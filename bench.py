@@ -35,7 +35,7 @@ import numpy as np  # noqa: E402
 
 
 _CLOCK_QUERY = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
-               "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+               "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
 
 def _clock_sampler_start(devs):
@@ -67,7 +67,9 @@ def _clocks_summary(samples):
     mx = max(int(s[1]) for s in samples if s[1].isdigit())
     names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
     reasons = [n for i, n in enumerate(names) if any(s[2 + i].lower().startswith("active") for s in samples)]
-    return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": reasons}
+    limits = [s[6] for s in samples if len(s) > 6]
+    return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": reasons,
+            "power_limit_w": float(limits[0]) if limits and limits[0].replace(".", "", 1).isdigit() else None}
 
 
 def _peak_hbm():
@@ -77,7 +79,7 @@ def _peak_hbm():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 def _host_cores():
@@ -329,7 +331,7 @@ def decision_run(torch, dist, Engine, synth, config, rank, world, local_rank, re
                        "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": None,
                        "algorithmic_bytes": int(alg), "peak_source": peak_src,
                        "note": "node state is shared-memory resident: the kernel is bound by issue slots / barrier latency per "
-                               "(template, group) step, not by HBM; see profiles/r02_summary.md for the ncu page"}
+                               "(template, group) step, not by HBM"}
     # ---- oracle on a template slice: parity of the timed result + the CPU arm of metric 2 + the §8(d) byte model
     try:
         tsel = _spread(enc.T, check_templates)
@@ -353,6 +355,35 @@ def decision_run(torch, dist, Engine, synth, config, rank, world, local_rank, re
     return out
 
 
+DUMP_BYTES = 48 << 20   # budget of the sampled bit matrix in --dump-outputs
+
+
+def dump_outputs(out_dir, torch, eng, T, Pl):
+    """What the last timed step left in HBM, i.e. what a caller of cae_feasibility receives: the fit histogram
+    fit_count[T] (after the exchange when N > 1) and the verdicts of this rank's pods, a fixed seeded sample of them
+    as 0/1 columns fit_bits[T][pods], with the sampled pod indices.  The synthetic inputs are seeded, so two builds
+    run with the same arguments can be compared array for array."""
+    def fetch(which, n):
+        ptr, nbytes = eng.device_buffer(which)
+        assert ptr and nbytes == 4 * n, "device buffer %d: %d bytes, expected %d" % (which, nbytes, 4 * n)
+
+        class _Wrap:
+            __cuda_array_interface__ = {"shape": (n,), "typestr": "<i4", "data": (ptr, False), "version": 3}
+        return torch.as_tensor(_Wrap(), device="cuda").cpu().numpy().view(np.uint32)
+
+    torch.cuda.synchronize()
+    Plw = (Pl + 31) // 32
+    count = fetch(0, T).view(np.int32)
+    bits = fetch(2, T * Plw).reshape(T, Plw)
+    n = min(Pl, max(1, DUMP_BYTES // (4 * max(T, 1))))
+    pods = np.sort(np.random.default_rng(0).choice(Pl, size=n, replace=False))
+    sample = (bits[:, pods // 32] >> (pods % 32).astype(np.uint32)) & np.uint32(1)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "fit_count.npy"), count.astype(np.float64))
+    np.save(os.path.join(out_dir, "fit_bits_sample.npy"), sample.astype(np.float32))
+    np.save(os.path.join(out_dir, "fit_bits_sample_pods.npy"), pods.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -367,6 +398,8 @@ def main():
     ap.add_argument("--counts-slice", default=None, help="reference arm: pb:pe:t0,t1,.. per-template fit counts (parity leg)")
     ap.add_argument("--cap", type=int, default=1000)
     ap.add_argument("--no-decision", action="store_true", help="engine arm: skip the decision-latency figures")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="engine arm: write what the last timed step computed to DIR/<name>.npy (rank 0)")
     ap.add_argument("--collective", default="peer", choices=["peer", "nccl"],
                     help="N>1: how the int32[T] fit histogram is reduced: fused P2P exchange in the kernel's last block, or NCCL")
     args = ap.parse_args()
@@ -408,7 +441,7 @@ def main():
     eng = Engine(device=local_rank, rank=rank, world_size=world, want_reasons=False, pods_presharded=world > 1)
     eng.load(enc)
     Pl = pe - pb
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")   # > 126 MB L2
+    flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")   # > 50 MB L2 of the H100
 
     count_t = None
     fused = False
@@ -432,8 +465,8 @@ def main():
     ar0 = torch.cuda.Event(enable_timing=True)
     ar1 = torch.cuda.Event(enable_timing=True)
     # The pass is a single ~10 us kernel: timed right after a host synchronize, the event window would mostly hold
-    # the HOST's launch latency (the GPU idles between the first event and the kernel's arrival: ~12 us for an
-    # empty kernel on this box, scripts/k1_floor.py).  So the L2 flush and a short spin kernel are queued on the
+    # the HOST's launch latency (the GPU idles between the first event and the kernel's arrival; scripts/k1_floor.py
+    # measures that floor with an empty kernel).  So the L2 flush and a short spin kernel are queued on the
     # engine's own stream first; event, kernel and event are then enqueued while the GPU is still busy and the
     # window measures device time only.  wall_ms_per_step keeps the host view.
     estream = torch.cuda.ExternalStream(eng.stream(), device=torch.device("cuda", local_rank))
@@ -484,6 +517,8 @@ def main():
         if count_t is not None:
             ar_ms.append(ar0.elapsed_time(ar1))
     launches = eng.stats().kernel_launches - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, torch, eng, T, Pl)
     for _ in range(10):                                        # host view of a step: launch + device + synchronize
         torch.cuda.synchronize()
         t0 = time.perf_counter()
@@ -638,32 +673,11 @@ def main():
     alg_bytes = Pl * (4 * Wd + 8) + T * 4 * Wd + Pl * T // 8 + 4 * T
     peak, peak_src = _peak_hbm()
     achieved = alg_bytes / (kern_ms * 1e-3) / 1e9
-    traffic = None
-    traffic_src = None
-    try:   # dram__bytes_read.sum + dram__bytes_write.sum of this kernel on this workload, one `ncu --set full` capture
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r01_k1_traffic.json")))
-        if args.config == 2 and P1 == 100_000 and T == 1000:
-            traffic = int(tj["dram__bytes_read.sum"]) + int(tj["dram__bytes_write.sum"])
-            traffic_src = "profiles/r01_k1_traffic.json (one `ncu --set full` capture of this kernel on this workload; not re-measured in this run)"
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "traffic_source": traffic_src, "kernel": "feasibility_lut_kernel", "algorithmic_bytes": alg_bytes,
-                "peak_source": peak_src,
+                "kernel": "feasibility_lut_kernel", "algorithmic_bytes": alg_bytes, "peak_source": peak_src,
                 "note": "the contract's HBM fraction; the kernel needs ~1 bit of DRAM traffic per evaluation and is bound by "
-                        "shared-memory wavefronts + fixed launch latency (see roofline_secondary and DESIGN.md)"}
-    # the kernel's own stated bound: shared-memory wavefronts (ncu l1tex__data_pipe_lsu_wavefronts_mem_shared of the capture above,
-    # 1.356 M per launch on C2) at one wavefront per SM per cycle
-    sm_mhz = None
+                        "shared-memory wavefronts + fixed launch latency (DESIGN.md)"}
     cs = _clocks_summary(samples)
-    if cs.get("sm_mhz"):
-        sm_mhz = cs["sm_mhz"]
-    roofline2 = None
-    if args.config == 2 and P1 == 100_000 and T == 1000 and sm_mhz:
-        wf = 1.356e6
-        floor_us = wf / 148.0 / (sm_mhz * 1e6) * 1e6
-        roofline2 = {"bound": "shared-memory wavefronts", "wavefronts_per_launch": wf, "floor_us": floor_us,
-                     "measured_us": kern_ms * 1e3, "frac": floor_us / (kern_ms * 1e3)}
 
     # ---- CPU baseline: the oracle on this box's cores, bounded sample of the same workload ---------------
     # (fresh processes: the oracle's worker pool must fork before any CUDA context exists)
@@ -692,7 +706,7 @@ def main():
         "step_ms_max_over_ranks": {"min": step_stats[0], "median": step_stats[1], "p99": step_stats[2], "max": step_stats[3]},
         "step_ms_rank0": [round(float(x), 5) for x in dev_ms],
         "collective": ("none" if world == 1 else ("fused exchange over NVLink peer memory inside the kernel" if fused else "NCCL all_reduce int32[T]")),
-        "wall_ms_per_step": float(np.mean(wall_ms)), "clocks": cs,
+        "wall_ms_per_step": float(np.mean(wall_ms)), "device": torch.cuda.get_device_name(local_rank), "clocks": cs,
         "e2e": {"value": (P1 * world) * T / (e2e_step * 1e-3), "unit": "evals/s", "ms_per_step": e2e_step,
                 "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                 "what": "per step: cae_load_pending (this step's pending-pod rows, host -> device, per-pod rows re-derived) + dense pass + "
@@ -700,7 +714,7 @@ def main():
                 "ms_per_step_full_load": e2e_full, "value_full_load": (P1 * world) * T / (e2e_full * 1e-3),
                 "ms_per_step_counts_only": e2e_counts, "value_counts_only": (P1 * world) * T / (e2e_counts * 1e-3)},
         "gpu_launches": int(launches), "parity_checked": bool(parity.get("checked")), "parity": parity,
-        "roofline": roofline, "roofline_secondary": roofline2, "cpu_baseline": cpu,
+        "roofline": roofline, "cpu_baseline": cpu,
         "dense_pass_large": dense_large, "decision_latency": headline_decision, "decisions": decisions}))
     if dist is not None:
         dist.destroy_process_group()

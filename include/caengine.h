@@ -1,5 +1,5 @@
 /*
- * caengine.h — C ABI of libcaengine.so, the B200-native scale-up simulation engine.
+ * caengine.h — C ABI of libcaengine.so, the H100-native scale-up simulation engine.
  *
  * This is the drop-in boundary for ONE hot path of the Cluster Autoscaler (reference
  * openshift/kubernetes-autoscaler, CA 1.35): pending pods x node-group templates through the
@@ -408,7 +408,8 @@ int32_t cae_expander_chain_ex(const int32_t* chain, int32_t chain_len, int32_t n
 int32_t cae_get_stats(cae_engine* e, cae_stats* out);
 
 /* Raw device pointers of the engine's result buffers, for zero-copy collectives (torch.distributed
- * / NCCL on the caller's side): 0 = fit_count int32[T], 1 = node_count|pod_count int32[2T]. */
+ * / NCCL on the caller's side): 0 = fit_count int32[T], 1 = node_count|pod_count int32[2T],
+ * 2 = fit_bits uint32[T][ceil(local pods / 32)] of the last cae_feasibility. */
 void* cae_device_buffer(cae_engine* e, int32_t which, size_t* bytes);
 
 /* The CUDA stream (cudaStream_t) every launch and copy of this engine is ordered on, for callers that order

@@ -589,7 +589,7 @@ static int32_t run_expander_chain(const int32_t* chain, int32_t chain_len, int T
 extern "C" {
 
 const char* cae_last_error(void) { return cae::g_err.c_str(); }
-const char* cae_version(void) { return "caengine/0.1 sm_100a"; }
+const char* cae_version(void) { return "caengine/0.1 sm_90a"; }
 
 int32_t cae_create(const cae_config* cfg, cae_engine** out) {
   if (!cfg || !out) return -2;
@@ -612,7 +612,11 @@ int32_t cae_create(const cae_config* cfg, cae_engine** out) {
   if (e->cfg.world_size < 1) e->cfg.world_size = 1;
   if (cudaSetDevice(cfg->device) != cudaSuccess) { cae::set_error("cudaSetDevice failed"); delete e; return -1; }
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, cfg->device) == cudaSuccess) { e->sm_count = prop.multiProcessorCount; e->smem_optin = (int)prop.sharedMemPerBlockOptin; }
+  if (cudaGetDeviceProperties(&prop, cfg->device) == cudaSuccess) {
+    e->sm_count = prop.multiProcessorCount;
+    e->smem_optin = (int)prop.sharedMemPerBlockOptin;
+    e->hbm_bytes = prop.totalGlobalMem;
+  }
   if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) { cae::set_error("stream create failed"); delete e; return -1; }
   cudaEventCreate(&e->ev0);
   cudaEventCreate(&e->ev1);
@@ -928,6 +932,7 @@ void* cae_device_buffer(cae_engine* h, int32_t which, size_t* bytes) {
   if (!e || !e->loaded) return nullptr;
   if (which == 0) { if (bytes) *bytes = sizeof(int32_t) * e->T; return e->d_fit_count; }
   if (which == 1) { if (bytes) *bytes = sizeof(int32_t) * 2 * e->T; return e->d_counts2; }
+  if (which == 2) { if (bytes) *bytes = sizeof(uint32_t) * (size_t)e->T * e->Plw; return e->d_fit_bits; }
   return nullptr;
 }
 

@@ -1542,7 +1542,7 @@ int launch_binpack(Engine* e) {
   p.scratch_per_cta = per_cta;
   int blocks = 0;
   if (launch_binpack_any(e, nt, smem, p, &blocks, true)) return -1;
-  const size_t budget = (size_t)24 << 30;  // keep the slabs within 24 GiB of the 180 GB HBM
+  const size_t budget = e->hbm_bytes / 8;  // keep the slabs within an eighth of the device memory (10 GB on an 80 GB H100)
   if (per_cta * blocks > budget) blocks = (int)std::max<size_t>(1, budget / per_cta);
   const size_t need = per_cta * blocks;
   const size_t sig = per_cta * 1000003u + Xg * 10007u + (size_t)p.dstride * 101u + (size_t)p.log_cap * 7u + (size_t)A1 + 0x9000000000ull;

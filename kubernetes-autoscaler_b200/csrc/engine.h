@@ -177,8 +177,9 @@ struct Engine {
   std::vector<int64_t> h_spec_req;        // [num_podspecs][R]
   std::vector<int64_t> h_cap_cpu, h_cap_mem;  // per template
   int num_podspecs = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   int smem_optin = 227 * 1024;             // opt-in shared memory per thread block
+  size_t hbm_bytes = (size_t)80 << 30;     // device memory (sizes the estimator's global slabs)
 };
 
 // kernels.cu

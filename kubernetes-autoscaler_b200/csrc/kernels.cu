@@ -1,4 +1,4 @@
-// kernels.cu — sm_100a kernels of the scale-up simulation engine.
+// kernels.cu — sm_90a kernels of the scale-up simulation engine.
 //
 //   class_matrix_kernel   (static class x universe node) -> reason/flag byte     [tables.cuh static_code]
 //   pack_ok_bits_kernel   byte matrix -> per-class template bit words

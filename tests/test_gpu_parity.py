@@ -509,3 +509,20 @@ def test_more_than_256_pods_per_node(eng, oracle):
     enc = encode([], [NodeInfo(node), NodeInfo(small)], groups)
     for caps in ([0, 0], [3, 7], [2, 2]):
         _check_estimate(eng, oracle, enc, caps)
+
+
+def test_device_buffers_hold_the_last_dense_pass(eng):
+    """cae_device_buffer 0 / 2 (what bench.py --dump-outputs reads): fit_count and fit_bits of the last cae_feasibility."""
+    import torch
+    enc = synth.generate(2, pods=3000, templates=70)
+    eng.load(enc)
+    bits, _, count = eng.feasibility()
+    torch.cuda.synchronize()
+    for which, want in ((0, count), (2, bits)):
+        ptr, nbytes = eng.device_buffer(which)
+        assert ptr and nbytes == want.nbytes
+
+        class _Wrap:
+            __cuda_array_interface__ = {"shape": (want.size,), "typestr": "<i4", "data": (ptr, False), "version": 3}
+        got = torch.as_tensor(_Wrap(), device="cuda").cpu().numpy()
+        assert np.array_equal(got.view(want.dtype).reshape(want.shape), want)
