@@ -87,6 +87,7 @@ struct PeerPush {
   int world, rank;           // world 0 = disabled
   int tag;                   // step number carried by every slot of this step (never 0)
   int2* data[8];             // every rank's [PEER_MAX][PEER_CAP] block of (count, tag) slots of this step's parity (P2P-mapped)
+  const int2* self;          // data[rank]
   int32_t* done_ctr;         // local: template chunks published
   int32_t* status;           // local: set to 1 when a peer never arrived
 };
@@ -127,6 +128,23 @@ __device__ __forceinline__ unsigned long long k1_globaltimer() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
+
+// Phase timeline of the dense pass, compiled in only with -DCAE_K1_PROF (scripts/k1_floor.py reads it through
+// cae_k1_prof_read): k1_prof[0] = %globaltimer when the stream reached the launch (a one-thread kernel queued just
+// before it), then per thread block K1_PROF_STAMPS stamps taken by thread 0: entry, loads done, compute done,
+// bit-matrix stores issued, exit.
+#ifdef CAE_K1_PROF
+constexpr int K1_PROF_MAX_BLOCKS = 8192, K1_PROF_STAMPS = 5;
+__device__ unsigned long long k1_prof[1 + K1_PROF_STAMPS * K1_PROF_MAX_BLOCKS];
+#define K1_STAMP(i)                                                                                 \
+  do {                                                                                              \
+    const int b_ = blockIdx.y * gridDim.x + blockIdx.x;                                             \
+    if (threadIdx.x == 0 && b_ < K1_PROF_MAX_BLOCKS) k1_prof[1 + K1_PROF_STAMPS * b_ + (i)] = k1_globaltimer(); \
+  } while (0)
+__global__ void k1_prof_mark_kernel() { k1_prof[0] = k1_globaltimer(); }
+#else
+#define K1_STAMP(i) do {} while (0)
+#endif
 
 // ---- epilogue shared by both variants -------------------------------------------------------------------
 // s_cnt holds this block's counts for templates t0 .. t0+K1_TCHUNK.  The LAST block of the chunk to arrive
@@ -170,11 +188,16 @@ __device__ __forceinline__ void k1_finish(const K1Args& a, const PeerPush& pp, c
   // which that peer wrote after it finished reading step s.
   __threadfence();
   const int tag = pp.tag;
-  for (int r = 0; r < pp.world; ++r) {
-    int2* dst = pp.data[r] + (size_t)pp.rank * Engine::PEER_CAP;
-    for (int t = tid; t < a.T; t += nthreads) k1_st_volatile_v2(dst + t, __ldcg(&a.fit_count[t]), tag);
+  // data[] is only indexed by unrolled constants and data[rank] comes as `self`: a run-time index would make every
+  // launch copy the whole struct to local memory, also at N = 1
+#pragma unroll
+  for (int r = 0; r < Engine::PEER_MAX; ++r) {
+    if (r < pp.world) {
+      int2* dst = pp.data[r] + (size_t)pp.rank * Engine::PEER_CAP;
+      for (int t = tid; t < a.T; t += nthreads) k1_st_volatile_v2(dst + t, __ldcg(&a.fit_count[t]), tag);
+    }
   }
-  const int2* mine = pp.data[pp.rank];
+  const int2* mine = pp.self;
   const unsigned long long t0ns = k1_globaltimer();
   int ok = 1;
   for (int t = tid; t < a.T && ok; t += nthreads) {
@@ -267,9 +290,14 @@ __device__ __forceinline__ uint32_t warp_transpose32(uint32_t x, int lane) {
 }
 
 // ---- LUT variant --------------------------------------------------------------------------------------------
+// Resident warps per SM the kernel is compiled for, the most that keeps it free of spills: 48 (at most 40 registers per
+// thread), 32 (64 registers) for the dim counts that would spill at 40, 16 for the reasons variant (its per-template
+// loop of byte stores is bound by memory, not by the warps in flight).
+template <int A, bool REASONS>
+constexpr int k1_lut_warps_per_sm() { return REASONS ? 16 : (A == 0 || A > 5) ? 32 : 48; }
 
 template <int A, bool REASONS, int NW>
-__global__ void __launch_bounds__(NW * 32, 48 / NW)
+__global__ void __launch_bounds__(NW * 32, k1_lut_warps_per_sm<A, REASONS>() / NW)
 feasibility_lut_kernel(K1Args a, int rows, PeerPush pp) {
   extern __shared__ uint32_t k1_smem[];
   constexpr int NT = NW * 32;
@@ -285,6 +313,7 @@ feasibility_lut_kernel(K1Args a, int rows, PeerPush pp) {
   const int npw = a.gq + ((int)blockIdx.x < a.gr ? 1 : 0);
   const int p = (pwb + warp) * 32 + lane;
   const bool valid = warp < npw && p < a.Pl;
+  K1_STAMP(0);
 
 #pragma unroll 1
   for (int i = tid; i < rows * K1_TW; i += NT) {
@@ -315,6 +344,7 @@ feasibility_lut_kernel(K1Args a, int rows, PeerPush pp) {
   }
   const TransposeConsts tc = transpose_consts(lane);
   __syncthreads();
+  K1_STAMP(1);
 
 #pragma unroll
   for (int tw = 0; tw < K1_TW; tw += 2) {
@@ -349,6 +379,7 @@ feasibility_lut_kernel(K1Args a, int rows, PeerPush pp) {
     atomicAdd(&s_cnt[(tw + 1) * 32 + lane], __popc(c1));
   }
   __syncthreads();
+  K1_STAMP(2);
   // flush: NW consecutive threads write the block's run of pod words of one template row
   if (a.fit_bits) {
     const int wv = tid % NW;
@@ -361,7 +392,9 @@ feasibility_lut_kernel(K1Args a, int rows, PeerPush pp) {
       for (int k = 0; k < kmax; ++k, dst += stride, src += 32) *dst = *src;
     }
   }
+  K1_STAMP(3);
   k1_finish(a, pp, s_cnt, t0, tid, NT);
+  K1_STAMP(4);
 }
 
 // ---- bit-sliced variant ---------------------------------------------------------------------------------------
@@ -462,6 +495,7 @@ static PeerPush peer_push_args(Engine* e) {
     pp.tag = (int)(e->peer_step & 0x7fffffff);
     if (pp.tag == 0) pp.tag = 1;
     for (int r = 0; r < e->peer_world; ++r) pp.data[r] = reinterpret_cast<int2*>(e->peer_base[r]) + par * blk;
+    pp.self = pp.data[pp.rank];
     pp.done_ctr = e->d_xbuf + 4 * blk + 8;
     pp.status = e->d_xbuf + 4 * blk + 9;
   }
@@ -495,7 +529,7 @@ template <int A, bool REASONS, int NW>
 static int launch_feas_lut_arw(Engine* e, K1Args a, const PeerPush& pp) {
   const int chunks = e->Twp / K1_TW;
   // one wave when it fits: the pod words are split evenly over as many blocks as the SMs hold at once
-  const int slots = e->sm_count * (48 / NW);
+  const int slots = e->sm_count * (k1_lut_warps_per_sm<A, REASONS>() / NW);
   const int g_min = (e->Plw + NW - 1) / NW;
   a.G = std::max(g_min, std::min(e->Plw, std::max(1, slots / chunks)));
   a.gq = e->Plw / a.G;
@@ -527,6 +561,14 @@ int launch_feasibility(Engine* e, bool want_reasons) {
     set_error("fused histogram exchange: more templates than the exchange buffer holds (use the NCCL all-reduce of cae_device_buffer(0))");
     return 1;
   }
+#ifdef CAE_K1_PROF
+  {
+    void* prof = nullptr;
+    CAE_CUDA(cudaGetSymbolAddress(&prof, k1_prof));
+    CAE_CUDA(cudaMemsetAsync(prof, 0, sizeof(k1_prof), e->stream));
+    k1_prof_mark_kernel<<<1, 1, 0, e->stream>>>();
+  }
+#endif
   const PeerPush pp = peer_push_args(e);
   const K1Args a = k1_args(e);
   if (!e->force_bitslice && e->lut_rows <= K1_LUT_MAX_ROWS) {
@@ -564,3 +606,12 @@ int launch_feasibility(Engine* e, bool want_reasons) {
 }
 
 }  // namespace cae
+
+#ifdef CAE_K1_PROF
+// the phase stamps of the last dense pass (synchronous): 1 + K1_PROF_STAMPS * blocks values, returns the count copied
+extern "C" int cae_k1_prof_read(unsigned long long* out, int n) {
+  n = std::max(0, std::min(n, 1 + cae::K1_PROF_STAMPS * cae::K1_PROF_MAX_BLOCKS));
+  if (cudaMemcpyFromSymbol(out, cae::k1_prof, sizeof(unsigned long long) * n) != cudaSuccess) return -1;
+  return n;
+}
+#endif
