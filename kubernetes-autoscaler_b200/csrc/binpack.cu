@@ -520,6 +520,9 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
       float rinv[A1];
 #pragma unroll
       for (int a = 0; a < A; ++a) { req[a] = rc.req[a]; rinv[a] = rc.rinv[a]; }
+      // no node holds more than LLONG_MAX / req[a] pods, so the capacities below start from at most kcap and
+      // k * req[a] cannot wrap int64
+      const int kcap = rc.kcap;
       const int sc = rc.sc;
       const int dc = rc.dc;
       const bool static_new = !(ord_cur & ORDER_NOT_ON_FRESH);
@@ -543,7 +546,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
 
       // spare capacity of node x for this pod by NodePorts + NodeResourcesFit alone (pod slots, free resources)
       auto res_cap_of = [&](auto frf, int slots, unsigned long long ports, int want) -> int {
-        int k = min(slots, want);
+        int k = min(min(slots, want), kcap);
         if (k > 0 && (ports & pconf)) k = 0;
 #pragma unroll
         for (int a = 0; a < A; ++a) {
@@ -583,7 +586,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
       auto fresh_cap = [&](int want) -> int {
         int k = 0;
         if (static_new) {
-          k = min(tslots, want);
+          k = min(min(tslots, want), kcap);
 #pragma unroll
           for (int a = 0; a < A; ++a) {
             if (req[a] > 0 && k > 0) {
@@ -1598,6 +1601,7 @@ __global__ void run_rec_kernel(DevObjects o, DynTables d, int runs, const int32_
   const int pb = run_off[r];
   g.n = run_off[r + 1] - pb;
   g.pad[0] = pb;
+  g.kcap = INT_MAX;
   const int spec = o.pend_spec[pods[pb]];
   g.spec = spec;
   g.sc = spec_sc[spec];
@@ -1612,6 +1616,7 @@ __global__ void run_rec_kernel(DevObjects o, DynTables d, int runs, const int32_
   for (int a = 0; a < n_act; ++a) {
     g.req[a] = o.ps_req[(size_t)spec * R + act_dim[a]];
     g.rinv[a] = g.req[a] > 0 ? __frcp_rn(__ll2float_rn(g.req[a])) : 0.f;
+    if (g.req[a] >> 32) g.kcap = min(g.kcap, (int)(LLONG_MAX / g.req[a]));
   }
   out[r] = g;
 }

@@ -23,7 +23,8 @@ void set_error(const std::string& msg);
 struct alignas(16) GroupRec {
   int32_t n, spec, sc, dc;            // pods, pod spec, static class, dynamic class (0 = plain)
   uint32_t flags;                     // GREC_*
-  int32_t pad[3];
+  int32_t pad[2];
+  int32_t kcap;                       // most pods of the group a node can hold without k x req wrapping int64
   unsigned long long pconf, pbit;     // host-port sets the pod collides with / the bit of its own set
   int64_t req[CAE_MAX_RES];           // request per ACTIVE resource dim
   float rinv[CAE_MAX_RES];            // 1 / req (0 when the dim is not requested)

@@ -231,6 +231,7 @@ __global__ void group_rec_kernel(DevObjects o, int E, ActDims act, int has_dyn, 
   GroupRec r{};
   const int pb = o.group_off[g];
   r.n = o.group_off[g + 1] - pb;
+  r.kcap = INT_MAX;
   if (r.n > 0) {
     const int spec = o.pend_spec[pb];
     r.spec = spec;
@@ -245,6 +246,7 @@ __global__ void group_rec_kernel(DevObjects o, int E, ActDims act, int has_dyn, 
     for (int a = 0; a < act.n; ++a) {
       r.req[a] = o.ps_req[(size_t)spec * R + act.dim[a]];
       r.rinv[a] = r.req[a] > 0 ? __frcp_rn(__ll2float_rn(r.req[a])) : 0.f;
+      if (r.req[a] >> 32) r.kcap = min(r.kcap, (int)(LLONG_MAX / r.req[a]));   // below 2^32, k < 2^31 cannot wrap
     }
   }
   out[g] = r;

@@ -83,12 +83,23 @@ class SplitMix64:
 
 
 RESERVED = {2: 70, 4: 80, 8: 90, 16: 110, 32: 150, 64: 230, 96: 310}
+# the resource dims of generate(dims=...) (CAE_MAX_RES of them), the unit of their request values, the requests of the
+# DaemonSet pods every node holds, and the default number of distinct request values per active dim
+DIMS = ("cpu", "memory", "ephemeral-storage", "example.com/r0", "example.com/r1", "example.com/r2", "example.com/r3",
+        "example.com/r4")
+DIM_UNIT = (50, 64 * MiB, GiB, 1, 1, 1, 1, 1)
+DS_REQ = [100, 200 * MiB, 0, 0, 0, 0, 0, 0]
+DIM_CARD = 3
 
 
 def generate(config: int = 2, pods: Optional[int] = None, templates: Optional[int] = None,
              cluster_nodes: Optional[int] = None, taints: Optional[bool] = None,
              spread: Optional[bool] = None, affinity: Optional[bool] = None,
-             seed: Optional[int] = None) -> EncodedObjects:
+             seed: Optional[int] = None, dims=None) -> EncodedObjects:
+    """dims = None: the requests of the module docstring (cpu, memory, nvidia.com/gpu as dim 3).  Otherwise the dims the
+    pending pods request, out of the 8 of ``DIMS``: a sequence of dim indices (DIM_CARD distinct values each), or a mapping
+    dim -> number of distinct request values.  Then a second stream draws every request and the allocatable of the active
+    dims (the first draws are unchanged), and there are at least as many groups as the largest count."""
     cfg = CONFIGS[config]
     P = cfg.pods if pods is None else pods
     T = cfg.templates if templates is None else templates
@@ -97,7 +108,8 @@ def generate(config: int = 2, pods: Optional[int] = None, templates: Optional[in
     use_spread = cfg.spread if spread is None else spread
     use_aff = cfg.affinity if affinity is None else affinity
     rng = SplitMix64((0xCA5CA1E0 + cfg.index) if seed is None else seed)
-    b = TableBuilder(num_res=4)
+    card = None if dims is None else (dict(dims) if isinstance(dims, dict) else {int(a): DIM_CARD for a in dims})
+    b = TableBuilder(num_res=4 if card is None else len(DIMS))
     b.hostname_key = K_HOST
     b.unschedulable_taint_key = -1
     for ns in range(32):
@@ -107,6 +119,8 @@ def generate(config: int = 2, pods: Optional[int] = None, templates: Optional[in
     V_ZONE0, V_POOL0, V_ITYPE0, V_TIER0, V_TAINTV0 = 0, 16, 24, 48, 52
     V_APP0 = 64
     E = max(1, P // 100)
+    if card:
+        E = max(E, max(card.values()))
     V_HOST0 = V_APP0 + E
     b.declare_value(V_HOST0 + T + NC + 1, None)
 
@@ -140,6 +154,14 @@ def generate(config: int = 2, pods: Optional[int] = None, templates: Optional[in
     pts_mind = rng.choice(E, [1, 3], [1, 1])
     u_aff = rng.uniform(E)
     aff_other = rng.randint(E, max(E, 1))
+    if card is not None:   # request of group g in dim a: DIM_UNIT[a] x (1 + level), every level of a dim used once E allows
+        rd = SplitMix64(((0xCA5CA1E0 + cfg.index) if seed is None else seed) ^ 0xD1B54A32D192ED03)
+        dim_req = np.zeros((E, len(DIMS)), np.int64)
+        for a, d in sorted(card.items()):
+            lvl = rd.randint(E, d)
+            n = min(E, d)
+            lvl[:n] = rd.next(n).argsort()
+            dim_req[:, a] = DIM_UNIT[a] * (1 + lvl)
 
     taint_ids = [(K_TAINT0 + k, V_TAINTV0 + v) for k in range(8) for v in range(2)]
     group_spec: List[int] = []
@@ -176,13 +198,13 @@ def generate(config: int = 2, pods: Optional[int] = None, templates: Optional[in
                 og = int(aff_other[g])
                 osel = b.selector([(K_APP, 0, (V_APP0 + og,))])
                 aff = b.affinity_list([(osel, K_ZONE, (int(ns_of[og]),), nothing)])
-        req = [int(cpu[g]), int(mem[g]), 0, int(gpu[g])]
+        req = [int(cpu[g]), int(mem[g]), 0, int(gpu[g])] if card is None else dim_req[g].tolist()
         group_spec.append(b.podspec(int(ns_of[g]), ls, req, b.toleration_list(tols), naff, -1, 0, pts, aff, anti))
 
     # ---- DaemonSet pods (kube-system = namespace 31, no labels anyone selects) --------------------
     ds_ls = b.labelset([(K_TIER, V_TIER0 + 3)])
     ds_tol = b.toleration_list([(-1, 1, -1, 0)])
-    ds_spec = [b.podspec(31, ds_ls, [100, 200 * MiB, 0, 0], ds_tol), b.podspec(31, ds_ls, [100, 200 * MiB, 0, 0], ds_tol)]
+    ds_spec = [b.podspec(31, ds_ls, DS_REQ[:4], ds_tol), b.podspec(31, ds_ls, DS_REQ[:4], ds_tol)]
 
     # ---- nodes ----------------------------------------------------------------------------------
     def node_shape(n: int, r: SplitMix64):
@@ -194,6 +216,10 @@ def generate(config: int = 2, pods: Optional[int] = None, templates: Optional[in
 
     def add_nodes(n: int, first_host: int, is_template: bool, resident: Optional[np.ndarray]):
         vcpu, mem_per, ngpu, zone, pool, u_t, tbits = node_shape(n, rng)
+        if card is not None:   # allocatable of an active dim: 1/2 .. 2x its largest request, on top of the DaemonSet pods
+            dim_alloc = np.zeros((n, len(DIMS)), np.int64)
+            for a, d in sorted(card.items()):
+                dim_alloc[:, a] = DS_REQ[a] + DIM_UNIT[a] * (d // 2 + rd.randint(n, 2 * d - d // 2 + 1))
         for i in range(n):
             v = int(vcpu[i])
             cap_cpu = v * 1000
@@ -211,8 +237,13 @@ def generate(config: int = 2, pods: Optional[int] = None, templates: Optional[in
             pods = list(ds_spec)
             if resident is not None:
                 pods += [group_spec[int(x)] for x in resident[i]]
+            alloc = [alloc_cpu, alloc_mem, 0, int(ngpu[i])]
+            if card is not None:
+                alloc = [alloc_cpu, alloc_mem] + [0] * (len(DIMS) - 2)
+                for a in card:
+                    alloc[a] = int(dim_alloc[i, a])
             args = dict(name=first_host + i, labelset=ls, taint_list=b.taint_list(tl), unschedulable=False,
-                        alloc=[alloc_cpu, alloc_mem, 0, int(ngpu[i])], allowed_pods=110, cap_cpu=cap_cpu,
+                        alloc=alloc, allowed_pods=110, cap_cpu=cap_cpu,
                         cap_mem=cap_mem, has_alloc_cpu=True, has_alloc_mem=True, pod_specs=pods)
             (b.template if is_template else b.cluster_node)(**args)
 

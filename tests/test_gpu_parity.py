@@ -526,3 +526,71 @@ def test_device_buffers_hold_the_last_dense_pass(eng):
             __cuda_array_interface__ = {"shape": (want.size,), "typestr": "<i4", "data": (ptr, False), "version": 3}
         got = torch.as_tensor(_Wrap(), device="cuda").cpu().numpy()
         assert np.array_equal(got.view(want.dtype).reshape(want.shape), want)
+
+
+def _quantities_enc(cluster, templates, groups):
+    """Snapshot at the integer level: dims cpu, memory, ephemeral-storage, example.com/bw.  cluster / templates:
+    (alloc, allowed pods, requests of the resident DaemonSet pods or None); groups: (requests, pod count)."""
+    from kubernetes_autoscaler_b200.encode import TableBuilder
+    b = TableBuilder(num_res=4)
+    b.hostname_key = 0
+    b.declare_namespace(0)
+    b.declare_value(len(cluster) + len(templates), None)
+    for i, (alloc, allowed, ds) in enumerate(cluster + templates):
+        pods = [] if ds is None else [b.podspec(0, 0, ds)]
+        node = b.template if i >= len(cluster) else b.cluster_node
+        node(name=i, labelset=b.labelset([(0, i)]), taint_list=0, unschedulable=False, alloc=alloc, allowed_pods=allowed,
+             cap_cpu=alloc[0], cap_mem=alloc[1], has_alloc_cpu=True, has_alloc_mem=True, pod_specs=pods)
+    for req, count in groups:
+        b.group(np.full(count, b.podspec(0, b.labelset([(1, len(b.group_off))]), req), np.int32))
+    return b.finish()
+
+
+_G, _T = 1 << 30, 1 << 40
+_BASE = [64_000, 256 * _G, 0]
+# (name, templates, groups, (nodes, pods) of the first template with unlimited caps)
+EXTREME_CASES = [
+    # k x request wraps int64: 10 x 2^61 = 2^62 (mod 2^64) <= 2^62 + 5, yet a node takes 2 pods
+    ("bw_product_wraps", [(_BASE + [(1 << 62) + 5], 110, None)], [([100, _G, 0, 1 << 61], 10)], (5, 10)),
+    # free = INT64_MAX, request 2^62: one pod per node; 2 x 2^62 = 2^63 wraps in the floor division's correction
+    ("free_int64_max", [(_BASE + [(1 << 63) - 1], 110, None)], [([100, _G, 0, 1 << 62], 10)], (10, 10)),
+    # requests exactly equal to free, in every dim at once
+    ("request_equals_free", [([3000, 6 * _G, 9 * _T, 3 << 60], 110, [1000, 2 * _G, 3 * _T, 1 << 60])],
+     [([1000, 2 * _G, 3 * _T, 1 << 60], 7)], (4, 7)),
+    # DaemonSet pods overcommit cpu on the first template: its free cpu is negative, only pods without a cpu request fit
+    ("negative_free", [([1000, 4 * _G, 0, 10], 110, [1500, _G, 0, 0]), (_BASE + [10], 110, [1500, _G, 0, 0])],
+     [([100, _G, 0, 1], 4), ([0, 0, 0, 3], 5)], (2, 5)),
+    # allocatable 2^62, request 1: the pod slots bind
+    ("alloc_2pow62_tiny_requests", [([1 << 62, 1 << 62, 1 << 62, 1 << 62], 110, None)], [([1, 1, 1, 1], 500)], (5, 500)),
+]
+
+
+def test_extreme_quantities(eng, oracle):
+    """Legal Kubernetes quantities at the edges of int64 in the estimator and the filter pass: k x request above 2^63
+    (the per-node capacity must still be cut by that dim), free close to INT64_MAX (the exact floor division must not wrap),
+    requests exactly equal to free, negative template free under overcommitting DaemonSet pods, allocatable 2^62 with tiny
+    requests, and more than 2^20 pods of a group on one node (the double-precision division)."""
+    for name, templates, groups, exp in EXTREME_CASES:
+        enc = _quantities_enc([], templates, groups)
+        _check_dense(eng, oracle, enc)
+        _check_estimate(eng, oracle, enc, np.full(enc.T, 3, np.int32))
+        nc, pc = _check_estimate(eng, oracle, enc, np.zeros(enc.T, np.int32))
+        assert (int(nc[0]), int(pc[0])) == exp, name
+
+    # more than 2^20 pods of one group on one node: the estimator's capacity takes the double-precision division.  The
+    # oracle places such a group pod by pod for many minutes; its answer is the closed form asserted here.
+    big = 1_100_000
+    enc = _quantities_enc([], [(_BASE[:2] + [0, 3 * 1_050_000 + 2], 3_000_000, None), (_BASE[:2] + [0, 1 << 62], 2_500_000, None)],
+                          [([0, 0, 0, 3], big)])
+    eng.load(enc)
+    nc, pc, sched, order = eng.estimate_all(np.zeros(enc.T, np.int32))
+    assert nc.tolist() == [2, 1] and pc.tolist() == [big, big] and sched.tolist() == [[big], [big]]
+
+    # the filter pass on cluster nodes: 2^62 + 5 of bw holds two pods of 2^61 each
+    enc = _quantities_enc([(_BASE + [(1 << 62) + 5], 110, None)] * 3, [(_BASE + [0], 110, None)], [([100, _G, 0, 1 << 61], 10)])
+    order = np.arange(enc.P, dtype=np.int32)
+    eng.load(enc)
+    got = eng.filter_schedulable(order)
+    want = oracle.filter_schedulable(enc, order)
+    assert np.array_equal(got[0], want[0]) and got[1:] == want[1:]
+    assert int((want[0] >= 0).sum()) == 6
