@@ -297,6 +297,55 @@ int32_t cae_load(cae_engine* e, const cae_objects* objs);
  * group -> spec sequence): call cae_load with the full snapshot instead.  Nothing is changed in that case. */
 int32_t cae_load_pending(cae_engine* e, int32_t num_pending, const int32_t* pend_spec, int32_t num_groups, const int32_t* group_off);
 
+/* The per-tick delta of the cluster nodes: new rows for EXISTING cluster nodes against the snapshot that is already resident.
+ * Replaces: the NodeInfo updates of DeltaSnapshotStore.SetClusterState between two loops (a pod bound or finished, a node
+ * cordoned, a taint added, allocatable changed) without re-interning, re-ranking and re-uploading the whole snapshot.
+ * The caller's interner is append-only: ids below the resident counts keep their meaning, and the new dictionary entries
+ * a changed row needs arrive as TAILS that continue the resident tables.  A dirty row carries its complete new state
+ * except the node name (the row's identity), the capacity and has_alloc_* (read for templates only).  After the call
+ * every entry point answers bit-identically to a cae_load of the updated objects.  Pending pods and templates are not
+ * touched (combine with cae_load_pending, in either order).
+ * Status -2 (malformed, nothing changed): NULL arrays with non-zero counts, rows out of range or not strictly increasing,
+ *   ids outside the resident tables plus the tails, offsets that do not start at 0 or decrease, label pairs not sorted
+ *   by strictly increasing key id, taint effects outside enum cae_effect.
+ * Status 2 (the delta does not apply: call cae_load with the full snapshot; nothing is changed):
+ *   - a dirty row's value of a topology key the resident counters use (PodTopologySpread / InterPodAffinity) changes,
+ *     appears or disappears — the topology domains would be renumbered;
+ *   - a new resident pod's spec has required anti-affinity terms and no pod of that spec was in the snapshot (pending or
+ *     resident) at the last cae_load — it could add an existing-anti-affinity counter;
+ *   - the resident pods of all nodes, or the entries of a dictionary table, would pass 2^31 - 1 (checked from the counts
+ *     and offsets alone, before any pod-spec id is read).
+ * Adding or removing nodes, template changes and pod specs the last cae_load did not have cannot be expressed: cae_load. */
+typedef struct cae_node_delta {
+  int32_t abi_version; /* CAE_ABI_VERSION */
+  /* dictionary tails: value ids [num_values, num_values + num_new_values) of the resident snapshot */
+  int32_t num_new_values;
+  const uint8_t* value_is_int; /* [num_new_values] */
+  const int64_t* value_int;    /* [num_new_values] */
+  /* label sets [num_labelsets, num_labelsets + num_new_labelsets); pairs sorted by key id as in cae_objects */
+  int32_t num_new_labelsets;
+  const int32_t* ls_off; /* [num_new_labelsets + 1], relative to the tail (ls_off[0] == 0) */
+  const int32_t* ls_key;
+  const int32_t* ls_val;
+  /* taint lists [num_taint_lists, num_taint_lists + num_new_taint_lists) */
+  int32_t num_new_taint_lists;
+  const int32_t* taint_off; /* [num_new_taint_lists + 1], relative to the tail */
+  const int32_t* taint_key;
+  const int32_t* taint_val;
+  const int32_t* taint_effect;
+  /* dirty cluster-node rows, strictly increasing, each < num_cluster_nodes */
+  int32_t num_dirty;
+  const int32_t* row;
+  const int32_t* labelset;
+  const int32_t* taint_list;
+  const uint8_t* unschedulable;
+  const int64_t* alloc;        /* [num_dirty * CAE_MAX_RES] Status.Allocatable */
+  const int32_t* allowed_pods;
+  const int32_t* pod_off;      /* [num_dirty + 1]: the COMPLETE new resident-pod list of each dirty row */
+  const int32_t* pod_spec;     /* pod-spec ids of the resident table */
+} cae_node_delta;
+int32_t cae_load_nodes(cae_engine* e, const cae_node_delta* d);
+
 int32_t cae_feasibility(cae_engine* e, uint32_t* fit_bits, uint8_t* reasons, int32_t* fit_count);
 
 /* Exemplar feasibility, what the orchestrator itself asks: group exemplar x template.

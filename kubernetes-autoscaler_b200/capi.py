@@ -91,6 +91,10 @@ class cae_price_inputs(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_price_inputs")
 
 
+class cae_node_delta(C.Structure):
+    _fields_ = _parse_struct(_SRC, "cae_node_delta")
+
+
 def declared_functions() -> List[str]:
     """Names of every function the header declares (used by the symbol-export test)."""
     return sorted(set(re.findall(r"\b(cae_\w+)\s*\(", _SRC)))
@@ -140,6 +144,8 @@ def load_engine_lib() -> C.CDLL:
     lib.cae_load.restype = C.c_int32
     lib.cae_load_pending.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.cae_load_pending.restype = C.c_int32
+    lib.cae_load_nodes.argtypes = [C.c_void_p, P(cae_node_delta)]
+    lib.cae_load_nodes.restype = C.c_int32
     lib.cae_feasibility.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.cae_feasibility.restype = C.c_int32
     lib.cae_feasibility_groups.argtypes = [C.c_void_p, C.c_void_p]

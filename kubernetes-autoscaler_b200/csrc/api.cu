@@ -108,6 +108,8 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
   auto nonempty = [&](const int32_t* off, int l) { return off[l + 1] > off[l]; };
   std::vector<uint8_t> spec_used(spec_pending);
   for (int i = 0; i < o->node_pod_off[NT]; ++i) spec_used[o->node_pod_spec[i]] = 1;
+  e->nh.spec_used = spec_used;
+  e->nh.key_val.clear();
   bool any = false;
   std::vector<int> keys;
   auto add_key = [&](int key) { if (std::find(keys.begin(), keys.end(), key) == keys.end()) keys.push_back(key); };
@@ -130,6 +132,7 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
   if ((int)keys.size() > DYN_MAX_KEYS) { set_error("more than 8 distinct topology keys"); return 1; }
   d.K = (int)keys.size();
   std::vector<int32_t> dom((size_t)d.K * NT, -1);
+  e->nh.key_val.assign((size_t)d.K * N, -1);
   for (int k = 0; k < d.K; ++k) {
     d.key_id[k] = keys[k];
     d.is_host[k] = keys[k] == o->hostname_key;
@@ -138,6 +141,7 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
       if (row == N) d.Dc[k] = (int)ids.size();
       int v;
       if (!host_label(o, o->node_labelset[row], keys[k], &v)) continue;
+      if (row < N) e->nh.key_val[(size_t)k * N + row] = v;
       auto it = ids.find(v);
       if (it == ids.end()) it = ids.emplace(v, (int)ids.size()).first;
       dom[(size_t)k * NT + row] = it->second;
@@ -181,6 +185,7 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
     if (o->group_off[g + 1] > o->group_off[g]) dc_ngroups[spec_dc[o->pend_spec[o->group_off[g]]]]++;
   d.DC = (int)dc_spec.size();
   d.Q = (int)q_kind.size();
+  d.pool = q_base_off.back();
   e->DC = d.DC;
   const int32_t* p32 = nullptr; const uint8_t* p8 = nullptr;
 #define UPV(vec, field) { if (upload(e, (vec).data(), (vec).size(), &field)) return -1; }
@@ -488,8 +493,25 @@ static int do_load(Engine* e, const cae_objects* o) {
   e->d_reasons = nullptr;
   if (e->cfg.want_reasons && dev_alloc(e, &e->d_reasons, (size_t)std::max(T, 1) * std::max(e->Pl, 1))) return -1;
 
-  // host copies for host-side steps (homogeneity check) and for the per-tick delta (cae_load_pending)
+  // host copies for host-side steps (homogeneity check) and for the per-tick deltas (cae_load_pending, cae_load_nodes)
   e->h_spec_pending = spec_pending;
+  {
+    Engine::NodeHost& nh = e->nh;   // spec_used and key_val come from build_dynamic
+    nh.num_values = o->num_values;
+    nh.num_labelsets = o->num_labelsets;
+    nh.num_taint_lists = o->num_taint_lists;
+    nh.taint_entries = o->taint_off[o->num_taint_lists];
+    const int np = o->ls_off[o->num_labelsets];
+    nh.ls_off.assign(o->ls_off, o->ls_off + o->num_labelsets + 1);
+    nh.ls_key.assign(o->ls_key, o->ls_key + np);
+    nh.ls_val.assign(o->ls_val, o->ls_val + np);
+    nh.pod_cnt.resize(N);
+    for (int n = 0; n < N; ++n) nh.pod_cnt[n] = o->node_pod_off[n + 1] - o->node_pod_off[n];
+    nh.pod_total = o->node_pod_off[NT];
+    nh.spec_anti.resize(S);
+    for (int s = 0; s < S; ++s) nh.spec_anti[s] = o->aff_off[o->ps_anti_list[s] + 1] > o->aff_off[o->ps_anti_list[s]];
+    e->h_spec_req.assign(o->ps_req, o->ps_req + (size_t)S * R);
+  }
   e->cap_P = e->P; e->cap_E = e->E; e->cap_Pl = e->Pl;
   { int rc = stage_pending(e, e->P, o->pend_spec, e->E, o->group_off, false); if (rc) return rc; }
 
@@ -520,6 +542,195 @@ static int do_load(Engine* e, const cae_objects* o) {
   cudaEventElapsedTime(&ms, e->ev0, e->ev1);
   e->stats.h2d_ms = ms;
   e->loaded = true;
+  return 0;
+}
+
+// Append a dictionary tail (already on the device, in the staged delta) to a DevObjects table.  The grown table lives in an
+// engine-owned buffer: the first delta after a load copies the arena's contents there once, later deltas append in place
+// while the headroom lasts.
+template <class T>
+static int grow_table(Engine* e, Engine::DevBuf& b, const T*& cur, size_t n_old, const void* d_tail, size_t n_tail) {
+  if (n_tail == 0) return 0;
+  const size_t need = (n_old + n_tail) * sizeof(T);
+  if (cur != b.p || need > b.cap) {
+    Engine::DevBuf nb = b;
+    if (need > b.cap) {
+      nb.cap = need + need / 2 + 4096;
+      CAE_CUDA(cudaMallocAsync(&nb.p, nb.cap, e->stream));
+    }
+    if (n_old) CAE_CUDA(cudaMemcpyAsync(nb.p, cur, n_old * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
+    if (nb.p != b.p && b.p) CAE_CUDA(cudaFreeAsync(b.p, e->stream));   // stream-ordered: after the copy out of it
+    b = nb;
+  }
+  CAE_CUDA(cudaMemcpyAsync(static_cast<T*>(b.p) + n_old, d_tail, n_tail * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
+  cur = static_cast<const T*>(b.p);
+  return 0;
+}
+
+// cae_load_nodes: every check on the host first (nothing is changed unless the whole delta applies), then the device work in
+// stream order without a host synchronisation: dictionary tails, dirty rows + resident CSR, pre_code of the dirty columns,
+// the topology counters and the tables derived from them.
+static int do_load_nodes(Engine* e, const cae_node_delta* dl) {
+  auto bad = [](const char* m) { set_error(std::string("cae_load_nodes: ") + m); return -2; };
+  auto refuse = [](const char* m) { set_error(std::string("cae_load_nodes: ") + m); return 2; };
+  if (dl->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
+  Engine::NodeHost& nh = e->nh;
+  const int N = e->N, S = e->num_podspecs, A = e->A;
+  const int nv = dl->num_new_values, nl = dl->num_new_labelsets, ntl = dl->num_new_taint_lists, nd = dl->num_dirty;
+  if (nv < 0 || nl < 0 || ntl < 0 || nd < 0) return bad("negative count");
+  if (nv && (!dl->value_is_int || !dl->value_int)) return bad("value tail without arrays");
+  if (nl && !dl->ls_off) return bad("label-set tail without offsets");
+  if (ntl && !dl->taint_off) return bad("taint-list tail without offsets");
+  if (nd && (!dl->row || !dl->labelset || !dl->taint_list || !dl->unschedulable || !dl->alloc || !dl->allowed_pods || !dl->pod_off))
+    return bad("dirty rows without arrays");
+  auto offsets_ok = [](const int32_t* off, int n) {
+    if (off[0] != 0) return false;
+    for (int i = 0; i < n; ++i) if (off[i + 1] < off[i]) return false;
+    return true;
+  };
+  if (nl && !offsets_ok(dl->ls_off, nl)) return bad("label-set offsets");
+  if (ntl && !offsets_ok(dl->taint_off, ntl)) return bad("taint-list offsets");
+  if (nd && !offsets_ok(dl->pod_off, nd)) return bad("resident-pod offsets");
+  const int64_t pairs = nl ? dl->ls_off[nl] : 0, tents = ntl ? dl->taint_off[ntl] : 0, npods = nd ? dl->pod_off[nd] : 0;
+  if (pairs && (!dl->ls_key || !dl->ls_val)) return bad("label pairs without arrays");
+  if (tents && (!dl->taint_key || !dl->taint_val || !dl->taint_effect)) return bad("taints without arrays");
+  if (npods && !dl->pod_spec) return bad("resident pods without pod_spec");
+  const int64_t NV = (int64_t)nh.num_values + nv, NL = (int64_t)nh.num_labelsets + nl, NTL = (int64_t)nh.num_taint_lists + ntl;
+  const int64_t old_pairs = nh.ls_off.back();
+  if (NV > INT32_MAX || NL >= INT32_MAX || NTL >= INT32_MAX || old_pairs + pairs > INT32_MAX || (int64_t)nh.taint_entries + tents > INT32_MAX)
+    return refuse("a dictionary table would pass 2^31 - 1 entries");
+  int64_t total = nh.pod_total;
+  for (int i = 0; i < nd; ++i) {
+    const int r = dl->row[i];
+    if (r < 0 || r >= N || (i > 0 && r <= dl->row[i - 1])) return bad("rows out of range or not strictly increasing");
+    if (dl->labelset[i] < 0 || dl->labelset[i] >= NL) return bad("label-set id out of range");
+    if (dl->taint_list[i] < 0 || dl->taint_list[i] >= NTL) return bad("taint-list id out of range");
+    total += (int64_t)(dl->pod_off[i + 1] - dl->pod_off[i]) - nh.pod_cnt[r];
+  }
+  if (total > INT32_MAX) return refuse("more than 2^31 - 1 resident pods");
+  for (int j = 0; j < nl; ++j)
+    for (int p = dl->ls_off[j]; p < dl->ls_off[j + 1]; ++p) {
+      if (dl->ls_key[p] < 0 || (p > dl->ls_off[j] && dl->ls_key[p] <= dl->ls_key[p - 1])) return bad("label pairs not sorted by key id");
+      if (dl->ls_val[p] < 0 || dl->ls_val[p] >= NV) return bad("label value id out of range");
+    }
+  for (int64_t p = 0; p < tents; ++p) {
+    if (dl->taint_key[p] < 0) return bad("taint key id out of range");
+    if (dl->taint_val[p] < -1 || dl->taint_val[p] >= NV) return bad("taint value id out of range");
+    if (dl->taint_effect[p] < CAE_EFFECT_NONE || dl->taint_effect[p] > CAE_EFFECT_NO_EXECUTE) return bad("taint effect out of range");
+  }
+  for (int64_t p = 0; p < npods; ++p)
+    if (dl->pod_spec[p] < 0 || dl->pod_spec[p] >= S) return bad("pod-spec id out of range");
+  // ---- status 2: the resident classes, counters and domains would not be the ones a cae_load builds ----
+  for (int64_t p = 0; p < npods; ++p) {
+    const int s = dl->pod_spec[p];
+    if (nh.spec_anti[s] && !nh.spec_used[s]) return refuse("a resident pod's spec has anti-affinity terms and was not in the snapshot");
+  }
+  auto label_of = [&](int ls, int key) -> int {   // value id of `key` in label set ls (resident table + tail), -1 absent
+    const bool tail = ls >= nh.num_labelsets;
+    const int32_t *off = tail ? dl->ls_off : nh.ls_off.data(), *k = tail ? dl->ls_key : nh.ls_key.data(), *v = tail ? dl->ls_val : nh.ls_val.data();
+    const int j = tail ? ls - nh.num_labelsets : ls;
+    for (int p = off[j]; p < off[j + 1]; ++p) if (k[p] == key) return v[p];
+    return -1;
+  };
+  const DynTables& dy = e->dyn;
+  for (int k = 0; k < (e->has_dynamic ? dy.K : 0); ++k)
+    for (int i = 0; i < nd; ++i)
+      if (label_of(dl->labelset[i], dy.key_id[k]) != nh.key_val[(size_t)k * N + dl->row[i]])
+        return refuse("a dirty node changes the value of a topology key the counters use");
+  e->stats.h2d_bytes = 0;
+  if (!nv && !nl && !ntl && !nd) return 0;
+
+  // ---- the delta applies: host state ----
+  const int old_nv = nh.num_values, old_nl = nh.num_labelsets, old_ntl = nh.num_taint_lists, old_tents = nh.taint_entries;
+  for (int j = 0; j < nl; ++j) nh.ls_off.push_back((int32_t)(old_pairs + dl->ls_off[j + 1]));
+  if (pairs) { nh.ls_key.insert(nh.ls_key.end(), dl->ls_key, dl->ls_key + pairs); nh.ls_val.insert(nh.ls_val.end(), dl->ls_val, dl->ls_val + pairs); }
+  nh.num_values = (int32_t)NV; nh.num_labelsets = (int32_t)NL; nh.num_taint_lists = (int32_t)NTL; nh.taint_entries += (int32_t)tents;
+  for (int i = 0; i < nd; ++i) nh.pod_cnt[dl->row[i]] = dl->pod_off[i + 1] - dl->pod_off[i];
+  nh.pod_total = total;
+  for (int64_t p = 0; p < npods; ++p) nh.spec_used[dl->pod_spec[p]] = 1;
+
+  // ---- one pinned staging blob, one H2D copy ----
+  size_t bytes = 0;
+  auto seg = [&](size_t n, size_t elem) { const size_t at = bytes; bytes = (bytes + n * elem + 7) & ~(size_t)7; return at; };
+  const size_t o_vint = seg(nv, 8), o_alloc = seg((size_t)nd * R, 8), o_cfree = seg((size_t)nd * A, 8);
+  const size_t o_lsoff = seg(nl, 4), o_lskey = seg(pairs, 4), o_lsval = seg(pairs, 4);
+  const size_t o_toff = seg(ntl, 4), o_tkey = seg(tents, 4), o_tval = seg(tents, 4), o_teff = seg(tents, 4);
+  const size_t o_row = seg(nd, 4), o_ls = seg(nd, 4), o_tl = seg(nd, 4), o_allowed = seg(nd, 4), o_slots = seg(nd, 4);
+  const size_t o_poff = seg((size_t)nd + 1, 4), o_pspec = seg(npods, 4), o_visint = seg(nv, 1), o_unsched = seg(nd, 1);
+  if (e->ev_nd) CAE_CUDA(cudaEventSynchronize(e->ev_nd));   // the previous delta's copy out of the staging (long finished)
+  else CAE_CUDA(cudaEventCreateWithFlags(&e->ev_nd, cudaEventDisableTiming));
+  if (bytes > e->nd_stage_bytes) {
+    if (e->h_nd_stage) cudaFreeHost(e->h_nd_stage);
+    e->h_nd_stage = nullptr;
+    e->nd_stage_bytes = 0;
+    const size_t cap = bytes + bytes / 4 + 4096;
+    CAE_CUDA(cudaHostAlloc(&e->h_nd_stage, cap, cudaHostAllocDefault));
+    e->nd_stage_bytes = cap;
+  }
+  char* h = static_cast<char*>(e->h_nd_stage);
+  auto put = [&](size_t at, const void* src, size_t n) { if (n) memcpy(h + at, src, n); };
+  put(o_vint, dl->value_int, (size_t)nv * 8);
+  put(o_visint, dl->value_is_int, (size_t)nv);
+  put(o_alloc, dl->alloc, (size_t)nd * R * 8);
+  for (int j = 0; j < nl; ++j) reinterpret_cast<int32_t*>(h + o_lsoff)[j] = (int32_t)(old_pairs + dl->ls_off[j + 1]);   // absolute
+  put(o_lskey, dl->ls_key, (size_t)pairs * 4);
+  put(o_lsval, dl->ls_val, (size_t)pairs * 4);
+  for (int j = 0; j < ntl; ++j) reinterpret_cast<int32_t*>(h + o_toff)[j] = old_tents + dl->taint_off[j + 1];
+  put(o_tkey, dl->taint_key, (size_t)tents * 4);
+  put(o_tval, dl->taint_val, (size_t)tents * 4);
+  put(o_teff, dl->taint_effect, (size_t)tents * 4);
+  put(o_row, dl->row, (size_t)nd * 4);
+  put(o_ls, dl->labelset, (size_t)nd * 4);
+  put(o_tl, dl->taint_list, (size_t)nd * 4);
+  put(o_allowed, dl->allowed_pods, (size_t)nd * 4);
+  put(o_unsched, dl->unschedulable, (size_t)nd);
+  if (nd) put(o_poff, dl->pod_off, ((size_t)nd + 1) * 4);
+  put(o_pspec, dl->pod_spec, (size_t)npods * 4);
+  // free capacity and pod slots of the dirty rows for the fallback placements: the int64 arithmetic of do_load
+  int64_t* cfree = reinterpret_cast<int64_t*>(h + o_cfree);
+  int32_t* cslots = reinterpret_cast<int32_t*>(h + o_slots);
+  for (int i = 0; i < nd; ++i) {
+    int64_t reqd[R] = {0};
+    for (int p = dl->pod_off[i]; p < dl->pod_off[i + 1]; ++p)
+      for (int r = 0; r < R; ++r) reqd[r] += e->h_spec_req[(size_t)dl->pod_spec[p] * R + r];
+    for (int a = 0; a < A; ++a) cfree[(size_t)i * A + a] = dl->alloc[(size_t)i * R + e->act_dim[a]] - reqd[e->act_dim[a]];
+    cslots[i] = dl->allowed_pods[i] - (dl->pod_off[i + 1] - dl->pod_off[i]);
+  }
+  if (devbuf_reserve(e, e->nd_blob, bytes)) return -1;
+  char* dv = static_cast<char*>(e->nd_blob.p);
+  CAE_CUDA(cudaMemcpyAsync(dv, h, bytes, cudaMemcpyHostToDevice, e->stream));
+  CAE_CUDA(cudaEventRecord(e->ev_nd, e->stream));
+  e->stats.h2d_bytes = (int64_t)bytes;
+
+  // ---- dictionary tails ----
+  DevObjects& d = e->dobj;
+  if (grow_table(e, e->nd_tab[0], d.value_is_int, old_nv, dv + o_visint, nv) || grow_table(e, e->nd_tab[1], d.value_int, old_nv, dv + o_vint, nv) ||
+      grow_table(e, e->nd_tab[2], d.ls_off, (size_t)old_nl + 1, dv + o_lsoff, nl) ||
+      grow_table(e, e->nd_tab[3], d.ls_key, (size_t)old_pairs, dv + o_lskey, pairs) ||
+      grow_table(e, e->nd_tab[4], d.ls_val, (size_t)old_pairs, dv + o_lsval, pairs) ||
+      grow_table(e, e->nd_tab[5], d.taint_off, (size_t)old_ntl + 1, dv + o_toff, ntl) ||
+      grow_table(e, e->nd_tab[6], d.taint_key, (size_t)old_tents, dv + o_tkey, tents) ||
+      grow_table(e, e->nd_tab[7], d.taint_val, (size_t)old_tents, dv + o_tval, tents) ||
+      grow_table(e, e->nd_tab[8], d.taint_effect, (size_t)old_tents, dv + o_teff, tents))
+    return -1;
+  d.num_values = (int32_t)NV;
+  e->group_reason_valid = false;
+  if (!nd) return 0;
+
+  // ---- dirty rows, resident CSR, then everything derived from the cluster rows ----
+  NodeDeltaDev dd{};
+  dd.nd = nd;
+  dd.row = reinterpret_cast<const int32_t*>(dv + o_row); dd.labelset = reinterpret_cast<const int32_t*>(dv + o_ls);
+  dd.taint_list = reinterpret_cast<const int32_t*>(dv + o_tl); dd.allowed = reinterpret_cast<const int32_t*>(dv + o_allowed);
+  dd.cslots = reinterpret_cast<const int32_t*>(dv + o_slots); dd.pod_off = reinterpret_cast<const int32_t*>(dv + o_poff);
+  dd.pod_spec = reinterpret_cast<const int32_t*>(dv + o_pspec); dd.unsched = reinterpret_cast<const uint8_t*>(dv + o_unsched);
+  dd.alloc = reinterpret_cast<const int64_t*>(dv + o_alloc); dd.cfree = reinterpret_cast<const int64_t*>(dv + o_cfree);
+  if (launch_node_rows(e, dd, total)) return -1;
+  if (launch_class_matrix_cols(e, dd.row, nd)) return -1;
+  if (e->has_dynamic) {
+    if (launch_dynamic_recount(e, dd.row, nd)) return -1;
+    if (launch_post_bits(e)) return -1;
+  }
   return 0;
 }
 
@@ -636,6 +847,11 @@ void cae_destroy(cae_engine* h) {
   if (e->d_fm_scratch) cudaFree(e->d_fm_scratch);
   if (e->d_fm_blob) cudaFree(e->d_fm_blob);
   if (e->h_pending_stage) cudaFreeHost(e->h_pending_stage);
+  for (Engine::DevBuf* b : {&e->nd_off[0], &e->nd_off[1], &e->nd_spec[0], &e->nd_spec[1], &e->nd_cnt, &e->nd_didx, &e->nd_cub, &e->nd_blob})
+    if (b->p) cudaFree(b->p);
+  for (auto& b : e->nd_tab) if (b.p) cudaFree(b.p);
+  if (e->h_nd_stage) cudaFreeHost(e->h_nd_stage);
+  if (e->ev_nd) cudaEventDestroy(e->ev_nd);
   if (e->ev2) { cudaEventDestroy(e->ev2); cudaEventDestroy(e->ev3); }
   if (e->ev0) cudaEventDestroy(e->ev0);
   if (e->ev1) cudaEventDestroy(e->ev1);
@@ -686,6 +902,14 @@ int32_t cae_load_pending(cae_engine* h, int32_t num_pending, const int32_t* pend
   if (cae::launch_group_records(e)) return -1;
   // no synchronize: the stream orders the copies and the two kernels before whatever the caller launches next
   return 0;
+}
+
+int32_t cae_load_nodes(cae_engine* h, const cae_node_delta* d) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_load_nodes before cae_load"); return -2; }
+  if (!d) { cae::set_error("cae_load_nodes: no delta"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_load_nodes(e, d);
 }
 
 int32_t cae_feasibility(cae_engine* h, uint32_t* fit_bits, uint8_t* reasons, int32_t* fit_count) {

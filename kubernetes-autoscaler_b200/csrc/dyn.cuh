@@ -50,6 +50,7 @@ struct DynTables {
   const int32_t* q_dc = nullptr;    // [Q] owning class
   const int32_t* q_p0 = nullptr;    // [Q] PTS: row in the pts_* arrays; AFF/ANTI: aterm id; EXIST: -
   const int32_t* q_base_off = nullptr;  // [Q+1] offsets into base_cnt / base_pres (Dc[k] entries each)
+  int pool = 0;                     // q_base_off[Q]: entries of base_cnt / base_pres
   // device-computed
   uint8_t* wmat = nullptr;          // [Q][S] weight of a pod of spec s for counter q
   uint8_t* q_self = nullptr;        // [Q] PTS: selector matches the pod's own labels (filtering.go:345-348)

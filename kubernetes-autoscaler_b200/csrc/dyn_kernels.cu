@@ -2,6 +2,7 @@
 // counter weights per pod spec, node eligibility, per-domain base counts over the cluster
 // (the reference's PreFilter scan, done ONCE per tick instead of once per SchedulePod), their min
 // statistics, and the resulting reason of every (dynamic class, template) pair for the dense pass.
+#include <algorithm>
 #include <climits>
 
 #include "engine.h"
@@ -70,11 +71,13 @@ __global__ void dyn_dcmeta_kernel(DevObjects o, DynTables d) {
   d.dc_aff_self[dc] = aff_self;
 }
 
-// does universe column u take part in counter q
-__global__ void dyn_elig_kernel(DevObjects o, DynTables d, int U, const uint8_t* __restrict__ pre_code) {
-  int u = blockIdx.x * blockDim.x + threadIdx.x;
+// does universe column u take part in counter q; cols = NULL: every column, else the ncols columns listed
+__global__ void dyn_elig_kernel(DevObjects o, DynTables d, int U, const int32_t* __restrict__ cols, int ncols,
+                                const uint8_t* __restrict__ pre_code) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
   int q = blockIdx.y;
-  if (u >= U || q >= d.Q) return;
+  if (i >= ncols || q >= d.Q) return;
+  const int u = cols ? cols[i] : i;
   UNode n = unode(o, u);
   bool ok;
   int val;
@@ -236,7 +239,7 @@ int launch_dynamic_tables(Engine* e, const uint8_t* d_spec_used, const int32_t* 
   dyn_weights_kernel<<<dim3((S + 127) / 128, Q), 128, 0, e->stream>>>(e->dobj, d);
   dyn_qmeta_kernel<<<(Q + 127) / 128, 128, 0, e->stream>>>(e->dobj, d, d_spec_used);
   dyn_dcmeta_kernel<<<(d.DC + 127) / 128, 128, 0, e->stream>>>(e->dobj, d);
-  dyn_elig_kernel<<<dim3((U + 127) / 128, Q), 128, 0, e->stream>>>(e->dobj, d, U, e->d_pre_code);
+  dyn_elig_kernel<<<dim3((U + 127) / 128, Q), 128, 0, e->stream>>>(e->dobj, d, U, nullptr, U, e->d_pre_code);
   if (e->N > 0) dyn_base_kernel<<<dim3((e->N + 127) / 128, Q), 128, 0, e->stream>>>(e->dobj, d, U);
   if (e->T > 0) dyn_dsw_kernel<<<dim3((e->T + 127) / 128, Q), 128, 0, e->stream>>>(e->dobj, d);
   dyn_stats_kernel<<<(Q * 32 + 127) / 128, 128, 0, e->stream>>>(e->dobj, d);
@@ -244,6 +247,27 @@ int launch_dynamic_tables(Engine* e, const uint8_t* d_spec_used, const int32_t* 
   if (e->T > 0) dyn_post_code_kernel<<<dim3((e->T + 127) / 128, d.DC), 128, 0, e->stream>>>(e->dobj, d, U, e->d_post_code);
   dyn_qrec_kernel<<<(Q + 127) / 128, 128, 0, e->stream>>>(e->dobj, d);
   e->stats.kernel_launches += 10;
+  CAE_KERNEL_OK();
+  return 0;
+}
+
+// After cae_load_nodes changed the cluster rows `cols` (pre_code of those columns already recomputed): their eligibility,
+// then every cluster-derived counter table from scratch.  Weights, classes, domains and the templates' DaemonSet weights
+// depend on neither the cluster rows nor their residents and stay.  The recount is the pass a load runs (one thread per
+// (counter, cluster node)); DESIGN.md §4 records why it is not an incremental subtract / add of the dirty rows.
+int launch_dynamic_recount(Engine* e, const int32_t* d_cols, int ncols) {
+  DynTables& d = e->dyn;
+  if (d.Q == 0) return 0;
+  const int Q = d.Q, U = e->U;
+  if (ncols > 0) dyn_elig_kernel<<<dim3((ncols + 127) / 128, Q), 128, 0, e->stream>>>(e->dobj, d, U, d_cols, ncols, e->d_pre_code);
+  CAE_CUDA(cudaMemsetAsync(d.base_cnt, 0, sizeof(int32_t) * std::max(d.pool, 1), e->stream));
+  CAE_CUDA(cudaMemsetAsync(d.base_pres, 0, sizeof(int32_t) * std::max(d.pool, 1), e->stream));
+  CAE_CUDA(cudaMemsetAsync(d.base_tot, 0, sizeof(int32_t) * Q, e->stream));
+  if (e->N > 0) dyn_base_kernel<<<dim3((e->N + 127) / 128, Q), 128, 0, e->stream>>>(e->dobj, d, U);
+  dyn_stats_kernel<<<(Q * 32 + 127) / 128, 128, 0, e->stream>>>(e->dobj, d);
+  if (e->T > 0) dyn_post_code_kernel<<<dim3((e->T + 127) / 128, d.DC), 128, 0, e->stream>>>(e->dobj, d, U, e->d_post_code);
+  dyn_qrec_kernel<<<(Q + 127) / 128, 128, 0, e->stream>>>(e->dobj, d);
+  e->stats.kernel_launches += 5;
   CAE_KERNEL_OK();
   return 0;
 }

@@ -178,6 +178,24 @@ struct Engine {
   std::vector<int64_t> h_spec_req;        // [num_podspecs][R]
   std::vector<int64_t> h_cap_cpu, h_cap_mem;  // per template
   int num_podspecs = 0;
+  // host state of the last load that cae_load_nodes validates against and updates (node_delta in api.cu)
+  struct NodeHost {
+    int32_t num_values = 0, num_labelsets = 0, num_taint_lists = 0, taint_entries = 0;
+    std::vector<int32_t> ls_off, ls_key, ls_val;   // resident label-set table, tails appended
+    std::vector<int32_t> pod_cnt;                  // [N] resident pods per cluster row
+    int64_t pod_total = 0;                         // node_pod_off[N + T]
+    std::vector<uint8_t> spec_used;                // [S] spec pending or resident (only grows between loads)
+    std::vector<uint8_t> spec_anti;                // [S] spec has required anti-affinity terms
+    std::vector<int32_t> key_val;                  // [K][N] value id of resident topology key k on cluster row n, -1 absent
+  } nh;
+  // engine-owned device buffers of cae_load_nodes (stream-ordered allocations; a cae_load points DevObjects back at its arena)
+  struct DevBuf { void* p = nullptr; size_t cap = 0; };
+  DevBuf nd_tab[9];                       // grown dictionary tables: value_is_int, value_int, ls_off|key|val, taint_off|key|val|effect
+  DevBuf nd_off[2], nd_spec[2];           // double-buffered resident CSR (node_pod_off / node_pod_spec)
+  DevBuf nd_cnt, nd_didx, nd_cub, nd_blob;  // per-row counts / dirty index, scan temp storage, device copy of the delta
+  void* h_nd_stage = nullptr;             // pinned staging of the delta
+  size_t nd_stage_bytes = 0;
+  cudaEvent_t ev_nd = nullptr;            // the last delta's H2D copy (guards the pinned staging)
   int sm_count = 132;
   int smem_optin = 227 * 1024;             // opt-in shared memory per thread block
   size_t hbm_bytes = (size_t)80 << 30;     // device memory (sizes the estimator's global slabs)
@@ -185,6 +203,16 @@ struct Engine {
 
 // kernels.cu
 int launch_class_matrix(Engine* e);      // pre_code[SC][U]: needs only the object tables + the static classes
+int launch_class_matrix_cols(Engine* e, const int32_t* d_cols, int ncols);   // pre_code[SC][cols] only
+int launch_dynamic_recount(Engine* e, const int32_t* d_cols, int ncols);     // elig of cols, cluster counters, post_code, qrec
+struct NodeDeltaDev {                    // device views into the staged cae_node_delta (node_delta.cu)
+  int nd;
+  const int32_t *row, *labelset, *taint_list, *allowed, *cslots, *pod_off, *pod_spec;
+  const uint8_t* unsched;
+  const int64_t *alloc, *cfree;          // [nd][R], [nd][A]
+};
+int launch_node_rows(Engine* e, const NodeDeltaDev& d, int64_t total);   // rows in place + resident CSR rebuilt into the spare buffer
+int devbuf_reserve(Engine* e, Engine::DevBuf& b, size_t bytes);          // stream-ordered growth, contents not kept
 int launch_pre_ok_bits(Engine* e);       // pre_ok[SC][Twp]: needs pre_code and the templates' pod slots
 int launch_post_bits(Engine* e);
 int launch_dynamic_tables(Engine* e, const uint8_t* d_spec_used, const int32_t* d_dc_ngroups);

@@ -21,11 +21,13 @@ namespace cae {
 // ------------------------------------------------------------------------------------------------
 // class matrices
 // ------------------------------------------------------------------------------------------------
+// cols = NULL: every universe column; else the ncols columns listed (dirty cluster rows of cae_load_nodes)
 __global__ void class_matrix_kernel(DevObjects o, const StaticClass* __restrict__ sclass, int SC, int U,
-                                    uint8_t* __restrict__ pre_code) {
-  int u = blockIdx.x * blockDim.x + threadIdx.x;
+                                    const int32_t* __restrict__ cols, int ncols, uint8_t* __restrict__ pre_code) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
   int c = blockIdx.y;
-  if (u >= U || c >= SC) return;
+  if (i >= ncols || c >= SC) return;
+  const int u = cols ? cols[i] : i;
   pre_code[(size_t)c * U + u] = static_code(o, sclass[c], u);
 }
 
@@ -98,7 +100,17 @@ int launch_group_feasibility(Engine* e) {
 int launch_class_matrix(Engine* e) {
   if (e->SC > 0 && e->U > 0) {
     dim3 grid((e->U + 127) / 128, e->SC);
-    class_matrix_kernel<<<grid, 128, 0, e->stream>>>(e->dobj, e->d_sclass, e->SC, e->U, e->d_pre_code);
+    class_matrix_kernel<<<grid, 128, 0, e->stream>>>(e->dobj, e->d_sclass, e->SC, e->U, nullptr, e->U, e->d_pre_code);
+    e->stats.kernel_launches++;
+  }
+  CAE_KERNEL_OK();
+  return 0;
+}
+
+int launch_class_matrix_cols(Engine* e, const int32_t* d_cols, int ncols) {
+  if (e->SC > 0 && ncols > 0) {
+    dim3 grid((ncols + 127) / 128, e->SC);
+    class_matrix_kernel<<<grid, 128, 0, e->stream>>>(e->dobj, e->d_sclass, e->SC, e->U, d_cols, ncols, e->d_pre_code);
     e->stats.kernel_launches++;
   }
   CAE_KERNEL_OK();

@@ -423,6 +423,66 @@ class EncodedObjects:
         out.struct = s
         return out
 
+    def with_pending(self, pend_spec, group_off) -> "EncodedObjects":
+        """The same snapshot with other pending-pod rows (every other table is shared): what cae_load_pending uploads."""
+        import copy
+        out = copy.copy(self)
+        out.arrays = dict(self.arrays)
+        out.arrays["pend_spec"] = np.ascontiguousarray(pend_spec, np.int32)
+        out.arrays["group_off"] = np.ascontiguousarray(group_off, np.int32)
+        out.struct = self._restruct(out.arrays, num_pending=int(out.arrays["group_off"][-1]),
+                                    num_groups=len(out.arrays["group_off"]) - 1)
+        return out
+
+    def apply_node_delta(self, delta: "NodeDelta") -> "EncodedObjects":
+        """The objects after cae_load_nodes(delta), stated on the host: the dictionary tails appended, the dirty cluster
+        rows rewritten and the resident-pod CSR rebuilt.  A cae_load of the result must answer like the engine after the
+        delta."""
+        import copy
+        a, d, s = dict(self.arrays), delta.arrays, self.struct
+        nv, nl, nt = s.num_values, s.num_labelsets, s.num_taint_lists
+        a["value_is_int"] = np.concatenate([a["value_is_int"][:nv], d["value_is_int"]]).astype(np.uint8)
+        a["value_int"] = np.concatenate([a["value_int"][:nv], d["value_int"]]).astype(np.int64)
+        p0 = int(a["ls_off"][nl])
+        a["ls_off"] = _i32(np.concatenate([a["ls_off"][:nl + 1], p0 + d["ls_off"][1:]]))
+        a["ls_key"] = _i32(np.concatenate([a["ls_key"][:p0], d["ls_key"]]))
+        a["ls_val"] = _i32(np.concatenate([a["ls_val"][:p0], d["ls_val"]]))
+        t0 = int(a["taint_off"][nt])
+        a["taint_off"] = _i32(np.concatenate([a["taint_off"][:nt + 1], t0 + d["taint_off"][1:]]))
+        for nm in ("taint_key", "taint_val", "taint_effect"):
+            a[nm] = _i32(np.concatenate([a[nm][:t0], d[nm]]))
+        rows = d["row"]
+        for nm, src in (("node_labelset", "labelset"), ("node_taint_list", "taint_list"),
+                        ("node_unschedulable", "unschedulable"), ("node_allowed_pods", "allowed_pods")):
+            a[nm] = a[nm].copy()
+            a[nm][rows] = d[src]
+        a["node_alloc"] = a["node_alloc"].copy()
+        a["node_alloc"][rows] = d["alloc"]
+        off, spec, po = a["node_pod_off"], a["node_pod_spec"], d["pod_off"]
+        dirty = {int(r): i for i, r in enumerate(rows)}
+        pieces, new_off = [], [0]
+        for r in range(len(off) - 1):
+            i = dirty.get(r)
+            pieces.append(spec[off[r]:off[r + 1]] if i is None else d["pod_spec"][po[i]:po[i + 1]])
+            new_off.append(new_off[-1] + len(pieces[-1]))
+        a["node_pod_off"] = _i32(new_off)
+        a["node_pod_spec"] = _i32(np.concatenate(pieces) if pieces else [])
+        out = copy.copy(self)
+        out.arrays = a
+        out.struct = self._restruct(a, num_values=len(a["value_is_int"]), num_labelsets=len(a["ls_off"]) - 1,
+                                    num_taint_lists=len(a["taint_off"]) - 1)
+        return out
+
+    def _restruct(self, arrays, **counts) -> "capi.cae_objects":
+        s = capi.cae_objects()
+        C.memmove(C.byref(s), C.byref(self.struct), C.sizeof(s))
+        for k, v in counts.items():
+            setattr(s, k, v)
+        for name, ctype in capi.cae_objects._fields_:
+            if name in arrays:
+                setattr(s, name, arrays[name].ctypes.data_as(ctype))
+        return s
+
     # convenience
     @property
     def P(self) -> int:
@@ -435,6 +495,47 @@ class EncodedObjects:
     @property
     def E(self) -> int:
         return self.struct.num_groups
+
+    def ptr(self):
+        return C.byref(self.struct)
+
+
+class NodeDelta:
+    """Owns the numpy arrays behind one ``cae_node_delta`` struct: the dictionary tails (values, label sets, taint lists
+    that continue the resident tables; offsets relative to the tail) and the complete new state of the dirty cluster
+    rows.  Field names are the header's."""
+
+    _I32 = ("ls_off", "ls_key", "ls_val", "taint_off", "taint_key", "taint_val", "taint_effect", "row", "labelset",
+            "taint_list", "allowed_pods", "pod_off", "pod_spec")
+
+    def __init__(self, **arrays) -> None:
+        a: Dict[str, np.ndarray] = {}
+        for nm in self._I32:
+            a[nm] = _i32(arrays.get(nm, [0] if nm in ("ls_off", "taint_off", "pod_off") else []))
+        a["value_is_int"] = np.ascontiguousarray(arrays.get("value_is_int", []), np.uint8)
+        a["value_int"] = np.ascontiguousarray(arrays.get("value_int", []), np.int64)
+        a["unschedulable"] = np.ascontiguousarray(arrays.get("unschedulable", []), np.uint8)
+        nd = len(a["row"])
+        a["alloc"] = np.ascontiguousarray(np.asarray(arrays.get("alloc", np.zeros((nd, MAX_RES))), np.int64).reshape(nd, MAX_RES))
+        self.arrays = a
+        s = capi.cae_node_delta()
+        s.abi_version = capi.CONST["CAE_ABI_VERSION"]
+        s.num_new_values = len(a["value_is_int"])
+        s.num_new_labelsets = len(a["ls_off"]) - 1
+        s.num_new_taint_lists = len(a["taint_off"]) - 1
+        s.num_dirty = nd
+        for name, ctype in capi.cae_node_delta._fields_:
+            if name in a:
+                setattr(s, name, a[name].ctypes.data_as(ctype))
+        self.struct = s
+
+    def replace(self, **arrays) -> "NodeDelta":
+        """A copy with some arrays replaced (the counts follow the arrays)."""
+        return NodeDelta(**{**self.arrays, **arrays})
+
+    @property
+    def num_dirty(self) -> int:
+        return self.struct.num_dirty
 
     def ptr(self):
         return C.byref(self.struct)
@@ -616,7 +717,83 @@ class Encoder:
         self._key(LABEL_HOSTNAME)
         self._key(TAINT_NODE_UNSCHEDULABLE)
         self.b.num_res = max(3, len(self.resources))
-        return self.b.finish()
+        enc = self.b.finish()
+        # what the engine holds after a load of `enc`: node_delta() emits what the interner adds beyond it as tails
+        self._emitted = (enc.struct.num_values, enc.struct.num_labelsets, enc.struct.num_taint_lists)
+        self._delta_ok = True
+        self._spec_wo_name: Optional[Dict[tuple, int]] = None
+        return enc
+
+    def _resident_spec(self, pod: Pod) -> int:
+        """Spec id of a resident pod of a changed node, among the specs of the last load.  No filter reads a resident pod's
+        spec.nodeName (only the incoming pod's), so the lookup ignores it: a pod bound since the last tick finds its
+        pending spec.  No match: Unsupported (the tick needs a full load)."""
+        b = self.b
+        n = len(b.ps_rows)
+        saved, self._podspec_cache = self._podspec_cache, {}
+        try:
+            sid = self.podspec(pod, resident=True)
+        finally:
+            self._podspec_cache = saved
+        if sid < n:
+            return sid
+        key = b.ps_rows.pop()           # the interner added a row: take it back and look for the same spec without nodeName
+        del b.ps_ids[key]
+        hit = b.ps_ids.get(key[:5] + (-1,) + key[6:])
+        if hit is None:
+            if self._spec_wo_name is None:
+                self._spec_wo_name = {}
+                for i, k in enumerate(b.ps_rows):
+                    self._spec_wo_name.setdefault(k[:5] + k[6:], i)
+            hit = self._spec_wo_name.get(key[:5] + key[6:])
+        if hit is None:
+            self._delta_ok = False
+            raise Unsupported("resident pod %s/%s has a spec the last load did not have" % (pod.namespace, pod.name))
+        return hit
+
+    def node_delta(self, changed: Sequence[Tuple[int, NodeInfo]]) -> NodeDelta:
+        """The shim's side of cae_load_nodes: the new state of changed cluster nodes (row of the last load, NodeInfo) as a
+        NodeDelta against what the engine holds.  The interner stays append-only; the values, label sets and taint lists
+        the changed rows add since the last load or delta become the delta's tails.  Unsupported = use a full load (and
+        a fresh Encoder: this one no longer matches the engine)."""
+        if not getattr(self, "_delta_ok", False):
+            raise Unsupported("no load to apply a node delta to, or an earlier delta was refused")
+        b = self.b
+        nv0, nl0, nt0 = self._emitted
+        if len(b.value_is_int) < nv0:
+            self._delta_ok = False
+            raise Unsupported("the value table of the last load was padded")
+        nres = len(self.resources)
+        items = sorted(changed, key=lambda x: x[0])
+        rows, lsets, tlists, unsched, alloc, allowed, pod_off, pod_spec = [], [], [], [], [], [], [0], []
+        for row, ni in items:
+            if not 0 <= row < b.num_cluster_nodes or (rows and row == rows[-1]):
+                raise ValueError("node delta row %d: not a cluster node of the last load, or given twice" % row)
+            n = ni.node
+            if self.node_names.ids.get(n.name) != b.node_rows[row][0]:
+                self._delta_ok = False
+                raise Unsupported("row %d is no longer node %s" % (row, n.name))
+            tl = b.taint_list([(self._key(t.key), self._val(t.value) if t.value else -1, _EFFECTS[t.effect]) for t in n.taints])
+            ls = self._labelset(n.labels)
+            vec = self._resource_vec(n.allocatable)
+            if len(self.resources) > nres:
+                self._delta_ok = False
+                raise Unsupported("node %s has a resource the last load did not have" % n.name)
+            specs = [self._resident_spec(p) for p in ni.pods]
+            rows.append(row); lsets.append(ls); tlists.append(tl); unsched.append(int(n.unschedulable))
+            alloc.append(vec); allowed.append(int(n.allocatable.get("pods", 0)))
+            pod_spec.extend(specs); pod_off.append(len(pod_spec))
+        L, Tn = b.labelsets, b.taints
+        lp0, tp0 = L.off[nl0], Tn.off[nt0]
+        delta = NodeDelta(
+            value_is_int=b.value_is_int[nv0:], value_int=b.value_int[nv0:],
+            ls_off=[o - lp0 for o in L.off[nl0:]], ls_key=L.cols[0][lp0:], ls_val=L.cols[1][lp0:],
+            taint_off=[o - tp0 for o in Tn.off[nt0:]], taint_key=Tn.cols[0][tp0:], taint_val=Tn.cols[1][tp0:],
+            taint_effect=Tn.cols[2][tp0:], row=rows, labelset=lsets, taint_list=tlists, unschedulable=unsched,
+            alloc=np.asarray(alloc, np.int64).reshape(len(rows), MAX_RES), allowed_pods=allowed, pod_off=pod_off,
+            pod_spec=pod_spec)
+        self._emitted = (len(b.value_is_int), L.n, Tn.n)
+        return delta
 
 
 def encode(cluster: Sequence[NodeInfo], templates: Sequence[NodeInfo],

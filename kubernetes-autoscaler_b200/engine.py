@@ -144,6 +144,16 @@ class Engine:
         self.enc = enc
         return True
 
+    def load_nodes(self, delta) -> bool:
+        """The per-tick delta of the cluster nodes (cae_load_nodes): new rows of existing cluster nodes plus the dictionary
+        tails they need (encode.NodeDelta).  Returns False when the engine answers "use a full load" (status 2); the engine
+        is unchanged then."""
+        rc = self.lib.cae_load_nodes(self.h, delta.ptr())
+        if rc == 2:
+            return False
+        self._check(rc)
+        return True
+
     def feasibility(self, want_bits: bool = True):
         """Dense pods x templates pass. Returns (fit_bits [T][ceil(Pl/32)] uint32 | None,
         reasons [T][Pl] uint8 | None, fit_count [T] int32) for this rank's pod shard."""

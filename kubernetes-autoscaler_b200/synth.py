@@ -256,3 +256,118 @@ def generate(config: int = 2, pods: Optional[int] = None, templates: Optional[in
     for g in range(E):
         b.group(np.full(int(counts[g]), group_spec[g], np.int32))
     return b.finish()
+
+
+def node_churn(enc: EncodedObjects, seed: int, n_dirty: int, bind: float = 0.3, evict: float = 0.3, move: float = 0.15,
+               cordon: float = 0.15, taint: float = 0.3, alloc: float = 0.25, relabel: float = 0.25):
+    """A deterministic random tick of cluster-node churn against a snapshot of ``generate`` (its key / value layout):
+    ``n_dirty`` distinct cluster rows, each changed with the given probabilities —
+      bind     pods of pending groups are bound to the node (every group keeps at least one pending pod, so the pending
+               delta still applies);
+      evict    resident pods finish;   move  resident pods move to another dirty node;
+      cordon   the node is cordoned / uncordoned;
+      taint    the node switches to an existing taint list or to a new one (some with a new value);
+      alloc    allocatable and allowed pods change, sometimes below what the residents request (negative free);
+      relabel  the node switches to a label set with the same hostname and zone but another pool (sometimes a new value)
+               and instance type, which nodeSelectors read.
+    Returns (delta, pending): the NodeDelta and ``enc`` with the bound pods removed from the pending rows.
+    ``pending.apply_node_delta(delta)`` is the snapshot after the tick."""
+    from .encode import NodeDelta
+    a, s = enc.arrays, enc.struct
+    N = s.num_cluster_nodes
+    rng = SplitMix64(0x5EED0000 + seed)
+    n_dirty = min(n_dirty, N)
+    rows = np.sort(rng.next(N).argsort()[:n_dirty]) if n_dirty else np.zeros(0, np.int64)
+    off, spec = a["node_pod_off"], a["node_pod_spec"]
+    lists = [list(spec[off[r]:off[r + 1]]) for r in rows]
+    go = a["group_off"]
+    left = np.diff(go).astype(np.int64)            # pending pods per group after the binds
+    gspec = np.where(left > 0, a["pend_spec"][np.minimum(go[:-1], max(len(a["pend_spec"]) - 1, 0))], -1) if len(go) > 1 else []
+    nv, nl, nt = s.num_values, s.num_labelsets, s.num_taint_lists
+    new_vals: List[int] = []
+    new_ls: dict = {}
+    new_tl: dict = {}
+
+    def new_value() -> int:
+        new_vals.append(len(new_vals))
+        return nv + len(new_vals) - 1
+
+    def labels_of(ls: int) -> dict:
+        return {int(k): int(v) for k, v in zip(a["ls_key"][a["ls_off"][ls]:a["ls_off"][ls + 1]],
+                                               a["ls_val"][a["ls_off"][ls]:a["ls_off"][ls + 1]])}
+
+    u = rng.uniform(8 * max(n_dirty, 1)).reshape(-1, 8)
+    r8 = rng.next(8 * max(n_dirty, 1)).reshape(-1, 8)
+    lsets, tlists, unsched, allocs, allowed = [], [], [], [], []
+    for i, r in enumerate(rows):
+        ui, ri = u[i], [int(x) for x in r8[i]]
+        pods = lists[i]
+        if ui[0] < evict and pods:
+            for _ in range(1 + ri[0] % 3):
+                if pods:
+                    pods.pop(ri[1] % len(pods))
+        if ui[1] < move and pods and n_dirty > 1:
+            j = (i + 1 + ri[2] % (n_dirty - 1)) % n_dirty
+            lists[j].append(pods.pop(ri[3] % len(pods)))
+        if ui[2] < bind and len(left):
+            for k in range(1 + ri[4] % 4):
+                g = (ri[5] + 7919 * k) % len(left)
+                if left[g] >= 2:
+                    left[g] -= 1
+                    pods.append(int(gspec[g]))
+        unsched.append(int(a["node_unschedulable"][r]) ^ int(ui[3] < cordon))
+        tl = int(a["node_taint_list"][r])
+        if ui[4] < taint:
+            if ri[6] % 3 == 0:   # a new list: one or two NoSchedule / NoExecute taints, sometimes on a new value
+                key = (K_TAINT0 + ri[6] % 8, new_value() if ri[7] % 4 == 0 else 52 + (ri[6] >> 3) % 2, 1 + 2 * ((ri[6] >> 5) % 2))
+                ent = (key,) if (ri[6] >> 7) % 2 else (key, (K_TAINT0 + (ri[6] >> 9) % 8, 52, 1))
+                ent = tuple(sorted(set(ent)))
+                tl = new_tl.setdefault(ent, nt + len(new_tl))
+            else:
+                tl = ri[6] % nt
+        tlists.append(tl)
+        al = a["node_alloc"][r].copy()
+        ap = int(a["node_allowed_pods"][r])
+        if ui[5] < alloc:
+            al[0] = max(1, int(al[0] * (0.5 + ui[6])))
+            al[1] = max(1, int(al[1] * (0.5 + ui[7])))
+            ap = int(ri[0] % 121)
+            if ri[1] % 5 == 0:
+                al[0] = 1           # residents request more than the node has: negative free
+        allocs.append(al)
+        allowed.append(ap)
+        ls = int(a["node_labelset"][r])
+        if ui[6] < relabel:
+            lab = labels_of(ls)
+            if K_POOL in lab:
+                lab[K_POOL] = new_value() if ri[2] % 10 == 0 else 16 + ri[2] % 8
+            if K_ITYPE in lab:
+                lab[K_ITYPE] = 24 + ri[3] % 24
+            key = tuple(sorted(lab.items()))
+            ls = new_ls.setdefault(key, nl + len(new_ls))
+        lsets.append(ls)
+    # allowed pods stay above the final resident count: the estimator's fallback onto cluster nodes that are already at
+    # their pod limit disagrees with the oracle (DESIGN.md §4), which is not what these deltas test
+    allowed = [max(ap, len(p) + 1) for ap, p in zip(allowed, lists)]
+    ls_items = sorted(new_ls.items(), key=lambda kv: kv[1])
+    tl_items = sorted(new_tl.items(), key=lambda kv: kv[1])
+    ls_off, tl_off = [0], [0]
+    for k, _ in ls_items:
+        ls_off.append(ls_off[-1] + len(k))
+    for k, _ in tl_items:
+        tl_off.append(tl_off[-1] + len(k))
+    pod_off = [0]
+    for p in lists:
+        pod_off.append(pod_off[-1] + len(p))
+    delta = NodeDelta(
+        value_is_int=[0] * len(new_vals), value_int=[0] * len(new_vals),
+        ls_off=ls_off, ls_key=[kk for k, _ in ls_items for kk, _v in k], ls_val=[v for k, _ in ls_items for _k, v in k],
+        taint_off=tl_off, taint_key=[e[0] for k, _ in tl_items for e in k], taint_val=[e[1] for k, _ in tl_items for e in k],
+        taint_effect=[e[2] for k, _ in tl_items for e in k],
+        row=rows, labelset=lsets, taint_list=tlists, unschedulable=unsched,
+        alloc=np.asarray(allocs, np.int64).reshape(len(rows), -1), allowed_pods=allowed, pod_off=pod_off,
+        pod_spec=[x for p in lists for x in p])
+    keep = np.concatenate([np.arange(go[g], go[g] + left[g]) for g in range(len(left))]) if len(left) else np.zeros(0, np.int64)
+    new_go = np.concatenate([[0], np.cumsum(left)]).astype(np.int32)
+    pending = enc.with_pending(a["pend_spec"][keep.astype(np.int64)], new_go)
+    return delta, pending

@@ -42,6 +42,19 @@ def main():
             got = eng.filter_schedulable(order_p)
             ref = pyoracle.filter_schedulable(enc, order_p)
             assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
+            # cluster-node delta (cae_load_nodes: row scatter, CSR rebuild, dirty-column class matrix, counter recount)
+            delta, pending = synth.node_churn(enc, cfg, 12)
+            assert eng.load_nodes(delta) and eng.load_pending(pending)
+            after = pending.apply_node_delta(delta)
+            eng.enc = after
+            _, reasons, _ = eng.feasibility()
+            assert np.array_equal(reasons, pyoracle.feasibility_dense(after)[0])
+            caps = np.full(after.T, 30, np.int32)
+            got_e, ref_e = eng.estimate_all(caps), pyoracle.estimate_all(after, caps)
+            assert all(np.array_equal(x, y) for x, y in zip(got_e, ref_e[:4]))
+            got = eng.filter_schedulable(order_p)
+            ref = pyoracle.filter_schedulable(after, order_p)
+            assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
         print("config", cfg, "ok: nodes", int(nc.sum()), "pods", int(pc.sum()), flush=True)
     eng.close()
     print("sanitize workload ok")
