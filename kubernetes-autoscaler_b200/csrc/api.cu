@@ -60,6 +60,32 @@ int Arena::flush(cudaStream_t st, int64_t* bytes) {
   return 0;
 }
 
+// ---- engine-owned buffers that grow: only their contents are per call ----
+int devbuf_reserve(Engine* e, Engine::DevBuf& b, size_t bytes) {   // 25 % headroom; the buffer is free when this is called
+  if (bytes <= b.cap) return 0;
+  if (b.p) CAE_CUDA(cudaFreeAsync(b.p, e->stream));
+  b.p = nullptr;
+  b.cap = 0;
+  const size_t cap = std::max<size_t>(bytes + bytes / 4, 4096);
+  CAE_CUDA(cudaMallocAsync(&b.p, cap, e->stream));
+  b.cap = cap;
+  return 0;
+}
+// The first allocation is exact (the pending rows of cae_load_pending never outgrow those of the load); a buffer that has
+// to grow gets 25 % headroom.
+int pinned_reserve(Engine* e, Engine::PinnedBuf& b, size_t bytes) {
+  if (b.ev) CAE_CUDA(cudaEventSynchronize(b.ev));   // normally long finished
+  else CAE_CUDA(cudaEventCreateWithFlags(&b.ev, cudaEventDisableTiming));
+  if (bytes <= b.cap) return 0;
+  const size_t cap = b.p ? bytes + bytes / 4 : bytes;
+  if (b.p) CAE_CUDA(cudaFreeHost(b.p));
+  b.p = nullptr;
+  b.cap = 0;
+  CAE_CUDA(cudaHostAlloc(&b.p, cap, cudaHostAllocDefault));
+  b.cap = cap;
+  return 0;
+}
+
 template <class T>
 static int upload(Engine* e, const T* host, size_t n, const T** dev) {
   void *p = nullptr, *h = nullptr;
@@ -202,7 +228,6 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
       dev_alloc(e, &d.st_min2, Q) || dev_alloc(e, &d.st_ndom, Q) || dev_alloc(e, &d.st_nmin, Q) || dev_alloc(e, &d.q_nfeed, Q, true) ||
       dev_alloc(e, &d.group_feeds, (size_t)std::max(e->E, 1), true) || dev_alloc(e, &d.qrec, Q))
     return -1;
-  e->h_dc_of_spec_valid = true;
   return 0;
 }
 
@@ -226,15 +251,6 @@ struct LoadTimer {   // CAE_LOAD_TIMING=1: host wall clock of the phases of cae_
 // the spec of every group and whether the groups are homogeneous.  `check_pending`: refuse specs that were not pending at
 // the last full load (returns 2).
 static int stage_pending(Engine* e, int P, const int32_t* pend_spec, int E, const int32_t* group_off, bool check_pending) {
-  const size_t words = (size_t)P + E + 1;
-  if (words > e->pending_stage_words) {
-    if (e->h_pending_stage) cudaFreeHost(e->h_pending_stage);
-    e->h_pending_stage = nullptr;
-    e->pending_stage_words = 0;
-    const size_t cap_words = std::max(words, (size_t)e->cap_P + e->cap_E + 1);
-    CAE_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&e->h_pending_stage), cap_words * 4, cudaHostAllocDefault));
-    e->pending_stage_words = cap_words;
-  }
   const int S = e->num_podspecs;
   // one pass per group: the exemplar's spec must have been pending at the last full load, the other pods must equal it
   std::vector<int32_t> gspec(E, -1);
@@ -254,13 +270,42 @@ static int stage_pending(Engine* e, int P, const int32_t* pend_spec, int E, cons
       const int s = pend_spec[p];
       if (s < 0 || s >= S || !e->h_spec_pending[s]) { set_error("cae_load_pending: a pod spec that was not pending at the last cae_load"); return 2; }
     }
-  if (P) memcpy(e->h_pending_stage, pend_spec, sizeof(int32_t) * P);
-  memcpy(e->h_pending_stage + P, group_off, sizeof(int32_t) * (E + 1));
-  e->h_pend_spec = e->h_pending_stage;
-  e->h_group_off = e->h_pending_stage + P;
+  if (pinned_reserve(e, e->pending_stage, sizeof(int32_t) * ((size_t)P + E + 1))) return -1;
+  int32_t* h = static_cast<int32_t*>(e->pending_stage.p);
+  if (P) memcpy(h, pend_spec, sizeof(int32_t) * P);
+  memcpy(h + P, group_off, sizeof(int32_t) * (E + 1));
+  e->h_pend_spec = h;
+  e->h_group_off = h + P;
   e->h_group_spec.swap(gspec);
   e->groups_homogeneous = homog;
   return 0;
+}
+
+// Pending pods [pb, pe) of this rank in the dense pass: a block partition whose shard starts are multiples of 32, so that the
+// ranks' bit rows concatenate word by word; all of them when the caller uploaded its own shard only
+static void pod_shard(const Engine* e, int P, int* pb, int* pe) {
+  const int W = std::max(1, e->cfg.world_size), rk = e->cfg.rank;
+  *pb = (int)((int64_t)P * rk / W) / 32 * 32;
+  *pe = (int)((int64_t)P * (rk + 1) / W);
+  if (rk + 1 < W) *pe = *pe / 32 * 32;
+  if (e->cfg.flags & CAE_CFG_PODS_PRESHARDED) { *pb = 0; *pe = P; }
+}
+
+// Requests of a row's resident pods, summed per resource dim
+static void resident_req(const int64_t* spec_req, const int32_t* pod_spec, int npods, int64_t reqd[R]) {
+  for (int r = 0; r < R; ++r) reqd[r] = 0;
+  for (int i = 0; i < npods; ++i)
+    for (int r = 0; r < R; ++r) reqd[r] += spec_req[(size_t)pod_spec[i] * R + r];
+}
+
+// Run state of a cluster row for the hostname-spread fallback (K3) and the filter-out-schedulable pass: free capacity per
+// active dim (`stride` elements apart) and free pod slots
+static void cluster_row_state(const Engine* e, const int64_t* alloc, int32_t allowed_pods, const int32_t* pod_spec, int npods,
+                              const int64_t* spec_req, int64_t* cfree, size_t stride, int32_t* cslots) {
+  int64_t reqd[R];
+  resident_req(spec_req, pod_spec, npods, reqd);
+  for (int a = 0; a < e->A; ++a) cfree[a * stride] = alloc[e->act_dim[a]] - reqd[e->act_dim[a]];
+  *cslots = allowed_pods - npods;
 }
 
 static int do_load(Engine* e, const cae_objects* o) {
@@ -277,12 +322,8 @@ static int do_load(Engine* e, const cae_objects* o) {
   e->Tw = (T + 31) / 32;
   e->Twp = (e->Tw + FEAS_TW - 1) / FEAS_TW * FEAS_TW;
   e->num_podspecs = o->num_podspecs;
+  pod_shard(e, e->P, &e->p_begin, &e->p_end);
   const int W = std::max(1, e->cfg.world_size), rk = e->cfg.rank;
-  e->p_begin = (int)((int64_t)e->P * rk / W);
-  e->p_end = (int)((int64_t)e->P * (rk + 1) / W);
-  e->p_begin = (e->p_begin / 32) * 32;  // word-aligned shards so bit rows concatenate
-  if (rk + 1 < W) e->p_end = (e->p_end / 32) * 32;
-  if (e->cfg.flags & CAE_CFG_PODS_PRESHARDED) { e->p_begin = 0; e->p_end = e->P; }   // the caller uploaded its own pod shard only
   e->Pl = e->p_end - e->p_begin;
   e->Plw = (e->Pl + 31) / 32;
   e->t_begin = (int)((int64_t)T * rk / W);
@@ -356,7 +397,6 @@ static int do_load(Engine* e, const cae_objects* o) {
   if (sclass.empty()) sclass.push_back({0, -1, -1, 0});
   e->SC = (int)sclass.size();
   e->DC = 1;  // class 0: no topology-spread / inter-pod-affinity involvement
-  e->h_dc_of_spec_valid = false;
   // The object tables and the static classes are complete: ship them and start the class matrix now, so that the
   // device works while the host goes on interning (dynamic classes, rank encoding).
   if (upload_mut(e, sclass, &e->d_sclass) || upload_mut(e, pc_of, &e->d_pc_of) || dev_alloc(e, &e->d_pre_code, (size_t)e->SC * e->U) ||
@@ -386,7 +426,6 @@ static int do_load(Engine* e, const cae_objects* o) {
   }
   int f_word[CAE_MAX_RES], f_shift[CAE_MAX_RES], f_bits[CAE_MAX_RES];
   e->W = 0;
-  for (int w = 0; w < FEAS_MAX_W; ++w) e->feas_guard[w] = 0;
   { int w = 0, shift = 0;
     for (int a = 0; a < e->A; ++a) {
       int bits = 1;
@@ -395,7 +434,6 @@ static int do_load(Engine* e, const cae_objects* o) {
       if (shift + bits > 32) { ++w; shift = 0; }
       if (w >= FEAS_MAX_W || bits > 32) { set_error("resource request cardinality too large for the rank encoding"); return 1; }
       f_word[a] = w; f_shift[a] = shift; f_bits[a] = bits;
-      e->feas_guard[w] |= 1u << (shift + bits - 1);
       shift += bits;
       e->W = w + 1;
     } }
@@ -411,23 +449,22 @@ static int do_load(Engine* e, const cae_objects* o) {
   std::vector<int64_t> free_all((size_t)R * T), free_act((size_t)A1 * T), cfree((size_t)A1 * std::max(N, 1));
   std::vector<int32_t> slots(T), cslots(std::max(N, 1));
   for (int row = 0; row < NT; ++row) {
-    int64_t reqd[R] = {0};
-    int npods = o->node_pod_off[row + 1] - o->node_pod_off[row];
-    for (int i = o->node_pod_off[row]; i < o->node_pod_off[row + 1]; ++i)
-      for (int r = 0; r < R; ++r) reqd[r] += o->ps_req[(size_t)o->node_pod_spec[i] * R + r];
-    if (row >= N) {
-      int t = row - N;
-      for (int r = 0; r < R; ++r) free_all[(size_t)r * T + t] = o->node_alloc[(size_t)row * R + r] - reqd[r];
-      for (int a = 0; a < e->A; ++a) free_act[(size_t)a * T + t] = free_all[(size_t)e->act_dim[a] * T + t];
-      slots[t] = o->node_allowed_pods[row] - npods;
-      for (int a = 0; a < e->A; ++a) {
-        int64_t f = free_act[(size_t)a * T + t];
-        uint32_t rank = (uint32_t)(std::upper_bound(rvals[a].begin(), rvals[a].end(), f) - rvals[a].begin());
-        tmpl_w[(size_t)f_word[a] * T + t] |= (rank | (1u << (f_bits[a] - 1))) << f_shift[a];
-      }
-    } else {   // cluster nodes: run state of the hostname-spread fallback (K3) and of the filter-out-schedulable pass
-      for (int a = 0; a < e->A; ++a) cfree[(size_t)a * N + row] = o->node_alloc[(size_t)row * R + e->act_dim[a]] - reqd[e->act_dim[a]];
-      cslots[row] = o->node_allowed_pods[row] - npods;
+    const int32_t* pods = o->node_pod_spec + o->node_pod_off[row];
+    const int npods = o->node_pod_off[row + 1] - o->node_pod_off[row];
+    if (row < N) {
+      cluster_row_state(e, o->node_alloc + (size_t)row * R, o->node_allowed_pods[row], pods, npods, o->ps_req, &cfree[row], N, &cslots[row]);
+      continue;
+    }
+    int64_t reqd[R];
+    resident_req(o->ps_req, pods, npods, reqd);
+    const int t = row - N;
+    for (int r = 0; r < R; ++r) free_all[(size_t)r * T + t] = o->node_alloc[(size_t)row * R + r] - reqd[r];
+    for (int a = 0; a < e->A; ++a) free_act[(size_t)a * T + t] = free_all[(size_t)e->act_dim[a] * T + t];
+    slots[t] = o->node_allowed_pods[row] - npods;
+    for (int a = 0; a < e->A; ++a) {
+      int64_t f = free_act[(size_t)a * T + t];
+      uint32_t rank = (uint32_t)(std::upper_bound(rvals[a].begin(), rvals[a].end(), f) - rvals[a].begin());
+      tmpl_w[(size_t)f_word[a] * T + t] |= (rank | (1u << (f_bits[a] - 1))) << f_shift[a];
     }
   }
   // bit-sliced free-capacity ranks for the dense pass (feas.cu): slice b, word tw holds bit b of the rank
@@ -473,7 +510,7 @@ static int do_load(Engine* e, const cae_objects* o) {
   }
   if (upload_mut(e, spec_sc, &e->d_spec_sc) || upload_mut(e, slots, &e->d_tmpl_slots) ||
       upload_mut(e, free_all, &e->d_tmpl_free_all) || upload_mut(e, free_act, &e->d_tmpl_free) || upload_mut(e, cfree, &e->d_c_free) ||
-      upload_mut(e, cslots, &e->d_c_slots) || upload_mut(e, spec_w, &e->d_spec_w) || upload_mut(e, tmpl_w, &e->d_tmpl_w) || upload_mut(e, spec_dc, &e->d_spec_dc))
+      upload_mut(e, cslots, &e->d_c_slots) || upload_mut(e, spec_w, &e->d_spec_w) || upload_mut(e, spec_dc, &e->d_spec_dc))
     return -1;
 
   lt.mark("ranks+tables");
@@ -483,13 +520,11 @@ static int do_load(Engine* e, const cae_objects* o) {
       dev_alloc(e, &e->d_pod_dc, (size_t)std::max(e->Pl, 1)) || dev_alloc(e, &e->d_fit_bits, (size_t)std::max(T, 1) * std::max(e->Plw, 1)) ||
       dev_alloc(e, &e->d_fit_count, (size_t)std::max(T, 1), true) || dev_alloc(e, &e->d_fit_acc, (size_t)std::max(T, 1), true) ||
       dev_alloc(e, &e->d_chunk_done, (size_t)std::max(e->Twp / FEAS_TW, 1), true) || dev_alloc(e, &e->d_group_reason, (size_t)std::max(T, 1) * std::max(e->E, 1)) ||
-      dev_alloc(e, &e->d_counts2, (size_t)2 * std::max(T, 1), true) || dev_alloc(e, &e->d_sched, (size_t)std::max(T, 1) * std::max(e->E, 1), true) ||
+      dev_alloc(e, &e->d_counts2, (size_t)2 * std::max(T, 1), true) || dev_alloc(e, &e->d_waste, (size_t)std::max(T, 1)) || dev_alloc(e, &e->d_sched, (size_t)std::max(T, 1) * std::max(e->E, 1), true) ||
       dev_alloc(e, &e->d_order, (size_t)std::max(T, 1) * std::max(e->E, 1)) || dev_alloc(e, &e->d_grec, (size_t)std::max(e->E, 1)) || dev_alloc(e, &e->d_order_n, (size_t)std::max(T, 1), true) ||
       dev_alloc(e, &e->d_max_nodes, (size_t)std::max(T, 1), true) || dev_alloc(e, &e->d_last_index_buf, (size_t)2 * std::max(T, 1), true) || dev_alloc(e, &e->d_tmpl_cost, (size_t)std::max(T, 1), true) ||
-      dev_alloc(e, &e->d_perm, (size_t)std::max(T, 1)) || dev_alloc(e, &e->d_work_counter, 4, true) ||
-      dev_alloc(e, &e->d_act_dim, CAE_MAX_RES))
+      dev_alloc(e, &e->d_perm, (size_t)std::max(T, 1)) || dev_alloc(e, &e->d_work_counter, 4, true))
     return -1;
-  e->d_score = nullptr;
   e->d_reasons = nullptr;
   if (e->cfg.want_reasons && dev_alloc(e, &e->d_reasons, (size_t)std::max(T, 1) * std::max(e->Pl, 1))) return -1;
 
@@ -517,7 +552,6 @@ static int do_load(Engine* e, const cae_objects* o) {
 
   lt.mark("dev_alloc+memsets");
   if (e->up.flush(e->stream, &e->stats.h2d_bytes)) return -1;   // ONE pinned H2D copy per arena chunk
-  CAE_CUDA(cudaMemcpyAsync(e->d_act_dim, e->act_dim, sizeof(int) * CAE_MAX_RES, cudaMemcpyHostToDevice, e->stream));
   if (launch_pre_ok_bits(e)) return -1;
   if (e->has_dynamic) {
     if (launch_dynamic_tables(e, e->d_spec_used, e->d_dc_ngroups)) return -1;
@@ -528,7 +562,6 @@ static int do_load(Engine* e, const cae_objects* o) {
     bool changed = false;
     for (int s = 0; s < S; ++s) if (spec_dc[s] && !act[spec_dc[s]]) { spec_dc[s] = 0; changed = true; }
     if (changed) CAE_CUDA(cudaMemcpyAsync(e->d_spec_dc, spec_dc.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, e->stream));
-    e->h_spec_dc = spec_dc;
     CAE_CUDA(cudaStreamSynchronize(e->stream));
   }
   if (launch_post_bits(e)) return -1;
@@ -553,14 +586,16 @@ static int grow_table(Engine* e, Engine::DevBuf& b, const T*& cur, size_t n_old,
   if (n_tail == 0) return 0;
   const size_t need = (n_old + n_tail) * sizeof(T);
   if (cur != b.p || need > b.cap) {
-    Engine::DevBuf nb = b;
+    void* np = b.p;
+    size_t ncap = b.cap;
     if (need > b.cap) {
-      nb.cap = need + need / 2 + 4096;
-      CAE_CUDA(cudaMallocAsync(&nb.p, nb.cap, e->stream));
+      ncap = need + need / 2 + 4096;
+      CAE_CUDA(cudaMallocAsync(&np, ncap, e->stream));
     }
-    if (n_old) CAE_CUDA(cudaMemcpyAsync(nb.p, cur, n_old * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
-    if (nb.p != b.p && b.p) CAE_CUDA(cudaFreeAsync(b.p, e->stream));   // stream-ordered: after the copy out of it
-    b = nb;
+    if (n_old) CAE_CUDA(cudaMemcpyAsync(np, cur, n_old * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
+    if (np != b.p && b.p) CAE_CUDA(cudaFreeAsync(b.p, e->stream));   // stream-ordered: after the copy out of it
+    b.p = np;
+    b.cap = ncap;
   }
   CAE_CUDA(cudaMemcpyAsync(static_cast<T*>(b.p) + n_old, d_tail, n_tail * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
   cur = static_cast<const T*>(b.p);
@@ -657,17 +692,8 @@ static int do_load_nodes(Engine* e, const cae_node_delta* dl) {
   const size_t o_toff = seg(ntl, 4), o_tkey = seg(tents, 4), o_tval = seg(tents, 4), o_teff = seg(tents, 4);
   const size_t o_row = seg(nd, 4), o_ls = seg(nd, 4), o_tl = seg(nd, 4), o_allowed = seg(nd, 4), o_slots = seg(nd, 4);
   const size_t o_poff = seg((size_t)nd + 1, 4), o_pspec = seg(npods, 4), o_visint = seg(nv, 1), o_unsched = seg(nd, 1);
-  if (e->ev_nd) CAE_CUDA(cudaEventSynchronize(e->ev_nd));   // the previous delta's copy out of the staging (long finished)
-  else CAE_CUDA(cudaEventCreateWithFlags(&e->ev_nd, cudaEventDisableTiming));
-  if (bytes > e->nd_stage_bytes) {
-    if (e->h_nd_stage) cudaFreeHost(e->h_nd_stage);
-    e->h_nd_stage = nullptr;
-    e->nd_stage_bytes = 0;
-    const size_t cap = bytes + bytes / 4 + 4096;
-    CAE_CUDA(cudaHostAlloc(&e->h_nd_stage, cap, cudaHostAllocDefault));
-    e->nd_stage_bytes = cap;
-  }
-  char* h = static_cast<char*>(e->h_nd_stage);
+  if (pinned_reserve(e, e->nd_stage, bytes)) return -1;
+  char* h = static_cast<char*>(e->nd_stage.p);
   auto put = [&](size_t at, const void* src, size_t n) { if (n) memcpy(h + at, src, n); };
   put(o_vint, dl->value_int, (size_t)nv * 8);
   put(o_visint, dl->value_is_int, (size_t)nv);
@@ -686,20 +712,15 @@ static int do_load_nodes(Engine* e, const cae_node_delta* dl) {
   put(o_unsched, dl->unschedulable, (size_t)nd);
   if (nd) put(o_poff, dl->pod_off, ((size_t)nd + 1) * 4);
   put(o_pspec, dl->pod_spec, (size_t)npods * 4);
-  // free capacity and pod slots of the dirty rows for the fallback placements: the int64 arithmetic of do_load
   int64_t* cfree = reinterpret_cast<int64_t*>(h + o_cfree);
   int32_t* cslots = reinterpret_cast<int32_t*>(h + o_slots);
-  for (int i = 0; i < nd; ++i) {
-    int64_t reqd[R] = {0};
-    for (int p = dl->pod_off[i]; p < dl->pod_off[i + 1]; ++p)
-      for (int r = 0; r < R; ++r) reqd[r] += e->h_spec_req[(size_t)dl->pod_spec[p] * R + r];
-    for (int a = 0; a < A; ++a) cfree[(size_t)i * A + a] = dl->alloc[(size_t)i * R + e->act_dim[a]] - reqd[e->act_dim[a]];
-    cslots[i] = dl->allowed_pods[i] - (dl->pod_off[i + 1] - dl->pod_off[i]);
-  }
+  for (int i = 0; i < nd; ++i)
+    cluster_row_state(e, dl->alloc + (size_t)i * R, dl->allowed_pods[i], dl->pod_spec + dl->pod_off[i], dl->pod_off[i + 1] - dl->pod_off[i],
+                      e->h_spec_req.data(), cfree + (size_t)i * A, 1, cslots + i);
   if (devbuf_reserve(e, e->nd_blob, bytes)) return -1;
   char* dv = static_cast<char*>(e->nd_blob.p);
   CAE_CUDA(cudaMemcpyAsync(dv, h, bytes, cudaMemcpyHostToDevice, e->stream));
-  CAE_CUDA(cudaEventRecord(e->ev_nd, e->stream));
+  CAE_CUDA(cudaEventRecord(e->nd_stage.ev, e->stream));
   e->stats.h2d_bytes = (int64_t)bytes;
 
   // ---- dictionary tails ----
@@ -832,7 +853,6 @@ int32_t cae_create(const cae_config* cfg, cae_engine** out) {
   cudaEventCreate(&e->ev0);
   cudaEventCreate(&e->ev1);
   { const char* v = getenv("CAE_K1_BITSLICE"); e->force_bitslice = v && v[0] == '1'; }
-  { const char* v = getenv("CAE_K1_WARPS"); if (v && atoi(v) == 8) e->k1_warps = 8; }
   *out = reinterpret_cast<cae_engine*>(e);
   return 0;
 }
@@ -843,20 +863,14 @@ void cae_destroy(cae_engine* h) {
   cudaSetDevice(e->cfg.device);
   e->up.release();
   e->scratch.release();
-  if (e->d_pack_scratch) cudaFree(e->d_pack_scratch);
-  if (e->d_fm_scratch) cudaFree(e->d_fm_scratch);
-  if (e->d_fm_blob) cudaFree(e->d_fm_blob);
-  if (e->h_pending_stage) cudaFreeHost(e->h_pending_stage);
-  for (Engine::DevBuf* b : {&e->nd_off[0], &e->nd_off[1], &e->nd_spec[0], &e->nd_spec[1], &e->nd_cnt, &e->nd_didx, &e->nd_cub, &e->nd_blob})
-    if (b->p) cudaFree(b->p);
-  for (auto& b : e->nd_tab) if (b.p) cudaFree(b.p);
-  if (e->h_nd_stage) cudaFreeHost(e->h_nd_stage);
-  if (e->ev_nd) cudaEventDestroy(e->ev_nd);
+  for (int r = 0; r < Engine::PEER_MAX; ++r)   // the other ranks' exchange buffers, opened by cae_peer_attach
+    if (r != e->cfg.rank && e->peer_base[r]) cudaIpcCloseMemHandle(e->peer_base[r]);
+  if (e->d_xbuf) cudaFree(e->d_xbuf);
   if (e->ev2) { cudaEventDestroy(e->ev2); cudaEventDestroy(e->ev3); }
   if (e->ev0) cudaEventDestroy(e->ev0);
   if (e->ev1) cudaEventDestroy(e->ev1);
   if (e->stream) cudaStreamDestroy(e->stream);
-  delete e;
+  delete e;   // frees the growable buffers (Engine::DevBuf, Engine::PinnedBuf)
 }
 
 int32_t cae_load(cae_engine* h, const cae_objects* objs) {
@@ -872,12 +886,8 @@ int32_t cae_load_pending(cae_engine* h, int32_t num_pending, const int32_t* pend
   if (num_pending < 0 || num_groups < 0 || (num_pending && !pend_spec) || !group_off) { cae::set_error("cae_load_pending: bad arguments"); return -2; }
   cudaSetDevice(e->cfg.device);
   const int P = num_pending, E = num_groups;
-  // shard of this rank under the same rule as cae_load
-  const int W = std::max(1, e->cfg.world_size), rk = e->cfg.rank;
-  int pb = (int)((int64_t)P * rk / W), pe = (int)((int64_t)P * (rk + 1) / W);
-  pb = (pb / 32) * 32;
-  if (rk + 1 < W) pe = (pe / 32) * 32;
-  if (e->cfg.flags & CAE_CFG_PODS_PRESHARDED) { pb = 0; pe = P; }
+  int pb = 0, pe = 0;
+  cae::pod_shard(e, P, &pb, &pe);
   const int Pl = pe - pb;
   if (P > e->cap_P || E > e->cap_E || Pl > e->cap_Pl) { cae::set_error("cae_load_pending: more pods / groups than the resident buffers hold"); return 2; }
   if (group_off[0] != 0 || group_off[E] != P) { cae::set_error("cae_load_pending: group_off does not cover the pending pods"); return -2; }
@@ -889,12 +899,11 @@ int32_t cae_load_pending(cae_engine* h, int32_t num_pending, const int32_t* pend
     }
     if (!same) { cae::set_error("cae_load_pending: the group -> spec sequence changed under topology counters"); return 2; }
   }
-  // wait for the previous delta's copies before the pinned rows are overwritten (normally long finished)
-  CAE_CUDA(cudaStreamSynchronize(e->stream));
   { int rc = cae::stage_pending(e, P, pend_spec, E, group_off, true); if (rc) return rc; }
   const size_t words = (size_t)P + E + 1;
   if (P) CAE_CUDA(cudaMemcpyAsync(const_cast<int32_t*>(e->dobj.pend_spec), e->h_pend_spec, sizeof(int32_t) * P, cudaMemcpyHostToDevice, e->stream));
   CAE_CUDA(cudaMemcpyAsync(const_cast<int32_t*>(e->dobj.group_off), e->h_group_off, sizeof(int32_t) * (E + 1), cudaMemcpyHostToDevice, e->stream));
+  CAE_CUDA(cudaEventRecord(e->pending_stage.ev, e->stream));
   e->stats.h2d_bytes = (int64_t)words * 4;
   e->P = P; e->E = E; e->p_begin = pb; e->p_end = pe; e->Pl = Pl; e->Plw = (Pl + 31) / 32;
   e->group_reason_valid = false;
@@ -1016,8 +1025,8 @@ int32_t cae_estimate_all_ex(cae_engine* h, const int32_t* max_nodes, const int32
     for (int t = e->t_begin; t < e->t_end; ++t) steps += order_n_host[t];
     e->stats.estimate_group_steps = steps;
   }
-  if (order && E)   // the device rows carry a flag bit per entry (ORDER_NOT_ON_FRESH); padding stays -1
-    for (size_t i = 0, nn = (size_t)T * E; i < nn; ++i) if (order[i] >= 0) order[i] &= ~cae::ORDER_NOT_ON_FRESH;
+  if (order && E)   // the device rows carry a flag bit per entry (ORDER_NOT_ON_FRESH); padding stays -1 (branch-free: it vectorises)
+    for (size_t i = 0, nn = (size_t)T * E; i < nn; ++i) order[i] &= order[i] < 0 ? ~0 : ~cae::ORDER_NOT_ON_FRESH;
   float ms = 0;
   cudaEventElapsedTime(&ms, e->ev0, e->ev1);
   e->stats.estimate_ms = ms;
@@ -1034,31 +1043,21 @@ int32_t cae_expander_best(cae_engine* h, const int32_t* chain, int32_t chain_len
   if (T == 0) return 0;
   // scores on the device: from the caller's (all-reduced) option table, or — sched_count == NULL —
   // straight from the device-resident result of the last cae_estimate_all (single-shard fast path)
-  int32_t *d_nc = nullptr, *d_sched = nullptr;
-  double* d_waste = nullptr;
-  std::vector<double> waste(T);
-  if (sched_count == nullptr) {
-    void* pw = nullptr;
-    if (e->scratch.alloc(&pw, nullptr, sizeof(double) * T)) return -1;
-    d_waste = static_cast<double*>(pw);
-    cudaEventRecord(e->ev0, e->stream);
-    if (cae::launch_expander(e, chain, chain_len, e->d_counts2, nullptr, e->d_sched, nullptr, d_waste)) return -1;
-    cudaEventRecord(e->ev1, e->stream);
-    CAE_CUDA(cudaMemcpyAsync(waste.data(), d_waste, sizeof(double) * T, cudaMemcpyDeviceToHost, e->stream));
-    CAE_CUDA(cudaStreamSynchronize(e->stream));
-  } else {
-    CAE_CUDA(cudaMalloc(&d_nc, sizeof(int32_t) * T));
-    CAE_CUDA(cudaMalloc(&d_sched, sizeof(int32_t) * (size_t)T * std::max(E, 1)));
-    CAE_CUDA(cudaMalloc(&d_waste, sizeof(double) * T));
-    CAE_CUDA(cudaMemcpyAsync(d_nc, node_count, sizeof(int32_t) * T, cudaMemcpyHostToDevice, e->stream));
-    if (E) CAE_CUDA(cudaMemcpyAsync(d_sched, sched_count, sizeof(int32_t) * (size_t)T * E, cudaMemcpyHostToDevice, e->stream));
-    cudaEventRecord(e->ev0, e->stream);
-    if (cae::launch_expander(e, chain, chain_len, d_nc, nullptr, d_sched, nullptr, d_waste)) return -1;
-    cudaEventRecord(e->ev1, e->stream);
-    CAE_CUDA(cudaMemcpyAsync(waste.data(), d_waste, sizeof(double) * T, cudaMemcpyDeviceToHost, e->stream));
-    CAE_CUDA(cudaStreamSynchronize(e->stream));
-    cudaFree(d_nc); cudaFree(d_sched); cudaFree(d_waste);
+  const int32_t *d_nc = e->d_counts2, *d_sched = e->d_sched;
+  if (sched_count) {
+    if (cae::devbuf_reserve(e, e->x_rows, sizeof(int32_t) * ((size_t)T + (size_t)T * std::max(E, 1)))) return -1;
+    int32_t* rows = static_cast<int32_t*>(e->x_rows.p);
+    CAE_CUDA(cudaMemcpyAsync(rows, node_count, sizeof(int32_t) * T, cudaMemcpyHostToDevice, e->stream));
+    if (E) CAE_CUDA(cudaMemcpyAsync(rows + T, sched_count, sizeof(int32_t) * (size_t)T * E, cudaMemcpyHostToDevice, e->stream));
+    d_nc = rows;
+    d_sched = rows + T;
   }
+  std::vector<double> waste(T);
+  cudaEventRecord(e->ev0, e->stream);
+  if (cae::launch_waste(e, d_nc, d_sched, e->d_waste)) return -1;
+  cudaEventRecord(e->ev1, e->stream);
+  CAE_CUDA(cudaMemcpyAsync(waste.data(), e->d_waste, sizeof(double) * T, cudaMemcpyDeviceToHost, e->stream));
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
   float ms = 0;
   cudaEventElapsedTime(&ms, e->ev0, e->ev1);
   e->stats.expander_ms = ms;
@@ -1072,11 +1071,8 @@ int32_t cae_waste_scores(cae_engine* h, double* waste_score) {
   cudaSetDevice(e->cfg.device);
   const int T = e->T;
   if (T == 0) return 0;
-  void* pw = nullptr;
-  if (e->scratch.alloc(&pw, nullptr, sizeof(double) * T)) return -1;
-  const int32_t chain0 = CAE_EXP_LEAST_WASTE;
-  if (cae::launch_expander(e, &chain0, 1, e->d_counts2, nullptr, e->d_sched, nullptr, static_cast<double*>(pw))) return -1;
-  CAE_CUDA(cudaMemcpyAsync(waste_score, pw, sizeof(double) * T, cudaMemcpyDeviceToHost, e->stream));
+  if (cae::launch_waste(e, e->d_counts2, e->d_sched, e->d_waste)) return -1;
+  CAE_CUDA(cudaMemcpyAsync(waste_score, e->d_waste, sizeof(double) * T, cudaMemcpyDeviceToHost, e->stream));
   CAE_CUDA(cudaStreamSynchronize(e->stream));
   for (int t = 0; t < T; ++t)
     if (t < e->t_begin || t >= e->t_end) waste_score[t] = 0.0;   // rows of other ranks: x + 0.0 == x, a sum all-reduce assembles the vector
@@ -1100,12 +1096,11 @@ int32_t cae_price_scores(cae_engine* h, const cae_price_inputs* in, const int32_
   cudaSetDevice(e->cfg.device);
   const int T = e->T, E = std::max(e->E, 1), S = e->num_podspecs;
   if (T == 0) return 0;
-  // one staging blob: node_price | pod_price | unfitness | score, then the byte vectors
+  // one device blob: node_price | pod_price | unfitness | score, then the byte vectors has_gpu | exists
   const size_t nd = (size_t)T + S + (in->unfitness ? T : 0) + T;
-  double* d_f = nullptr;
-  uint8_t* d_b = nullptr;
-  CAE_CUDA(cudaMalloc(&d_f, nd * sizeof(double)));
-  CAE_CUDA(cudaMalloc(&d_b, (size_t)3 * T));
+  if (cae::devbuf_reserve(e, e->x_price, nd * sizeof(double) + (size_t)2 * T)) return -1;
+  double* d_f = static_cast<double*>(e->x_price.p);
+  uint8_t* d_b = reinterpret_cast<uint8_t*>(d_f + nd);
   cae_price_inputs dev = *in;
   size_t off = 0;
   CAE_CUDA(cudaMemcpyAsync(d_f + off, in->node_price, sizeof(double) * T, cudaMemcpyHostToDevice, e->stream)); dev.node_price = d_f + off; off += T;
@@ -1115,10 +1110,10 @@ int32_t cae_price_scores(cae_engine* h, const cae_price_inputs* in, const int32_
   dev.has_gpu = dev.exists = dev.price_error = nullptr;
   if (in->has_gpu) { CAE_CUDA(cudaMemcpyAsync(d_b, in->has_gpu, T, cudaMemcpyHostToDevice, e->stream)); dev.has_gpu = d_b; }
   if (in->exists) { CAE_CUDA(cudaMemcpyAsync(d_b + T, in->exists, T, cudaMemcpyHostToDevice, e->stream)); dev.exists = d_b + T; }
-  int32_t *d_nc = e->d_counts2, *d_sched = e->d_sched, *d_order = e->d_order, *d_tmp = nullptr;
+  int32_t *d_nc = e->d_counts2, *d_sched = e->d_sched, *d_order = e->d_order;
   if (node_count) {
-    CAE_CUDA(cudaMalloc(&d_tmp, sizeof(int32_t) * ((size_t)T + (size_t)2 * T * E)));
-    d_nc = d_tmp; d_sched = d_tmp + T; d_order = d_sched + (size_t)T * E;
+    if (cae::devbuf_reserve(e, e->x_rows, sizeof(int32_t) * ((size_t)T + (size_t)2 * T * E))) return -1;
+    d_nc = static_cast<int32_t*>(e->x_rows.p); d_sched = d_nc + T; d_order = d_sched + (size_t)T * E;
     CAE_CUDA(cudaMemcpyAsync(d_nc, node_count, sizeof(int32_t) * T, cudaMemcpyHostToDevice, e->stream));
     CAE_CUDA(cudaMemcpyAsync(d_sched, sched_count, sizeof(int32_t) * (size_t)T * E, cudaMemcpyHostToDevice, e->stream));
     CAE_CUDA(cudaMemcpyAsync(d_order, order, sizeof(int32_t) * (size_t)T * E, cudaMemcpyHostToDevice, e->stream));
@@ -1131,8 +1126,6 @@ int32_t cae_price_scores(cae_engine* h, const cae_price_inputs* in, const int32_
   if (rc) return rc;
   CAE_CUDA(cudaMemcpyAsync(score, d_score, sizeof(double) * T, cudaMemcpyDeviceToHost, e->stream));
   CAE_CUDA(cudaStreamSynchronize(e->stream));
-  cudaFree(d_f); cudaFree(d_b);
-  if (d_tmp) cudaFree(d_tmp);
   return 0;
 }
 
@@ -1217,13 +1210,8 @@ int32_t cae_filter_schedulable(cae_engine* h, const int32_t* pod_order, int32_t 
   const size_t o_mark = off; off += words(std::max(n_classes, 1));
   const size_t o_over = off; off += words(std::max(nctrl, 1));
   (void)o_in_end;
-  if (off > e->fm_blob_words) {
-    if (e->d_fm_blob) cudaFree(e->d_fm_blob);
-    e->d_fm_blob = nullptr;
-    e->fm_blob_words = 0;
-    CAE_CUDA(cudaMalloc(&e->d_fm_blob, off * 4));
-    e->fm_blob_words = off;
-  }
+  if (cae::devbuf_reserve(e, e->fm_blob, off * 4)) return -1;
+  int32_t* blob = static_cast<int32_t*>(e->fm_blob.p);
   std::vector<int32_t> hostblob(o_in_end2, 0);
   std::copy(run_off.begin(), run_off.end(), hostblob.begin() + o_run);
   if (n_pods) std::copy(pod_order, pod_order + n_pods, hostblob.begin() + o_pods);
@@ -1231,26 +1219,26 @@ int32_t cae_filter_schedulable(cae_engine* h, const int32_t* pod_order, int32_t 
   if (sim_class) std::copy(sim_class, sim_class + P, hostblob.begin() + o_cls);
   if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, hostblob.begin() + o_cc);
   if (node_ok && N) memcpy(hostblob.data() + o_nodeok, node_ok, N);
-  CAE_CUDA(cudaMemcpyAsync(e->d_fm_blob, hostblob.data(), o_in_end2 * 4, cudaMemcpyHostToDevice, e->stream));
-  CAE_CUDA(cudaMemsetAsync(e->d_fm_blob + o_asg, 0xFF, (size_t)std::max(P, 1) * 4, e->stream));   // -1 = stays unschedulable
-  CAE_CUDA(cudaMemsetAsync(e->d_fm_blob + o_out, 0, (off - o_out) * 4, e->stream));
+  CAE_CUDA(cudaMemcpyAsync(blob, hostblob.data(), o_in_end2 * 4, cudaMemcpyHostToDevice, e->stream));
+  CAE_CUDA(cudaMemsetAsync(blob + o_asg, 0xFF, (size_t)std::max(P, 1) * 4, e->stream));   // -1 = stays unschedulable
+  CAE_CUDA(cudaMemsetAsync(blob + o_out, 0, (off - o_out) * 4, e->stream));
   cae::FilterLaunch f{};
   f.runs = runs; f.n_pods = n_pods; f.last_index = last_index_in; f.break_on_failure = break_on_failure ? 1 : 0; f.nctrl = nctrl;
-  f.run_off = e->d_fm_blob + o_run; f.pods = e->d_fm_blob + o_pods;
-  f.hint = hint_node ? e->d_fm_blob + o_hint : nullptr;
-  f.cls = sim_class ? e->d_fm_blob + o_cls : nullptr;
-  f.class_ctrl = e->d_fm_blob + o_cc;
-  f.node_ok = node_ok ? reinterpret_cast<const uint8_t*>(e->d_fm_blob + o_nodeok) : nullptr;
-  f.assigned = e->d_fm_blob + o_asg; f.out = e->d_fm_blob + o_out; f.ctrl_cnt = e->d_fm_blob + o_cnt;
-  f.class_mark = reinterpret_cast<uint8_t*>(e->d_fm_blob + o_mark);
-  f.ctrl_over = reinterpret_cast<uint8_t*>(e->d_fm_blob + o_over);
+  f.run_off = blob + o_run; f.pods = blob + o_pods;
+  f.hint = hint_node ? blob + o_hint : nullptr;
+  f.cls = sim_class ? blob + o_cls : nullptr;
+  f.class_ctrl = blob + o_cc;
+  f.node_ok = node_ok ? reinterpret_cast<const uint8_t*>(blob + o_nodeok) : nullptr;
+  f.assigned = blob + o_asg; f.out = blob + o_out; f.ctrl_cnt = blob + o_cnt;
+  f.class_mark = reinterpret_cast<uint8_t*>(blob + o_mark);
+  f.ctrl_over = reinterpret_cast<uint8_t*>(blob + o_over);
   cudaEventRecord(e->ev0, e->stream);
   if (runs > 0 && cae::launch_filter(e, f)) return -1;
   cudaEventRecord(e->ev1, e->stream);
   int32_t out[4] = {last_index_raw, 0, 0, 0}, status = 0;
-  if (P) CAE_CUDA(cudaMemcpyAsync(assigned_node, e->d_fm_blob + o_asg, (size_t)P * 4, cudaMemcpyDeviceToHost, e->stream));
+  if (P) CAE_CUDA(cudaMemcpyAsync(assigned_node, blob + o_asg, (size_t)P * 4, cudaMemcpyDeviceToHost, e->stream));
   if (runs > 0) {
-    CAE_CUDA(cudaMemcpyAsync(out, e->d_fm_blob + o_out, sizeof(out), cudaMemcpyDeviceToHost, e->stream));
+    CAE_CUDA(cudaMemcpyAsync(out, blob + o_out, sizeof(out), cudaMemcpyDeviceToHost, e->stream));
     CAE_CUDA(cudaMemcpyAsync(&status, e->d_work_counter + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
   }
   CAE_CUDA(cudaStreamSynchronize(e->stream));

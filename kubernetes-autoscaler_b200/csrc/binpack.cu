@@ -1503,6 +1503,27 @@ __global__ void lpt_rank_kernel(const long long* __restrict__ cost, int t_begin,
   if (i < nt) perm[rank] = t_begin + i;
 }
 
+// Bytes of one thread block's global slab (the layout at the top of binpack_kernel), 256-byte aligned
+static size_t slab_per_cta(int A1, size_t Xg, int dstride, int log_cap) {
+  const size_t b = 16 + Xg * ((size_t)A1 * 8 + 8 + 4 + 4 + 4 + 4) + (size_t)3 * DYN_MAX_Q * dstride * 4 + (size_t)log_cap * 12 + Xg;
+  return (b + 255) & ~(size_t)255;
+}
+
+// `need` bytes of slab for the layout p describes (Xg slab nodes per block).  The slot versions in a block's slab persist
+// across launches but are only meaningful within one layout: bytes that a new allocation or a new layout hands out are zeroed.
+static int slab_reserve(Engine* e, Engine::Slab& s, BpParams& p, int A1, size_t Xg, size_t need) {
+  const size_t sig = p.scratch_per_cta * 1000003u + Xg * 10007u + (size_t)p.dstride * 101u + (size_t)p.log_cap * 7u + (size_t)A1;
+  const void* old = s.buf.p;
+  if (devbuf_reserve(e, s.buf, need)) return -1;
+  if (s.buf.p != old || sig != s.sig) { s.sig = sig; s.zeroed = 0; }
+  if (need > s.zeroed) {
+    CAE_CUDA(cudaMemsetAsync(static_cast<unsigned char*>(s.buf.p) + s.zeroed, 0, need - s.zeroed, e->stream));
+    s.zeroed = need;
+  }
+  p.scratch = static_cast<unsigned char*>(s.buf.p);
+  return 0;
+}
+
 static int launch_binpack_any(Engine* e, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, bool filter = false) {
   const int A = std::min(e->A, 8);
   if (A <= 2) return bp_launch_part0(e, A, blocks_wanted, smem, p, blocks_out, query_only, filter);
@@ -1540,28 +1561,13 @@ int launch_binpack(Engine* e) {
   for (int k = 0; k < e->dyn.K; ++k) dmax = std::max(dmax, e->dyn.Dc[k] + 1 + (e->dyn.is_host[k] ? cap : 0));
   p.dstride = p.has_dyn ? dmax : 1;
   p.log_cap = p.has_dyn ? (int)std::min<size_t>(4 * ((size_t)Neff + cap) + 1024, (size_t)1 << 24) : 1;
-  size_t per_cta = 16 + Xg * ((size_t)A1 * 8 + 8 + 4 + 4 + 4 + 4) + (size_t)3 * DYN_MAX_Q * p.dstride * 4 + (size_t)p.log_cap * 12 + Xg;
-  per_cta = (per_cta + 255) & ~(size_t)255;
+  const size_t per_cta = slab_per_cta(A1, Xg, p.dstride, p.log_cap);
   p.scratch_per_cta = per_cta;
   int blocks = 0;
   if (launch_binpack_any(e, nt, smem, p, &blocks, true)) return -1;
   const size_t budget = e->hbm_bytes / 8;  // keep the slabs within an eighth of the device memory (10 GB on an 80 GB H100)
   if (per_cta * blocks > budget) blocks = (int)std::max<size_t>(1, budget / per_cta);
-  const size_t need = per_cta * blocks;
-  const size_t sig = per_cta * 1000003u + Xg * 10007u + (size_t)p.dstride * 101u + (size_t)p.log_cap * 7u + (size_t)A1 + 0x9000000000ull;
-  if (need > e->pack_scratch_bytes) {
-    if (e->d_pack_scratch) cudaFree(e->d_pack_scratch);
-    e->d_pack_scratch = nullptr;
-    e->pack_scratch_bytes = 0;
-    CAE_CUDA(cudaMalloc(&e->d_pack_scratch, need));
-    e->pack_scratch_bytes = need;
-    e->pack_layout_sig = 0;
-  }
-  if (sig != e->pack_layout_sig) {  // slot versions are only meaningful within one slab layout
-    CAE_CUDA(cudaMemsetAsync(e->d_pack_scratch, 0, need, e->stream));
-    e->pack_layout_sig = sig;
-  }
-  p.scratch = static_cast<unsigned char*>(e->d_pack_scratch);
+  if (slab_reserve(e, e->pack_slab, p, A1, Xg, per_cta * blocks)) return -1;
   CAE_CUDA(cudaMemsetAsync(e->d_work_counter, 0, sizeof(int32_t) * 2, e->stream));
   // longest processing time first: the heaviest templates start first, the tail of the pass is made of light ones
   lpt_rank_kernel<<<(nt + 255) / 256, 256, 0, e->stream>>>(e->d_tmpl_cost, e->t_begin, nt, e->d_perm);
@@ -1592,32 +1598,15 @@ int launch_binpack(Engine* e) {
 
 // ---- filter-out-schedulable pass -----------------------------------------------------------------------------------------
 __global__ void run_rec_kernel(DevObjects o, DynTables d, int runs, const int32_t* __restrict__ run_off, const int32_t* __restrict__ pods,
-                               int n_act, const int* __restrict__ act_dim, int has_dyn, const int32_t* __restrict__ spec_sc,
-                               const int32_t* __restrict__ spec_dc, const int32_t* __restrict__ pc_of,
-                               const unsigned long long* __restrict__ port_conf, GroupRec* __restrict__ out) {
+                               GroupRecSrc s, GroupRec* __restrict__ out) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= runs) return;
-  GroupRec g{};
   const int pb = run_off[r];
-  g.n = run_off[r + 1] - pb;
-  g.pad[0] = pb;
-  g.kcap = INT_MAX;
   const int spec = o.pend_spec[pods[pb]];
-  g.spec = spec;
-  g.sc = spec_sc[spec];
-  g.dc = has_dyn ? spec_dc[spec] : 0;
-  const int plist = o.ps_port_list[spec];
-  const bool has_ports = o.port_off[plist + 1] > o.port_off[plist];
-  g.pconf = has_ports ? port_conf[plist] : 0ull;
-  g.pbit = has_ports ? (1ull << pc_of[plist]) : 0ull;
   bool feeds = false;   // runs are not groups: log every placement that some counter counts
-  if (has_dyn) for (int q = 0; q < d.Q && !feeds; ++q) feeds = d.wmat[(size_t)q * d.S + spec] != 0;
-  g.flags = (has_ports ? GREC_HAS_PORTS : 0u) | (feeds ? GREC_FEEDS : 0u) | (o.ps_hostname_spread[spec] ? GREC_HOST_SPREAD : 0u);
-  for (int a = 0; a < n_act; ++a) {
-    g.req[a] = o.ps_req[(size_t)spec * R + act_dim[a]];
-    g.rinv[a] = g.req[a] > 0 ? __frcp_rn(__ll2float_rn(g.req[a])) : 0.f;
-    if (g.req[a] >> 32) g.kcap = min(g.kcap, (int)(LLONG_MAX / g.req[a]));
-  }
+  if (s.has_dyn) for (int q = 0; q < d.Q && !feeds; ++q) feeds = d.wmat[(size_t)q * d.S + spec] != 0;
+  GroupRec g = build_group_rec(o, s, spec, run_off[r + 1] - pb, feeds);
+  g.pad[0] = pb;
   out[r] = g;
 }
 
@@ -1642,30 +1631,13 @@ int launch_filter(Engine* e, const FilterLaunch& f) {
   for (int k = 0; k < e->dyn.K; ++k) dmax = std::max(dmax, e->dyn.Dc[k] + 2);
   p.dstride = p.has_dyn ? dmax : 1;
   p.log_cap = p.has_dyn ? f.n_pods + 1024 : 1;   // one entry per placement at most
-  size_t per_cta = 16 + Xg * ((size_t)A1 * 8 + 8 + 4 + 4 + 4 + 4) + (size_t)3 * DYN_MAX_Q * p.dstride * 4 + (size_t)p.log_cap * 12 + Xg;
-  per_cta = (per_cta + 255) & ~(size_t)255;
-  p.scratch_per_cta = per_cta;
-  const size_t rec_bytes = ((size_t)std::max(f.runs, 1) * sizeof(GroupRec) + 255) & ~(size_t)255;
-  const size_t need = per_cta + rec_bytes;
-  const size_t sig = per_cta * 1000003u + Xg * 10007u + (size_t)p.dstride * 101u + (size_t)p.log_cap * 7u + (size_t)A1 + 0x7000000000ull;
-  if (need > e->fm_scratch_bytes) {
-    if (e->d_fm_scratch) cudaFree(e->d_fm_scratch);
-    e->d_fm_scratch = nullptr;
-    e->fm_scratch_bytes = 0;
-    CAE_CUDA(cudaMalloc(&e->d_fm_scratch, need));
-    e->fm_scratch_bytes = need;
-    e->fm_layout_sig = 0;
-  }
-  if (sig != e->fm_layout_sig) {
-    CAE_CUDA(cudaMemsetAsync(e->d_fm_scratch, 0, need, e->stream));
-    e->fm_layout_sig = sig;
-  }
-  p.scratch = static_cast<unsigned char*>(e->d_fm_scratch);
-  GroupRec* d_rec = reinterpret_cast<GroupRec*>(p.scratch + per_cta);
+  p.scratch_per_cta = slab_per_cta(A1, Xg, p.dstride, p.log_cap);
+  const size_t rec_bytes = ((size_t)std::max(f.runs, 1) * sizeof(GroupRec) + 255) & ~(size_t)255;   // the run records follow the one slab
+  if (slab_reserve(e, e->fm_slab, p, A1, Xg, p.scratch_per_cta + rec_bytes)) return -1;
+  GroupRec* d_rec = reinterpret_cast<GroupRec*>(p.scratch + p.scratch_per_cta);
   p.grec = d_rec;
   CAE_CUDA(cudaMemsetAsync(e->d_work_counter, 0, sizeof(int32_t) * 2, e->stream));
-  run_rec_kernel<<<(f.runs + 127) / 128, 128, 0, e->stream>>>(e->dobj, e->dyn, f.runs, f.run_off, f.pods, e->A, e->d_act_dim, p.has_dyn,
-                                                             e->d_spec_sc, e->d_spec_dc, e->d_pc_of, e->d_port_conf, d_rec);
+  run_rec_kernel<<<(f.runs + 127) / 128, 128, 0, e->stream>>>(e->dobj, e->dyn, f.runs, f.run_off, f.pods, group_rec_src(e), d_rec);
   { int unused = 0; if (launch_binpack_any(e, 1, 0, p, &unused, false, true)) return -1; }
   e->stats.kernel_launches += 2;
   CAE_KERNEL_OK();

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <climits>
 #include <cstdint>
 #include <string>
 #include <vector>
@@ -31,6 +32,35 @@ struct alignas(16) GroupRec {
 };
 static_assert(sizeof(GroupRec) == 144, "GroupRec is fetched as nine 16-byte chunks");
 enum : uint32_t { GREC_HAS_PORTS = 1u, GREC_FEEDS = 2u, GREC_HOST_SPREAD = 4u };
+
+// The engine tables a GroupRec is built from (group_rec_src), beside the spec, pod count and feeds flag of the group
+struct GroupRecSrc {
+  int has_dyn, n_act;
+  int act_dim[CAE_MAX_RES];
+  const int32_t *spec_sc, *spec_dc, *pc_of;
+  const unsigned long long* port_conf;
+};
+// The record of n pods of one spec: a pod group (group_rec_kernel) or a run of the filter pass (run_rec_kernel)
+__device__ __forceinline__ GroupRec build_group_rec(const DevObjects& o, const GroupRecSrc& s, int spec, int n, bool feeds) {
+  GroupRec r{};
+  r.n = n;
+  r.kcap = INT_MAX;
+  if (n <= 0) return r;
+  r.spec = spec;
+  r.sc = s.spec_sc[spec];
+  r.dc = s.has_dyn ? s.spec_dc[spec] : 0;
+  const int plist = o.ps_port_list[spec];
+  const bool has_ports = o.port_off[plist + 1] > o.port_off[plist];
+  r.pconf = has_ports ? s.port_conf[plist] : 0ull;
+  r.pbit = has_ports ? (1ull << s.pc_of[plist]) : 0ull;
+  r.flags = (has_ports ? GREC_HAS_PORTS : 0u) | (feeds ? GREC_FEEDS : 0u) | (o.ps_hostname_spread[spec] ? GREC_HOST_SPREAD : 0u);
+  for (int a = 0; a < s.n_act; ++a) {
+    r.req[a] = o.ps_req[(size_t)spec * R + s.act_dim[a]];
+    r.rinv[a] = r.req[a] > 0 ? __frcp_rn(__ll2float_rn(r.req[a])) : 0.f;
+    if (r.req[a] >> 32) r.kcap = min(r.kcap, (int)(LLONG_MAX / r.req[a]));   // below 2^32, k < 2^31 cannot wrap
+  }
+  return r;
+}
 constexpr int ORDER_NOT_ON_FRESH = 1 << 30;   // order entry flag: the group's static filters fail on the SANITIZED template
 
 #define CAE_CUDA(expr)                                                                        \
@@ -77,9 +107,6 @@ struct Engine {
   const int32_t* d_dc_ngroups = nullptr;
   int64_t* d_c_free = nullptr;            // [A][N] free capacity of the cluster nodes (fallback placements)
   int32_t* d_c_slots = nullptr;           // [N]
-  int* d_act_dim = nullptr;               // [CAE_MAX_RES]
-  std::vector<int32_t> h_spec_dc;
-  bool h_dc_of_spec_valid = false;
   cae_stats stats{};
   bool loaded = false;
 
@@ -105,11 +132,9 @@ struct Engine {
   uint8_t* d_post_code = nullptr;         // [DC][T] PTS / IPA reason on the empty template (0 = ok)
   uint32_t* d_post_ok = nullptr;          // [DC][Twp]
   int W = 0;                              // 32-bit words of the packed rank encoding (feas.cu)
-  uint32_t feas_guard[4] = {0, 0, 0, 0};  // guard-bit mask per word
   uint32_t* d_spec_w = nullptr;           // [num_podspecs][FEAS_MAX_W] packed request ranks
   uint32_t* d_pod_w = nullptr;            // [W][Pl] per pending pod
   uint16_t* d_pod_row = nullptr;          // [A][Pl] threshold-row id per active dim (LUT variant)
-  uint32_t* d_tmpl_w = nullptr;           // [W][T] packed free-capacity ranks + guard bits
   int feas_B = 0;                         // bit slices of the free-capacity ranks (all fields)
   uint32_t feas_fstart = 0;               // bit b set: slice b is the most significant bit of a field
   uint8_t feas_sword[32] = {0}, feas_sshift[32] = {0};  // where bit b sits in the packed pod words
@@ -122,14 +147,12 @@ struct Engine {
   uint32_t* d_rlut = nullptr;             // [lut_rows][Twp]
   long long* d_tmpl_cost = nullptr;       // [T] pods in the schedulable groups of a template (order kernel)
   int32_t* d_perm = nullptr;              // [T] work order of the pack
-  int k1_warps = 16;                      // warps per thread block of the LUT variant (CAE_K1_WARPS=8|16)
   bool force_bitslice = false;            // CAE_K1_BITSLICE=1: always take the bit-sliced comparator (tests)
   int32_t* d_pod_sc = nullptr;            // [P]
   int32_t* d_pod_dc = nullptr;            // [P]
   int64_t* d_tmpl_free = nullptr;         // [A][T] allocatable - DaemonSet requested
   int64_t* d_tmpl_free_all = nullptr;     // [R][T] same over all R dims (pack kernel)
   int32_t* d_tmpl_slots = nullptr;        // [T] allowed pods - DaemonSet pods
-  int64_t* d_spec_req_t = nullptr;        // [num_podspecs][R] request (raw)
   // results kept on device
   uint32_t* d_fit_bits = nullptr;         // [T][Plw]
   uint8_t* d_reasons = nullptr;           // [T][Pl] (want_reasons)
@@ -143,7 +166,7 @@ struct Engine {
   int32_t* d_order = nullptr;             // [T][E]
   int32_t* d_order_n = nullptr;           // [T]
   GroupRec* d_grec = nullptr;             // [E]
-  double* d_score = nullptr;              // [T][E]
+  double* d_waste = nullptr;              // [T] least-waste score per option
   int32_t* d_max_nodes = nullptr;         // [T]
   int32_t* d_last_index_buf = nullptr;    // [2T] lastIndex in | out (cae_estimate_all_ex)
   const int32_t* d_last_index_in = nullptr;   // set per call: NULL = every Estimate starts at 0
@@ -151,15 +174,29 @@ struct Engine {
   int32_t* d_pc_of = nullptr;             // [num_port_lists] compact id of a pending pod's port list, -1 otherwise
   unsigned long long* d_port_conf = nullptr;  // [num_port_lists] conflict mask over compact ids
   int pack_cap = 1 << 30;                 // node capacity of a pack slab (from the limiter caps)
-  // pack scratch
-  void* d_pack_scratch = nullptr;
-  size_t pack_scratch_bytes = 0;
-  size_t pack_layout_sig = 0;
-  // filter-out-schedulable pass (binpack.cu, FM): own slab + input blob
-  void* d_fm_scratch = nullptr;
-  size_t fm_scratch_bytes = 0, fm_layout_sig = 0;
-  int32_t* d_fm_blob = nullptr;
-  size_t fm_blob_words = 0;
+  // Engine-owned buffers that grow and are kept across loads (devbuf_reserve / pinned_reserve in api.cu), freed with the engine.
+  struct DevBuf {
+    void* p = nullptr;
+    size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
+  };
+  struct PinnedBuf {                      // host staging of H2D copies: the host waits for the last copy out of it before writing
+    void* p = nullptr;
+    size_t cap = 0;
+    cudaEvent_t ev = nullptr;             // recorded after the last H2D copy that reads the buffer
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf&) = delete;
+    PinnedBuf& operator=(const PinnedBuf&) = delete;
+    ~PinnedBuf() { if (p) cudaFreeHost(p); if (ev) cudaEventDestroy(ev); }
+  };
+  struct Slab { DevBuf buf; size_t sig = 0, zeroed = 0; };   // estimator slab: layout signature, bytes zeroed under it
+  Slab pack_slab, fm_slab;                // estimator / filter-out-schedulable pass (binpack.cu)
+  DevBuf fm_blob;                         // inputs and outputs of the filter pass
+  DevBuf x_rows;                          // caller-supplied option rows: node_count | sched | order
+  DevBuf x_price;                         // price inputs: node_price | pod_price | unfitness | score, then has_gpu | exists
   // fused histogram exchange over peer memory (feas.cu)
   static constexpr int PEER_MAX = 8, PEER_CAP = 1 << 16;
   int32_t* d_xbuf = nullptr;              // [2 parities][PEER_MAX][PEER_CAP] (count, step tag) slots + done counter, status
@@ -168,15 +205,13 @@ struct Engine {
   int64_t peer_step = 0;
   int32_t* d_work_counter = nullptr;
   // host copies needed by host-side steps
-  const int32_t *h_group_off = nullptr, *h_pend_spec = nullptr;   // host copy of the pending-pod rows: views into h_pending_stage
+  const int32_t *h_group_off = nullptr, *h_pend_spec = nullptr;   // host copy of the pending-pod rows: views into pending_stage
   std::vector<int32_t> h_group_spec;      // [E] spec of each group's pods (-1 = empty group)
   bool groups_homogeneous = true;         // every group holds pods of ONE spec (equivalence.BuildPodGroups guarantees it)
   std::vector<uint8_t> h_spec_pending;    // [num_podspecs] spec carried by a pending pod at the last full load
   int cap_P = 0, cap_E = 0, cap_Pl = 0;   // capacities of the resident per-pod / per-group buffers (cae_load_pending)
-  int32_t* h_pending_stage = nullptr;     // pinned staging of pend_spec | group_off for the delta upload
-  size_t pending_stage_words = 0;
+  PinnedBuf pending_stage;                // pend_spec | group_off, source of cae_load_pending's H2D copy
   std::vector<int64_t> h_spec_req;        // [num_podspecs][R]
-  std::vector<int64_t> h_cap_cpu, h_cap_mem;  // per template
   int num_podspecs = 0;
   // host state of the last load that cae_load_nodes validates against and updates (node_delta in api.cu)
   struct NodeHost {
@@ -188,18 +223,19 @@ struct Engine {
     std::vector<uint8_t> spec_anti;                // [S] spec has required anti-affinity terms
     std::vector<int32_t> key_val;                  // [K][N] value id of resident topology key k on cluster row n, -1 absent
   } nh;
-  // engine-owned device buffers of cae_load_nodes (stream-ordered allocations; a cae_load points DevObjects back at its arena)
-  struct DevBuf { void* p = nullptr; size_t cap = 0; };
+  // buffers of cae_load_nodes (a cae_load points DevObjects back at its arena)
   DevBuf nd_tab[9];                       // grown dictionary tables: value_is_int, value_int, ls_off|key|val, taint_off|key|val|effect
   DevBuf nd_off[2], nd_spec[2];           // double-buffered resident CSR (node_pod_off / node_pod_spec)
   DevBuf nd_cnt, nd_didx, nd_cub, nd_blob;  // per-row counts / dirty index, scan temp storage, device copy of the delta
-  void* h_nd_stage = nullptr;             // pinned staging of the delta
-  size_t nd_stage_bytes = 0;
-  cudaEvent_t ev_nd = nullptr;            // the last delta's H2D copy (guards the pinned staging)
+  PinnedBuf nd_stage;                     // the delta, source of its one H2D copy
   int sm_count = 132;
   int smem_optin = 227 * 1024;             // opt-in shared memory per thread block
   size_t hbm_bytes = (size_t)80 << 30;     // device memory (sizes the estimator's global slabs)
 };
+
+// api.cu: growth of the engine-owned buffers; the contents are not kept
+int devbuf_reserve(Engine* e, Engine::DevBuf& b, size_t bytes);          // stream-ordered
+int pinned_reserve(Engine* e, Engine::PinnedBuf& b, size_t bytes);       // after the last copy out of b has finished
 
 // kernels.cu
 int launch_class_matrix(Engine* e);      // pre_code[SC][U]: needs only the object tables + the static classes
@@ -212,7 +248,6 @@ struct NodeDeltaDev {                    // device views into the staged cae_nod
   const int64_t *alloc, *cfree;          // [nd][R], [nd][A]
 };
 int launch_node_rows(Engine* e, const NodeDeltaDev& d, int64_t total);   // rows in place + resident CSR rebuilt into the spare buffer
-int devbuf_reserve(Engine* e, Engine::DevBuf& b, size_t bytes);          // stream-ordered growth, contents not kept
 int launch_pre_ok_bits(Engine* e);       // pre_ok[SC][Twp]: needs pre_code and the templates' pod slots
 int launch_post_bits(Engine* e);
 int launch_dynamic_tables(Engine* e, const uint8_t* d_spec_used, const int32_t* d_dc_ngroups);
@@ -222,6 +257,7 @@ int launch_feasibility(Engine* e, bool want_reasons);
 int launch_group_feasibility(Engine* e);
 int launch_order(Engine* e);
 int launch_group_records(Engine* e);     // GroupRec[E] (after the class / counter tables of a load)
+GroupRecSrc group_rec_src(const Engine* e);
 int launch_binpack(Engine* e);   // K3: block-per-template estimator (binpack.cu)
 struct FilterLaunch {
   int runs, n_pods, last_index, break_on_failure, nctrl;
@@ -233,7 +269,6 @@ struct FilterLaunch {
 int launch_filter(Engine* e, const FilterLaunch& f);
 int launch_price(Engine* e, const cae_price_inputs& in_dev, const int32_t* d_node_count, const int32_t* d_sched, const int32_t* d_order,
                  double* d_score);
-int launch_expander(Engine* e, const int32_t* chain, int chain_len, const int32_t* d_node_count,
-                    const int32_t* d_pod_count, const int32_t* d_sched, uint8_t* d_mask, double* d_waste);
+int launch_waste(Engine* e, const int32_t* d_node_count, const int32_t* d_sched, double* d_waste);
 
 }  // namespace cae

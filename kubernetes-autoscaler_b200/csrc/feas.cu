@@ -544,8 +544,6 @@ static int launch_feas_lut_arw(Engine* e, K1Args a, const PeerPush& pp) {
 
 template <int A>
 static int launch_feas_lut_a(Engine* e, bool want_reasons, const K1Args& a, const PeerPush& pp) {
-  if (e->k1_warps == 8)
-    return want_reasons ? launch_feas_lut_arw<A, true, 8>(e, a, pp) : launch_feas_lut_arw<A, false, 8>(e, a, pp);
   return want_reasons ? launch_feas_lut_arw<A, true, 16>(e, a, pp) : launch_feas_lut_arw<A, false, 16>(e, a, pp);
 }
 

@@ -151,8 +151,7 @@ int launch_port_conflicts(Engine* e, int num_port_lists) {
 // ------------------------------------------------------------------------------------------------
 __global__ void order_kernel(DevObjects o, int E, int T, int N, int t_begin, int n_sort,
                              const uint8_t* __restrict__ group_reason, const uint8_t* __restrict__ pre_code,
-                             const int32_t* __restrict__ spec_sc, double* __restrict__ score_out,
-                             int32_t* __restrict__ order, int32_t* __restrict__ order_n, long long* __restrict__ tmpl_cost) {
+                             const int32_t* __restrict__ spec_sc, int32_t* __restrict__ order, int32_t* __restrict__ order_n, long long* __restrict__ tmpl_cost) {
   extern __shared__ unsigned char smem_raw[];
   __shared__ unsigned long long s_cost;   // pods in this template's schedulable groups: the pack's work estimate
   double* s_key = reinterpret_cast<double*>(smem_raw);
@@ -177,7 +176,6 @@ __global__ void order_kernel(DevObjects o, int E, int T, int N, int t_begin, int
       // the nodes Estimate adds are SANITIZED copies (fresh name and hostname label): flag the groups whose static
       // filters pass on the template but not on its copy (nodeName / matchFields / hostname selectors)
       if (pre_code[(size_t)spec_sc[spec] * (N + 2 * T) + N + T + t] & 0x0F) idx |= ORDER_NOT_ON_FRESH;
-      if (score_out) score_out[(size_t)t * E + g] = sc;
       if (tmpl_cost) atomicAdd(&s_cost, (unsigned long long)(o.group_off[g + 1] - o.group_off[g]));
     }
     s_key[g] = sc;
@@ -226,51 +224,34 @@ int launch_order(Engine* e) {
   if (smem > 200 * 1024) { set_error("too many pod groups for the in-smem orderer"); return 1; }
   CAE_CUDA(cudaFuncSetAttribute(order_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   order_kernel<<<nt, 256, smem, e->stream>>>(e->dobj, e->E, e->T, e->N, e->t_begin, n_sort, e->d_group_reason,
-                                              e->d_pre_code, e->d_spec_sc, e->d_score, e->d_order, e->d_order_n, e->d_tmpl_cost);
+                                              e->d_pre_code, e->d_spec_sc, e->d_order, e->d_order_n, e->d_tmpl_cost);
   e->stats.kernel_launches++;
   CAE_KERNEL_OK();
   return 0;
 }
 
-struct ActDims { int n; int dim[CAE_MAX_RES]; };
+GroupRecSrc group_rec_src(const Engine* e) {
+  GroupRecSrc s{};
+  s.has_dyn = e->has_dynamic ? 1 : 0;
+  s.n_act = e->A;
+  for (int a = 0; a < CAE_MAX_RES; ++a) s.act_dim[a] = e->act_dim[a];
+  s.spec_sc = e->d_spec_sc;
+  s.spec_dc = e->d_spec_dc;
+  s.pc_of = e->d_pc_of;
+  s.port_conf = e->d_port_conf;
+  return s;
+}
 
-__global__ void group_rec_kernel(DevObjects o, int E, ActDims act, int has_dyn, const int32_t* __restrict__ spec_sc,
-                                 const int32_t* __restrict__ spec_dc, const int32_t* __restrict__ pc_of,
-                                 const unsigned long long* __restrict__ port_conf, const uint8_t* __restrict__ group_feeds,
-                                 GroupRec* __restrict__ out) {
+__global__ void group_rec_kernel(DevObjects o, int E, GroupRecSrc s, const uint8_t* __restrict__ group_feeds, GroupRec* __restrict__ out) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= E) return;
-  GroupRec r{};
-  const int pb = o.group_off[g];
-  r.n = o.group_off[g + 1] - pb;
-  r.kcap = INT_MAX;
-  if (r.n > 0) {
-    const int spec = o.pend_spec[pb];
-    r.spec = spec;
-    r.sc = spec_sc[spec];
-    r.dc = has_dyn ? spec_dc[spec] : 0;
-    const int plist = o.ps_port_list[spec];
-    const bool has_ports = o.port_off[plist + 1] > o.port_off[plist];
-    r.pconf = has_ports ? port_conf[plist] : 0ull;
-    r.pbit = has_ports ? (1ull << pc_of[plist]) : 0ull;
-    r.flags = (has_ports ? GREC_HAS_PORTS : 0u) | ((has_dyn && group_feeds[g]) ? GREC_FEEDS : 0u) |
-              (o.ps_hostname_spread[spec] ? GREC_HOST_SPREAD : 0u);
-    for (int a = 0; a < act.n; ++a) {
-      r.req[a] = o.ps_req[(size_t)spec * R + act.dim[a]];
-      r.rinv[a] = r.req[a] > 0 ? __frcp_rn(__ll2float_rn(r.req[a])) : 0.f;
-      if (r.req[a] >> 32) r.kcap = min(r.kcap, (int)(LLONG_MAX / r.req[a]));   // below 2^32, k < 2^31 cannot wrap
-    }
-  }
-  out[g] = r;
+  const int pb = o.group_off[g], n = o.group_off[g + 1] - pb;
+  out[g] = build_group_rec(o, s, n > 0 ? o.pend_spec[pb] : -1, n, n > 0 && s.has_dyn && group_feeds[g]);
 }
 
 int launch_group_records(Engine* e) {
   if (e->E == 0) return 0;
-  ActDims act{};
-  act.n = e->A;
-  for (int a = 0; a < CAE_MAX_RES; ++a) act.dim[a] = e->act_dim[a];
-  group_rec_kernel<<<(e->E + 127) / 128, 128, 0, e->stream>>>(e->dobj, e->E, act, e->has_dynamic ? 1 : 0, e->d_spec_sc, e->d_spec_dc,
-                                                               e->d_pc_of, e->d_port_conf, e->dyn.group_feeds, e->d_grec);
+  group_rec_kernel<<<(e->E + 127) / 128, 128, 0, e->stream>>>(e->dobj, e->E, group_rec_src(e), e->dyn.group_feeds, e->d_grec);
   e->stats.kernel_launches++;
   CAE_KERNEL_OK();
   return 0;
@@ -409,8 +390,7 @@ int launch_price(Engine* e, const cae_price_inputs& in_dev, const int32_t* d_nod
   return 0;
 }
 
-int launch_expander(Engine* e, const int32_t*, int, const int32_t* d_node_count, const int32_t*,
-                    const int32_t* d_sched, uint8_t*, double* d_waste) {
+int launch_waste(Engine* e, const int32_t* d_node_count, const int32_t* d_sched, double* d_waste) {
   if (e->T == 0) return 0;
   int threads = 128, warps_per_block = threads / 32;
   waste_kernel<<<(e->T + warps_per_block - 1) / warps_per_block, threads, 0, e->stream>>>(e->dobj, e->E, e->T, e->N,

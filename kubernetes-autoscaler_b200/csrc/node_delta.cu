@@ -10,18 +10,6 @@
 
 namespace cae {
 
-// stream-ordered (re)allocation with 25 % headroom; the old contents are NOT kept (the buffer is free when this is called)
-int devbuf_reserve(Engine* e, Engine::DevBuf& b, size_t bytes) {
-  if (bytes <= b.cap) return 0;
-  if (b.p) CAE_CUDA(cudaFreeAsync(b.p, e->stream));
-  b.p = nullptr;
-  b.cap = 0;
-  const size_t cap = std::max<size_t>(bytes + bytes / 4, 4096);
-  CAE_CUDA(cudaMallocAsync(&b.p, cap, e->stream));
-  b.cap = cap;
-  return 0;
-}
-
 // resident pods per row of the current CSR; cnt[NT] = 0 closes the scan; every row starts clean (didx = -1)
 __global__ void nd_count_kernel(const int32_t* __restrict__ off, int NT, int32_t* __restrict__ cnt, int32_t* __restrict__ didx) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;

@@ -48,7 +48,7 @@ class PinnedArray:
 
 def shard_pods(P: int, rank: int, world_size: int) -> Tuple[int, int]:
     """Block partition of the pending pods for the dense pass; shard starts are multiples of 32 so the
-    template-major bit rows of the ranks concatenate word by word (must match do_load in csrc/api.cu)."""
+    template-major bit rows of the ranks concatenate word by word (must match pod_shard in csrc/api.cu)."""
     b = (P * rank // world_size) // 32 * 32
     e = P * (rank + 1) // world_size
     if rank + 1 < world_size:

@@ -2,8 +2,8 @@
 than thread blocks, fewer templates than one word, ragged P and T, many template words.  Bit matrix, histogram and
 (with reasons) the first failing plugin must equal the oracle bit for bit, also on a second pass over the same load.
 
-Every instantiation of the pass: A = 0..8 active resource dims (not a prefix of the dims for most A) on the LUT kernel at
-16 and 8 warps and on the bit-sliced kernel, and the boundaries of the rank layout (a second rank word, the largest
+Every instantiation of the pass: A = 0..8 active resource dims (not a prefix of the dims for most A) on the LUT kernel,
+also with several pod words per thread block, and on the bit-sliced kernel, and the boundaries of the rank layout (a second rank word, the largest
 threshold table, the 32-slice limit).  The non-GPU test at the end checks that these inputs really have those layouts."""
 import functools
 
@@ -22,7 +22,12 @@ SHAPES = [
 
 # the shape of the instantiation sweep: ragged P and T, 3 template chunks of 512, G > 1 pod blocks per chunk
 SWEEP_P, SWEEP_T = 3001, 1181
-VARIANTS = {"lut16": {}, "lut8": {"CAE_K1_WARPS": "8"}, "bitslice": {"CAE_K1_BITSLICE": "1"}}
+# one template chunk and more pod words than an H100 holds LUT blocks at once: every block takes several pod words, and the
+# words do not split evenly over the blocks
+MULTIWORD_P, MULTIWORD_T = 20011, 500
+# variant -> (environment, shape)
+VARIANTS = {"lut16": ({}, (SWEEP_P, SWEEP_T)), "lut16_multiword": ({}, (MULTIWORD_P, MULTIWORD_T)),
+            "bitslice": ({"CAE_K1_BITSLICE": "1"}, (SWEEP_P, SWEEP_T))}
 
 # rank-layout boundaries: dim -> distinct request values, and the layout that must result
 _SMALL6 = {0: 3, 1: 2, 2: 3, 4: 2, 5: 3}                            # 18 threshold rows, 10 slices
@@ -36,8 +41,8 @@ BOUNDARIES = {
 
 
 @functools.lru_cache(maxsize=None)
-def _sweep_enc(A):
-    return synth.generate(2, pods=SWEEP_P, templates=SWEEP_T, dims=rank_layout.DIM_SETS[A])
+def _sweep_enc(A, shape=(SWEEP_P, SWEEP_T)):
+    return synth.generate(2, pods=shape[0], templates=shape[1], dims=rank_layout.DIM_SETS[A])
 
 
 @functools.lru_cache(maxsize=None)
@@ -86,14 +91,16 @@ def test_dense_decomposition_edges(oracle, pods, templates, want_reasons):
 @pytest.mark.parametrize("variant", list(VARIANTS))
 @pytest.mark.parametrize("A", range(9))
 def test_dense_every_dim_count(oracle, monkeypatch, A, variant, want_reasons):
-    """feasibility_lut_kernel<A, REASONS, 16 | 8> for A = 0..8, and the bit-sliced kernel at the slice counts these give."""
+    """feasibility_lut_kernel<A, REASONS, 16> for A = 0..8 (at one and at several pod words per block), and the bit-sliced
+    kernel at the slice counts these give."""
     import __graft_entry__ as g
     g.build()
     from kubernetes_autoscaler_b200.engine import Engine
-    for k, v in VARIANTS[variant].items():
+    env, shape = VARIANTS[variant]
+    for k, v in env.items():
         monkeypatch.setenv(k, v)
-    enc = _sweep_enc(A)
-    want = _oracle_dense(oracle, ("sweep", A), enc)
+    enc = _sweep_enc(A, shape)
+    want = _oracle_dense(oracle, ("sweep", A, shape), enc)
     e = Engine(device=0, want_reasons=want_reasons)
     try:
         _check_passes(e, enc, want, want_reasons)
@@ -145,6 +152,9 @@ def test_dense_parametrization_covers_every_cell():
     assert SWEEP_P % 32 and SWEEP_T % 32
     assert -(-Tw // 16) == 3           # template chunks of FEAS_TW = 16 words
     assert -(-Plw // 16) > 1           # even a 16-warp block takes a part of the pod words: G > 1 blocks per chunk
+    Tw_m, Plw_m = -(-MULTIWORD_T // 32), -(-MULTIWORD_P // 32)
+    assert -(-Tw_m // 16) == 1         # one template chunk
+    assert Plw_m > 3 * 132 and all(Plw_m % g for g in (132, 264, 396))   # 132 SMs x 1..3 LUT blocks: >= 2 words for some blocks, uneven
     bitsliced = set()                  # instantiations feasibility_kernel<B> run, B = slices rounded up to 4
     for A in range(9):
         enc = _sweep_enc(A)
@@ -152,6 +162,8 @@ def test_dense_parametrization_covers_every_cell():
         assert (lay["A"], lay["act_dims"], lay["W"], lay["path"]) == (A, rank_layout.DIM_SETS[A], 1 if A else 0, "lut"), lay
         assert rank_layout.layout_of(enc, force_bitslice=True)["path"] == "bitslice"
         bitsliced.add(-(-lay["slices"] // 4) * 4)
+        lay_m = rank_layout.layout_of(_sweep_enc(A, (MULTIWORD_P, MULTIWORD_T)))
+        assert (lay_m["A"], lay_m["act_dims"], lay_m["path"]) == (A, rank_layout.DIM_SETS[A], "lut"), lay_m
     assert sum(s != tuple(range(len(s))) for s in rank_layout.DIM_SETS.values()) >= 6   # mostly non-prefix active sets
     for name, (_, want) in BOUNDARIES.items():
         lay = rank_layout.layout_of(_boundary_enc(name))
