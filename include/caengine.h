@@ -410,6 +410,34 @@ int32_t cae_filter_schedulable(cae_engine* e, const int32_t* pod_order, int32_t 
                                int32_t last_index_in, int32_t break_on_failure, int32_t* assigned_node,
                                int32_t* last_index_out, int32_t* overflowing_controllers);
 
+/* The scale-down removal simulation: RemovalSimulator.SimulateNodeRemoval(candidate, destinationMap) called on every
+ * candidate in order, on ONE RemovalSimulator (one HintingSimulator: hints and lastIndex carried from call to call)
+ * (cluster-autoscaler/simulator/cluster.go:126-217).  Runs on the tables of the last cae_load, whose pending pods are the
+ * to-move copies (nodeName cleared) of the candidates' pods at load time; templates are ignored (T = 0 is fine).
+ * Per candidate, in order: the node leaves the snapshot (topology domains, inter-pod counts, lastIndex positions);
+ * its pods are tried with breakOnFailure on the acceptable destinations (dest_ok, never the candidate or a removed
+ * node), SimilarPodsScheduling restarting per candidate; with `persist` a success commits (the node is gone, its pods
+ * stay on their destinations and are appended to those nodes' pods, so they move again if that node is a later
+ * candidate), anything else is undone.  Hints set by placed pods and lastIndex survive every simulation.
+ *   n_cand, cand_node [n_cand]  cluster row of each candidate, -1 = a name the caller could not find (duplicates allowed)
+ *   move_off [n_cand + 1], move_pod []  pending pods the candidate held at load time, in the order they are tried (the
+ *                               same pod may not be listed under two different rows)
+ *   dest_ok [N]                 destinationMap, NULL = every node
+ *   hint_node [num_pending]     hinted cluster row, -1 = none; NULL = no hints
+ *   sim_class, class_ctrl, n_classes  SimilarPodsScheduling classes as for cae_filter_schedulable
+ *   last_index_in               SchedulerPluginRunner.lastIndex before the first candidate (may be raw)
+ * Outputs: result [n_cand] (cae_removal_result); last_index_out; log [log_cap][3] = (candidate, pending pod, cluster row or
+ * -1), one entry per pod tried, in processing order (moved-in pods included), from which the caller rebuilds
+ * pods_to_reschedule, the hints and the persisted cluster; log_len = entries written.  If the log needs more than
+ * log_cap entries the call still runs every simulation, sets log_len to the size needed and returns 1 with no other output
+ * defined: call again with that capacity.  Malformed input returns -2 before anything runs. */
+enum cae_removal_result { CAE_REMOVAL_REMOVABLE = 0, CAE_REMOVAL_NO_PLACE = 1, CAE_REMOVAL_NO_NODE_INFO = 2 };
+int32_t cae_simulate_removals(cae_engine* e, int32_t n_cand, const int32_t* cand_node, const int32_t* move_off,
+                              const int32_t* move_pod, const uint8_t* dest_ok, const int32_t* hint_node,
+                              const int32_t* sim_class, const int32_t* class_ctrl, int32_t n_classes, int32_t last_index_in,
+                              int32_t persist, int32_t* result, int32_t* last_index_out, int32_t* log, int32_t log_cap,
+                              int32_t* log_len);
+
 /* The two halves of cae_expander_best for templates sharded over ranks (no [T][E] matrix ever leaves a GPU):
  * cae_waste_scores returns the least-waste score (expander/waste/waste.go:44-72) of this rank's template shard from
  * the device-resident result of the last cae_estimate_all, 0.0 for the rows of other ranks, so that a SUM all-reduce of

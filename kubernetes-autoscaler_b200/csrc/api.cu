@@ -1251,6 +1251,114 @@ int32_t cae_filter_schedulable(cae_engine* h, const int32_t* pod_order, int32_t 
   return 0;
 }
 
+int32_t cae_simulate_removals(cae_engine* h, int32_t n_cand, const int32_t* cand_node, const int32_t* move_off,
+                              const int32_t* move_pod, const uint8_t* dest_ok, const int32_t* hint_node,
+                              const int32_t* sim_class, const int32_t* class_ctrl, int32_t n_classes, int32_t last_index_in,
+                              int32_t persist, int32_t* result, int32_t* last_index_out, int32_t* log, int32_t log_cap,
+                              int32_t* log_len) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_simulate_removals before cae_load"); return -2; }
+  if (n_cand < 0 || (n_cand > 0 && (!cand_node || !move_off || !result)) || !last_index_out || !log_len || log_cap < 0 ||
+      (log_cap > 0 && !log) || (sim_class && n_classes > 0 && !class_ctrl)) {
+    cae::set_error("cae_simulate_removals: bad arguments");
+    return -2;
+  }
+  const int P = e->P, N = e->N;
+  if (!sim_class) n_classes = 0;
+  // everything is checked before the first device write
+  const int M = n_cand > 0 ? move_off[n_cand] : 0;
+  if (n_cand > 0 && move_off[0] != 0) { cae::set_error("cae_simulate_removals: move_off[0] must be 0"); return -2; }
+  for (int c = 0; c < n_cand; ++c) {
+    if (cand_node[c] < -1 || cand_node[c] >= N) { cae::set_error("cae_simulate_removals: candidate row out of range"); return -2; }
+    if (move_off[c + 1] < move_off[c]) { cae::set_error("cae_simulate_removals: move_off decreases"); return -2; }
+  }
+  if (M > 0 && !move_pod) { cae::set_error("cae_simulate_removals: bad arguments"); return -2; }
+  {
+    // a pending pod sits on one node: listed under one row only, once per candidate
+    std::vector<int32_t>& owner = e->rm_owner;
+    std::vector<int32_t>& seen = e->rm_seen;
+    owner.assign(std::max(P, 1), INT_MIN);
+    seen.assign(std::max(P, 1), -1);
+    for (int c = 0; c < n_cand; ++c)
+      for (int k = move_off[c]; k < move_off[c + 1]; ++k) {
+        const int pod = move_pod[k];
+        if (pod < 0 || pod >= P) { cae::set_error("cae_simulate_removals: pod index out of range"); return -2; }
+        if (seen[pod] == c || (owner[pod] != INT_MIN && owner[pod] != cand_node[c])) {
+          cae::set_error("cae_simulate_removals: a pod is listed twice or under two nodes");
+          return -2;
+        }
+        seen[pod] = c; owner[pod] = cand_node[c];
+      }
+  }
+  if (hint_node)
+    for (int i = 0; i < P; ++i)
+      if (hint_node[i] < -1 || hint_node[i] >= N) { cae::set_error("cae_simulate_removals: hinted row out of range"); return -2; }
+  int nctrl = 0;
+  for (int c = 0; c < n_classes; ++c) {
+    if (class_ctrl[c] < 0) { cae::set_error("cae_simulate_removals: negative controller id"); return -2; }
+    nctrl = std::max(nctrl, class_ctrl[c] + 1);
+  }
+  if (sim_class)
+    for (int i = 0; i < P; ++i)
+      if (sim_class[i] < -1 || sim_class[i] >= n_classes) { cae::set_error("cae_simulate_removals: similarity class out of range"); return -2; }
+  if (n_cand == 0) { *last_index_out = last_index_in; *log_len = 0; return 0; }
+  cudaSetDevice(e->cfg.device);
+  // one blob: cand | move_off | move_pod | hint | class | class_ctrl | dest_ok (bytes), then result | out[2] | log
+  auto words = [](size_t bytes) { return (bytes + 3) / 4; };
+  size_t off = 0;
+  const size_t o_cand = off; off += n_cand;
+  const size_t o_moff = off; off += n_cand + 1;
+  const size_t o_mpod = off; off += std::max(M, 1);
+  const size_t o_hint = off; off += hint_node ? P : 0;
+  const size_t o_cls = off; off += sim_class ? P : 0;
+  const size_t o_cc = off; off += std::max(n_classes, 1);
+  const size_t o_dest = off; off += dest_ok ? words(N) : 0;
+  const size_t o_in_end = off;
+  const size_t o_res = off; off += n_cand;
+  const size_t o_out = off; off += 2;
+  const size_t o_log = off; off += (size_t)std::max(log_cap, 1) * 3;
+  if (cae::devbuf_reserve(e, e->fm_blob, off * 4)) return -1;
+  if (cae::pinned_reserve(e, e->rm_stage, o_in_end * 4)) return -1;
+  int32_t* blob = static_cast<int32_t*>(e->fm_blob.p);
+  int32_t* hb = static_cast<int32_t*>(e->rm_stage.p);
+  std::copy(cand_node, cand_node + n_cand, hb + o_cand);
+  std::copy(move_off, move_off + n_cand + 1, hb + o_moff);
+  if (M) std::copy(move_pod, move_pod + M, hb + o_mpod);
+  if (hint_node) std::copy(hint_node, hint_node + P, hb + o_hint);
+  if (sim_class) std::copy(sim_class, sim_class + P, hb + o_cls);
+  if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, hb + o_cc);
+  if (dest_ok && N) memcpy(hb + o_dest, dest_ok, N);
+  CAE_CUDA(cudaMemcpyAsync(blob, hb, o_in_end * 4, cudaMemcpyHostToDevice, e->stream));
+  CAE_CUDA(cudaEventRecord(e->rm_stage.ev, e->stream));
+  cae::RemovalLaunch r{};
+  r.ncand = n_cand; r.persist = persist ? 1 : 0; r.ncls = n_classes; r.nctrl = nctrl; r.log_cap = log_cap;
+  r.last_index = last_index_in; r.n_move = M;
+  r.cand = blob + o_cand; r.move_off = blob + o_moff; r.move_pod = blob + o_mpod;
+  r.hint = hint_node ? blob + o_hint : nullptr;
+  r.cls = sim_class ? blob + o_cls : nullptr;
+  r.class_ctrl = blob + o_cc;
+  r.dest_ok = dest_ok ? reinterpret_cast<const uint8_t*>(blob + o_dest) : nullptr;
+  r.result = blob + o_res; r.out = blob + o_out; r.log = blob + o_log;
+  cudaEventRecord(e->ev0, e->stream);
+  if (cae::launch_removals(e, r)) return -1;
+  cudaEventRecord(e->ev1, e->stream);
+  int32_t out[2] = {0, 0}, status = 0;
+  CAE_CUDA(cudaMemcpyAsync(out, blob + o_out, sizeof(out), cudaMemcpyDeviceToHost, e->stream));
+  CAE_CUDA(cudaMemcpyAsync(&status, e->d_work_counter + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
+  e->stats.estimate_ms = ms;
+  if (status) { cae::set_error("placement log overflow in the removal batch"); return -1; }
+  *log_len = out[1];
+  if (out[1] > log_cap) { cae::set_error("cae_simulate_removals: the log needs more entries than log_cap"); return 1; }
+  CAE_CUDA(cudaMemcpyAsync(result, blob + o_res, sizeof(int32_t) * n_cand, cudaMemcpyDeviceToHost, e->stream));
+  if (out[1]) CAE_CUDA(cudaMemcpyAsync(log, blob + o_log, sizeof(int32_t) * 3 * (size_t)out[1], cudaMemcpyDeviceToHost, e->stream));
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
+  *last_index_out = out[0];
+  return 0;
+}
+
 void* cae_stream(cae_engine* h) {
   Engine* e = reinterpret_cast<Engine*>(h);
   return e ? reinterpret_cast<void*>(e->stream) : nullptr;

@@ -67,6 +67,8 @@ struct BpParams {
   uint8_t *fm_class_mark, *fm_ctrl_over;  // [classes] known unschedulable, [controllers] overflowing (zeroed)
   unsigned char* scratch;
   size_t scratch_per_cta;
+  // scale-down batch (RM, cae_simulate_removals): work item t is candidate t; the fm_* buffers above are refilled per candidate
+  RemovalState rm;
 };
 
 constexpr int BP_HIST = 256;   // capacities up to this use the histogram; above, a binary search
@@ -89,6 +91,7 @@ struct BpShared {
   int ri[2][32][3];
   int hist[BP_HIST + 1];      // #nodes per capacity value (closed-form lap count)
   int t, L, rem, pre_s, log_n, overflow, newly, need_log, mlast, lastnode;
+  int rm_mode, rm_len, rm_runs, rm_li, rm_nlive, rm_li_raw, rm_log_n;   // RM: see rm_begin / rm_end in binpack_kernel
   long long dead[4][CAE_MAX_RES];   // requests (no host ports) whose sweep found no room since the node state last changed
 };
 
@@ -213,7 +216,11 @@ __device__ __forceinline__ int bp_div_f(int64_t f, int64_t r, float rinv, int kb
 // pods arrive as runs of consecutive identical pods in the caller's order.  Plain runs are dealt in closed form (lap by lap,
 // because every pod's node is reported), hinted pods and pods under topology counters one by one, with the
 // SimilarPodsScheduling shortcut (similar_pods.go:59-104).
-template <int A, int TPB, bool WIN, bool FM>
+// RM = true (implies FM): RemovalSimulator.SimulateNodeRemoval called on every candidate in order (simulator/cluster.go:
+// 126-217), one work item per candidate on the same block.  rm_begin takes the candidate out of a working copy of the
+// snapshot (live mask, counter tables), builds its pod list and runs; the FM body simulates; rm_end records the outcome
+// and, for a persisted success, makes the working copy the committed one.
+template <int A, int TPB, bool WIN, bool FM, bool RM = false>
 __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack_kernel(DevObjects o, DynTables d, BpParams p) {
   constexpr int NW = TPB / 32;
   constexpr int A1 = A > 0 ? A : 1;
@@ -277,7 +284,8 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
     __syncthreads();
     if (tid == 0) {
       const int i = atomicAdd(p.work_counter, 1);
-      if (FM) S.t = i == 0 ? 0 : p.t_end;
+      if (RM) S.t = min(i, p.t_end);
+      else if (FM) S.t = i == 0 ? 0 : p.t_end;
       else S.t = i >= p.t_end - p.t_begin ? p.t_end : (p.perm ? p.perm[i] : p.t_begin + i);
       S.log_n = 0; S.overflow = 0;
     }
@@ -285,6 +293,146 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
     const int t = S.t;
     if (t >= p.t_end) break;
     const long long prof_tmpl0 = (p.prof && tid == 0) ? clock64() : 0;
+    if constexpr (RM) {
+      // ---- rm_begin: candidate t leaves a working copy of the committed snapshot (cluster.go:184-217) ----
+      const RemovalState& r = p.rm;
+      const int NTd = N + p.T;
+      if (t == 0) {   // the committed snapshot starts as the load's
+        for (int x = tid; x < N; x += TPB) {
+#pragma unroll
+          for (int a = 0; a < A; ++a) r.cfree[(size_t)a * N + x] = p.c_free[(size_t)a * N + x];
+          r.cslots[x] = p.c_slots[x]; r.cports[x] = 0ull; r.live[x] = 1; r.head[x] = -1; r.tail[x] = -1;
+        }
+        for (int i = tid; i < d.pool; i += TPB) { r.ccnt[i] = d.base_cnt[i]; r.cpres[i] = d.base_pres[i]; }
+        for (int q = tid; q < d.Q; q += TPB) r.ctot[q] = d.base_tot[q];
+        if (tid == 0) { S.rm_li_raw = r.li_in; S.rm_log_n = 0; }
+        __syncthreads();
+      }
+      const int cand = r.cand[t];
+      const bool exists = cand >= 0 && r.live[cand];
+      if (!exists) {
+        if (tid == 0) { S.rm_mode = 0; S.rm_runs = 0; S.rm_len = 0; S.rm_li = 0; }
+      } else {
+        // working copy: counters, live mask, destinations (the candidate, removed nodes and nodes outside the map are none)
+        for (int i = tid; i < d.pool; i += TPB) { r.wcnt[i] = r.ccnt[i]; r.wpres[i] = r.cpres[i]; }
+        for (int q = tid; q < d.Q; q += TPB) r.wtot[q] = r.ctot[q];
+        for (int x = tid; x < N; x += TPB) {
+          const uint8_t lw = r.live[x] && x != cand;
+          r.live_w[x] = lw;
+          const_cast<uint8_t*>(p.fm_node_ok)[x] = lw && (!r.dest_ok || r.dest_ok[x]);
+        }
+        __syncthreads();
+        // the candidate's resident pods and the pods earlier persisted simulations moved onto it stop counting, and its
+        // domains lose one eligible node (dyn_base_kernel's sums without this row)
+        for (int q = tid; q < d.Q; q += TPB) {
+          if (!d.elig[(size_t)q * p.U + cand]) continue;
+          const int dm = d.dom[(size_t)d.q_k[q] * NTd + cand];
+          if (dm < 0) continue;
+          int w = 0;
+          for (int i = o.node_pod_off[cand]; i < o.node_pod_off[cand + 1]; ++i) w += d.wmat[(size_t)q * d.S + o.node_pod_spec[i]];
+          for (int pod = r.head[cand]; pod >= 0; pod = r.next[pod]) w += d.wmat[(size_t)q * d.S + o.pend_spec[pod]];
+          const int off = d.q_base_off[q];
+          r.wcnt[off + dm] -= w; r.wtot[q] -= w; r.wpres[off + dm] -= 1;
+        }
+        // the pods to move: the load-time list, then the moved-in pods in arrival order
+        const int mb = r.move_off[t], L0 = r.move_off[t + 1] - mb;
+        int32_t* list = const_cast<int32_t*>(p.fm_pods);
+        for (int i = tid; i < L0; i += TPB) list[i] = r.move_pod[mb + i];
+        if (tid == 0) {
+          int L = L0;
+          for (int pod = r.head[cand]; pod >= 0; pod = r.next[pod]) list[L++] = pod;
+          S.rm_len = L;
+        }
+        __syncthreads();
+        // statistics of every counter over the reduced node set (dyn_stats_kernel on the working copy): one warp per counter
+        for (int q = warp; q < d.Q; q += NW) {
+          const int off = d.q_base_off[q], len = d.q_base_off[q + 1] - off;
+          int m1 = INT_MAX, nd = 0;
+          for (int i = lane; i < len; i += 32) if (r.wpres[off + i] > 0) { ++nd; m1 = min(m1, r.wcnt[off + i]); }
+          m1 = bp_wmin(m1); nd = bp_wsum(nd);
+          int nm = 0;
+          for (int i = lane; i < len; i += 32) nm += r.wpres[off + i] > 0 && r.wcnt[off + i] == m1;
+          nm = bp_wsum(nm);
+          if (lane == 0) { r.stat[q * 3] = m1; r.stat[q * 3 + 1] = nm; r.stat[q * 3 + 2] = nd; }
+        }
+        // rank of every row among the live nodes (one block prefix per candidate)
+        int basecnt = 0;
+        for (int base = 0; base < N; base += TPB) {
+          const int x = base + tid;
+          const bool lv = x < N && r.live_w[x];
+          const unsigned mm = __ballot_sync(0xffffffffu, lv);
+          if (lane == 0) S.ri[par][warp][0] = __popc(mm);
+          __syncthreads();
+          const int v = lane < NW ? S.ri[par][lane][0] : 0;
+          int inc = v;
+#pragma unroll
+          for (int off = 1; off < 32; off <<= 1) {
+            const int u = __shfl_up_sync(0xffffffffu, inc, off);
+            if (lane >= off) inc += u;
+          }
+          const int wpre = __shfl_sync(0xffffffffu, inc - v, warp);
+          if (x < N) r.rank[x] = basecnt + wpre + __popc(mm & ((1u << lane) - 1));
+          basecnt += __shfl_sync(0xffffffffu, inc, 31);
+          par ^= 1;
+        }
+        const int nlive = basecnt, L = S.rm_len;
+        // lastIndex arrives as a position among the live nodes (raw: modulo their number, plugin_runner.go:81): to a row
+        const int li_rank = nlive > 0 ? (int)((((long long)S.rm_li_raw % nlive) + nlive) % nlive) : 0;
+        for (int x = tid; x < N; x += TPB) if (r.live_w[x] && r.rank[x] == li_rank) S.rm_li = x;
+        if (tid == 0) { S.rm_nlive = nlive; if (nlive == 0) S.rm_li = 0; }
+        // per-call state: assignments, SimilarPodsScheduling; a hint to a node outside the simulation's snapshot is none
+        for (int i = tid; i < L; i += TPB) {
+          const int pod = list[i], h = r.hint[pod];
+          p.fm_assigned[pod] = -1;
+          const_cast<int32_t*>(p.fm_hint)[pod] = h >= 0 && r.live_w[h] ? h : -1;
+        }
+        for (int c = tid; c < r.ncls; c += TPB) p.fm_class_mark[c] = 0;
+        for (int c = tid; c < r.nctrl; c += TPB) { p.fm_ctrl_cnt[c] = 0; p.fm_ctrl_over[c] = 0; }
+        __syncthreads();
+        // runs of consecutive identical pods (cae_filter_schedulable's rule), compacted with a block prefix
+        int nruns = 0;
+        for (int base = 0; base < L; base += TPB) {
+          const int i = base + tid;
+          bool st = false;
+          if (i < L) {
+            const int pod = list[i];
+            st = i == 0;
+            if (!st) {
+              const int prev = list[i - 1];
+              st = o.pend_spec[pod] != o.pend_spec[prev] || p.fm_hint[pod] >= 0 || p.fm_hint[prev] >= 0 ||
+                   (p.fm_class && p.fm_class[pod] != p.fm_class[prev]);
+            }
+          }
+          const unsigned mm = __ballot_sync(0xffffffffu, st);
+          if (lane == 0) S.ri[par][warp][0] = __popc(mm);
+          __syncthreads();
+          const int v = lane < NW ? S.ri[par][lane][0] : 0;
+          int inc = v;
+#pragma unroll
+          for (int off = 1; off < 32; off <<= 1) {
+            const int u = __shfl_up_sync(0xffffffffu, inc, off);
+            if (lane >= off) inc += u;
+          }
+          const int wpre = __shfl_sync(0xffffffffu, inc - v, warp);
+          if (st) r.run_off[nruns + wpre + __popc(mm & ((1u << lane) - 1))] = i;
+          nruns += __shfl_sync(0xffffffffu, inc, 31);
+          par ^= 1;
+        }
+        if (tid == 0) { r.run_off[nruns] = L; S.rm_runs = nruns; S.rm_mode = L > 0 ? 1 : 2; }
+        __syncthreads();
+        GroupRec* recs = const_cast<GroupRec*>(p.grec);
+        for (int k = tid; k < nruns; k += TPB) {
+          const int pb = r.run_off[k], spec = o.pend_spec[list[pb]];
+          bool feeds = false;
+          if (p.has_dyn) for (int q = 0; q < d.Q && !feeds; ++q) feeds = d.wmat[(size_t)q * d.S + spec] != 0;
+          GroupRec g = build_group_rec(o, r.grs, spec, r.run_off[k + 1] - pb, feeds);
+          g.pad[0] = pb;
+          recs[k] = g;
+        }
+        __threadfence_block();
+      }
+      __syncthreads();
+    }
 
     int64_t tfree[A1];
 #pragma unroll
@@ -294,16 +442,24 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
     const int col_new = N + p.T + t;  // universe column of the sanitized template
     // lastIndex may come in RAW (left by a longer node list): plugin_runner.go:81 uses it modulo the CURRENT list length
     // until a scan places a pod (:123), so every scan start below is taken through li_eff()
-    int n_new = 0, nodes_with_pods = 0, pods_total = 0, last_index = FM ? p.fm_last_index : (p.last_index_in ? p.last_index_in[t] : 0);
+    int n_new = 0, nodes_with_pods = 0, pods_total = 0,
+        last_index = RM ? S.rm_li : FM ? p.fm_last_index : (p.last_index_in ? p.last_index_in[t] : 0);
     auto li_eff = [&]() -> int { const int len = N + n_new; return len > 0 ? last_index % len : 0; };
     bool new_nodes_available = !FM, cl_init = false, fm_stop = false, fm_moved = false;
     auto ensure_cluster = [&]() {  // run state of the cluster nodes, needed once a placement can reach them
       if (cl_init) return;
       for (int x = tid; x < N; x += TPB) {
+        if constexpr (RM) {   // the committed snapshot: node state is restored from it for every candidate
 #pragma unroll
-        for (int a = 0; a < A; ++a) g_free[(size_t)a * Xg + x] = p.c_free[(size_t)a * N + x];
-        g_slots[x] = p.c_slots[x];
-        g_ports[x] = 0ull;
+          for (int a = 0; a < A; ++a) g_free[(size_t)a * Xg + x] = p.rm.cfree[(size_t)a * N + x];
+          g_slots[x] = p.rm.cslots[x];
+          g_ports[x] = p.rm.cports[x];
+        } else {
+#pragma unroll
+          for (int a = 0; a < A; ++a) g_free[(size_t)a * Xg + x] = p.c_free[(size_t)a * N + x];
+          g_slots[x] = p.c_slots[x];
+          g_ports[x] = 0ull;
+        }
         g_sched[x] = 0;
       }
       cl_init = true;
@@ -344,7 +500,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
       for (int a = 0; a < A; ++a) maxfree[a] = bp_wmax_ll(lane < NW ? S.rb[par][lane][a] : LLONG_MIN);
       par ^= 1;
     };
-    const int n_groups = FM ? p.fm_runs : p.order_n[t];
+    const int n_groups = RM ? S.rm_runs : FM ? p.fm_runs : p.order_n[t];
 
     auto log_append = [&](int x, int spec, int cnt) {  // any thread
       const int idx = atomicAdd(&S.log_n, 1);
@@ -837,6 +993,10 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
               wd.wown[i] = r.wown; wd.self[i] = r.self; wd.maxskew[i] = r.maxskew; wd.mindom[i] = r.mindom;
               wd.elig_new[i] = en; wd.dsw[i] = dsw; wd.tot[i] = r.base_tot; wd.boff[i] = r.boff;
               wd.minv[i] = r.st_min1; wd.nmin[i] = r.st_nmin; wd.ndom[i] = r.st_ndom;
+              if constexpr (RM) {   // the counters of the candidate's simulation, not the load's
+                wd.tot[i] = p.rm.wtot[q];
+                wd.minv[i] = p.rm.stat[q * 3]; wd.nmin[i] = p.rm.stat[q * 3 + 1]; wd.ndom[i] = p.rm.stat[q * 3 + 2];
+              }
               wd.nfeed[i] = r.nfeed;
               S.flag[i] = 0;
             }
@@ -856,13 +1016,15 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
         // Working counters are copy-on-write over the cluster base counts: a slot is valid only when its
         // version equals this group's, otherwise it reads as its default (base count for cluster domains,
         // DaemonSet weight for the fresh hostname domain of an added node, 0 for a template-only value).
+        const int32_t* base_cnt = RM ? p.rm.wcnt : d.base_cnt;
+        const int32_t* base_pres = RM ? p.rm.wpres : d.base_pres;
         auto def_cnt = [&](int q, int sl) -> int {
           const int Dc = wd.Dc[q];
-          return sl < Dc ? d.base_cnt[wd.boff[q] + sl] : (sl == Dc ? 0 : (wd.elig_new[q] ? wd.dsw[q] : 0));
+          return sl < Dc ? base_cnt[wd.boff[q] + sl] : (sl == Dc ? 0 : (wd.elig_new[q] ? wd.dsw[q] : 0));
         };
         auto def_pres = [&](int q, int sl) -> int {
           const int Dc = wd.Dc[q];
-          return sl < Dc ? d.base_pres[wd.boff[q] + sl] : (sl == Dc ? 0 : (wd.elig_new[q] ? 1 : 0));
+          return sl < Dc ? base_pres[wd.boff[q] + sl] : (sl == Dc ? 0 : (wd.elig_new[q] ? 1 : 0));
         };
         auto rd_cnt = [&](int q, int sl) -> int {
           const size_t o2 = (size_t)q * p.dstride + sl;
@@ -1072,7 +1234,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
               h_caps(x, cp, ci);
               const int k_other = min(rc, ci);
               g_kc[x] = min(k_other, cp);
-              if (k_other == 0 && hp >= 0) {
+              if (k_other == 0 && hp >= 0 && (!RM || p.rm.live_w[x])) {   // a removed node is no domain's eligible node
                 const int sl = slot_of(hp, x);
                 if (sl >= 0 && elig_of(hp, x) && rd_cnt(hp, sl) == 0 && rd_pres(hp, sl) == 1) blocked = 1;
               }
@@ -1423,7 +1585,61 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
       ord_next = ord_next2;
     }
     if (p.prof && tid == 0) atomicAdd((unsigned long long*)&p.prof[7], (unsigned long long)(clock64() - prof_tmpl0));
-    if constexpr (FM) {
+    if constexpr (RM) {
+      // ---- rm_end: outcome, log, hints, lastIndex; a persisted success commits the working copy ----
+      const RemovalState& r = p.rm;
+      const int mode = S.rm_mode, L = S.rm_len, base = S.rm_log_n;
+      const int cand = r.cand[t];
+      const bool ok = pods_total == L;      // breakOnFailure: every pod placed, or the simulation stopped
+      for (int i = tid; i < L; i += TPB) {  // one log entry per pod tried; hints set by placed pods survive in every case
+        const int pod = p.fm_pods[i], x = p.fm_assigned[pod];
+        if (base + i < r.log_cap) { r.log[(size_t)(base + i) * 3] = t; r.log[(size_t)(base + i) * 3 + 1] = pod; r.log[(size_t)(base + i) * 3 + 2] = x; }
+        if (x >= 0) r.hint[pod] = x;
+      }
+      if (mode != 0 && ok && r.persist) {
+        // Commit.  Undo needs no log: every candidate starts from a full copy of the committed state (rm_begin copies the
+        // counters, ensure_cluster the node state), so a simulation that is not committed leaves nothing behind, and one that
+        // is committed is copied back whole — the committed state is always exactly what the loop of single calls leaves.
+        for (int x = tid; x < N; x += TPB) {
+#pragma unroll
+          for (int a = 0; a < A; ++a) r.cfree[(size_t)a * N + x] = g_free[(size_t)a * Xg + x];
+          r.cslots[x] = g_slots[x];
+          r.cports[x] = g_ports[x];
+        }
+        // the moved pods count on their destinations from now on (the placements the FM body logged into its own copies)
+        for (int k = tid; k < L * d.Q; k += TPB) {
+          const int i = k / d.Q, q = k - i * d.Q;
+          const int pod = p.fm_pods[i], x = p.fm_assigned[pod];
+          const int w = d.wmat[(size_t)q * d.S + o.pend_spec[pod]];
+          if (w == 0 || !d.elig[(size_t)q * p.U + x]) continue;
+          const int dm = d.dom[(size_t)d.q_k[q] * (N + p.T) + x];
+          if (dm < 0) continue;
+          atomicAdd(&r.wcnt[d.q_base_off[q] + dm], w);
+          atomicAdd(&r.wtot[q], w);
+        }
+        __syncthreads();
+        for (int i = tid; i < d.pool; i += TPB) { r.ccnt[i] = r.wcnt[i]; r.cpres[i] = r.wpres[i]; }
+        for (int q = tid; q < d.Q; q += TPB) r.ctot[q] = r.wtot[q];
+        if (tid == 0) {
+          r.live[cand] = 0;
+          for (int i = 0; i < L; ++i) {   // NodeInfo order: appended to their destination in processing order
+            const int pod = p.fm_pods[i], x = p.fm_assigned[pod];
+            r.next[pod] = -1;
+            if (r.tail[x] < 0) r.head[x] = pod; else r.next[r.tail[x]] = pod;
+            r.tail[x] = pod;
+          }
+        }
+      }
+      if (tid == 0) {
+        r.result[t] = mode == 0 ? CAE_REMOVAL_NO_NODE_INFO : ok ? CAE_REMOVAL_REMOVABLE : CAE_REMOVAL_NO_PLACE;
+        // lastIndex leaves as a position among the live nodes; it stays raw when no scan placed a pod (plugin_runner.go:123)
+        if (fm_moved && S.rm_nlive > 0) S.rm_li_raw = r.rank[last_index] % S.rm_nlive;
+        S.rm_log_n = base + L;
+        r.out[0] = S.rm_li_raw; r.out[1] = S.rm_log_n;
+        if (S.overflow && p.status) atomicExch(p.status, 1);
+      }
+      __syncthreads();
+    } else if constexpr (FM) {
       int over = 0, zero = 0;
       for (int c = tid; c < p.fm_nctrl; c += TPB) over += p.fm_ctrl_over[c] != 0;
       blk_sum_max<NW>(S, par, over, zero);
@@ -1447,14 +1663,19 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
 #ifndef BP_PART
 #define BP_PART 0
 #endif
-int bp_launch_part0(Engine* e, int A, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, bool filter);
-int bp_launch_part1(Engine* e, int A, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, bool filter);
-int bp_launch_part2(Engine* e, int A, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, bool filter);
+// filter: 0 = estimator, 1 = filter-out-schedulable pass, 2 = scale-down batch
+int bp_launch_part0(Engine* e, int A, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, int filter);
+int bp_launch_part1(Engine* e, int A, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, int filter);
+int bp_launch_part2(Engine* e, int A, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, int filter);
 
 template <int A>
-static int bp_launch_a(Engine* e, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, bool filter) {
-  if (filter) {
+static int bp_launch_a(Engine* e, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, int filter) {
+  if (filter == 1) {
     binpack_kernel<A, 512, false, true><<<1, 512, 0, e->stream>>>(e->dobj, e->dyn, p);
+    return 0;
+  }
+  if (filter == 2) {
+    binpack_kernel<A, 512, false, true, true><<<1, 512, 0, e->stream>>>(e->dobj, e->dyn, p);
     return 0;
   }
   auto kern = p.win ? binpack_kernel<A, 256, true, false> : binpack_kernel<A, 256, false, false>;
@@ -1469,15 +1690,15 @@ static int bp_launch_a(Engine* e, int blocks_wanted, size_t smem, const BpParams
   return 0;
 }
 #if BP_PART == 0
-int bp_launch_part0(Engine* e, int A, int bw, size_t smem, const BpParams& p, int* bo, bool q, bool f) {
+int bp_launch_part0(Engine* e, int A, int bw, size_t smem, const BpParams& p, int* bo, bool q, int f) {
   return A == 0 ? bp_launch_a<0>(e, bw, smem, p, bo, q, f) : A == 1 ? bp_launch_a<1>(e, bw, smem, p, bo, q, f) : bp_launch_a<2>(e, bw, smem, p, bo, q, f);
 }
 #elif BP_PART == 1
-int bp_launch_part1(Engine* e, int A, int bw, size_t smem, const BpParams& p, int* bo, bool q, bool f) {
+int bp_launch_part1(Engine* e, int A, int bw, size_t smem, const BpParams& p, int* bo, bool q, int f) {
   return A == 3 ? bp_launch_a<3>(e, bw, smem, p, bo, q, f) : A == 4 ? bp_launch_a<4>(e, bw, smem, p, bo, q, f) : bp_launch_a<5>(e, bw, smem, p, bo, q, f);
 }
 #else
-int bp_launch_part2(Engine* e, int A, int bw, size_t smem, const BpParams& p, int* bo, bool q, bool f) {
+int bp_launch_part2(Engine* e, int A, int bw, size_t smem, const BpParams& p, int* bo, bool q, int f) {
   return A == 6 ? bp_launch_a<6>(e, bw, smem, p, bo, q, f) : A == 7 ? bp_launch_a<7>(e, bw, smem, p, bo, q, f) : bp_launch_a<8>(e, bw, smem, p, bo, q, f);
 }
 #endif
@@ -1524,7 +1745,7 @@ static int slab_reserve(Engine* e, Engine::Slab& s, BpParams& p, int A1, size_t 
   return 0;
 }
 
-static int launch_binpack_any(Engine* e, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, bool filter = false) {
+static int launch_binpack_any(Engine* e, int blocks_wanted, size_t smem, const BpParams& p, int* blocks_out, bool query_only, int filter = 0) {
   const int A = std::min(e->A, 8);
   if (A <= 2) return bp_launch_part0(e, A, blocks_wanted, smem, p, blocks_out, query_only, filter);
   if (A <= 5) return bp_launch_part1(e, A, blocks_wanted, smem, p, blocks_out, query_only, filter);
@@ -1638,8 +1859,69 @@ int launch_filter(Engine* e, const FilterLaunch& f) {
   p.grec = d_rec;
   CAE_CUDA(cudaMemsetAsync(e->d_work_counter, 0, sizeof(int32_t) * 2, e->stream));
   run_rec_kernel<<<(f.runs + 127) / 128, 128, 0, e->stream>>>(e->dobj, e->dyn, f.runs, f.run_off, f.pods, group_rec_src(e), d_rec);
-  { int unused = 0; if (launch_binpack_any(e, 1, 0, p, &unused, false, true)) return -1; }
+  { int unused = 0; if (launch_binpack_any(e, 1, 0, p, &unused, false, 1)) return -1; }
   e->stats.kernel_launches += 2;
+  CAE_KERNEL_OK();
+  return 0;
+}
+
+// RemovalSimulator.SimulateNodeRemoval over every candidate in order (one thread block, one launch).  `rl` = device views of
+// the inputs and outputs laid out by cae_simulate_removals (api.cu); the batch state goes to the engine-owned e->rm_state.
+int launch_removals(Engine* e, const RemovalLaunch& rl) {
+  BpParams p{};
+  p.E = e->E; p.T = e->T; p.N = e->N; p.U = e->U;
+  p.has_dyn = e->has_dynamic ? 1 : 0;
+  for (int a = 0; a < CAE_MAX_RES; ++a) p.act_dim[a] = e->act_dim[a];
+  p.pre_code = e->d_pre_code; p.spec_sc = e->d_spec_sc; p.spec_dc = e->d_spec_dc;
+  p.pc_of = e->d_pc_of; p.port_conf = e->d_port_conf; p.c_free = e->d_c_free; p.c_slots = e->d_c_slots;
+  p.work_counter = e->d_work_counter; p.status = e->d_work_counter + 1;
+  p.t_begin = 0; p.t_end = rl.ncand; p.cap = 0; p.win = 0;
+  p.fm_break = 1; p.fm_nctrl = rl.nctrl; p.fm_class = rl.cls; p.fm_class_ctrl = rl.class_ctrl;
+  const int N = e->N, P = std::max(e->P, 1), Q = e->dyn.Q, pool = std::max(e->dyn.pool, 1);
+  const int A1 = std::max(e->A, 1);
+  // batch state, one buffer: sub-arrays 256-byte aligned
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_cfree = take((size_t)8 * A1 * N), o_cslots = take(4 * (size_t)N), o_cports = take(8 * (size_t)N);
+  const size_t o_live = take(N), o_livew = take(N), o_ok = take(N), o_rank = take(4 * (size_t)N);
+  const size_t o_ccnt = take(4 * (size_t)pool), o_cpres = take(4 * (size_t)pool), o_wcnt = take(4 * (size_t)pool), o_wpres = take(4 * (size_t)pool);
+  const size_t o_ctot = take(4 * (size_t)std::max(Q, 1)), o_wtot = take(4 * (size_t)std::max(Q, 1)), o_stat = take(12 * (size_t)std::max(Q, 1));
+  const size_t o_hint = take(4 * (size_t)P), o_hinte = take(4 * (size_t)P), o_asg = take(4 * (size_t)P), o_list = take(4 * (size_t)P);
+  const size_t o_head = take(4 * (size_t)N), o_tail = take(4 * (size_t)N), o_next = take(4 * (size_t)P), o_run = take(4 * ((size_t)P + 1));
+  const size_t o_rec = take(sizeof(GroupRec) * (size_t)P);
+  const size_t o_mark = take(std::max(rl.ncls, 1)), o_ccnt2 = take(4 * (size_t)std::max(rl.nctrl, 1)), o_over = take(std::max(rl.nctrl, 1));
+  if (devbuf_reserve(e, e->rm_state, off)) return -1;
+  unsigned char* b = static_cast<unsigned char*>(e->rm_state.p);
+  RemovalState& r = p.rm;
+  r.ncand = rl.ncand; r.persist = rl.persist; r.log_cap = rl.log_cap; r.li_in = rl.last_index; r.ncls = rl.ncls; r.nctrl = rl.nctrl;
+  r.cand = rl.cand; r.move_off = rl.move_off; r.move_pod = rl.move_pod; r.dest_ok = rl.dest_ok;
+  r.result = rl.result; r.log = rl.log; r.out = rl.out;
+  r.cfree = reinterpret_cast<int64_t*>(b + o_cfree); r.cslots = reinterpret_cast<int32_t*>(b + o_cslots);
+  r.cports = reinterpret_cast<unsigned long long*>(b + o_cports);
+  r.live = b + o_live; r.live_w = b + o_livew; r.rank = reinterpret_cast<int32_t*>(b + o_rank);
+  r.ccnt = reinterpret_cast<int32_t*>(b + o_ccnt); r.cpres = reinterpret_cast<int32_t*>(b + o_cpres);
+  r.wcnt = reinterpret_cast<int32_t*>(b + o_wcnt); r.wpres = reinterpret_cast<int32_t*>(b + o_wpres);
+  r.ctot = reinterpret_cast<int32_t*>(b + o_ctot); r.wtot = reinterpret_cast<int32_t*>(b + o_wtot); r.stat = reinterpret_cast<int32_t*>(b + o_stat);
+  r.hint = reinterpret_cast<int32_t*>(b + o_hint);
+  r.head = reinterpret_cast<int32_t*>(b + o_head); r.tail = reinterpret_cast<int32_t*>(b + o_tail); r.next = reinterpret_cast<int32_t*>(b + o_next);
+  r.run_off = reinterpret_cast<int32_t*>(b + o_run);
+  r.grs = group_rec_src(e);
+  p.fm_node_ok = b + o_ok; p.fm_hint = reinterpret_cast<int32_t*>(b + o_hinte); p.fm_assigned = reinterpret_cast<int32_t*>(b + o_asg);
+  p.fm_pods = reinterpret_cast<int32_t*>(b + o_list); p.grec = reinterpret_cast<GroupRec*>(b + o_rec);
+  p.fm_class_mark = b + o_mark; p.fm_ctrl_cnt = reinterpret_cast<int32_t*>(b + o_ccnt2); p.fm_ctrl_over = b + o_over;
+  if (rl.hint) CAE_CUDA(cudaMemcpyAsync(r.hint, rl.hint, sizeof(int32_t) * e->P, cudaMemcpyDeviceToDevice, e->stream));
+  else CAE_CUDA(cudaMemsetAsync(r.hint, 0xFF, sizeof(int32_t) * P, e->stream));
+  // the FM slab, laid out as for cae_filter_schedulable: one placement log entry per pod of a candidate at most
+  const size_t Xg = (size_t)N;
+  int dmax = 1;
+  for (int k = 0; k < e->dyn.K; ++k) dmax = std::max(dmax, e->dyn.Dc[k] + 2);
+  p.dstride = p.has_dyn ? dmax : 1;
+  p.log_cap = p.has_dyn ? e->P + 1024 : 1;
+  p.scratch_per_cta = slab_per_cta(A1, Xg, p.dstride, p.log_cap);
+  if (slab_reserve(e, e->fm_slab, p, A1, Xg, p.scratch_per_cta)) return -1;
+  CAE_CUDA(cudaMemsetAsync(e->d_work_counter, 0, sizeof(int32_t) * 2, e->stream));
+  { int unused = 0; if (launch_binpack_any(e, 1, 0, p, &unused, false, 2)) return -1; }
+  e->stats.kernel_launches += 1;
   CAE_KERNEL_OK();
   return 0;
 }

@@ -194,7 +194,10 @@ struct Engine {
   };
   struct Slab { DevBuf buf; size_t sig = 0, zeroed = 0; };   // estimator slab: layout signature, bytes zeroed under it
   Slab pack_slab, fm_slab;                // estimator / filter-out-schedulable pass (binpack.cu)
-  DevBuf fm_blob;                         // inputs and outputs of the filter pass
+  DevBuf fm_blob;                         // inputs and outputs of the filter pass / the scale-down batch
+  DevBuf rm_state;                        // scale-down batch state (RemovalState)
+  PinnedBuf rm_stage;                     // host staging of the scale-down batch's inputs
+  std::vector<int32_t> rm_owner, rm_seen; // [P] argument checks of the scale-down batch (kept to avoid per-call allocation)
   DevBuf x_rows;                          // caller-supplied option rows: node_count | sched | order
   DevBuf x_price;                         // price inputs: node_price | pod_price | unfitness | score, then has_gpu | exists
   // fused histogram exchange over peer memory (feas.cu)
@@ -267,6 +270,34 @@ struct FilterLaunch {
   uint8_t *class_mark, *ctrl_over;
 };
 int launch_filter(Engine* e, const FilterLaunch& f);
+// cae_simulate_removals (api.cu lays out the inputs and outputs, launch_removals the batch state behind them)
+struct RemovalLaunch {
+  int ncand, persist, ncls, nctrl, log_cap, last_index, n_move;
+  const int32_t *cand, *move_off, *move_pod, *hint, *cls, *class_ctrl;   // hint [P] (-1 = none) is read once
+  const uint8_t* dest_ok;                                                // [N] or NULL
+  int32_t *result, *log, *out;                                           // out = {lastIndex, log length}
+};
+// Device view of a batch: inputs and outputs of RemovalLaunch, the committed state of the snapshot (what the persisted
+// simulations left) and the working copy of the candidate being simulated.  All of it lives in one engine-owned buffer.
+struct RemovalState {
+  int ncand, persist, log_cap, li_in, ncls, nctrl;
+  const int32_t *cand, *move_off, *move_pod;
+  const uint8_t* dest_ok;
+  int32_t *result, *log, *out;
+  int64_t* cfree;                  // [A1][N] committed free resources
+  int32_t* cslots;                 // [N]     committed pod slots
+  unsigned long long* cports;      // [N]     committed host-port sets of moved pods
+  uint8_t *live, *live_w;          // [N]     node in the committed snapshot / in the candidate's simulation
+  int32_t* rank;                   // [N]     live_w rows before row x (lastIndex is a position among live nodes)
+  int32_t *ccnt, *cpres, *ctot;    // committed counters: [pool] counts, [pool] eligible nodes, [Q] totals
+  int32_t *wcnt, *wpres, *wtot;    // the same for the candidate's simulation (its node removed)
+  int32_t* stat;                   // [Q][3] min count, #domains at the min, #present domains of wcnt / wpres
+  int32_t* hint;                   // [P] hinted node of a pending pod, updated as pods are placed
+  int32_t *head, *tail, *next;     // [N], [N], [P] pods moved onto a node by persisted simulations, in arrival order
+  int32_t* run_off;                // [P + 1] runs of the candidate's pod list
+  GroupRecSrc grs;
+};
+int launch_removals(Engine* e, const RemovalLaunch& r);
 int launch_price(Engine* e, const cae_price_inputs& in_dev, const int32_t* d_node_count, const int32_t* d_sched, const int32_t* d_order,
                  double* d_score);
 int launch_waste(Engine* e, const int32_t* d_node_count, const int32_t* d_sched, double* d_waste);

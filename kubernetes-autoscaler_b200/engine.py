@@ -277,6 +277,43 @@ class Engine:
                                                     vp(assigned), vp(li), vp(ov)))
         return assigned[:enc.P], int(li[0]), int(ov[0])
 
+    def simulate_removals(self, cand_node, move_off, move_pod, dest_ok=None, hint_node=None, sim_class=None, class_ctrl=None,
+                          last_index: int = 0, persist: bool = False, log_cap: Optional[int] = None):
+        """RemovalSimulator.SimulateNodeRemoval on every candidate in order, on the snapshot of the last load
+        (cae_simulate_removals).  Returns (result[n_cand] CAE_REMOVAL_*, lastIndex afterwards, log [n][3] = (candidate,
+        pending pod, cluster row or -1) per pod tried).  A log that outgrows `log_cap` (default: one entry per listed pod
+        plus room for moved-in pods) is fetched again at the size the engine reports."""
+        move_off = np.ascontiguousarray(move_off, np.int32)
+        cap = int(log_cap) if log_cap is not None else int(move_off[-1]) + 64 if len(move_off) else 0
+        rc, res, li, log = self._simulate_removals_raw(cand_node, move_off, move_pod, dest_ok, hint_node, sim_class, class_ctrl,
+                                                        last_index, persist, cap)
+        if rc == 1:   # the log needed more room: once more at the size it reported
+            rc, res, li, log = self._simulate_removals_raw(cand_node, move_off, move_pod, dest_ok, hint_node, sim_class,
+                                                            class_ctrl, last_index, persist, len(log))
+        self._check(rc)
+        return res, li, log
+
+    def _simulate_removals_raw(self, cand_node, move_off, move_pod, dest_ok, hint_node, sim_class, class_ctrl, last_index,
+                               persist, log_cap):
+        """One cae_simulate_removals call: (status, result, lastIndex, log); on status 1 the log is zeros of the needed length."""
+        cn = np.ascontiguousarray(cand_node, np.int32)
+        mo = np.ascontiguousarray(move_off, np.int32)
+        mp = np.ascontiguousarray(move_pod, np.int32)
+        ok = None if dest_ok is None else np.ascontiguousarray(dest_ok, np.uint8)
+        hn = None if hint_node is None else np.ascontiguousarray(hint_node, np.int32)
+        sc = None if sim_class is None else np.ascontiguousarray(sim_class, np.int32)
+        cc = None if class_ctrl is None else np.ascontiguousarray(class_ctrl, np.int32)
+        res = np.zeros(max(len(cn), 1), np.int32)
+        log = np.zeros((max(log_cap, 1), 3), np.int32)
+        li, n = np.zeros(1, np.int32), np.zeros(1, np.int32)
+        vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+        rc = self.lib.cae_simulate_removals(self.h, len(cn), vp(cn), vp(mo), vp(mp), vp(ok), vp(hn), vp(sc), vp(cc),
+                                            0 if cc is None else len(cc), int(last_index), int(bool(persist)), vp(res), vp(li),
+                                            vp(log), int(log_cap), vp(n))
+        if rc == 1:
+            return rc, None, None, np.zeros((int(n[0]), 3), np.int32)
+        return rc, res[:len(cn)], int(li[0]), log[:int(n[0])]
+
     # ---- fused histogram exchange over peer memory (multi-GPU dense pass) -------------------------
     def peer_handle(self) -> bytes:
         buf = C.create_string_buffer(capi.CONST["CAE_PEER_HANDLE_BYTES"])

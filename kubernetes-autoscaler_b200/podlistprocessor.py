@@ -72,11 +72,9 @@ class TryScheduleInputs:
     node_ok: Optional[np.ndarray]
 
 
-def prepare_try_schedule(cluster_snapshot: Sequence[NodeInfo], pods: Sequence[Pod], hints: Optional[Hints] = None,
-                         isNodeAcceptable: Callable[[NodeInfo], bool] = ScheduleAnywhere,
-                         namespaces: Sequence[Namespace] = ()) -> TryScheduleInputs:
-    pods = list(pods)
-    cluster = list(cluster_snapshot)
+def _encode_pending(cluster: List[NodeInfo], pods: List[Pod], hints: Optional[Hints], namespaces: Sequence[Namespace]):
+    """The snapshot with `pods` as the pending pods: (enc, id(pod) -> pending index, hinted row per pending pod,
+    SimilarPodsScheduling class per pending pod, controller per class)."""
     groups = build_pod_groups(pods)
     enc = encode(cluster, [], groups, namespaces)
     index_of: Dict[int, int] = {}
@@ -87,7 +85,6 @@ def prepare_try_schedule(cluster_snapshot: Sequence[NodeInfo], pods: Sequence[Po
             k += 1
     pend_spec = enc.arrays["pend_spec"]
     node_index = {ni.node.name: i for i, ni in enumerate(cluster)}
-    order = [index_of[id(p)] for p in pods]
     hint = np.full(enc.P, -1, np.int32)
     if hints is not None:
         for p in pods:
@@ -107,11 +104,90 @@ def prepare_try_schedule(cluster_snapshot: Sequence[NodeInfo], pods: Sequence[Po
                 classes[key] = len(class_ctrl)
                 class_ctrl.append(ctrls.setdefault(p.owner_uid, len(ctrls)))
             sim[i] = classes[key]
+    return enc, index_of, hint, sim, class_ctrl
+
+
+def prepare_try_schedule(cluster_snapshot: Sequence[NodeInfo], pods: Sequence[Pod], hints: Optional[Hints] = None,
+                         isNodeAcceptable: Callable[[NodeInfo], bool] = ScheduleAnywhere,
+                         namespaces: Sequence[Namespace] = ()) -> TryScheduleInputs:
+    pods = list(pods)
+    cluster = list(cluster_snapshot)
+    enc, index_of, hint, sim, class_ctrl = _encode_pending(cluster, pods, hints, namespaces)
+    order = [index_of[id(p)] for p in pods]
     ok = None
     if isNodeAcceptable is not ScheduleAnywhere:
         ok = np.array([1 if isNodeAcceptable(ni) else 0 for ni in cluster], np.uint8)
     return TryScheduleInputs(enc, cluster, pods, index_of, order, hint if (hint >= 0).any() else None,
                              sim if class_ctrl else None, class_ctrl or None, ok)
+
+
+@dataclass
+class RemovalInputs:
+    """What cae_simulate_removals takes, built from objects: the WHOLE snapshot encoded once, its pending pods the
+    to-move copies (nodeName cleared) of every candidate's load-time pods, one per pod key."""
+    enc: object
+    cluster: List[NodeInfo]
+    candidates: List[str]
+    pods: List[Pod]                   # pending pod index -> the to-move copy
+    cand_node: np.ndarray             # [K] cluster row, -1 = not in the snapshot
+    move_off: np.ndarray              # [K + 1]
+    move_pod: np.ndarray              # pending-pod indices of every candidate's load-time list
+    to_move: List[List[Pod]]          # [K] the caller's objects behind move_pod (what pods_to_reschedule reports)
+    dest_ok: Optional[np.ndarray]
+    hint: Optional[np.ndarray]
+    sim_class: Optional[np.ndarray]
+    class_ctrl: Optional[List[int]]
+
+
+def prepare_removals(cluster_snapshot: Sequence[NodeInfo], candidates: Sequence[str], destinationMap: Dict[str, bool],
+                     pods_to_move: Optional[Sequence[Optional[Sequence[Pod]]]] = None, hints: Optional[Hints] = None,
+                     namespaces: Sequence[Namespace] = ()) -> RemovalInputs:
+    """One encode for a whole scale-down batch.  pods_to_move[i] (or None) replaces the default list of candidate i: the
+    node's non-DaemonSet pods in NodeInfo order (removal.RemovalSimulator.SimulateNodeRemoval)."""
+    if isinstance(candidates, str) or not all(isinstance(c, str) for c in candidates):
+        raise TypeError("candidates must be a sequence of node names")
+    candidates = list(candidates)
+    if pods_to_move is not None and len(pods_to_move) != len(candidates):
+        raise ValueError("pods_to_move needs one entry per candidate (%d != %d)" % (len(pods_to_move), len(candidates)))
+    cluster = list(cluster_snapshot)
+    row_of = {ni.node.name: i for i, ni in enumerate(cluster)}
+    pods: List[Pod] = []
+    key_index: Dict[Tuple[str, str], Tuple[int, int]] = {}     # pod key -> (pending index, row it is listed under)
+    cand_node, lists, to_move = [], [], []
+    for i, name in enumerate(candidates):
+        row = row_of.get(name, -1)
+        cand_node.append(row)
+        explicit = pods_to_move[i] if pods_to_move is not None else None
+        objs = [] if row < 0 else (list(explicit) if explicit is not None else
+                                   [p for p in cluster[row].pods if p.owner_kind != "DaemonSet"])
+        idx = []
+        for p in objs:
+            k = HintKeyFromPod(p)
+            if k in key_index:
+                j, r = key_index[k]
+                if r != row or j in idx:
+                    raise ValueError("pod %s/%s is listed twice or under two nodes" % k)
+            else:
+                q = p.clone()
+                q.node_name = ""
+                j = len(pods)
+                pods.append(q)
+                key_index[k] = (j, row)
+            idx.append(j)
+        lists.append(idx)
+        to_move.append(objs)
+    enc, index_of, hint, sim, class_ctrl = _encode_pending(cluster, pods, hints, namespaces)
+    perm = [index_of[id(q)] for q in pods]   # list position -> pending index of the encode
+    move_off = np.zeros(len(candidates) + 1, np.int32)
+    move_off[1:] = np.cumsum([len(ix) for ix in lists]) if lists else []
+    move_pod = np.array([perm[j] for ix in lists for j in ix], np.int32)
+    by_index: List[Optional[Pod]] = [None] * enc.P
+    for q in pods:
+        by_index[index_of[id(q)]] = q
+    dest = np.array([1 if destinationMap.get(ni.node.name) else 0 for ni in cluster], np.uint8)
+    return RemovalInputs(enc, cluster, candidates, by_index, np.array(cand_node, np.int32), move_off, move_pod, to_move,
+                         None if dest.all() else dest, hint if (hint >= 0).any() else None,
+                         sim if class_ctrl else None, class_ctrl or None)
 
 
 class HintingSimulator:

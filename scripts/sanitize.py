@@ -6,7 +6,7 @@ self-cleaning accumulators, last-block election, shared-memory state and block-w
     compute-sanitizer --tool racecheck python scripts/sanitize.py
 
 Dense pass (K1, both variants), Estimate() of every template (K0 + K3: plain closed form, capacity form with the cluster
-fallback, per-pod loop), expander scores, the filter-out-schedulable pass — on miniatures of C2, C3 and C4 — each checked
+fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals) — on miniatures of C2, C3 and C4 — each checked
 against the CPU oracle so that a "clean" run also means "correct results under the tool"."""
 import os
 import sys
@@ -54,6 +54,14 @@ def main():
             assert all(np.array_equal(x, y) for x, y in zip(got_e, ref_e[:4]))
             got = eng.filter_schedulable(order_p)
             ref = pyoracle.filter_schedulable(after, order_p)
+            assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
+            # scale-down batch (cae_simulate_removals): every cluster node a candidate, each listing its own slice of pending
+            # pods, persisted; the filter pass on the same load is unchanged afterwards
+            n = enc.struct.num_cluster_nodes
+            cand = np.arange(n, dtype=np.int32)
+            move_off = np.minimum(np.arange(n + 1, dtype=np.int32) * 4, len(order_p)).astype(np.int32)
+            eng.simulate_removals(cand, move_off, order_p[:move_off[-1]], persist=True)
+            got = eng.filter_schedulable(order_p)
             assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
         print("config", cfg, "ok: nodes", int(nc.sum()), "pods", int(pc.sum()), flush=True)
     eng.close()
