@@ -315,7 +315,10 @@ int32_t cae_load_pending(cae_engine* e, int32_t num_pending, const int32_t* pend
  *     resident) at the last cae_load — it could add an existing-anti-affinity counter;
  *   - the resident pods of all nodes, or the entries of a dictionary table, would pass 2^31 - 1 (checked from the counts
  *     and offsets alone, before any pod-spec id is read).
- * Adding or removing nodes, template changes and pod specs the last cae_load did not have cannot be expressed: cae_load. */
+ * Adding or removing nodes: cae_load_node_churn.  Template changes and pod specs the last cae_load did not have cannot be
+ * expressed: cae_load.
+ * The interner is append-only across deltas: hostname_key and unschedulable_taint_key stay those of the last cae_load (a
+ * caller that needs them to change does a full load). */
 typedef struct cae_node_delta {
   int32_t abi_version; /* CAE_ABI_VERSION */
   /* dictionary tails: value ids [num_values, num_values + num_new_values) of the resident snapshot */
@@ -345,6 +348,43 @@ typedef struct cae_node_delta {
   const int32_t* pod_spec;     /* pod-spec ids of the resident table */
 } cae_node_delta;
 int32_t cae_load_nodes(cae_engine* e, const cae_node_delta* d);
+
+/* The per-tick delta of the cluster-node LIST: nodes removed (a scale-down, a node that left) and nodes added (a scale-up's
+ * nodes registering), together with the dirty rows of the surviving nodes, against the snapshot that is already resident.
+ * Replaces: the node adds / removes of DeltaSnapshotStore.SetClusterState between two loops, which cae_load_nodes cannot
+ * express because a row's identity is its index.
+ * The new cluster list is the surviving rows in their old order, then the added rows in the given order; template t moves
+ * to row N' + t.  Every row index the caller holds (hints, node_ok, dest_ok, cand_node) refers to the new list after the
+ * call.  After the call every entry point answers bit-identically to a cae_load of the objects in that order.  Pending pods
+ * and templates are not touched; the call combines with cae_load_pending and cae_load_nodes in any order.  Unlike
+ * cae_load_nodes, a dirty or added row may carry any value of a topology key: the topology domains are rebuilt.  An added
+ * node carries no capacity or has_alloc_* (read for templates only).  hostname_key and unschedulable_taint_key stay those
+ * of the last cae_load.
+ * Status -2 (malformed, nothing changed): every cause of cae_load_nodes on `changed`; removed rows out of range, not
+ *   strictly increasing or also dirty; added-row arrays NULL with num_added > 0; ids of added rows outside the resident
+ *   tables plus the tails (a node-name id must be >= 0); added-row offsets that do not start at 0 or decrease.
+ * Status 2 (the churn does not apply: call cae_load with the full snapshot; nothing is changed):
+ *   - an added or dirty row's resident pod has a spec with required anti-affinity terms and no pod of that spec was in the
+ *     snapshot at the last cae_load;
+ *   - the node rows and template copies (N' + 2T), the resident pods of all nodes, or the entries of a dictionary table
+ *     would pass 2^31 - 1 (checked from the counts and offsets alone, before any id is read). */
+typedef struct cae_node_churn {
+  int32_t abi_version;             /* CAE_ABI_VERSION */
+  const cae_node_delta* changed;   /* dirty rows (row numbers of the snapshot BEFORE the call) and the dictionary tails that
+                                      the dirty AND the added rows use; NULL = none */
+  int32_t num_removed;
+  const int32_t* removed;          /* rows before the call, strictly increasing, none of them also dirty */
+  int32_t num_added;               /* new cluster nodes, appended after the surviving rows in this order */
+  const int32_t* name;             /* node-name id */
+  const int32_t* labelset;
+  const int32_t* taint_list;
+  const uint8_t* unschedulable;
+  const int64_t* alloc;            /* [num_added * CAE_MAX_RES] */
+  const int32_t* allowed_pods;
+  const int32_t* pod_off;          /* [num_added + 1] */
+  const int32_t* pod_spec;         /* resident pod-spec ids */
+} cae_node_churn;
+int32_t cae_load_node_churn(cae_engine* e, const cae_node_churn* c);
 
 int32_t cae_feasibility(cae_engine* e, uint32_t* fit_bits, uint8_t* reasons, int32_t* fit_count);
 

@@ -10,7 +10,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import re
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 REPO_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(REPO_ROOT, "include", "caengine.h")
@@ -25,7 +25,8 @@ def _strip_comments(src: str) -> str:
     return re.sub(r"/\*.*?\*/", "", src, flags=re.S)
 
 
-def _parse_struct(src: str, name: str) -> List[Tuple[str, object]]:
+def _parse_struct(src: str, name: str, structs: Optional[Dict[str, type]] = None) -> List[Tuple[str, object]]:
+    """``structs``: ABI structs a field may point to, by their C name."""
     m = re.search(r"typedef struct %s \{(.*?)\} %s;" % (name, name), src, flags=re.S)
     if not m:
         raise RuntimeError("struct %s not found in %s" % (name, HEADER))
@@ -37,7 +38,7 @@ def _parse_struct(src: str, name: str) -> List[Tuple[str, object]]:
         mm = re.match(r"(const\s+)?(\w+)\s*(\*?)\s*([\w, ]+?)(\[(\d+)\])?$", decl)
         if not mm:
             raise RuntimeError("cannot parse field %r of %s" % (decl, name))
-        ctype = _SCALARS[mm.group(2)]
+        ctype = _SCALARS[mm.group(2)] if mm.group(2) in _SCALARS else (structs or {})[mm.group(2)]
         for fname in [f.strip() for f in mm.group(4).split(",")]:
             if mm.group(3):
                 fields.append((fname, C.POINTER(ctype)))
@@ -95,6 +96,10 @@ class cae_node_delta(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_node_delta")
 
 
+class cae_node_churn(C.Structure):
+    _fields_ = _parse_struct(_SRC, "cae_node_churn", {"cae_node_delta": cae_node_delta})
+
+
 def declared_functions() -> List[str]:
     """Names of every function the header declares (used by the symbol-export test)."""
     return sorted(set(re.findall(r"\b(cae_\w+)\s*\(", _SRC)))
@@ -146,6 +151,8 @@ def load_engine_lib() -> C.CDLL:
     lib.cae_load_pending.restype = C.c_int32
     lib.cae_load_nodes.argtypes = [C.c_void_p, P(cae_node_delta)]
     lib.cae_load_nodes.restype = C.c_int32
+    lib.cae_load_node_churn.argtypes = [C.c_void_p, P(cae_node_churn)]
+    lib.cae_load_node_churn.restype = C.c_int32
     lib.cae_feasibility.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.cae_feasibility.restype = C.c_int32
     lib.cae_feasibility_groups.argtypes = [C.c_void_p, C.c_void_p]

@@ -122,6 +122,26 @@ static bool host_label(const cae_objects* o, int ls, int key, int* val) {
   return false;
 }
 
+// Topology domains of one key over the NT rows (val[row] = value id, -1 = label absent): domain ids in order of first
+// appearance, cluster rows [0, N) first, then the templates.  Dc = domains that occur on cluster rows, D = all of them.
+// id_of maps value id -> domain while it runs and is all -1 again on return.
+static void assign_domains(const int32_t* val, int N, int NT, std::vector<int32_t>& id_of, int32_t* dom, int* Dc, int* D) {
+  int n = 0;
+  *Dc = 0;
+  for (int row = 0; row < NT; ++row) {
+    if (row == N) *Dc = n;
+    const int v = val[row];
+    dom[row] = -1;
+    if (v < 0) continue;
+    if ((size_t)v >= id_of.size()) id_of.resize((size_t)v + 1, -1);
+    if (id_of[v] < 0) id_of[v] = n++;
+    dom[row] = id_of[v];
+  }
+  if (N == NT) *Dc = n;
+  *D = n;
+  for (int row = 0; row < NT; ++row) if (val[row] >= 0) id_of[val[row]] = -1;
+}
+
 // Interning for the pod-state dependent plugins (dyn.cuh): topology keys -> compact ids, label values
 // -> domain indices, pod specs -> dynamic classes, and the list of counters each class needs.
 // Structure only; every match / count is computed on the device (dyn_kernels.cu).
@@ -136,6 +156,8 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
   for (int i = 0; i < o->node_pod_off[NT]; ++i) spec_used[o->node_pod_spec[i]] = 1;
   e->nh.spec_used = spec_used;
   e->nh.key_val.clear();
+  e->nh.tkey_val.clear();
+  e->nh.q_k.clear();
   bool any = false;
   std::vector<int> keys;
   auto add_key = [&](int key) { if (std::find(keys.begin(), keys.end(), key) == keys.end()) keys.push_back(key); };
@@ -157,23 +179,19 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
   if (!any) return 0;
   if ((int)keys.size() > DYN_MAX_KEYS) { set_error("more than 8 distinct topology keys"); return 1; }
   d.K = (int)keys.size();
-  std::vector<int32_t> dom((size_t)d.K * NT, -1);
+  std::vector<int32_t> dom((size_t)d.K * NT, -1), val(NT);
   e->nh.key_val.assign((size_t)d.K * N, -1);
+  e->nh.tkey_val.assign((size_t)d.K * T, -1);
   for (int k = 0; k < d.K; ++k) {
     d.key_id[k] = keys[k];
     d.is_host[k] = keys[k] == o->hostname_key;
-    std::map<int, int> ids;
     for (int row = 0; row < NT; ++row) {
-      if (row == N) d.Dc[k] = (int)ids.size();
       int v;
-      if (!host_label(o, o->node_labelset[row], keys[k], &v)) continue;
-      if (row < N) e->nh.key_val[(size_t)k * N + row] = v;
-      auto it = ids.find(v);
-      if (it == ids.end()) it = ids.emplace(v, (int)ids.size()).first;
-      dom[(size_t)k * NT + row] = it->second;
+      val[row] = host_label(o, o->node_labelset[row], keys[k], &v) ? v : -1;
     }
-    if (T == 0) d.Dc[k] = (int)ids.size();
-    d.D[k] = (int)ids.size();
+    std::copy(val.begin(), val.begin() + N, e->nh.key_val.begin() + (size_t)k * N);
+    std::copy(val.begin() + N, val.end(), e->nh.tkey_val.begin() + (size_t)k * T);
+    assign_domains(val.data(), N, NT, e->nh.dom_scratch, dom.data() + (size_t)k * NT, &d.Dc[k], &d.D[k]);
   }
   auto kidx = [&](int key) { return (int)(std::find(keys.begin(), keys.end(), key) - keys.begin()); };
   // dynamic classes
@@ -212,6 +230,7 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
   d.DC = (int)dc_spec.size();
   d.Q = (int)q_kind.size();
   d.pool = q_base_off.back();
+  e->nh.q_k = q_k;
   e->DC = d.DC;
   const int32_t* p32 = nullptr; const uint8_t* p8 = nullptr;
 #define UPV(vec, field) { if (upload(e, (vec).data(), (vec).size(), &field)) return -1; }
@@ -602,22 +621,63 @@ static int grow_table(Engine* e, Engine::DevBuf& b, const T*& cur, size_t n_old,
   return 0;
 }
 
-// cae_load_nodes: every check on the host first (nothing is changed unless the whole delta applies), then the device work in
-// stream order without a host synchronisation: dictionary tails, dirty rows + resident CSR, pre_code of the dirty columns,
-// the topology counters and the tables derived from them.
-static int do_load_nodes(Engine* e, const cae_node_delta* dl) {
-  auto bad = [](const char* m) { set_error(std::string("cae_load_nodes: ") + m); return -2; };
-  auto refuse = [](const char* m) { set_error(std::string("cae_load_nodes: ") + m); return 2; };
+// The new state of cluster rows a node delta carries: the dirty rows of a cae_node_delta, the added nodes of a churn
+struct RowsIn {
+  int n = 0;
+  const int32_t *labelset = nullptr, *taint_list = nullptr, *allowed = nullptr, *pod_off = nullptr, *pod_spec = nullptr;
+  const uint8_t* unsched = nullptr;
+  const int64_t* alloc = nullptr;
+};
+
+// One cae_load_nodes or cae_load_node_churn call: its input, then what check_nodes derived from it
+struct NodePlan {
+  const cae_node_delta* dl = nullptr;   // dictionary tails and dirty rows (row numbers before the call)
+  RowsIn dirty, added;
+  const int32_t *removed = nullptr, *name = nullptr;   // churn: removed rows, node names of the added rows
+  int nr = 0;
+  int64_t pairs = 0, tents = 0, npods_d = 0, npods_a = 0, NV = 0, NL = 0, NTL = 0, total = 0;
+  int32_t old_nv = 0, old_nl = 0, old_ntl = 0, old_tents = 0, old_pairs = 0;
+};
+
+static RowsIn dirty_rows(const cae_node_delta* dl) {
+  RowsIn r;
+  r.n = dl->num_dirty; r.labelset = dl->labelset; r.taint_list = dl->taint_list; r.allowed = dl->allowed_pods;
+  r.pod_off = dl->pod_off; r.pod_spec = dl->pod_spec; r.unsched = dl->unschedulable; r.alloc = dl->alloc;
+  return r;
+}
+
+// value id of `key` in label set ls of the resident table or of the delta's tail, -1 absent
+static int label_of(const Engine::NodeHost& nh, const cae_node_delta* dl, int ls, int key) {
+  const bool tail = ls >= nh.num_labelsets;
+  const int32_t *off = tail ? dl->ls_off : nh.ls_off.data(), *k = tail ? dl->ls_key : nh.ls_key.data(), *v = tail ? dl->ls_val : nh.ls_val.data();
+  const int j = tail ? ls - nh.num_labelsets : ls;   // a tail's offsets and pairs are numbered from 0
+  for (int p = off[j]; p < off[j + 1]; ++p) if (k[p] == key) return v[p];
+  return -1;
+}
+
+// Every check of a node delta or churn, on the host, before anything changes.  Returns 0, -2 (malformed) or 2 (the call
+// does not apply: use cae_load).  `topo_fixed` (cae_load_nodes): a dirty row may not change the value of a topology key
+// the counters use, because the domains are not rebuilt.
+static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed) {
+  auto bad = [who](const char* m) { set_error(std::string(who) + ": " + m); return -2; };
+  auto refuse = [who](const char* m) { set_error(std::string(who) + ": " + m); return 2; };
+  const cae_node_delta* dl = p.dl;
   if (dl->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
-  Engine::NodeHost& nh = e->nh;
-  const int N = e->N, S = e->num_podspecs, A = e->A;
+  const Engine::NodeHost& nh = e->nh;
+  const int N = e->N, S = e->num_podspecs;
   const int nv = dl->num_new_values, nl = dl->num_new_labelsets, ntl = dl->num_new_taint_lists, nd = dl->num_dirty;
-  if (nv < 0 || nl < 0 || ntl < 0 || nd < 0) return bad("negative count");
+  const int na = p.added.n, nr = p.nr;
+  if (nv < 0 || nl < 0 || ntl < 0 || nd < 0 || na < 0 || nr < 0) return bad("negative count");
   if (nv && (!dl->value_is_int || !dl->value_int)) return bad("value tail without arrays");
   if (nl && !dl->ls_off) return bad("label-set tail without offsets");
   if (ntl && !dl->taint_off) return bad("taint-list tail without offsets");
-  if (nd && (!dl->row || !dl->labelset || !dl->taint_list || !dl->unschedulable || !dl->alloc || !dl->allowed_pods || !dl->pod_off))
-    return bad("dirty rows without arrays");
+  auto rows_null = [](const RowsIn& r) {
+    return r.n && (!r.labelset || !r.taint_list || !r.unsched || !r.alloc || !r.allowed || !r.pod_off);
+  };
+  if (rows_null(p.dirty) || (nd && !dl->row)) return bad("dirty rows without arrays");
+  if (nr && !p.removed) return bad("removed rows without an array");
+  if (rows_null(p.added) || (na && !p.name)) return bad("added rows without arrays");
+  if ((int64_t)N - nr + na + 2 * (int64_t)e->T > INT32_MAX) return refuse("the node rows and template copies would pass 2^31 - 1");
   auto offsets_ok = [](const int32_t* off, int n) {
     if (off[0] != 0) return false;
     for (int i = 0; i < n; ++i) if (off[i + 1] < off[i]) return false;
@@ -626,130 +686,286 @@ static int do_load_nodes(Engine* e, const cae_node_delta* dl) {
   if (nl && !offsets_ok(dl->ls_off, nl)) return bad("label-set offsets");
   if (ntl && !offsets_ok(dl->taint_off, ntl)) return bad("taint-list offsets");
   if (nd && !offsets_ok(dl->pod_off, nd)) return bad("resident-pod offsets");
-  const int64_t pairs = nl ? dl->ls_off[nl] : 0, tents = ntl ? dl->taint_off[ntl] : 0, npods = nd ? dl->pod_off[nd] : 0;
-  if (pairs && (!dl->ls_key || !dl->ls_val)) return bad("label pairs without arrays");
-  if (tents && (!dl->taint_key || !dl->taint_val || !dl->taint_effect)) return bad("taints without arrays");
-  if (npods && !dl->pod_spec) return bad("resident pods without pod_spec");
-  const int64_t NV = (int64_t)nh.num_values + nv, NL = (int64_t)nh.num_labelsets + nl, NTL = (int64_t)nh.num_taint_lists + ntl;
+  if (na && !offsets_ok(p.added.pod_off, na)) return bad("resident-pod offsets of the added rows");
+  p.pairs = nl ? dl->ls_off[nl] : 0;
+  p.tents = ntl ? dl->taint_off[ntl] : 0;
+  p.npods_d = nd ? dl->pod_off[nd] : 0;
+  p.npods_a = na ? p.added.pod_off[na] : 0;
+  if (p.pairs && (!dl->ls_key || !dl->ls_val)) return bad("label pairs without arrays");
+  if (p.tents && (!dl->taint_key || !dl->taint_val || !dl->taint_effect)) return bad("taints without arrays");
+  if ((p.npods_d && !dl->pod_spec) || (p.npods_a && !p.added.pod_spec)) return bad("resident pods without pod_spec");
+  p.NV = (int64_t)nh.num_values + nv; p.NL = (int64_t)nh.num_labelsets + nl; p.NTL = (int64_t)nh.num_taint_lists + ntl;
   const int64_t old_pairs = nh.ls_off.back();
-  if (NV > INT32_MAX || NL >= INT32_MAX || NTL >= INT32_MAX || old_pairs + pairs > INT32_MAX || (int64_t)nh.taint_entries + tents > INT32_MAX)
+  if (p.NV > INT32_MAX || p.NL >= INT32_MAX || p.NTL >= INT32_MAX || old_pairs + p.pairs > INT32_MAX ||
+      (int64_t)nh.taint_entries + p.tents > INT32_MAX)
     return refuse("a dictionary table would pass 2^31 - 1 entries");
   int64_t total = nh.pod_total;
   for (int i = 0; i < nd; ++i) {
     const int r = dl->row[i];
     if (r < 0 || r >= N || (i > 0 && r <= dl->row[i - 1])) return bad("rows out of range or not strictly increasing");
-    if (dl->labelset[i] < 0 || dl->labelset[i] >= NL) return bad("label-set id out of range");
-    if (dl->taint_list[i] < 0 || dl->taint_list[i] >= NTL) return bad("taint-list id out of range");
+    if (dl->labelset[i] < 0 || dl->labelset[i] >= p.NL) return bad("label-set id out of range");
+    if (dl->taint_list[i] < 0 || dl->taint_list[i] >= p.NTL) return bad("taint-list id out of range");
     total += (int64_t)(dl->pod_off[i + 1] - dl->pod_off[i]) - nh.pod_cnt[r];
   }
+  for (int i = 0, j = 0; i < nr; ++i) {   // j walks the dirty rows alongside
+    const int r = p.removed[i];
+    if (r < 0 || r >= N || (i > 0 && r <= p.removed[i - 1])) return bad("removed rows out of range or not strictly increasing");
+    while (j < nd && dl->row[j] < r) ++j;
+    if (j < nd && dl->row[j] == r) return bad("a removed row is also dirty");
+    total -= nh.pod_cnt[r];
+  }
+  for (int i = 0; i < na; ++i) {
+    if (p.name[i] < 0) return bad("node-name id of an added row out of range");
+    if (p.added.labelset[i] < 0 || p.added.labelset[i] >= p.NL) return bad("label-set id of an added row out of range");
+    if (p.added.taint_list[i] < 0 || p.added.taint_list[i] >= p.NTL) return bad("taint-list id of an added row out of range");
+  }
+  total += p.npods_a;
   if (total > INT32_MAX) return refuse("more than 2^31 - 1 resident pods");
   for (int j = 0; j < nl; ++j)
-    for (int p = dl->ls_off[j]; p < dl->ls_off[j + 1]; ++p) {
-      if (dl->ls_key[p] < 0 || (p > dl->ls_off[j] && dl->ls_key[p] <= dl->ls_key[p - 1])) return bad("label pairs not sorted by key id");
-      if (dl->ls_val[p] < 0 || dl->ls_val[p] >= NV) return bad("label value id out of range");
+    for (int q = dl->ls_off[j]; q < dl->ls_off[j + 1]; ++q) {
+      if (dl->ls_key[q] < 0 || (q > dl->ls_off[j] && dl->ls_key[q] <= dl->ls_key[q - 1])) return bad("label pairs not sorted by key id");
+      if (dl->ls_val[q] < 0 || dl->ls_val[q] >= p.NV) return bad("label value id out of range");
     }
-  for (int64_t p = 0; p < tents; ++p) {
-    if (dl->taint_key[p] < 0) return bad("taint key id out of range");
-    if (dl->taint_val[p] < -1 || dl->taint_val[p] >= NV) return bad("taint value id out of range");
-    if (dl->taint_effect[p] < CAE_EFFECT_NONE || dl->taint_effect[p] > CAE_EFFECT_NO_EXECUTE) return bad("taint effect out of range");
+  for (int64_t q = 0; q < p.tents; ++q) {
+    if (dl->taint_key[q] < 0) return bad("taint key id out of range");
+    if (dl->taint_val[q] < -1 || dl->taint_val[q] >= p.NV) return bad("taint value id out of range");
+    if (dl->taint_effect[q] < CAE_EFFECT_NONE || dl->taint_effect[q] > CAE_EFFECT_NO_EXECUTE) return bad("taint effect out of range");
   }
-  for (int64_t p = 0; p < npods; ++p)
-    if (dl->pod_spec[p] < 0 || dl->pod_spec[p] >= S) return bad("pod-spec id out of range");
+  for (int64_t q = 0; q < p.npods_d; ++q)
+    if (dl->pod_spec[q] < 0 || dl->pod_spec[q] >= S) return bad("pod-spec id out of range");
+  for (int64_t q = 0; q < p.npods_a; ++q)
+    if (p.added.pod_spec[q] < 0 || p.added.pod_spec[q] >= S) return bad("pod-spec id of an added row out of range");
   // ---- status 2: the resident classes, counters and domains would not be the ones a cae_load builds ----
-  for (int64_t p = 0; p < npods; ++p) {
-    const int s = dl->pod_spec[p];
+  for (int64_t q = 0; q < p.npods_d + p.npods_a; ++q) {
+    const int s = q < p.npods_d ? dl->pod_spec[q] : p.added.pod_spec[q - p.npods_d];
     if (nh.spec_anti[s] && !nh.spec_used[s]) return refuse("a resident pod's spec has anti-affinity terms and was not in the snapshot");
   }
-  auto label_of = [&](int ls, int key) -> int {   // value id of `key` in label set ls (resident table + tail), -1 absent
-    const bool tail = ls >= nh.num_labelsets;
-    const int32_t *off = tail ? dl->ls_off : nh.ls_off.data(), *k = tail ? dl->ls_key : nh.ls_key.data(), *v = tail ? dl->ls_val : nh.ls_val.data();
-    const int j = tail ? ls - nh.num_labelsets : ls;
-    for (int p = off[j]; p < off[j + 1]; ++p) if (k[p] == key) return v[p];
-    return -1;
-  };
   const DynTables& dy = e->dyn;
-  for (int k = 0; k < (e->has_dynamic ? dy.K : 0); ++k)
-    for (int i = 0; i < nd; ++i)
-      if (label_of(dl->labelset[i], dy.key_id[k]) != nh.key_val[(size_t)k * N + dl->row[i]])
-        return refuse("a dirty node changes the value of a topology key the counters use");
-  e->stats.h2d_bytes = 0;
-  if (!nv && !nl && !ntl && !nd) return 0;
+  if (topo_fixed)
+    for (int k = 0; k < (e->has_dynamic ? dy.K : 0); ++k)
+      for (int i = 0; i < nd; ++i)
+        if (label_of(nh, dl, dl->labelset[i], dy.key_id[k]) != nh.key_val[(size_t)k * N + dl->row[i]])
+          return refuse("a dirty node changes the value of a topology key the counters use");
+  p.total = total;
+  return 0;
+}
 
-  // ---- the delta applies: host state ----
-  const int old_nv = nh.num_values, old_nl = nh.num_labelsets, old_ntl = nh.num_taint_lists, old_tents = nh.taint_entries;
-  for (int j = 0; j < nl; ++j) nh.ls_off.push_back((int32_t)(old_pairs + dl->ls_off[j + 1]));
-  if (pairs) { nh.ls_key.insert(nh.ls_key.end(), dl->ls_key, dl->ls_key + pairs); nh.ls_val.insert(nh.ls_val.end(), dl->ls_val, dl->ls_val + pairs); }
-  nh.num_values = (int32_t)NV; nh.num_labelsets = (int32_t)NL; nh.num_taint_lists = (int32_t)NTL; nh.taint_entries += (int32_t)tents;
-  for (int i = 0; i < nd; ++i) nh.pod_cnt[dl->row[i]] = dl->pod_off[i + 1] - dl->pod_off[i];
-  nh.pod_total = total;
-  for (int64_t p = 0; p < npods; ++p) nh.spec_used[dl->pod_spec[p]] = 1;
+// The host state every applied delta updates: the dictionary tails, the specs in the snapshot, the resident total
+static void commit_nodes(Engine* e, NodePlan& p) {
+  Engine::NodeHost& nh = e->nh;
+  const cae_node_delta* dl = p.dl;
+  p.old_nv = nh.num_values; p.old_nl = nh.num_labelsets; p.old_ntl = nh.num_taint_lists; p.old_tents = nh.taint_entries;
+  p.old_pairs = nh.ls_off.back();
+  for (int j = 0; j < dl->num_new_labelsets; ++j) nh.ls_off.push_back((int32_t)(p.old_pairs + dl->ls_off[j + 1]));
+  if (p.pairs) {
+    nh.ls_key.insert(nh.ls_key.end(), dl->ls_key, dl->ls_key + p.pairs);
+    nh.ls_val.insert(nh.ls_val.end(), dl->ls_val, dl->ls_val + p.pairs);
+  }
+  nh.num_values = (int32_t)p.NV; nh.num_labelsets = (int32_t)p.NL; nh.num_taint_lists = (int32_t)p.NTL; nh.taint_entries += (int32_t)p.tents;
+  nh.pod_total = p.total;
+  for (int64_t q = 0; q < p.npods_d; ++q) nh.spec_used[dl->pod_spec[q]] = 1;
+  for (int64_t q = 0; q < p.npods_a; ++q) nh.spec_used[p.added.pod_spec[q]] = 1;
+}
 
-  // ---- one pinned staging blob, one H2D copy ----
+// One pinned staging blob and one H2D copy: the dictionary tails, the staged rows (dirty rows, then added ones) with their
+// run state (cluster_row_state), and the caller's `extra` segments (device addresses in xdev); then the dictionary tables
+// grow on the device.  After commit_nodes.
+static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<std::pair<const void*, size_t>>& extra, NodeDeltaDev* dd,
+                       std::vector<const char*>* xdev) {
+  const cae_node_delta* dl = p.dl;
+  const int A = e->A;
+  const int nv = dl->num_new_values, nl = dl->num_new_labelsets, ntl = dl->num_new_taint_lists;
+  const int nd = p.dirty.n, na = p.added.n, ns = nd + na;
+  const int64_t pairs = p.pairs, tents = p.tents, npods = p.npods_d + p.npods_a;
   size_t bytes = 0;
   auto seg = [&](size_t n, size_t elem) { const size_t at = bytes; bytes = (bytes + n * elem + 7) & ~(size_t)7; return at; };
-  const size_t o_vint = seg(nv, 8), o_alloc = seg((size_t)nd * R, 8), o_cfree = seg((size_t)nd * A, 8);
+  const size_t o_vint = seg(nv, 8), o_alloc = seg((size_t)ns * R, 8), o_cfree = seg((size_t)ns * A, 8);
   const size_t o_lsoff = seg(nl, 4), o_lskey = seg(pairs, 4), o_lsval = seg(pairs, 4);
   const size_t o_toff = seg(ntl, 4), o_tkey = seg(tents, 4), o_tval = seg(tents, 4), o_teff = seg(tents, 4);
-  const size_t o_row = seg(nd, 4), o_ls = seg(nd, 4), o_tl = seg(nd, 4), o_allowed = seg(nd, 4), o_slots = seg(nd, 4);
-  const size_t o_poff = seg((size_t)nd + 1, 4), o_pspec = seg(npods, 4), o_visint = seg(nv, 1), o_unsched = seg(nd, 1);
+  const size_t o_row = seg(nd, 4), o_name = seg(na, 4), o_ls = seg(ns, 4), o_tl = seg(ns, 4), o_allowed = seg(ns, 4), o_slots = seg(ns, 4);
+  const size_t o_poff = seg((size_t)ns + 1, 4), o_pspec = seg(npods, 4), o_visint = seg(nv, 1), o_unsched = seg(ns, 1);
+  std::vector<size_t> o_extra;
+  for (const auto& x : extra) o_extra.push_back(seg(x.second, 1));
   if (pinned_reserve(e, e->nd_stage, bytes)) return -1;
   char* h = static_cast<char*>(e->nd_stage.p);
   auto put = [&](size_t at, const void* src, size_t n) { if (n) memcpy(h + at, src, n); };
   put(o_vint, dl->value_int, (size_t)nv * 8);
   put(o_visint, dl->value_is_int, (size_t)nv);
-  put(o_alloc, dl->alloc, (size_t)nd * R * 8);
-  for (int j = 0; j < nl; ++j) reinterpret_cast<int32_t*>(h + o_lsoff)[j] = (int32_t)(old_pairs + dl->ls_off[j + 1]);   // absolute
+  for (int j = 0; j < nl; ++j) reinterpret_cast<int32_t*>(h + o_lsoff)[j] = (int32_t)(p.old_pairs + dl->ls_off[j + 1]);   // absolute
   put(o_lskey, dl->ls_key, (size_t)pairs * 4);
   put(o_lsval, dl->ls_val, (size_t)pairs * 4);
-  for (int j = 0; j < ntl; ++j) reinterpret_cast<int32_t*>(h + o_toff)[j] = old_tents + dl->taint_off[j + 1];
+  for (int j = 0; j < ntl; ++j) reinterpret_cast<int32_t*>(h + o_toff)[j] = p.old_tents + dl->taint_off[j + 1];
   put(o_tkey, dl->taint_key, (size_t)tents * 4);
   put(o_tval, dl->taint_val, (size_t)tents * 4);
   put(o_teff, dl->taint_effect, (size_t)tents * 4);
   put(o_row, dl->row, (size_t)nd * 4);
-  put(o_ls, dl->labelset, (size_t)nd * 4);
-  put(o_tl, dl->taint_list, (size_t)nd * 4);
-  put(o_allowed, dl->allowed_pods, (size_t)nd * 4);
-  put(o_unsched, dl->unschedulable, (size_t)nd);
-  if (nd) put(o_poff, dl->pod_off, ((size_t)nd + 1) * 4);
-  put(o_pspec, dl->pod_spec, (size_t)npods * 4);
+  put(o_name, p.name, (size_t)na * 4);
+  int32_t* poff = reinterpret_cast<int32_t*>(h + o_poff);
+  poff[0] = 0;
   int64_t* cfree = reinterpret_cast<int64_t*>(h + o_cfree);
   int32_t* cslots = reinterpret_cast<int32_t*>(h + o_slots);
-  for (int i = 0; i < nd; ++i)
-    cluster_row_state(e, dl->alloc + (size_t)i * R, dl->allowed_pods[i], dl->pod_spec + dl->pod_off[i], dl->pod_off[i + 1] - dl->pod_off[i],
-                      e->h_spec_req.data(), cfree + (size_t)i * A, 1, cslots + i);
+  for (int part = 0, i0 = 0; part < 2; ++part) {   // the dirty rows, then the added ones
+    const RowsIn& r = part ? p.added : p.dirty;
+    put(o_ls + (size_t)i0 * 4, r.labelset, (size_t)r.n * 4);
+    put(o_tl + (size_t)i0 * 4, r.taint_list, (size_t)r.n * 4);
+    put(o_allowed + (size_t)i0 * 4, r.allowed, (size_t)r.n * 4);
+    put(o_unsched + (size_t)i0, r.unsched, (size_t)r.n);
+    put(o_alloc + (size_t)i0 * R * 8, r.alloc, (size_t)r.n * R * 8);
+    put(o_pspec + (size_t)poff[i0] * 4, r.pod_spec, (size_t)(r.n ? r.pod_off[r.n] : 0) * 4);
+    for (int i = 0; i < r.n; ++i) {
+      poff[i0 + i + 1] = poff[i0] + r.pod_off[i + 1];
+      cluster_row_state(e, r.alloc + (size_t)i * R, r.allowed[i], r.pod_spec + r.pod_off[i], r.pod_off[i + 1] - r.pod_off[i],
+                        e->h_spec_req.data(), cfree + (size_t)(i0 + i) * A, 1, cslots + i0 + i);
+    }
+    i0 += r.n;
+  }
+  for (size_t x = 0; x < extra.size(); ++x) put(o_extra[x], extra[x].first, extra[x].second);
   if (devbuf_reserve(e, e->nd_blob, bytes)) return -1;
   char* dv = static_cast<char*>(e->nd_blob.p);
   CAE_CUDA(cudaMemcpyAsync(dv, h, bytes, cudaMemcpyHostToDevice, e->stream));
   CAE_CUDA(cudaEventRecord(e->nd_stage.ev, e->stream));
   e->stats.h2d_bytes = (int64_t)bytes;
+  if (xdev) for (size_t at : o_extra) xdev->push_back(dv + at);
 
   // ---- dictionary tails ----
   DevObjects& d = e->dobj;
-  if (grow_table(e, e->nd_tab[0], d.value_is_int, old_nv, dv + o_visint, nv) || grow_table(e, e->nd_tab[1], d.value_int, old_nv, dv + o_vint, nv) ||
-      grow_table(e, e->nd_tab[2], d.ls_off, (size_t)old_nl + 1, dv + o_lsoff, nl) ||
-      grow_table(e, e->nd_tab[3], d.ls_key, (size_t)old_pairs, dv + o_lskey, pairs) ||
-      grow_table(e, e->nd_tab[4], d.ls_val, (size_t)old_pairs, dv + o_lsval, pairs) ||
-      grow_table(e, e->nd_tab[5], d.taint_off, (size_t)old_ntl + 1, dv + o_toff, ntl) ||
-      grow_table(e, e->nd_tab[6], d.taint_key, (size_t)old_tents, dv + o_tkey, tents) ||
-      grow_table(e, e->nd_tab[7], d.taint_val, (size_t)old_tents, dv + o_tval, tents) ||
-      grow_table(e, e->nd_tab[8], d.taint_effect, (size_t)old_tents, dv + o_teff, tents))
+  if (grow_table(e, e->nd_tab[0], d.value_is_int, p.old_nv, dv + o_visint, nv) || grow_table(e, e->nd_tab[1], d.value_int, p.old_nv, dv + o_vint, nv) ||
+      grow_table(e, e->nd_tab[2], d.ls_off, (size_t)p.old_nl + 1, dv + o_lsoff, nl) ||
+      grow_table(e, e->nd_tab[3], d.ls_key, (size_t)p.old_pairs, dv + o_lskey, pairs) ||
+      grow_table(e, e->nd_tab[4], d.ls_val, (size_t)p.old_pairs, dv + o_lsval, pairs) ||
+      grow_table(e, e->nd_tab[5], d.taint_off, (size_t)p.old_ntl + 1, dv + o_toff, ntl) ||
+      grow_table(e, e->nd_tab[6], d.taint_key, (size_t)p.old_tents, dv + o_tkey, tents) ||
+      grow_table(e, e->nd_tab[7], d.taint_val, (size_t)p.old_tents, dv + o_tval, tents) ||
+      grow_table(e, e->nd_tab[8], d.taint_effect, (size_t)p.old_tents, dv + o_teff, tents))
     return -1;
-  d.num_values = (int32_t)NV;
+  d.num_values = (int32_t)p.NV;
   e->group_reason_valid = false;
-  if (!nd) return 0;
+  if (dd) {
+    *dd = NodeDeltaDev{};
+    dd->nd = nd; dd->na = na;
+    dd->row = reinterpret_cast<const int32_t*>(dv + o_row); dd->name = reinterpret_cast<const int32_t*>(dv + o_name);
+    dd->labelset = reinterpret_cast<const int32_t*>(dv + o_ls); dd->taint_list = reinterpret_cast<const int32_t*>(dv + o_tl);
+    dd->allowed = reinterpret_cast<const int32_t*>(dv + o_allowed); dd->cslots = reinterpret_cast<const int32_t*>(dv + o_slots);
+    dd->pod_off = reinterpret_cast<const int32_t*>(dv + o_poff); dd->pod_spec = reinterpret_cast<const int32_t*>(dv + o_pspec);
+    dd->unsched = reinterpret_cast<const uint8_t*>(dv + o_unsched);
+    dd->alloc = reinterpret_cast<const int64_t*>(dv + o_alloc); dd->cfree = reinterpret_cast<const int64_t*>(dv + o_cfree);
+  }
+  return 0;
+}
 
-  // ---- dirty rows, resident CSR, then everything derived from the cluster rows ----
+// cae_load_nodes: every check on the host first (nothing is changed unless the whole delta applies), then the device work in
+// stream order without a host synchronisation: dictionary tails, dirty rows + resident CSR, pre_code of the dirty columns,
+// the topology counters and the tables derived from them.
+static int do_load_nodes(Engine* e, const cae_node_delta* dl) {
+  NodePlan p;
+  p.dl = dl;
+  p.dirty = dirty_rows(dl);
+  { const int rc = check_nodes(e, "cae_load_nodes", p, true); if (rc) return rc; }
+  e->stats.h2d_bytes = 0;
+  const int nd = dl->num_dirty;
+  if (!dl->num_new_values && !dl->num_new_labelsets && !dl->num_new_taint_lists && !nd) return 0;
+  commit_nodes(e, p);
+  for (int i = 0; i < nd; ++i) e->nh.pod_cnt[dl->row[i]] = dl->pod_off[i + 1] - dl->pod_off[i];
   NodeDeltaDev dd{};
-  dd.nd = nd;
-  dd.row = reinterpret_cast<const int32_t*>(dv + o_row); dd.labelset = reinterpret_cast<const int32_t*>(dv + o_ls);
-  dd.taint_list = reinterpret_cast<const int32_t*>(dv + o_tl); dd.allowed = reinterpret_cast<const int32_t*>(dv + o_allowed);
-  dd.cslots = reinterpret_cast<const int32_t*>(dv + o_slots); dd.pod_off = reinterpret_cast<const int32_t*>(dv + o_poff);
-  dd.pod_spec = reinterpret_cast<const int32_t*>(dv + o_pspec); dd.unsched = reinterpret_cast<const uint8_t*>(dv + o_unsched);
-  dd.alloc = reinterpret_cast<const int64_t*>(dv + o_alloc); dd.cfree = reinterpret_cast<const int64_t*>(dv + o_cfree);
-  if (launch_node_rows(e, dd, total)) return -1;
+  if (stage_nodes(e, p, {}, &dd, nullptr)) return -1;
+  if (!nd) return 0;
+  // ---- dirty rows, resident CSR, then everything derived from the cluster rows ----
+  if (launch_node_rows(e, dd, p.total)) return -1;
   if (launch_class_matrix_cols(e, dd.row, nd)) return -1;
   if (e->has_dynamic) {
     if (launch_dynamic_recount(e, dd.row, nd)) return -1;
+    if (launch_post_bits(e)) return -1;
+  }
+  return 0;
+}
+
+// cae_load_node_churn: the same checks and staging as cae_load_nodes plus the removed and added rows; then the row list is
+// rebuilt.  The host computes the new row -> source map, the resident counts and topology values of the new list and its
+// topology domains (assign_domains, as cae_load does); the device gathers the node columns and the resident CSR through
+// the map and reruns what a load derives from the node list: the class matrix over the whole universe, the template bits
+// and, with topology counters, the recount over every column.
+static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
+  if (c->abi_version != CAE_ABI_VERSION) { set_error("cae_load_node_churn: abi_version mismatch"); return -2; }
+  cae_node_delta none{};
+  none.abi_version = CAE_ABI_VERSION;
+  NodePlan p;
+  p.dl = c->changed ? c->changed : &none;
+  p.dirty = dirty_rows(p.dl);
+  p.added.n = c->num_added; p.added.labelset = c->labelset; p.added.taint_list = c->taint_list; p.added.allowed = c->allowed_pods;
+  p.added.pod_off = c->pod_off; p.added.pod_spec = c->pod_spec; p.added.unsched = c->unschedulable; p.added.alloc = c->alloc;
+  p.removed = c->removed; p.name = c->name; p.nr = c->num_removed;
+  { const int rc = check_nodes(e, "cae_load_node_churn", p, false); if (rc) return rc; }
+  e->stats.h2d_bytes = 0;
+  const cae_node_delta* dl = p.dl;
+  const int nd = p.dirty.n, na = p.added.n, nr = p.nr;
+  if (!dl->num_new_values && !dl->num_new_labelsets && !dl->num_new_taint_lists && !nd && !na && !nr) return 0;
+  commit_nodes(e, p);
+  if (!nd && !na && !nr) return stage_nodes(e, p, {}, nullptr, nullptr);
+
+  // ---- the new row list on the host: survivors in their old order, the added nodes, the templates ----
+  Engine::NodeHost& nh = e->nh;
+  DynTables& dy = e->dyn;
+  const int oldN = e->N, T = e->T, N = oldN - nr + na, NT = N + T;
+  const int K = e->has_dynamic ? dy.K : 0;
+  std::vector<int32_t> src(NT), pod_cnt(N), key_val((size_t)K * N);
+  int r = 0;
+  for (int o = 0, ir = 0, id = 0; o < oldN; ++o) {
+    if (ir < nr && p.removed[ir] == o) { ++ir; continue; }
+    const bool dirty = id < nd && dl->row[id] == o;
+    src[r] = dirty ? -1 - id : o;
+    pod_cnt[r] = dirty ? dl->pod_off[id + 1] - dl->pod_off[id] : nh.pod_cnt[o];
+    for (int k = 0; k < K; ++k)
+      key_val[(size_t)k * N + r] = dirty ? label_of(nh, dl, dl->labelset[id], dy.key_id[k]) : nh.key_val[(size_t)k * oldN + o];
+    id += dirty;
+    ++r;
+  }
+  for (int j = 0; j < na; ++j, ++r) {
+    src[r] = -1 - (nd + j);
+    pod_cnt[r] = p.added.pod_off[j + 1] - p.added.pod_off[j];
+    for (int k = 0; k < K; ++k) key_val[(size_t)k * N + r] = label_of(nh, dl, p.added.labelset[j], dy.key_id[k]);
+  }
+  for (int t = 0; t < T; ++t) src[N + t] = oldN + t;
+  // topology domains of the new list, and the counter pool they size
+  std::vector<int32_t> dom((size_t)K * NT), qbo(1, 0), val(NT);
+  int Dc[DYN_MAX_KEYS] = {0}, D[DYN_MAX_KEYS] = {0};
+  for (int k = 0; k < K; ++k) {
+    std::copy(key_val.begin() + (size_t)k * N, key_val.begin() + (size_t)(k + 1) * N, val.begin());
+    std::copy(nh.tkey_val.begin() + (size_t)k * T, nh.tkey_val.begin() + (size_t)(k + 1) * T, val.begin() + N);
+    assign_domains(val.data(), N, NT, nh.dom_scratch, dom.data() + (size_t)k * NT, &Dc[k], &D[k]);
+  }
+  if (e->has_dynamic)
+    for (int q = 0; q < dy.Q; ++q) qbo.push_back(qbo.back() + Dc[nh.q_k[q]]);
+  NodeDeltaDev dd{};
+  std::vector<const char*> xd;
+  if (stage_nodes(e, p, {{src.data(), 4 * src.size()}, {dom.data(), 4 * dom.size()}, {qbo.data(), 4 * qbo.size()}}, &dd, &xd)) return -1;
+  nh.pod_cnt.swap(pod_cnt);
+  nh.key_val.swap(key_val);
+
+  // ---- device: node columns + resident CSR, then everything a load derives from the node list ----
+  if (launch_node_churn(e, dd, reinterpret_cast<const int32_t*>(xd[0]), N, p.total)) return -1;
+  e->N = N;
+  e->U = N + 2 * T;
+  if (devbuf_reserve(e, e->ch_pre, (size_t)std::max(e->SC, 1) * std::max(e->U, 1))) return -1;
+  e->d_pre_code = static_cast<uint8_t*>(e->ch_pre.p);
+  if (launch_class_matrix(e) || launch_pre_ok_bits(e)) return -1;
+  if (e->has_dynamic) {
+    const size_t Q1 = std::max(dy.Q, 1), pool = std::max(qbo.back(), 1);
+    size_t off = 0;
+    auto take = [&](size_t b) { const size_t o = off; off += (std::max<size_t>(b, 1) + 255) & ~(size_t)255; return o; };
+    const size_t o_dom = take(4 * dom.size()), o_qbo = take(4 * qbo.size()), o_cnt = take(4 * pool), o_pres = take(4 * pool);
+    const size_t o_elig = take(Q1 * std::max(e->U, 1));
+    if (devbuf_reserve(e, e->ch_dyn, off)) return -1;
+    char* b = static_cast<char*>(e->ch_dyn.p);
+    if (!dom.empty()) CAE_CUDA(cudaMemcpyAsync(b + o_dom, xd[1], 4 * dom.size(), cudaMemcpyDeviceToDevice, e->stream));
+    CAE_CUDA(cudaMemcpyAsync(b + o_qbo, xd[2], 4 * qbo.size(), cudaMemcpyDeviceToDevice, e->stream));
+    dy.dom = reinterpret_cast<const int32_t*>(b + o_dom);
+    dy.q_base_off = reinterpret_cast<const int32_t*>(b + o_qbo);
+    dy.base_cnt = reinterpret_cast<int32_t*>(b + o_cnt);
+    dy.base_pres = reinterpret_cast<int32_t*>(b + o_pres);
+    dy.elig = reinterpret_cast<uint8_t*>(b + o_elig);
+    dy.pool = qbo.back();
+    for (int k = 0; k < K; ++k) { dy.Dc[k] = Dc[k]; dy.D[k] = D[k]; }
+    if (launch_dynamic_recount(e, nullptr, e->U)) return -1;
     if (launch_post_bits(e)) return -1;
   }
   return 0;
@@ -919,6 +1135,14 @@ int32_t cae_load_nodes(cae_engine* h, const cae_node_delta* d) {
   if (!d) { cae::set_error("cae_load_nodes: no delta"); return -2; }
   cudaSetDevice(e->cfg.device);
   return cae::do_load_nodes(e, d);
+}
+
+int32_t cae_load_node_churn(cae_engine* h, const cae_node_churn* c) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_load_node_churn before cae_load"); return -2; }
+  if (!c) { cae::set_error("cae_load_node_churn: no churn"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_load_node_churn(e, c);
 }
 
 int32_t cae_feasibility(cae_engine* h, uint32_t* fit_bits, uint8_t* reasons, int32_t* fit_count) {

@@ -255,6 +255,7 @@ int launch_dynamic_tables(Engine* e, const uint8_t* d_spec_used, const int32_t* 
 // then every cluster-derived counter table from scratch.  Weights, classes, domains and the templates' DaemonSet weights
 // depend on neither the cluster rows nor their residents and stay.  The recount is the pass a load runs (one thread per
 // (counter, cluster node)); DESIGN.md §4 records why it is not an incremental subtract / add of the dirty rows.
+// cae_load_node_churn passes cols = NULL, ncols = U (every column) after it has rebuilt the domains and the counter pool.
 int launch_dynamic_recount(Engine* e, const int32_t* d_cols, int ncols) {
   DynTables& d = e->dyn;
   if (d.Q == 0) return 0;

@@ -216,7 +216,7 @@ struct Engine {
   PinnedBuf pending_stage;                // pend_spec | group_off, source of cae_load_pending's H2D copy
   std::vector<int64_t> h_spec_req;        // [num_podspecs][R]
   int num_podspecs = 0;
-  // host state of the last load that cae_load_nodes validates against and updates (node_delta in api.cu)
+  // host state of the last load that cae_load_nodes / cae_load_node_churn validate against and update (api.cu)
   struct NodeHost {
     int32_t num_values = 0, num_labelsets = 0, num_taint_lists = 0, taint_entries = 0;
     std::vector<int32_t> ls_off, ls_key, ls_val;   // resident label-set table, tails appended
@@ -225,12 +225,19 @@ struct Engine {
     std::vector<uint8_t> spec_used;                // [S] spec pending or resident (only grows between loads)
     std::vector<uint8_t> spec_anti;                // [S] spec has required anti-affinity terms
     std::vector<int32_t> key_val;                  // [K][N] value id of resident topology key k on cluster row n, -1 absent
+    std::vector<int32_t> tkey_val;                 // [K][T] the same on the templates (domain rebuild of a churn)
+    std::vector<int32_t> q_k;                      // [Q] topology key of each counter (its pool segment has Dc[q_k] entries)
+    std::vector<int32_t> dom_scratch;              // value id -> domain while the domains are assigned (all -1 in between)
   } nh;
   // buffers of cae_load_nodes (a cae_load points DevObjects back at its arena)
   DevBuf nd_tab[9];                       // grown dictionary tables: value_is_int, value_int, ls_off|key|val, taint_off|key|val|effect
   DevBuf nd_off[2], nd_spec[2];           // double-buffered resident CSR (node_pod_off / node_pod_spec)
-  DevBuf nd_cnt, nd_didx, nd_cub, nd_blob;  // per-row counts / dirty index, scan temp storage, device copy of the delta
+  DevBuf nd_cnt, nd_didx, nd_cub, nd_blob;  // per-row counts / source rows, scan temp storage, device copy of the delta
   PinnedBuf nd_stage;                     // the delta, source of its one H2D copy
+  // buffers of cae_load_node_churn: the tables whose size follows the node count, until the next cae_load
+  DevBuf ch_nodes[2];                     // double-buffered node columns [N+T] + c_free [A][N] + c_slots [N] (node_delta.cu)
+  DevBuf ch_pre;                          // pre_code [SC][U]
+  DevBuf ch_dyn;                          // dom [K][N+T] | q_base_off [Q+1] | base_cnt, base_pres [pool] | elig [Q][U]
   int sm_count = 132;
   int smem_optin = 227 * 1024;             // opt-in shared memory per thread block
   size_t hbm_bytes = (size_t)80 << 30;     // device memory (sizes the estimator's global slabs)
@@ -244,13 +251,16 @@ int pinned_reserve(Engine* e, Engine::PinnedBuf& b, size_t bytes);       // afte
 int launch_class_matrix(Engine* e);      // pre_code[SC][U]: needs only the object tables + the static classes
 int launch_class_matrix_cols(Engine* e, const int32_t* d_cols, int ncols);   // pre_code[SC][cols] only
 int launch_dynamic_recount(Engine* e, const int32_t* d_cols, int ncols);     // elig of cols, cluster counters, post_code, qrec
-struct NodeDeltaDev {                    // device views into the staged cae_node_delta (node_delta.cu)
-  int nd;
-  const int32_t *row, *labelset, *taint_list, *allowed, *cslots, *pod_off, *pod_spec;
+struct NodeDeltaDev {                    // device views into the staged rows of a delta or a churn (node_delta.cu)
+  int nd, na;                            // staged rows [0, nd) are dirty rows, [nd, nd + na) added nodes (churn)
+  const int32_t *row, *name;             // [nd] old row of a dirty row, [na] node name of an added one
+  const int32_t *labelset, *taint_list, *allowed, *cslots, *pod_off, *pod_spec;
   const uint8_t* unsched;
-  const int64_t *alloc, *cfree;          // [nd][R], [nd][A]
+  const int64_t *alloc, *cfree;          // [nd + na][R], [nd + na][A]
 };
 int launch_node_rows(Engine* e, const NodeDeltaDev& d, int64_t total);   // rows in place + resident CSR rebuilt into the spare buffer
+// cae_load_node_churn: node columns, run state and resident CSR of the new row list; src [N'+T] = old row, or -1 - staged row
+int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int N_new, int64_t total);
 int launch_pre_ok_bits(Engine* e);       // pre_ok[SC][Twp]: needs pre_code and the templates' pod slots
 int launch_post_bits(Engine* e);
 int launch_dynamic_tables(Engine* e, const uint8_t* d_spec_used, const int32_t* d_dc_ngroups);

@@ -473,6 +473,34 @@ class EncodedObjects:
                                     num_taint_lists=len(a["taint_off"]) - 1)
         return out
 
+    def apply_node_churn(self, churn: "NodeChurn") -> "EncodedObjects":
+        """The objects after cae_load_node_churn(churn), stated on the host: the tails and dirty rows of ``churn.changed``
+        applied (row numbers before the call), then the removed rows dropped and the added rows appended after the
+        surviving cluster rows, before the templates.  An added node has no capacity and no has_alloc_* (read for
+        templates only).  A cae_load of the result must answer like the engine after the churn."""
+        import copy
+        out = self.apply_node_delta(churn.changed) if churn.changed is not None else self
+        a, c = dict(out.arrays), churn.arrays
+        N = out.struct.num_cluster_nodes
+        na = len(c["name"])
+        keep = np.setdiff1d(np.arange(N), c["removed"])
+        zeros = {"node_cap_cpu": np.int64, "node_cap_mem": np.int64, "node_has_alloc_cpu": np.uint8, "node_has_alloc_mem": np.uint8}
+        added = {"node_name": c["name"], "node_labelset": c["labelset"], "node_taint_list": c["taint_list"],
+                 "node_unschedulable": c["unschedulable"], "node_allowed_pods": c["allowed_pods"], "node_alloc": c["alloc"]}
+        for nm in list(added) + list(zeros):
+            col = a[nm]
+            new = added[nm] if nm in added else np.zeros(na, zeros[nm])
+            a[nm] = np.ascontiguousarray(np.concatenate([col[keep], np.asarray(new, col.dtype).reshape((na,) + col.shape[1:]), col[N:]]))
+        off, spec, po = a["node_pod_off"], a["node_pod_spec"], c["pod_off"]
+        pieces = [spec[off[r]:off[r + 1]] for r in keep] + [c["pod_spec"][po[j]:po[j + 1]] for j in range(na)] + \
+                 [spec[off[r]:off[r + 1]] for r in range(N, len(off) - 1)]
+        a["node_pod_off"] = _i32(np.concatenate([[0], np.cumsum([len(p) for p in pieces], dtype=np.int64)]))
+        a["node_pod_spec"] = _i32(np.concatenate(pieces) if pieces else [])
+        res = copy.copy(out)
+        res.arrays = a
+        res.struct = out._restruct(a, num_cluster_nodes=len(keep) + na)
+        return res
+
     def _restruct(self, arrays, **counts) -> "capi.cae_objects":
         s = capi.cae_objects()
         C.memmove(C.byref(s), C.byref(self.struct), C.sizeof(s))
@@ -536,6 +564,49 @@ class NodeDelta:
     @property
     def num_dirty(self) -> int:
         return self.struct.num_dirty
+
+    def ptr(self):
+        return C.byref(self.struct)
+
+
+class NodeChurn:
+    """Owns the numpy arrays behind one ``cae_node_churn`` struct: ``changed`` (a NodeDelta with the dirty rows and the
+    dictionary tails the dirty and the added rows use, or None), the removed rows and the added nodes.  Field names are
+    the header's."""
+
+    _I32 = ("removed", "name", "labelset", "taint_list", "allowed_pods", "pod_off", "pod_spec")
+
+    def __init__(self, changed: Optional[NodeDelta] = None, **arrays) -> None:
+        a: Dict[str, np.ndarray] = {}
+        for nm in self._I32:
+            a[nm] = _i32(arrays.get(nm, [0] if nm == "pod_off" else []))
+        a["unschedulable"] = np.ascontiguousarray(arrays.get("unschedulable", np.zeros(len(a["name"]))), np.uint8)
+        na = len(a["name"])
+        a["alloc"] = np.ascontiguousarray(np.asarray(arrays.get("alloc", np.zeros((na, MAX_RES))), np.int64).reshape(na, MAX_RES))
+        self.arrays = a
+        self.changed = changed
+        s = capi.cae_node_churn()
+        s.abi_version = capi.CONST["CAE_ABI_VERSION"]
+        s.changed = C.pointer(changed.struct) if changed is not None else None
+        s.num_removed = len(a["removed"])
+        s.num_added = na
+        for name, ctype in capi.cae_node_churn._fields_:
+            if name in a:
+                setattr(s, name, a[name].ctypes.data_as(ctype))
+        self.struct = s
+
+    def replace(self, **arrays) -> "NodeChurn":
+        """A copy with some arrays (or ``changed``) replaced (the counts follow the arrays)."""
+        changed = arrays.pop("changed", self.changed)
+        return NodeChurn(changed, **{**self.arrays, **arrays})
+
+    @property
+    def num_removed(self) -> int:
+        return self.struct.num_removed
+
+    @property
+    def num_added(self) -> int:
+        return self.struct.num_added
 
     def ptr(self):
         return C.byref(self.struct)
@@ -722,6 +793,11 @@ class Encoder:
         self._emitted = (enc.struct.num_values, enc.struct.num_labelsets, enc.struct.num_taint_lists)
         self._delta_ok = True
         self._spec_wo_name: Optional[Dict[tuple, int]] = None
+        # the cluster rows the engine holds: (node-name id, row state) per row, kept current by node_delta / node_churn
+        b, off = self.b, self.b.node_pod_off
+        self._cluster = [(b.node_rows[r][0], (b.node_rows[r][1], b.node_rows[r][2], b.node_rows[r][3], tuple(b.node_alloc[r]),
+                                              b.node_rows[r][4], tuple(b.node_pod_spec[off[r]:off[r + 1]])))
+                         for r in range(b.num_cluster_nodes)]
         return enc
 
     def _resident_spec(self, pod: Pod) -> int:
@@ -756,44 +832,109 @@ class Encoder:
         NodeDelta against what the engine holds.  The interner stays append-only; the values, label sets and taint lists
         the changed rows add since the last load or delta become the delta's tails.  Unsupported = use a full load (and
         a fresh Encoder: this one no longer matches the engine)."""
+        self._check_resident()
+        items = sorted(changed, key=lambda x: x[0])
+        rows: List[int] = []
+        states = []
+        for row, ni in items:
+            if not 0 <= row < len(self._cluster) or (rows and row == rows[-1]):
+                raise ValueError("node delta row %d: not a cluster node of the last load, or given twice" % row)
+            if self.node_names.ids.get(ni.node.name) != self._cluster[row][0]:
+                self._delta_ok = False
+                raise Unsupported("row %d is no longer node %s" % (row, ni.node.name))
+            rows.append(row)
+            states.append(self._row_state(ni))
+        delta = self._tails_and_rows(rows, states)
+        for row, st in zip(rows, states):
+            self._cluster[row] = (self._cluster[row][0], st)
+        return delta
+
+    def _check_resident(self) -> None:
+        """Unsupported unless the interner still matches what the engine holds."""
         if not getattr(self, "_delta_ok", False):
             raise Unsupported("no load to apply a node delta to, or an earlier delta was refused")
-        b = self.b
-        nv0, nl0, nt0 = self._emitted
-        if len(b.value_is_int) < nv0:
+        if len(self.b.value_is_int) < self._emitted[0]:
             self._delta_ok = False
             raise Unsupported("the value table of the last load was padded")
+
+    def _row_state(self, ni: NodeInfo) -> tuple:
+        """(label set, taint list, unschedulable, allocatable, allowed pods, resident specs) of a cluster node, interned
+        append-only against the last load."""
+        n, b = ni.node, self.b
         nres = len(self.resources)
-        items = sorted(changed, key=lambda x: x[0])
-        rows, lsets, tlists, unsched, alloc, allowed, pod_off, pod_spec = [], [], [], [], [], [], [0], []
-        for row, ni in items:
-            if not 0 <= row < b.num_cluster_nodes or (rows and row == rows[-1]):
-                raise ValueError("node delta row %d: not a cluster node of the last load, or given twice" % row)
-            n = ni.node
-            if self.node_names.ids.get(n.name) != b.node_rows[row][0]:
-                self._delta_ok = False
-                raise Unsupported("row %d is no longer node %s" % (row, n.name))
-            tl = b.taint_list([(self._key(t.key), self._val(t.value) if t.value else -1, _EFFECTS[t.effect]) for t in n.taints])
-            ls = self._labelset(n.labels)
-            vec = self._resource_vec(n.allocatable)
-            if len(self.resources) > nres:
-                self._delta_ok = False
-                raise Unsupported("node %s has a resource the last load did not have" % n.name)
-            specs = [self._resident_spec(p) for p in ni.pods]
-            rows.append(row); lsets.append(ls); tlists.append(tl); unsched.append(int(n.unschedulable))
-            alloc.append(vec); allowed.append(int(n.allocatable.get("pods", 0)))
-            pod_spec.extend(specs); pod_off.append(len(pod_spec))
+        tl = b.taint_list([(self._key(t.key), self._val(t.value) if t.value else -1, _EFFECTS[t.effect]) for t in n.taints])
+        ls = self._labelset(n.labels)
+        vec = self._resource_vec(n.allocatable)
+        if len(self.resources) > nres:
+            self._delta_ok = False
+            raise Unsupported("node %s has a resource the last load did not have" % n.name)
+        specs = tuple(self._resident_spec(p) for p in ni.pods)
+        return (ls, tl, int(n.unschedulable), tuple(vec), int(n.allocatable.get("pods", 0)), specs)
+
+    def _tails_and_rows(self, rows: Sequence[int], states: Sequence[tuple]) -> NodeDelta:
+        """The NodeDelta of dirty rows `rows` with row states `states`, carrying as tails what the interner added since the
+        last load or delta."""
+        b = self.b
+        nv0, nl0, nt0 = self._emitted
+        pod_off, pod_spec = [0], []
+        for st in states:
+            pod_spec.extend(st[5])
+            pod_off.append(len(pod_spec))
         L, Tn = b.labelsets, b.taints
         lp0, tp0 = L.off[nl0], Tn.off[nt0]
         delta = NodeDelta(
             value_is_int=b.value_is_int[nv0:], value_int=b.value_int[nv0:],
             ls_off=[o - lp0 for o in L.off[nl0:]], ls_key=L.cols[0][lp0:], ls_val=L.cols[1][lp0:],
             taint_off=[o - tp0 for o in Tn.off[nt0:]], taint_key=Tn.cols[0][tp0:], taint_val=Tn.cols[1][tp0:],
-            taint_effect=Tn.cols[2][tp0:], row=rows, labelset=lsets, taint_list=tlists, unschedulable=unsched,
-            alloc=np.asarray(alloc, np.int64).reshape(len(rows), MAX_RES), allowed_pods=allowed, pod_off=pod_off,
-            pod_spec=pod_spec)
+            taint_effect=Tn.cols[2][tp0:], row=rows, labelset=[st[0] for st in states], taint_list=[st[1] for st in states],
+            unschedulable=[st[2] for st in states], alloc=np.asarray([st[3] for st in states], np.int64).reshape(len(rows), MAX_RES),
+            allowed_pods=[st[4] for st in states], pod_off=pod_off, pod_spec=pod_spec)
         self._emitted = (len(b.value_is_int), L.n, Tn.n)
         return delta
+
+    def node_churn(self, new_cluster: Sequence[NodeInfo]) -> "NodeChurn":
+        """The shim's side of cae_load_node_churn: the complete new cluster-node list as a NodeChurn against what the engine
+        holds.  Nodes are matched by name: names that are gone are removed, new names are added, survivors whose state
+        changed become dirty rows.  The survivors must keep their relative order and the new nodes must all come after
+        them (Unsupported otherwise: a full load).  Resident specs are found as for node_delta."""
+        self._check_resident()
+        old = {nid: r for r, (nid, _) in enumerate(self._cluster)}
+        names = [ni.node.name for ni in new_cluster]
+        if len(set(names)) != len(names):
+            raise ValueError("node churn: a node name is given twice")
+        last, seen_new = -1, False
+        for nm in names:
+            r = old.get(self.node_names.ids.get(nm, -1))
+            if r is None:
+                seen_new = True
+            elif seen_new or r < last:
+                raise Unsupported("node churn: the surviving nodes are reordered or a new node comes before one of them")
+            else:
+                last = r
+        kept = {old[self.node_names.ids[nm]] for nm in names if self.node_names.ids.get(nm, -1) in old}
+        removed = [r for r in range(len(self._cluster)) if r not in kept]
+        rows, dirty_states, new_list, added = [], [], [], []
+        for ni in new_cluster:
+            st = self._row_state(ni)
+            r = old.get(self.node_names.ids.get(ni.node.name, -1))
+            if r is None:
+                nid = self.node_names(ni.node.name)
+                added.append((nid, st))
+                continue
+            if st != self._cluster[r][1]:
+                rows.append(r)
+                dirty_states.append(st)
+            new_list.append((self._cluster[r][0], st))
+        changed = self._tails_and_rows(rows, dirty_states)
+        po = [0]
+        for _, st in added:
+            po.append(po[-1] + len(st[5]))
+        churn = NodeChurn(changed, removed=removed, name=[nid for nid, _ in added], labelset=[st[0] for _, st in added],
+                          taint_list=[st[1] for _, st in added], unschedulable=[st[2] for _, st in added],
+                          alloc=np.asarray([st[3] for _, st in added], np.int64).reshape(len(added), MAX_RES),
+                          allowed_pods=[st[4] for _, st in added], pod_off=po, pod_spec=[x for _, st in added for x in st[5]])
+        self._cluster = new_list + added
+        return churn
 
 
 def encode(cluster: Sequence[NodeInfo], templates: Sequence[NodeInfo],

@@ -154,6 +154,16 @@ class Engine:
         self._check(rc)
         return True
 
+    def load_node_churn(self, churn) -> bool:
+        """The per-tick delta of the cluster-node list (cae_load_node_churn): removed and added cluster nodes plus the
+        dirty rows of the survivors (encode.NodeChurn).  Returns False when the engine answers "use a full load" (status 2);
+        the engine is unchanged then."""
+        rc = self.lib.cae_load_node_churn(self.h, churn.ptr())
+        if rc == 2:
+            return False
+        self._check(rc)
+        return True
+
     def feasibility(self, want_bits: bool = True):
         """Dense pods x templates pass. Returns (fit_bits [T][ceil(Pl/32)] uint32 | None,
         reasons [T][Pl] uint8 | None, fit_count [T] int32) for this rank's pod shard."""

@@ -371,3 +371,84 @@ def node_churn(enc: EncodedObjects, seed: int, n_dirty: int, bind: float = 0.3, 
     new_go = np.concatenate([[0], np.cumsum(left)]).astype(np.int32)
     pending = enc.with_pending(a["pend_spec"][keep.astype(np.int64)], new_go)
     return delta, pending
+
+
+def node_scale(enc: EncodedObjects, seed: int, n_remove: int, n_add: int, n_dirty: int = 0):
+    """A deterministic random tick that changes the cluster-node list of a snapshot of ``generate``: ``n_remove`` random
+    cluster rows leave, ``n_add`` nodes shaped like the generator's cluster nodes join, and ``n_dirty`` other rows change
+    as in ``node_churn`` (same seed).  Every added node has a new hostname value; about one in four has a new zone value
+    (a domain appears); when ``n_remove`` allows, the removals include every node of the smallest zone (a domain
+    disappears).  Residents of the added nodes are drawn from the specs resident at the load; allowed pods stay above the
+    resident count (DESIGN.md §4).
+    Returns (churn, pending): the NodeChurn and ``enc`` with the pods bound by the dirty rows removed from the pending rows.
+    ``pending.apply_node_churn(churn)`` is the snapshot after the tick."""
+    from .encode import NodeChurn, NodeDelta
+    a, s = enc.arrays, enc.struct
+    N = s.num_cluster_nodes
+    delta, pending = node_churn(enc, seed, n_dirty) if n_dirty else (None, enc)
+    dirty = set(int(r) for r in delta.arrays["row"]) if delta is not None else set()
+    rng = SplitMix64(0x5CA1E000 + seed)
+    # removals: the smallest zone first (when it fits), then random clean rows
+    zone = np.full(N, -1, np.int64)
+    for r in range(N):
+        ls = int(a["node_labelset"][r])
+        for i in range(a["ls_off"][ls], a["ls_off"][ls + 1]):
+            if a["ls_key"][i] == K_ZONE:
+                zone[r] = a["ls_val"][i]
+    clean = [r for r in range(N) if r not in dirty]
+    n_remove = min(n_remove, len(clean))
+    removed: List[int] = []
+    zones, counts = np.unique(zone[zone >= 0], return_counts=True)
+    if len(zones):
+        z = int(zones[int(np.argmin(counts))])
+        members = [r for r in range(N) if zone[r] == z]
+        if members and all(r not in dirty for r in members) and len(members) <= n_remove:
+            removed = members
+    rest = [r for r in clean if r not in set(removed)]
+    order = rng.next(len(rest)).argsort() if rest else np.zeros(0, np.int64)
+    removed = sorted(removed + [rest[int(i)] for i in order[:n_remove - len(removed)]])
+    # dictionary tails: those of the dirty rows, then new hostname / zone values and the added nodes' label sets
+    nv0 = s.num_values + (delta.struct.num_new_values if delta is not None else 0)
+    nl0 = s.num_labelsets + (delta.struct.num_new_labelsets if delta is not None else 0)
+    nt = s.num_taint_lists + (delta.struct.num_new_taint_lists if delta is not None else 0)
+    new_zone = nv0 + n_add          # one new zone value shared by the nodes that take it
+    vcpu = rng.choice(max(n_add, 1), [2, 4, 8, 16, 32, 64, 96], [1] * 7).astype(np.int64)
+    mem_per = rng.choice(max(n_add, 1), [2, 4, 8], [1, 1, 1]).astype(np.int64)
+    ngpu = np.where(rng.uniform(max(n_add, 1)) < 0.15, rng.choice(max(n_add, 1), [1, 4, 8], [1, 1, 1]), 0).astype(np.int64)
+    u = rng.uniform(max(n_add, 1))
+    zr, pr, tr, nres = (rng.randint(max(n_add, 1), h) for h in (16, 8, max(nt, 1), 31))
+    resident_pool = a["node_pod_spec"]
+    name0 = int(a["node_name"].max()) + 1 if len(a["node_name"]) else 0
+    ls_items, names, tls, allocs, allowed, pod_off, pod_spec = [], [], [], [], [], [0], []
+    for j in range(n_add):
+        v = int(vcpu[j])
+        z = new_zone if u[j] < 0.25 else int(zr[j])
+        ls_items.append(((K_HOST, nv0 + j), (K_ZONE, z), (K_POOL, 16 + int(pr[j])), (K_ITYPE, 24 + v % 24)))
+        names.append(name0 + j)
+        tls.append(int(tr[j]) if nt else 0)
+        cap_mem = v * int(mem_per[j]) * GiB
+        allocs.append([v * 1000 - RESERVED[v], cap_mem - cap_mem // 20, 0, int(ngpu[j])])
+        k = int(nres[j]) if len(resident_pool) else 0
+        pods = [int(resident_pool[i]) for i in rng.randint(k, len(resident_pool))] if k else []
+        pod_spec.extend(pods)
+        pod_off.append(len(pod_spec))
+        allowed.append(max(110, len(pods) + 1))
+    n_new_vals = n_add + (1 if n_add else 0)
+    ls_off = list(delta.arrays["ls_off"]) if delta is not None else [0]
+    for it in ls_items:
+        ls_off.append(ls_off[-1] + len(it))
+    changed_arrays = dict(delta.arrays) if delta is not None else {}
+    changed_arrays.update(
+        value_is_int=np.concatenate([changed_arrays.get("value_is_int", np.zeros(0, np.uint8)), np.zeros(n_new_vals, np.uint8)]),
+        value_int=np.concatenate([changed_arrays.get("value_int", np.zeros(0, np.int64)), np.zeros(n_new_vals, np.int64)]),
+        ls_off=ls_off,
+        ls_key=np.concatenate([changed_arrays.get("ls_key", np.zeros(0, np.int32)), [k for it in ls_items for k, _ in it]]),
+        ls_val=np.concatenate([changed_arrays.get("ls_val", np.zeros(0, np.int32)), [v for it in ls_items for _, v in it]]))
+    changed = NodeDelta(**changed_arrays)
+    alloc = np.zeros((n_add, len(a["node_alloc"][0]) if len(a["node_alloc"]) else 8), np.int64)
+    if n_add:
+        alloc[:, :4] = np.asarray(allocs, np.int64)
+    churn = NodeChurn(changed, removed=removed, name=names, labelset=[nl0 + j for j in range(n_add)], taint_list=tls,
+                      unschedulable=np.zeros(n_add, np.uint8), alloc=alloc, allowed_pods=allowed, pod_off=pod_off,
+                      pod_spec=pod_spec)
+    return churn, pending

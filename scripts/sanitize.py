@@ -6,7 +6,8 @@ self-cleaning accumulators, last-block election, shared-memory state and block-w
     compute-sanitizer --tool racecheck python scripts/sanitize.py
 
 Dense pass (K1, both variants), Estimate() of every template (K0 + K3: plain closed form, capacity form with the cluster
-fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals) — on miniatures of C2, C3 and C4 — each checked
+fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals), a cluster-node delta
+(cae_load_nodes) and a cluster-node churn (cae_load_node_churn) — on miniatures of C2, C3 and C4 — each checked
 against the CPU oracle so that a "clean" run also means "correct results under the tool"."""
 import os
 import sys
@@ -62,6 +63,19 @@ def main():
             move_off = np.minimum(np.arange(n + 1, dtype=np.int32) * 4, len(order_p)).astype(np.int32)
             eng.simulate_removals(cand, move_off, order_p[:move_off[-1]], persist=True)
             got = eng.filter_schedulable(order_p)
+            assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
+            # cluster-node churn (cae_load_node_churn: column gather, CSR rebuild, domains, full class matrix, recount)
+            churn, pending = synth.node_scale(after, cfg, 4, 4, 6)
+            assert eng.load_node_churn(churn) and eng.load_pending(pending)
+            after = pending.apply_node_churn(churn)
+            eng.enc = after
+            _, reasons, _ = eng.feasibility()
+            assert np.array_equal(reasons, pyoracle.feasibility_dense(after)[0])
+            caps = np.full(after.T, 30, np.int32)
+            got_e, ref_e = eng.estimate_all(caps), pyoracle.estimate_all(after, caps)
+            assert all(np.array_equal(x, y) for x, y in zip(got_e, ref_e[:4]))
+            got = eng.filter_schedulable(order_p)
+            ref = pyoracle.filter_schedulable(after, order_p)
             assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
         print("config", cfg, "ok: nodes", int(nc.sum()), "pods", int(pc.sum()), flush=True)
     eng.close()
