@@ -315,7 +315,7 @@ int32_t cae_load_pending(cae_engine* e, int32_t num_pending, const int32_t* pend
  *     resident) at the last cae_load — it could add an existing-anti-affinity counter;
  *   - the resident pods of all nodes, or the entries of a dictionary table, would pass 2^31 - 1 (checked from the counts
  *     and offsets alone, before any pod-spec id is read).
- * Adding or removing nodes: cae_load_node_churn.  Template changes and pod specs the last cae_load did not have cannot be
+ * Adding or removing nodes: cae_load_node_churn.  New pod specs: cae_load_pods first.  Template changes cannot be
  * expressed: cae_load.
  * The interner is append-only across deltas: hostname_key and unschedulable_taint_key stay those of the last cae_load (a
  * caller that needs them to change does a full load). */
@@ -385,6 +385,108 @@ typedef struct cae_node_churn {
   const int32_t* pod_spec;         /* resident pod-spec ids */
 } cae_node_churn;
 int32_t cae_load_node_churn(cae_engine* e, const cae_node_churn* c);
+
+/* The per-tick delta of the pod specs: new pod specs (a new Deployment, a rollout, a Job) and the complete new pending list
+ * against the snapshot that is already resident.  The dictionary entries the new specs need arrive as TAILS that continue
+ * the resident tables (ids [resident count, resident count + n)); the offsets of a tail start at 0 and index that
+ * tail's own child table (ls_off -> its pairs, sel_req_off -> its requirements, aff_off -> its terms, ...).  The new specs
+ * get ids [num_podspecs, num_podspecs + num_new_specs).
+ * After the call every entry point (dense pass, group reasons, estimate_all(_ex), waste and price scores,
+ * cae_filter_schedulable, cae_simulate_removals) answers bit-identically to a cae_load of the resident objects with the
+ * tails and specs appended and this pending list: the engine reruns the derivation a load runs on the pending set over
+ * the resident node side, which is neither uploaded nor recomputed.  Any spec may be pending (also one that was only
+ * resident), the grouping may change in any way, and P and E may exceed those of the load.  Nodes and templates are not
+ * touched; the call combines with cae_load_pending, cae_load_nodes and cae_load_node_churn in any order, and a later node
+ * call's tails continue after this call's.  Afterwards a node call may name the new specs as resident pods, and the rules
+ * those calls state relative to "the last cae_load" (cae_load_pending's pending-spec check, the anti-affinity refusal of
+ * the node calls) are judged against the last cae_load or cae_load_pods.  The pending list has the meaning (and, under
+ * CAE_CFG_PODS_PRESHARDED, the sharding) it has in cae_objects.  Every check runs on the host before any device write.
+ * Status -2 (malformed, nothing changed): NULL arrays with non-zero counts, ids outside the resident table plus its tail,
+ *   offsets that do not start at 0 or decrease, a tail's offsets past its child tail, label pairs not sorted by strictly
+ *   increasing key id, enum fields out of range, group_off not covering pend_spec.
+ * Status 1 (nothing changed): a limit for which cae_load answers status 1 (more than 8 topology keys, more than 12
+ *   counters for one pod, more than 64 host-port sets, the width of the rank encoding): use the stock path.
+ * Status 2 (nothing changed): a table would pass 2^31 - 1 entries (checked from the counts and offsets alone), or a new
+ *   spec requests a dim at or past the load's num_res (a new resource dimension): cae_load.
+ * Node-name ids (ps_node_name, field_node_name) are an open id space, as in cae_objects: only -1 / >= 0 is checked.
+ * Template changes and label changes of an existing Namespace: cae_load. */
+typedef struct cae_pod_delta {
+  int32_t abi_version; /* CAE_ABI_VERSION */
+  int32_t num_new_values;
+  const uint8_t* value_is_int;
+  const int64_t* value_int;
+  int32_t num_new_namespaces;
+  const int32_t* ns_labelset;
+  const uint8_t* ns_exists;
+  int32_t num_new_labelsets;
+  const int32_t* ls_off; /* [num_new_labelsets + 1] */
+  const int32_t* ls_key;
+  const int32_t* ls_val;
+  int32_t num_new_reqs;
+  const int32_t* req_key;
+  const int32_t* req_op;
+  const int32_t* req_val_off; /* [num_new_reqs + 1] */
+  const int32_t* req_vals;
+  int32_t num_new_selectors;
+  const int32_t* sel_kind;
+  const int32_t* sel_req_off; /* [num_new_selectors + 1] -> the requirement tail */
+  int32_t num_new_naff;
+  const int32_t* naff_nodesel;
+  const uint8_t* naff_has_required;
+  const int32_t* naff_term_off; /* [num_new_naff + 1] -> the term tail */
+  int32_t num_new_naff_terms;
+  const int32_t* term_expr_sel;
+  const int32_t* term_field_off; /* [num_new_naff_terms + 1] */
+  const int32_t* field_op;
+  const int32_t* field_node_name;
+  int32_t num_new_tol_lists;
+  const int32_t* tol_off; /* [num_new_tol_lists + 1] */
+  const int32_t* tol_key;
+  const int32_t* tol_op;
+  const int32_t* tol_val;
+  const int32_t* tol_effect;
+  int32_t num_new_port_lists;
+  const int32_t* port_off; /* [num_new_port_lists + 1] */
+  const int32_t* port_ip;
+  const int32_t* port_proto;
+  const int32_t* port_num;
+  int32_t num_new_pts_lists;
+  const int32_t* pts_off; /* [num_new_pts_lists + 1] */
+  const int32_t* pts_max_skew;
+  const int32_t* pts_key;
+  const int32_t* pts_selector;
+  const int32_t* pts_min_domains;
+  const int32_t* pts_node_affinity_policy;
+  const int32_t* pts_node_taints_policy;
+  int32_t num_new_aff_lists;
+  const int32_t* aff_off; /* [num_new_aff_lists + 1] -> the term tail */
+  int32_t num_new_aterms;
+  const int32_t* aterm_selector;
+  const int32_t* aterm_key;
+  const int32_t* aterm_ns_off; /* [num_new_aterms + 1] */
+  const int32_t* aterm_ns;
+  const int32_t* aterm_ns_selector;
+  /* pod specs [num_podspecs, num_podspecs + num_new_specs): the columns of cae_objects */
+  int32_t num_new_specs;
+  const int32_t* ps_namespace;
+  const int32_t* ps_labelset;
+  const int64_t* ps_req; /* [num_new_specs * CAE_MAX_RES] */
+  const int32_t* ps_tol_list;
+  const int32_t* ps_naff;
+  const int32_t* ps_node_name;
+  const int32_t* ps_port_list;
+  const int32_t* ps_pts_list;
+  const int32_t* ps_aff_list;
+  const int32_t* ps_anti_list;
+  const uint8_t* ps_terminating;
+  const uint8_t* ps_hostname_spread;
+  /* the complete new pending list */
+  int32_t num_groups;
+  int32_t num_pending;
+  const int32_t* group_off; /* [num_groups + 1] */
+  const int32_t* pend_spec; /* [num_pending] */
+} cae_pod_delta;
+int32_t cae_load_pods(cae_engine* e, const cae_pod_delta* d);
 
 int32_t cae_feasibility(cae_engine* e, uint32_t* fit_bits, uint8_t* reasons, int32_t* fit_count);
 

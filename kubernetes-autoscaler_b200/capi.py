@@ -100,6 +100,10 @@ class cae_node_churn(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_node_churn", {"cae_node_delta": cae_node_delta})
 
 
+class cae_pod_delta(C.Structure):
+    _fields_ = _parse_struct(_SRC, "cae_pod_delta")
+
+
 def declared_functions() -> List[str]:
     """Names of every function the header declares (used by the symbol-export test)."""
     return sorted(set(re.findall(r"\b(cae_\w+)\s*\(", _SRC)))
@@ -153,6 +157,8 @@ def load_engine_lib() -> C.CDLL:
     lib.cae_load_nodes.restype = C.c_int32
     lib.cae_load_node_churn.argtypes = [C.c_void_p, P(cae_node_churn)]
     lib.cae_load_node_churn.restype = C.c_int32
+    lib.cae_load_pods.argtypes = [C.c_void_p, P(cae_pod_delta)]
+    lib.cae_load_pods.restype = C.c_int32
     lib.cae_feasibility.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.cae_feasibility.restype = C.c_int32
     lib.cae_feasibility_groups.argtypes = [C.c_void_p, C.c_void_p]

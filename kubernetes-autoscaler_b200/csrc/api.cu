@@ -87,17 +87,17 @@ int pinned_reserve(Engine* e, Engine::PinnedBuf& b, size_t bytes) {
 }
 
 template <class T>
-static int upload(Engine* e, const T* host, size_t n, const T** dev) {
+static int upload(Arena& a, const T* host, size_t n, const T** dev) {
   void *p = nullptr, *h = nullptr;
-  if (e->up.alloc(&p, &h, n * sizeof(T))) return -1;
+  if (a.alloc(&p, &h, n * sizeof(T))) return -1;
   if (n) memcpy(h, host, n * sizeof(T));
   *dev = static_cast<const T*>(p);
   return 0;
 }
 template <class T>
-static int upload_mut(Engine* e, const std::vector<T>& v, T** dev) {
+static int upload_mut(Arena& a, const std::vector<T>& v, T** dev) {
   const T* p = nullptr;
-  if (upload(e, v.data(), v.size(), &p)) return -1;
+  if (upload(a, v.data(), v.size(), &p)) return -1;
   *dev = const_cast<T*>(p);
   return 0;
 }
@@ -114,7 +114,7 @@ static int dev_alloc(Engine* e, T** dev, size_t n, bool zero = false) {
 }
 
 #define UP(field, count)                                                           \
-  if (upload(e, o->field, (size_t)(count), &e->dobj.field)) return -1
+  if (upload(e->up, o->field, (size_t)(count), &e->dobj.field)) return -1
 
 static bool host_label(const cae_objects* o, int ls, int key, int* val) {
   for (int i = o->ls_off[ls]; i < o->ls_off[ls + 1]; ++i)
@@ -142,22 +142,41 @@ static void assign_domains(const int32_t* val, int N, int NT, std::vector<int32_
   for (int row = 0; row < NT; ++row) if (val[row] >= 0) id_of[val[row]] = -1;
 }
 
+// What the pending-side derivation (derive_pending) works out on the host before it changes any engine state: the classes
+// of the pending specs, the dynamic tables and the rank encoding.  Every status-1 limit is met while this is filled in.
+struct PendPlan {
+  std::vector<uint8_t> spec_pending, spec_used;
+  std::vector<StaticClass> sclass;
+  std::vector<int32_t> spec_sc, spec_dc, pc_of;
+  bool any = false;                               // dynamic tables
+  DynTables dyn;
+  std::vector<int32_t> key_val, tkey_val, dom, dc_spec, dc_sc, dc_q_off, dc_ngroups, q_k, q_dc, q_p0, q_base_off;
+  std::vector<uint8_t> q_kind;
+  int A = 0, W = 0, act_dim[CAE_MAX_RES] = {0};   // rank encoding
+  int f_word[CAE_MAX_RES] = {0}, f_shift[CAE_MAX_RES] = {0}, f_bits[CAE_MAX_RES] = {0};
+  std::vector<std::vector<int64_t>> rvals;
+  RankArgs ra{};                                  // the device half (pod_delta.cu)
+  const int64_t* d_rvals = nullptr;
+  uint32_t* d_tmpl_w = nullptr;
+};
+
 // Interning for the pod-state dependent plugins (dyn.cuh): topology keys -> compact ids, label values
 // -> domain indices, pod specs -> dynamic classes, and the list of counters each class needs.
 // Structure only; every match / count is computed on the device (dyn_kernels.cu).
-static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint8_t>& spec_pending,
-                         const std::vector<int32_t>& spec_sc, std::vector<int32_t>& spec_dc) {
-  DynTables& d = e->dyn;
-  d = DynTables();
+static int plan_dynamic(Engine* e, const cae_objects* o, const std::vector<uint8_t>* resident, PendPlan& pl) {
+  DynTables& d = pl.dyn;
   const int N = e->N, T = e->T, NT = N + T, S = o->num_podspecs;
+  const std::vector<uint8_t>& spec_pending = pl.spec_pending;
+  const std::vector<int32_t>& spec_sc = pl.spec_sc;
+  std::vector<int32_t>& spec_dc = pl.spec_dc;
   d.S = S;
   auto nonempty = [&](const int32_t* off, int l) { return off[l + 1] > off[l]; };
-  std::vector<uint8_t> spec_used(spec_pending);
-  for (int i = 0; i < o->node_pod_off[NT]; ++i) spec_used[o->node_pod_spec[i]] = 1;
-  e->nh.spec_used = spec_used;
-  e->nh.key_val.clear();
-  e->nh.tkey_val.clear();
-  e->nh.q_k.clear();
+  std::vector<uint8_t>& spec_used = pl.spec_used;
+  spec_used = spec_pending;
+  if (resident)
+    for (int s = 0; s < S; ++s) spec_used[s] |= (*resident)[s];
+  else
+    for (int i = 0; i < o->node_pod_off[NT]; ++i) spec_used[o->node_pod_spec[i]] = 1;
   bool any = false;
   std::vector<int> keys;
   auto add_key = [&](int key) { if (std::find(keys.begin(), keys.end(), key) == keys.end()) keys.push_back(key); };
@@ -171,17 +190,19 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
       if (std::find(exist_keys.begin(), exist_keys.end(), o->aterm_key[t]) == exist_keys.end()) exist_keys.push_back(o->aterm_key[t]);
     }
     if (!spec_pending[s]) continue;
-    int pl = o->ps_pts_list[s], fl = o->ps_aff_list[s];
-    for (int c = o->pts_off[pl]; c < o->pts_off[pl + 1]; ++c) { any = true; add_key(o->pts_key[c]); }
+    int pl_ = o->ps_pts_list[s], fl = o->ps_aff_list[s];
+    for (int c = o->pts_off[pl_]; c < o->pts_off[pl_ + 1]; ++c) { any = true; add_key(o->pts_key[c]); }
     for (int t = o->aff_off[fl]; t < o->aff_off[fl + 1]; ++t) { any = true; add_key(o->aterm_key[t]); }
   }
-  e->has_dynamic = any;
+  pl.any = any;
   if (!any) return 0;
   if ((int)keys.size() > DYN_MAX_KEYS) { set_error("more than 8 distinct topology keys"); return 1; }
   d.K = (int)keys.size();
-  std::vector<int32_t> dom((size_t)d.K * NT, -1), val(NT);
-  e->nh.key_val.assign((size_t)d.K * N, -1);
-  e->nh.tkey_val.assign((size_t)d.K * T, -1);
+  std::vector<int32_t>& dom = pl.dom;
+  std::vector<int32_t> val(NT);
+  dom.assign((size_t)d.K * NT, -1);
+  pl.key_val.assign((size_t)d.K * N, -1);
+  pl.tkey_val.assign((size_t)d.K * T, -1);
   for (int k = 0; k < d.K; ++k) {
     d.key_id[k] = keys[k];
     d.is_host[k] = keys[k] == o->hostname_key;
@@ -189,22 +210,23 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
       int v;
       val[row] = host_label(o, o->node_labelset[row], keys[k], &v) ? v : -1;
     }
-    std::copy(val.begin(), val.begin() + N, e->nh.key_val.begin() + (size_t)k * N);
-    std::copy(val.begin() + N, val.end(), e->nh.tkey_val.begin() + (size_t)k * T);
+    std::copy(val.begin(), val.begin() + N, pl.key_val.begin() + (size_t)k * N);
+    std::copy(val.begin() + N, val.end(), pl.tkey_val.begin() + (size_t)k * T);
     assign_domains(val.data(), N, NT, e->nh.dom_scratch, dom.data() + (size_t)k * NT, &d.Dc[k], &d.D[k]);
   }
   auto kidx = [&](int key) { return (int)(std::find(keys.begin(), keys.end(), key) - keys.begin()); };
   // dynamic classes
   std::map<std::tuple<int, int, int, int, int, int>, int> dc_ids;
-  std::vector<int32_t> dc_spec(1, 0), dc_sc(1, 0), dc_q_off(1, 0), dc_ngroups(1, 0);
-  std::vector<uint8_t> q_kind;
-  std::vector<int32_t> q_k, q_dc, q_p0, q_base_off(1, 0);
+  std::vector<int32_t> &dc_spec = pl.dc_spec, &dc_sc = pl.dc_sc, &dc_q_off = pl.dc_q_off, &dc_ngroups = pl.dc_ngroups;
+  std::vector<uint8_t>& q_kind = pl.q_kind;
+  std::vector<int32_t> &q_k = pl.q_k, &q_dc = pl.q_dc, &q_p0 = pl.q_p0, &q_base_off = pl.q_base_off;
+  dc_spec.assign(1, 0); dc_sc.assign(1, 0); dc_q_off.assign(1, 0); dc_ngroups.assign(1, 0); q_base_off.assign(1, 0);
   dc_q_off.push_back(0);
   for (int s = 0; s < S; ++s) {
     if (!spec_pending[s]) continue;
-    int pl = o->ps_pts_list[s], fl = o->ps_aff_list[s], al = o->ps_anti_list[s];
-    if (!nonempty(o->pts_off, pl) && !nonempty(o->aff_off, fl) && !nonempty(o->aff_off, al) && exist_keys.empty()) continue;
-    auto key = std::make_tuple(o->ps_namespace[s], o->ps_labelset[s], pl, fl, al, spec_sc[s]);
+    int pl_ = o->ps_pts_list[s], fl = o->ps_aff_list[s], al = o->ps_anti_list[s];
+    if (!nonempty(o->pts_off, pl_) && !nonempty(o->aff_off, fl) && !nonempty(o->aff_off, al) && exist_keys.empty()) continue;
+    auto key = std::make_tuple(o->ps_namespace[s], o->ps_labelset[s], pl_, fl, al, spec_sc[s]);
     auto it = dc_ids.find(key);
     if (it == dc_ids.end()) {
       int dc = (int)dc_spec.size();
@@ -216,7 +238,7 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
         q_kind.push_back((uint8_t)kind); q_k.push_back(k); q_dc.push_back(dc); q_p0.push_back(p0);
         q_base_off.push_back(q_base_off.back() + d.Dc[k]);
       };
-      for (int c = o->pts_off[pl]; c < o->pts_off[pl + 1]; ++c) add_q(Q_PTS, kidx(o->pts_key[c]), c);
+      for (int c = o->pts_off[pl_]; c < o->pts_off[pl_ + 1]; ++c) add_q(Q_PTS, kidx(o->pts_key[c]), c);
       for (int t = o->aff_off[fl]; t < o->aff_off[fl + 1]; ++t) add_q(Q_AFF, kidx(o->aterm_key[t]), t);
       for (int t = o->aff_off[al]; t < o->aff_off[al + 1]; ++t) add_q(Q_ANTI, kidx(o->aterm_key[t]), t);
       for (int key2 : exist_keys) add_q(Q_EXIST, kidx(key2), -1);
@@ -230,16 +252,29 @@ static int build_dynamic(Engine* e, const cae_objects* o, const std::vector<uint
   d.DC = (int)dc_spec.size();
   d.Q = (int)q_kind.size();
   d.pool = q_base_off.back();
-  e->nh.q_k = q_k;
+  return 0;
+}
+
+// The dynamic tables of a plan into the engine: host state, uploads, device buffers
+static int apply_dynamic(Engine* e, PendPlan& pl) {
+  DynTables& d = e->dyn;
+  d = pl.dyn;
+  const int T = e->T, S = d.S;
+  e->nh.spec_used = pl.spec_used;
+  e->nh.key_val.swap(pl.key_val);
+  e->nh.tkey_val.swap(pl.tkey_val);
+  e->nh.q_k.swap(pl.q_k);
+  e->has_dynamic = pl.any;
+  if (!pl.any) { e->nh.key_val.clear(); e->nh.tkey_val.clear(); e->nh.q_k.clear(); return 0; }
   e->DC = d.DC;
   const int32_t* p32 = nullptr; const uint8_t* p8 = nullptr;
-#define UPV(vec, field) { if (upload(e, (vec).data(), (vec).size(), &field)) return -1; }
-  UPV(dom, d.dom); UPV(dc_spec, d.dc_spec); UPV(dc_sc, d.dc_sc); UPV(dc_q_off, d.dc_q_off); UPV(q_kind, d.q_kind);
-  UPV(q_k, d.q_k); UPV(q_dc, d.q_dc); UPV(q_p0, d.q_p0); UPV(q_base_off, d.q_base_off);
-  UPV(spec_used, p8); e->d_spec_used = p8;
-  UPV(dc_ngroups, p32); e->d_dc_ngroups = p32;
+#define UPV(vec, field) { if (upload(e->pup, (vec).data(), (vec).size(), &field)) return -1; }
+  UPV(pl.dom, d.dom); UPV(pl.dc_spec, d.dc_spec); UPV(pl.dc_sc, d.dc_sc); UPV(pl.dc_q_off, d.dc_q_off); UPV(pl.q_kind, d.q_kind);
+  UPV(e->nh.q_k, d.q_k); UPV(pl.q_dc, d.q_dc); UPV(pl.q_p0, d.q_p0); UPV(pl.q_base_off, d.q_base_off);
+  UPV(pl.spec_used, p8); e->d_spec_used = p8;
+  UPV(pl.dc_ngroups, p32); e->d_dc_ngroups = p32;
 #undef UPV
-  const size_t Q = std::max(d.Q, 1), pool = std::max(q_base_off.back(), 1);
+  const size_t Q = std::max(d.Q, 1), pool = std::max(pl.q_base_off.back(), 1);
   if (dev_alloc(e, &d.wmat, Q * S) || dev_alloc(e, &d.q_self, Q) || dev_alloc(e, &d.q_wown, Q) || dev_alloc(e, &d.q_active, Q) ||
       dev_alloc(e, &d.dc_aff_self, (size_t)d.DC) || dev_alloc(e, &d.dc_active, (size_t)d.DC) || dev_alloc(e, &d.elig, Q * e->U) ||
       dev_alloc(e, &d.base_cnt, pool, true) || dev_alloc(e, &d.base_pres, pool, true) || dev_alloc(e, &d.base_tot, Q, true) ||
@@ -254,7 +289,8 @@ struct LoadTimer {   // CAE_LOAD_TIMING=1: host wall clock of the phases of cae_
   bool on;
   std::chrono::steady_clock::time_point t0;
   std::string out;
-  LoadTimer() : on(getenv("CAE_LOAD_TIMING") != nullptr), t0(std::chrono::steady_clock::now()) {}
+  const char* who;
+  explicit LoadTimer(const char* who_ = "cae_load") : on(getenv("CAE_LOAD_TIMING") != nullptr), t0(std::chrono::steady_clock::now()), who(who_) {}
   void mark(const char* what) {
     if (!on) return;
     auto t1 = std::chrono::steady_clock::now();
@@ -263,7 +299,7 @@ struct LoadTimer {   // CAE_LOAD_TIMING=1: host wall clock of the phases of cae_
     out += buf;
     t0 = t1;
   }
-  ~LoadTimer() { if (on) fprintf(stderr, "cae_load:%s\n", out.c_str()); }
+  ~LoadTimer() { if (on) fprintf(stderr, "%s:%s\n", who, out.c_str()); }
 };
 
 // Host copy of the pending-pod rows in pinned memory (source of the H2D copy of cae_load_pending, read by the filter pass),
@@ -327,24 +363,267 @@ static void cluster_row_state(const Engine* e, const int64_t* alloc, int32_t all
   *cslots = allowed_pods - npods;
 }
 
+struct Key4 { int a, b, c, d; bool operator==(const Key4& k) const { return a == k.a && b == k.b && c == k.c && d == k.d; } };
+struct Key4Hash {
+  size_t operator()(const Key4& k) const {
+    uint64_t h = (uint64_t)(uint32_t)k.a * 0x9E3779B97F4A7C15ull;
+    h = (h ^ (uint32_t)k.b) * 0xBF58476D1CE4E5B9ull;
+    h = (h ^ (uint32_t)k.c) * 0x94D049BB133111EBull;
+    h = (h ^ (uint32_t)k.d) * 0x9E3779B97F4A7C15ull;
+    return (size_t)(h ^ (h >> 29));
+  }
+};
+
+// ---- host-side interning of pod specs into classes (no predicate is evaluated here) ----
+static int plan_static(const cae_objects* o, PendPlan& pl) {
+  const int S = o->num_podspecs;
+  std::vector<uint8_t>& spec_pending = pl.spec_pending;
+  spec_pending.assign(S, 0);
+  for (int p = 0, prev = -1; p < o->num_pending; ++p)   // pods of a group are adjacent and share a spec: touch the flag on changes only
+    if (o->pend_spec[p] != prev) { prev = o->pend_spec[p]; spec_pending[prev] = 1; }
+  std::unordered_map<Key4, int, Key4Hash> sc_ids;
+  sc_ids.reserve((size_t)S * 2);
+  std::vector<StaticClass>& sclass = pl.sclass;
+  sclass.reserve(S);
+  pl.spec_sc.assign(S, 0);
+  pl.spec_dc.assign(S, 0);
+  for (int s = 0; s < S; ++s) {
+    if (!spec_pending[s]) continue;
+    const Key4 key{o->ps_tol_list[s], o->ps_naff[s], o->ps_node_name[s], o->ps_port_list[s]};
+    auto ins = sc_ids.emplace(key, (int)sclass.size());   // ids in order of first appearance
+    if (ins.second) sclass.push_back({key.a, key.b, key.c, key.d});
+    pl.spec_sc[s] = ins.first->second;
+  }
+  // host-port lists of pending pods get compact ids (one bit each in a node's used-port mask)
+  pl.pc_of.assign(o->num_port_lists, -1);
+  int npc = 0;
+  for (int s = 0; s < S; ++s) {
+    int p = o->ps_port_list[s];
+    if (!spec_pending[s] || o->port_off[p + 1] == o->port_off[p] || pl.pc_of[p] >= 0) continue;
+    if (npc == 64) { set_error("more than 64 distinct host-port sets among pending pods"); return 1; }
+    pl.pc_of[p] = npc++;
+  }
+  if (sclass.empty()) sclass.push_back({0, -1, -1, 0});
+  return 0;
+}
+
+// Ships the static classes and starts the class matrix, so that the device works while the host goes on (dynamic
+// classes, rank encoding).  The derivation's arenas start over here.
+static int apply_static(Engine* e, const cae_objects* o, PendPlan& pl) {
+  e->pup.reset();
+  e->scratch.reset();
+  e->SC = (int)pl.sclass.size();
+  e->DC = 1;  // class 0: no topology-spread / inter-pod-affinity involvement
+  if (upload_mut(e->pup, pl.sclass, &e->d_sclass) || upload_mut(e->pup, pl.pc_of, &e->d_pc_of) ||
+      dev_alloc(e, &e->d_pre_code, (size_t)e->SC * e->U) || dev_alloc(e, &e->d_port_conf, (size_t)std::max(o->num_port_lists, 1)))
+    return -1;
+  if (e->up.flush(e->stream, &e->stats.h2d_bytes) || e->pup.flush(e->stream, &e->stats.h2d_bytes)) return -1;
+  if (launch_port_conflicts(e, o->num_port_lists)) return -1;
+  if (launch_class_matrix(e)) return -1;
+  return 0;
+}
+
+// active resource dims and the order-preserving rank encoding of the request / free-capacity operands (feas.cu)
+static int plan_ranks(const cae_objects* o, PendPlan& pl) {
+  const int S = o->num_podspecs;
+  const std::vector<uint8_t>& spec_pending = pl.spec_pending;
+  pl.A = 0;
+  for (int r = 0; r < R; ++r) {
+    bool used = false;
+    for (int s = 0; s < S && !used; ++s) used = spec_pending[s] && o->ps_req[(size_t)s * R + r] > 0;
+    if (used) pl.act_dim[pl.A++] = r;
+  }
+  pl.rvals.assign(pl.A, {});
+  for (int a = 0; a < pl.A; ++a) {
+    std::vector<int64_t>& rv = pl.rvals[a];
+    for (int s = 0; s < S; ++s) if (spec_pending[s] && o->ps_req[(size_t)s * R + pl.act_dim[a]] > 0) rv.push_back(o->ps_req[(size_t)s * R + pl.act_dim[a]]);
+    std::sort(rv.begin(), rv.end());
+    rv.erase(std::unique(rv.begin(), rv.end()), rv.end());
+  }
+  pl.W = 0;
+  int w = 0, shift = 0, slices = 0;
+  for (int a = 0; a < pl.A; ++a) {
+    int bits = 1;
+    while ((1ll << bits) <= (long long)pl.rvals[a].size()) ++bits;   // ranks 0..D need `bits` bits
+    bits += 1;                                                        // + guard bit
+    if (shift + bits > 32) { ++w; shift = 0; }
+    if (w >= FEAS_MAX_W || bits > 32) { set_error("resource request cardinality too large for the rank encoding"); return 1; }
+    pl.f_word[a] = w; pl.f_shift[a] = shift; pl.f_bits[a] = bits;
+    shift += bits;
+    pl.W = w + 1;
+    slices += bits - 1;
+  }
+  if (slices > 32) { set_error("resource request cardinality too large for the bit-sliced encoding"); return 1; }
+  return 0;
+}
+
+// The rank fields of the specs, the layout of the template rank fields and threshold bitmaps, and the device buffers of
+// the free capacity over the active dims; launch_rank_tables (pod_delta.cu) fills the per-row tables after the flush
+static int apply_ranks(Engine* e, const cae_objects* o, PendPlan& pl) {
+  const int S = o->num_podspecs, N = e->N, T = e->T;
+  e->A = pl.A;
+  e->W = pl.W;
+  for (int a = 0; a < pl.A; ++a) e->act_dim[a] = pl.act_dim[a];
+  const int A1 = std::max(e->A, 1);
+  const int *f_word = pl.f_word, *f_shift = pl.f_shift, *f_bits = pl.f_bits;
+  const std::vector<std::vector<int64_t>>& rvals = pl.rvals;
+  std::vector<uint32_t> spec_w((size_t)S * FEAS_MAX_W, 0);
+  for (int s = 0; s < S; ++s) {
+    if (!pl.spec_pending[s]) continue;
+    for (int a = 0; a < e->A; ++a) {
+      int64_t v = o->ps_req[(size_t)s * R + e->act_dim[a]];
+      uint32_t rank = v > 0 ? (uint32_t)(std::lower_bound(rvals[a].begin(), rvals[a].end(), v) - rvals[a].begin()) + 1 : 0;
+      spec_w[(size_t)s * FEAS_MAX_W + f_word[a]] |= rank << f_shift[a];
+    }
+  }
+  // bit-sliced free-capacity ranks for the dense pass (feas.cu): slice b, word tw holds bit b of the rank
+  // of templates tw*32 .. tw*32+31; slices run MSB-first inside a field, fields concatenated
+  e->feas_B = 0;
+  e->feas_fstart = 0;
+  for (int a = 0; a < e->A; ++a) {
+    const int nb = f_bits[a] - 1;
+    for (int i = nb - 1; i >= 0; --i) {
+      e->feas_sword[e->feas_B] = (uint8_t)f_word[a];
+      e->feas_sshift[e->feas_B] = (uint8_t)(f_shift[a] + i);
+      if (i == nb - 1) e->feas_fstart |= 1u << e->feas_B;
+      ++e->feas_B;
+    }
+  }
+  // threshold bitmaps for the LUT variant of the dense pass: one row per (dim, request rank)
+  e->lut_rows = 0;
+  for (int a = 0; a < e->A; ++a) {
+    e->lut_base[a] = e->lut_rows;
+    e->lut_rows += (int)rvals[a].size() + 1;
+    e->lut_word[a] = (uint8_t)f_word[a];
+    e->lut_shift[a] = (uint8_t)f_shift[a];
+    e->lut_mask[a] = (1u << (f_bits[a] - 1)) - 1u;
+  }
+  RankArgs& ra = pl.ra;
+  ra = RankArgs{};
+  ra.A = e->A; ra.N = N; ra.T = T; ra.Tw = e->Tw; ra.Twp = e->Twp; ra.W = e->W; ra.lut_rows = e->lut_rows; ra.feas_B = e->feas_B;
+  ra.Bpad = std::max(4, (e->feas_B + 3) / 4 * 4);
+  std::vector<int64_t> rv;
+  ra.rv_off[0] = 0;
+  for (int a = 0; a < e->A; ++a) {
+    ra.act[a] = e->act_dim[a]; ra.f_word[a] = f_word[a]; ra.f_shift[a] = f_shift[a]; ra.f_bits[a] = f_bits[a];
+    ra.lut_base[a] = e->lut_base[a]; ra.lut_mask[a] = e->lut_mask[a];
+    rv.insert(rv.end(), rvals[a].begin(), rvals[a].end());
+    ra.rv_off[a + 1] = (int)rv.size();
+  }
+  for (int b = 0; b < e->feas_B; ++b) { ra.sword[b] = e->feas_sword[b]; ra.sshift[b] = e->feas_sshift[b]; }
+  e->d_tslice = nullptr;
+  if ((e->force_bitslice || e->lut_rows > FEAS_LUT_MAX_ROWS) &&   // only the fallback variant of the dense pass reads the slices
+      dev_alloc(e, &e->d_tslice, (size_t)ra.Bpad * std::max(e->Tw, 1)))
+    return -1;
+  const int64_t* d_rv = nullptr;
+  if (upload(e->pup, rv.data(), rv.size(), &d_rv)) return -1;
+  pl.d_rvals = d_rv;
+  if (dev_alloc(e, &pl.d_tmpl_w, (size_t)std::max(e->W, 1) * std::max(T, 1)) ||
+      dev_alloc(e, &e->d_rlut, (size_t)std::max(e->lut_rows, 1) * std::max(e->Twp, 1)) ||
+      dev_alloc(e, &e->d_tmpl_free, (size_t)A1 * T) || dev_alloc(e, &e->d_c_free, (size_t)A1 * std::max(N, 1)))
+    return -1;
+  if (upload_mut(e->pup, pl.spec_sc, &e->d_spec_sc) || upload_mut(e->pup, spec_w, &e->d_spec_w) || upload_mut(e->pup, pl.spec_dc, &e->d_spec_dc))
+    return -1;
+  return 0;
+}
+
+// Everything derived from the pending set, for cae_load and cae_load_pods alike: spec_pending / spec_used, the static
+// classes with pre_code and pre_ok and the port classes, the dynamic tables (keys, domains, classes, counters and what
+// the device derives from them), the active dims and the rank encoding, pod rows, group records and every buffer sized
+// by P, E or Pl.  It reads the node side from `o` only through node_labelset and the resident CSR (on the host), and
+// through the resident device tables (pod_delta.cu).
+// cae_load (`resident` NULL: the specs of the resident pods are read from `o`): the class matrix starts before the rest is
+// planned, a status-1 limit met later leaves the engine unloaded.  cae_load_pods (`resident` [S] flags, read from the
+// device): every limit is checked first, then `commit` grows the object tables, then the derivation changes the engine.
+template <class Commit>
+static int derive_pending(Engine* e, const cae_objects* o, LoadTimer& lt, const std::vector<uint8_t>* resident, Commit commit) {
+  const bool atomic = resident != nullptr;
+  PendPlan pl;
+  { const int rc = plan_static(o, pl); if (rc) return rc; }
+  if (!atomic && apply_static(e, o, pl)) return -1;
+  lt.mark("stage+classes");
+  { int rc = plan_dynamic(e, o, resident, pl); if (!rc) rc = plan_ranks(o, pl); if (rc) return rc; }
+  if (atomic) {
+    if (commit()) return -1;
+    cudaEventRecord(e->ev0, e->stream);
+    if (apply_static(e, o, pl)) return -1;
+  }
+  const int S = o->num_podspecs, T = e->T;
+  e->num_podspecs = S;
+  e->E = o->num_groups; e->P = o->num_pending;
+  pod_shard(e, e->P, &e->p_begin, &e->p_end);
+  e->Pl = e->p_end - e->p_begin;
+  e->Plw = (e->Pl + 31) / 32;
+  if (upload(e->pup, o->group_off, (size_t)o->num_groups + 1, &e->dobj.group_off) ||
+      upload(e->pup, o->pend_spec, (size_t)o->num_pending, &e->dobj.pend_spec))
+    return -1;
+  if (apply_dynamic(e, pl)) return -1;
+  lt.mark("build_dynamic");
+  if (apply_ranks(e, o, pl)) return -1;
+  std::vector<int32_t>& spec_dc = pl.spec_dc;
+
+  lt.mark("ranks+tables");
+  if (dev_alloc(e, &e->d_pre_ok, (size_t)e->SC * std::max(e->Twp, 1)) ||
+      dev_alloc(e, &e->d_post_code, (size_t)e->DC * std::max(T, 1), true) || dev_alloc(e, &e->d_post_ok, (size_t)e->DC * std::max(e->Twp, 1)) ||
+      dev_alloc(e, &e->d_pod_w, (size_t)std::max(e->W, 1) * std::max(e->Pl, 1)) || dev_alloc(e, &e->d_pod_row, (size_t)std::max(e->A, 1) * std::max(e->Pl, 1)) || dev_alloc(e, &e->d_pod_sc, (size_t)std::max(e->Pl, 1)) ||
+      dev_alloc(e, &e->d_pod_dc, (size_t)std::max(e->Pl, 1)) || dev_alloc(e, &e->d_fit_bits, (size_t)std::max(T, 1) * std::max(e->Plw, 1)) ||
+      dev_alloc(e, &e->d_fit_count, (size_t)std::max(T, 1), true) || dev_alloc(e, &e->d_fit_acc, (size_t)std::max(T, 1), true) ||
+      dev_alloc(e, &e->d_chunk_done, (size_t)std::max(e->Twp / FEAS_TW, 1), true) || dev_alloc(e, &e->d_group_reason, (size_t)std::max(T, 1) * std::max(e->E, 1)) ||
+      dev_alloc(e, &e->d_counts2, (size_t)2 * std::max(T, 1), true) || dev_alloc(e, &e->d_waste, (size_t)std::max(T, 1)) || dev_alloc(e, &e->d_sched, (size_t)std::max(T, 1) * std::max(e->E, 1), true) ||
+      dev_alloc(e, &e->d_order, (size_t)std::max(T, 1) * std::max(e->E, 1)) || dev_alloc(e, &e->d_grec, (size_t)std::max(e->E, 1)) || dev_alloc(e, &e->d_order_n, (size_t)std::max(T, 1), true) ||
+      dev_alloc(e, &e->d_max_nodes, (size_t)std::max(T, 1), true) || dev_alloc(e, &e->d_last_index_buf, (size_t)2 * std::max(T, 1), true) || dev_alloc(e, &e->d_tmpl_cost, (size_t)std::max(T, 1), true) ||
+      dev_alloc(e, &e->d_perm, (size_t)std::max(T, 1)) || dev_alloc(e, &e->d_work_counter, 4, true))
+    return -1;
+  e->d_reasons = nullptr;
+  if (e->cfg.want_reasons && dev_alloc(e, &e->d_reasons, (size_t)std::max(T, 1) * std::max(e->Pl, 1))) return -1;
+
+  // host copies for host-side steps (homogeneity check) and for the per-tick deltas (cae_load_pending)
+  e->h_spec_pending = pl.spec_pending;
+  e->cap_P = e->P; e->cap_E = e->E; e->cap_Pl = e->Pl;
+  { int rc = stage_pending(e, e->P, o->pend_spec, e->E, o->group_off, false); if (rc) return rc; }
+
+  lt.mark("dev_alloc+memsets");
+  if (e->pup.flush(e->stream, &e->stats.h2d_bytes)) return -1;   // ONE pinned H2D copy per arena chunk
+  if (launch_rank_tables(e, pl.ra, pl.d_rvals, pl.d_tmpl_w)) return -1;
+  if (launch_pre_ok_bits(e)) return -1;
+  if (e->has_dynamic) {
+    if (launch_dynamic_tables(e, e->d_spec_used, e->d_dc_ngroups)) return -1;
+    // classes none of whose counters can ever be non-zero are plain: fold them back into class 0
+    std::vector<uint8_t> act(e->dyn.DC);
+    CAE_CUDA(cudaMemcpyAsync(act.data(), e->dyn.dc_active, act.size(), cudaMemcpyDeviceToHost, e->stream));
+    CAE_CUDA(cudaStreamSynchronize(e->stream));
+    bool changed = false;
+    for (int s = 0; s < S; ++s) if (spec_dc[s] && !act[spec_dc[s]]) { spec_dc[s] = 0; changed = true; }
+    if (changed) CAE_CUDA(cudaMemcpyAsync(e->d_spec_dc, spec_dc.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, e->stream));
+    CAE_CUDA(cudaStreamSynchronize(e->stream));
+  }
+  if (launch_post_bits(e)) return -1;
+  if (launch_expand_pods(e)) return -1;
+  if (launch_group_records(e)) return -1;
+  cudaEventRecord(e->ev1, e->stream);
+  lt.mark("launches");
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
+  lt.mark("sync");
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
+  e->stats.h2d_ms = ms;
+  e->group_reason_valid = false;
+  return 0;
+}
+
 static int do_load(Engine* e, const cae_objects* o) {
   LoadTimer lt;
   if (o->abi_version != CAE_ABI_VERSION) { set_error("cae_objects.abi_version mismatch"); return -2; }
   if (o->num_res < 3 || o->num_res > CAE_MAX_RES) { set_error("num_res out of range"); return 1; }
   e->up.reset();
-  e->scratch.reset();
   e->loaded = false;
   e->group_reason_valid = false;
   e->stats.h2d_bytes = 0;
   const int N = o->num_cluster_nodes, T = o->num_templates, NT = N + T;
-  e->N = N; e->T = T; e->U = N + 2 * T; e->E = o->num_groups; e->P = o->num_pending;
+  e->N = N; e->T = T; e->U = N + 2 * T;
   e->Tw = (T + 31) / 32;
   e->Twp = (e->Tw + FEAS_TW - 1) / FEAS_TW * FEAS_TW;
-  e->num_podspecs = o->num_podspecs;
-  pod_shard(e, e->P, &e->p_begin, &e->p_end);
   const int W = std::max(1, e->cfg.world_size), rk = e->cfg.rank;
-  e->Pl = e->p_end - e->p_begin;
-  e->Plw = (e->Pl + 31) / 32;
   e->t_begin = (int)((int64_t)T * rk / W);
   e->t_end = (int)((int64_t)T * (rk + 1) / W);
 
@@ -375,182 +654,29 @@ static int do_load(Engine* e, const cae_objects* o) {
   UP(node_alloc, (size_t)NT * R); UP(node_allowed_pods, NT); UP(node_cap_cpu, NT); UP(node_cap_mem, NT);
   UP(node_has_alloc_cpu, NT); UP(node_has_alloc_mem, NT);
   UP(node_pod_off, NT + 1); UP(node_pod_spec, o->node_pod_off[NT]);
-  UP(group_off, o->num_groups + 1); UP(pend_spec, o->num_pending);
 
-  // ---- host-side interning of pod specs into classes (no predicate is evaluated here) ----
+  // node side: free capacity of the templates over all R dims, free pod slots of every row
   const int S = o->num_podspecs;
-  std::vector<uint8_t> spec_pending(S, 0);
-  for (int p = 0, prev = -1; p < o->num_pending; ++p)   // pods of a group are adjacent and share a spec: touch the flag on changes only
-    if (o->pend_spec[p] != prev) { prev = o->pend_spec[p]; spec_pending[prev] = 1; }
-  struct Key4 { int a, b, c, d; bool operator==(const Key4& k) const { return a == k.a && b == k.b && c == k.c && d == k.d; } };
-  struct Key4Hash {
-    size_t operator()(const Key4& k) const {
-      uint64_t h = (uint64_t)(uint32_t)k.a * 0x9E3779B97F4A7C15ull;
-      h = (h ^ (uint32_t)k.b) * 0xBF58476D1CE4E5B9ull;
-      h = (h ^ (uint32_t)k.c) * 0x94D049BB133111EBull;
-      h = (h ^ (uint32_t)k.d) * 0x9E3779B97F4A7C15ull;
-      return (size_t)(h ^ (h >> 29));
-    }
-  };
-  std::unordered_map<Key4, int, Key4Hash> sc_ids;
-  sc_ids.reserve((size_t)S * 2);
-  std::vector<StaticClass> sclass;
-  sclass.reserve(S);
-  std::vector<int32_t> spec_sc(S, 0), spec_dc(S, 0);
-  for (int s = 0; s < S; ++s) {
-    if (!spec_pending[s]) continue;
-    const Key4 key{o->ps_tol_list[s], o->ps_naff[s], o->ps_node_name[s], o->ps_port_list[s]};
-    auto ins = sc_ids.emplace(key, (int)sclass.size());   // ids in order of first appearance
-    if (ins.second) sclass.push_back({key.a, key.b, key.c, key.d});
-    spec_sc[s] = ins.first->second;
-  }
-  // host-port lists of pending pods get compact ids (one bit each in a node's used-port mask)
-  std::vector<int32_t> pc_of(o->num_port_lists, -1);
-  int npc = 0;
-  for (int s = 0; s < S; ++s) {
-    int pl = o->ps_port_list[s];
-    if (!spec_pending[s] || o->port_off[pl + 1] == o->port_off[pl] || pc_of[pl] >= 0) continue;
-    if (npc == 64) { set_error("more than 64 distinct host-port sets among pending pods"); return 1; }
-    pc_of[pl] = npc++;
-  }
-  if (sclass.empty()) sclass.push_back({0, -1, -1, 0});
-  e->SC = (int)sclass.size();
-  e->DC = 1;  // class 0: no topology-spread / inter-pod-affinity involvement
-  // The object tables and the static classes are complete: ship them and start the class matrix now, so that the
-  // device works while the host goes on interning (dynamic classes, rank encoding).
-  if (upload_mut(e, sclass, &e->d_sclass) || upload_mut(e, pc_of, &e->d_pc_of) || dev_alloc(e, &e->d_pre_code, (size_t)e->SC * e->U) ||
-      dev_alloc(e, &e->d_port_conf, (size_t)std::max(o->num_port_lists, 1)))
-    return -1;
-  if (e->up.flush(e->stream, &e->stats.h2d_bytes)) return -1;
-  if (launch_port_conflicts(e, o->num_port_lists)) return -1;
-  if (launch_class_matrix(e)) return -1;
-  lt.mark("stage+classes");
-  { int rc = build_dynamic(e, o, spec_pending, spec_sc, spec_dc); if (rc) return rc; }
-  lt.mark("build_dynamic");
-
-  // active resource dims + free capacity of templates and cluster nodes
-  e->A = 0;
-  for (int r = 0; r < R; ++r) {
-    bool used = false;
-    for (int s = 0; s < S && !used; ++s) used = spec_pending[s] && o->ps_req[(size_t)s * R + r] > 0;
-    if (used) e->act_dim[e->A++] = r;
-  }
-  const int A1 = std::max(e->A, 1);
-  // order-preserving rank encoding of the request / free-capacity operands (feas.cu)
-  std::vector<std::vector<int64_t>> rvals(e->A);
-  for (int a = 0; a < e->A; ++a) {
-    for (int s = 0; s < S; ++s) if (spec_pending[s] && o->ps_req[(size_t)s * R + e->act_dim[a]] > 0) rvals[a].push_back(o->ps_req[(size_t)s * R + e->act_dim[a]]);
-    std::sort(rvals[a].begin(), rvals[a].end());
-    rvals[a].erase(std::unique(rvals[a].begin(), rvals[a].end()), rvals[a].end());
-  }
-  int f_word[CAE_MAX_RES], f_shift[CAE_MAX_RES], f_bits[CAE_MAX_RES];
-  e->W = 0;
-  { int w = 0, shift = 0;
-    for (int a = 0; a < e->A; ++a) {
-      int bits = 1;
-      while ((1ll << bits) <= (long long)rvals[a].size()) ++bits;   // ranks 0..D need `bits` bits
-      bits += 1;                                                     // + guard bit
-      if (shift + bits > 32) { ++w; shift = 0; }
-      if (w >= FEAS_MAX_W || bits > 32) { set_error("resource request cardinality too large for the rank encoding"); return 1; }
-      f_word[a] = w; f_shift[a] = shift; f_bits[a] = bits;
-      shift += bits;
-      e->W = w + 1;
-    } }
-  std::vector<uint32_t> spec_w((size_t)S * FEAS_MAX_W, 0), tmpl_w((size_t)std::max(e->W, 1) * std::max(T, 1), 0);
-  for (int s = 0; s < S; ++s) {
-    if (!spec_pending[s]) continue;
-    for (int a = 0; a < e->A; ++a) {
-      int64_t v = o->ps_req[(size_t)s * R + e->act_dim[a]];
-      uint32_t rank = v > 0 ? (uint32_t)(std::lower_bound(rvals[a].begin(), rvals[a].end(), v) - rvals[a].begin()) + 1 : 0;
-      spec_w[(size_t)s * FEAS_MAX_W + f_word[a]] |= rank << f_shift[a];
-    }
-  }
-  std::vector<int64_t> free_all((size_t)R * T), free_act((size_t)A1 * T), cfree((size_t)A1 * std::max(N, 1));
+  Engine::PodHost& ph = e->ph;
+  std::vector<int64_t> free_all((size_t)R * T);
   std::vector<int32_t> slots(T), cslots(std::max(N, 1));
   for (int row = 0; row < NT; ++row) {
-    const int32_t* pods = o->node_pod_spec + o->node_pod_off[row];
     const int npods = o->node_pod_off[row + 1] - o->node_pod_off[row];
     if (row < N) {
-      cluster_row_state(e, o->node_alloc + (size_t)row * R, o->node_allowed_pods[row], pods, npods, o->ps_req, &cfree[row], N, &cslots[row]);
+      cslots[row] = o->node_allowed_pods[row] - npods;
       continue;
     }
     int64_t reqd[R];
-    resident_req(o->ps_req, pods, npods, reqd);
+    resident_req(o->ps_req, o->node_pod_spec + o->node_pod_off[row], npods, reqd);
     const int t = row - N;
     for (int r = 0; r < R; ++r) free_all[(size_t)r * T + t] = o->node_alloc[(size_t)row * R + r] - reqd[r];
-    for (int a = 0; a < e->A; ++a) free_act[(size_t)a * T + t] = free_all[(size_t)e->act_dim[a] * T + t];
     slots[t] = o->node_allowed_pods[row] - npods;
-    for (int a = 0; a < e->A; ++a) {
-      int64_t f = free_act[(size_t)a * T + t];
-      uint32_t rank = (uint32_t)(std::upper_bound(rvals[a].begin(), rvals[a].end(), f) - rvals[a].begin());
-      tmpl_w[(size_t)f_word[a] * T + t] |= (rank | (1u << (f_bits[a] - 1))) << f_shift[a];
-    }
   }
-  // bit-sliced free-capacity ranks for the dense pass (feas.cu): slice b, word tw holds bit b of the rank
-  // of templates tw*32 .. tw*32+31; slices run MSB-first inside a field, fields concatenated
-  e->feas_B = 0;
-  e->feas_fstart = 0;
-  for (int a = 0; a < e->A; ++a) {
-    const int nb = f_bits[a] - 1;
-    for (int i = nb - 1; i >= 0; --i) {
-      if (e->feas_B >= 32) { set_error("resource request cardinality too large for the bit-sliced encoding"); return 1; }
-      e->feas_sword[e->feas_B] = (uint8_t)f_word[a];
-      e->feas_sshift[e->feas_B] = (uint8_t)(f_shift[a] + i);
-      if (i == nb - 1) e->feas_fstart |= 1u << e->feas_B;
-      ++e->feas_B;
-    }
-  }
-  // threshold bitmaps for the LUT variant of the dense pass: one row per (dim, request rank)
-  e->lut_rows = 0;
-  for (int a = 0; a < e->A; ++a) {
-    e->lut_base[a] = e->lut_rows;
-    e->lut_rows += (int)rvals[a].size() + 1;
-    e->lut_word[a] = (uint8_t)f_word[a];
-    e->lut_shift[a] = (uint8_t)f_shift[a];
-    e->lut_mask[a] = (1u << (f_bits[a] - 1)) - 1u;
-  }
-  e->d_tslice = nullptr;
-  if (e->force_bitslice || e->lut_rows > FEAS_LUT_MAX_ROWS) {   // only the fallback variant of the dense pass reads the slices
-    const int Bpad = std::max(4, (e->feas_B + 3) / 4 * 4);
-    std::vector<uint32_t> tslice((size_t)Bpad * std::max(e->Tw, 1), 0);
-    for (int b = 0; b < e->feas_B; ++b)
-      for (int t = 0; t < T; ++t)
-        tslice[(size_t)b * e->Tw + t / 32] |= ((tmpl_w[(size_t)e->feas_sword[b] * T + t] >> e->feas_sshift[b]) & 1u) << (t % 32);
-    if (upload_mut(e, tslice, &e->d_tslice)) return -1;
-  }
-  {
-    std::vector<uint32_t> rlut((size_t)std::max(e->lut_rows, 1) * std::max(e->Twp, 1), 0);
-    for (int a = 0; a < e->A; ++a)
-      for (int t = 0; t < T; ++t) {
-        const uint32_t rank_free = (tmpl_w[(size_t)f_word[a] * T + t] >> f_shift[a]) & e->lut_mask[a];
-        for (uint32_t k = 0; k <= rank_free; ++k) rlut[(size_t)(e->lut_base[a] + k) * e->Twp + t / 32] |= 1u << (t % 32);
-      }
-    if (upload_mut(e, rlut, &e->d_rlut)) return -1;
-  }
-  if (upload_mut(e, spec_sc, &e->d_spec_sc) || upload_mut(e, slots, &e->d_tmpl_slots) ||
-      upload_mut(e, free_all, &e->d_tmpl_free_all) || upload_mut(e, free_act, &e->d_tmpl_free) || upload_mut(e, cfree, &e->d_c_free) ||
-      upload_mut(e, cslots, &e->d_c_slots) || upload_mut(e, spec_w, &e->d_spec_w) || upload_mut(e, spec_dc, &e->d_spec_dc))
+  if (upload_mut(e->up, slots, &e->d_tmpl_slots) || upload_mut(e->up, free_all, &e->d_tmpl_free_all) || upload_mut(e->up, cslots, &e->d_c_slots))
     return -1;
-
-  lt.mark("ranks+tables");
-  if (dev_alloc(e, &e->d_pre_ok, (size_t)e->SC * std::max(e->Twp, 1)) ||
-      dev_alloc(e, &e->d_post_code, (size_t)e->DC * std::max(T, 1), true) || dev_alloc(e, &e->d_post_ok, (size_t)e->DC * std::max(e->Twp, 1)) ||
-      dev_alloc(e, &e->d_pod_w, (size_t)std::max(e->W, 1) * std::max(e->Pl, 1)) || dev_alloc(e, &e->d_pod_row, (size_t)std::max(e->A, 1) * std::max(e->Pl, 1)) || dev_alloc(e, &e->d_pod_sc, (size_t)std::max(e->Pl, 1)) ||
-      dev_alloc(e, &e->d_pod_dc, (size_t)std::max(e->Pl, 1)) || dev_alloc(e, &e->d_fit_bits, (size_t)std::max(T, 1) * std::max(e->Plw, 1)) ||
-      dev_alloc(e, &e->d_fit_count, (size_t)std::max(T, 1), true) || dev_alloc(e, &e->d_fit_acc, (size_t)std::max(T, 1), true) ||
-      dev_alloc(e, &e->d_chunk_done, (size_t)std::max(e->Twp / FEAS_TW, 1), true) || dev_alloc(e, &e->d_group_reason, (size_t)std::max(T, 1) * std::max(e->E, 1)) ||
-      dev_alloc(e, &e->d_counts2, (size_t)2 * std::max(T, 1), true) || dev_alloc(e, &e->d_waste, (size_t)std::max(T, 1)) || dev_alloc(e, &e->d_sched, (size_t)std::max(T, 1) * std::max(e->E, 1), true) ||
-      dev_alloc(e, &e->d_order, (size_t)std::max(T, 1) * std::max(e->E, 1)) || dev_alloc(e, &e->d_grec, (size_t)std::max(e->E, 1)) || dev_alloc(e, &e->d_order_n, (size_t)std::max(T, 1), true) ||
-      dev_alloc(e, &e->d_max_nodes, (size_t)std::max(T, 1), true) || dev_alloc(e, &e->d_last_index_buf, (size_t)2 * std::max(T, 1), true) || dev_alloc(e, &e->d_tmpl_cost, (size_t)std::max(T, 1), true) ||
-      dev_alloc(e, &e->d_perm, (size_t)std::max(T, 1)) || dev_alloc(e, &e->d_work_counter, 4, true))
-    return -1;
-  e->d_reasons = nullptr;
-  if (e->cfg.want_reasons && dev_alloc(e, &e->d_reasons, (size_t)std::max(T, 1) * std::max(e->Pl, 1))) return -1;
-
-  // host copies for host-side steps (homogeneity check) and for the per-tick deltas (cae_load_pending, cae_load_nodes)
-  e->h_spec_pending = spec_pending;
+  // host state the per-tick deltas validate against and update (cae_load_pending, cae_load_nodes, cae_load_pods)
   {
-    Engine::NodeHost& nh = e->nh;   // spec_used and key_val come from build_dynamic
+    Engine::NodeHost& nh = e->nh;   // spec_used and key_val come from the derivation
     nh.num_values = o->num_values;
     nh.num_labelsets = o->num_labelsets;
     nh.num_taint_lists = o->num_taint_lists;
@@ -565,34 +691,30 @@ static int do_load(Engine* e, const cae_objects* o) {
     nh.spec_anti.resize(S);
     for (int s = 0; s < S; ++s) nh.spec_anti[s] = o->aff_off[o->ps_anti_list[s] + 1] > o->aff_off[o->ps_anti_list[s]];
     e->h_spec_req.assign(o->ps_req, o->ps_req + (size_t)S * R);
+    ph.hostname_key = o->hostname_key;
+    ph.num_res = o->num_res;
+    ph.num_namespaces = o->num_namespaces;
+    ph.num_reqs = o->num_reqs;
+    ph.req_vals = o->num_reqs ? o->req_val_off[o->num_reqs] : 0;
+    ph.num_selectors = o->num_selectors;
+    ph.num_naff = o->num_naff;
+    ph.num_naff_terms = o->num_naff_terms;
+    ph.fields = o->term_field_off[o->num_naff_terms];
+    ph.num_tol_lists = o->num_tol_lists;
+    ph.tol_entries = o->tol_off[o->num_tol_lists];
+    ph.num_aterms = o->num_aterms;
+    ph.aterm_ns = o->aterm_ns_off[o->num_aterms];
+    auto col = [S](std::vector<int32_t>& v, const int32_t* src) { v.assign(src, src + S); };
+    col(ph.ps_namespace, o->ps_namespace); col(ph.ps_labelset, o->ps_labelset); col(ph.ps_tol_list, o->ps_tol_list);
+    col(ph.ps_naff, o->ps_naff); col(ph.ps_node_name, o->ps_node_name); col(ph.ps_port_list, o->ps_port_list);
+    col(ph.ps_pts_list, o->ps_pts_list); col(ph.ps_aff_list, o->ps_aff_list); col(ph.ps_anti_list, o->ps_anti_list);
+    ph.port_off.assign(o->port_off, o->port_off + o->num_port_lists + 1);
+    ph.pts_off.assign(o->pts_off, o->pts_off + o->num_pts_lists + 1);
+    ph.pts_key.assign(o->pts_key, o->pts_key + o->pts_off[o->num_pts_lists]);
+    ph.aff_off.assign(o->aff_off, o->aff_off + o->num_aff_lists + 1);
+    ph.aterm_key.assign(o->aterm_key, o->aterm_key + o->num_aterms);
   }
-  e->cap_P = e->P; e->cap_E = e->E; e->cap_Pl = e->Pl;
-  { int rc = stage_pending(e, e->P, o->pend_spec, e->E, o->group_off, false); if (rc) return rc; }
-
-  lt.mark("dev_alloc+memsets");
-  if (e->up.flush(e->stream, &e->stats.h2d_bytes)) return -1;   // ONE pinned H2D copy per arena chunk
-  if (launch_pre_ok_bits(e)) return -1;
-  if (e->has_dynamic) {
-    if (launch_dynamic_tables(e, e->d_spec_used, e->d_dc_ngroups)) return -1;
-    // classes none of whose counters can ever be non-zero are plain: fold them back into class 0
-    std::vector<uint8_t> act(e->dyn.DC);
-    CAE_CUDA(cudaMemcpyAsync(act.data(), e->dyn.dc_active, act.size(), cudaMemcpyDeviceToHost, e->stream));
-    CAE_CUDA(cudaStreamSynchronize(e->stream));
-    bool changed = false;
-    for (int s = 0; s < S; ++s) if (spec_dc[s] && !act[spec_dc[s]]) { spec_dc[s] = 0; changed = true; }
-    if (changed) CAE_CUDA(cudaMemcpyAsync(e->d_spec_dc, spec_dc.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, e->stream));
-    CAE_CUDA(cudaStreamSynchronize(e->stream));
-  }
-  if (launch_post_bits(e)) return -1;
-  if (launch_expand_pods(e)) return -1;
-  if (launch_group_records(e)) return -1;
-  cudaEventRecord(e->ev1, e->stream);
-  lt.mark("launches");
-  CAE_CUDA(cudaStreamSynchronize(e->stream));
-  lt.mark("sync");
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
-  e->stats.h2d_ms = ms;
+  { const int rc = derive_pending(e, o, lt, nullptr, [] { return 0; }); if (rc) return rc; }
   e->loaded = true;
   return 0;
 }
@@ -600,10 +722,9 @@ static int do_load(Engine* e, const cae_objects* o) {
 // Append a dictionary tail (already on the device, in the staged delta) to a DevObjects table.  The grown table lives in an
 // engine-owned buffer: the first delta after a load copies the arena's contents there once, later deltas append in place
 // while the headroom lasts.
-template <class T>
-static int grow_table(Engine* e, Engine::DevBuf& b, const T*& cur, size_t n_old, const void* d_tail, size_t n_tail) {
+static int grow_bytes(Engine* e, Engine::DevBuf& b, const void*& cur, size_t elem, size_t n_old, const void* d_tail, size_t n_tail) {
   if (n_tail == 0) return 0;
-  const size_t need = (n_old + n_tail) * sizeof(T);
+  const size_t need = (n_old + n_tail) * elem;
   if (cur != b.p || need > b.cap) {
     void* np = b.p;
     size_t ncap = b.cap;
@@ -611,14 +732,22 @@ static int grow_table(Engine* e, Engine::DevBuf& b, const T*& cur, size_t n_old,
       ncap = need + need / 2 + 4096;
       CAE_CUDA(cudaMallocAsync(&np, ncap, e->stream));
     }
-    if (n_old) CAE_CUDA(cudaMemcpyAsync(np, cur, n_old * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
-    if (np != b.p && b.p) CAE_CUDA(cudaFreeAsync(b.p, e->stream));   // stream-ordered: after the copy out of it
+    if (n_old) CAE_CUDA(cudaMemcpyAsync(np, cur, n_old * elem, cudaMemcpyDeviceToDevice, e->stream));
+    if (np != b.p && b.p) CAE_CUDA(cudaFreeAsync(b.p, e->stream));
     b.p = np;
     b.cap = ncap;
   }
-  CAE_CUDA(cudaMemcpyAsync(static_cast<T*>(b.p) + n_old, d_tail, n_tail * sizeof(T), cudaMemcpyDeviceToDevice, e->stream));
-  cur = static_cast<const T*>(b.p);
+  CAE_CUDA(cudaMemcpyAsync(static_cast<char*>(b.p) + n_old * elem, d_tail, n_tail * elem, cudaMemcpyDeviceToDevice, e->stream));
+  cur = b.p;
   return 0;
+}
+
+template <class T>
+static int grow_table(Engine* e, Engine::DevBuf& b, const T*& cur, size_t n_old, const void* d_tail, size_t n_tail) {
+  const void* c = cur;
+  const int rc = grow_bytes(e, b, c, sizeof(T), n_old, d_tail, n_tail);
+  cur = static_cast<const T*>(c);
+  return rc;
 }
 
 // The new state of cluster rows a node delta carries: the dirty rows of a cae_node_delta, the added nodes of a churn
@@ -971,6 +1100,226 @@ static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
   return 0;
 }
 
+static int do_load_pods(Engine* e, const cae_pod_delta* d) {
+  LoadTimer lt("cae_load_pods");
+  auto bad = [](const char* m) { set_error(std::string("cae_load_pods: ") + m); return -2; };
+  if (d->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
+  Engine::NodeHost& nh = e->nh;
+  Engine::PodHost& ph = e->ph;
+  const int S0 = e->num_podspecs;
+  const int nv = d->num_new_values, nns = d->num_new_namespaces, nl = d->num_new_labelsets, nrq = d->num_new_reqs;
+  const int nsel = d->num_new_selectors, nnf = d->num_new_naff, ntm = d->num_new_naff_terms, ntol = d->num_new_tol_lists;
+  const int npl = d->num_new_port_lists, npts = d->num_new_pts_lists, nal = d->num_new_aff_lists, nat = d->num_new_aterms;
+  const int nsp = d->num_new_specs, P = d->num_pending, E = d->num_groups;
+  if ((nv | nns | nl | nrq | nsel | nnf | ntm | ntol | npl | npts | nal | nat | nsp | P | E) < 0) return bad("negative count");
+  if ((nv && (!d->value_is_int || !d->value_int)) || (nns && (!d->ns_labelset || !d->ns_exists)) || (nl && !d->ls_off) ||
+      (nrq && (!d->req_key || !d->req_op || !d->req_val_off)) || (nsel && (!d->sel_kind || !d->sel_req_off)) ||
+      (nnf && (!d->naff_nodesel || !d->naff_has_required || !d->naff_term_off)) || (ntm && (!d->term_expr_sel || !d->term_field_off)) ||
+      (ntol && !d->tol_off) || (npl && !d->port_off) || (npts && !d->pts_off) || (nal && !d->aff_off) ||
+      (nat && (!d->aterm_selector || !d->aterm_key || !d->aterm_ns_off || !d->aterm_ns_selector)) ||
+      (nsp && (!d->ps_namespace || !d->ps_labelset || !d->ps_req || !d->ps_tol_list || !d->ps_naff || !d->ps_node_name ||
+               !d->ps_port_list || !d->ps_pts_list || !d->ps_aff_list || !d->ps_anti_list || !d->ps_terminating || !d->ps_hostname_spread)) ||
+      !d->group_off || (P && !d->pend_spec))
+    return bad("NULL array with a non-zero count");
+  auto offsets_ok = [](const int32_t* off, int n) {
+    if (n == 0) return true;
+    if (off[0] != 0) return false;
+    for (int i = 0; i < n; ++i) if (off[i + 1] < off[i]) return false;
+    return true;
+  };
+  if (!offsets_ok(d->ls_off, nl) || !offsets_ok(d->req_val_off, nrq) || !offsets_ok(d->sel_req_off, nsel) ||
+      !offsets_ok(d->naff_term_off, nnf) || !offsets_ok(d->term_field_off, ntm) || !offsets_ok(d->tol_off, ntol) ||
+      !offsets_ok(d->port_off, npl) || !offsets_ok(d->pts_off, npts) || !offsets_ok(d->aff_off, nal) ||
+      !offsets_ok(d->aterm_ns_off, nat) || d->group_off[0] != 0 || !offsets_ok(d->group_off, E) || d->group_off[E] != P)
+    return bad("offsets that do not start at 0, decrease, or group_off not covering pend_spec");
+  auto end = [](const int32_t* off, int n) -> int64_t { return n ? off[n] : 0; };
+  const int64_t pairs = end(d->ls_off, nl), rvals = end(d->req_val_off, nrq), fields = end(d->term_field_off, ntm);
+  const int64_t tents = end(d->tol_off, ntol), pents = end(d->port_off, npl), cents = end(d->pts_off, npts), nsents = end(d->aterm_ns_off, nat);
+  if (end(d->sel_req_off, nsel) > nrq || end(d->naff_term_off, nnf) > ntm || end(d->aff_off, nal) > nat)
+    return bad("a tail's offsets run past its child tail");
+  if ((pairs && (!d->ls_key || !d->ls_val)) || (rvals && !d->req_vals) || (fields && (!d->field_op || !d->field_node_name)) ||
+      (tents && (!d->tol_key || !d->tol_op || !d->tol_val || !d->tol_effect)) || (pents && (!d->port_ip || !d->port_proto || !d->port_num)) ||
+      (cents && (!d->pts_max_skew || !d->pts_key || !d->pts_selector || !d->pts_min_domains || !d->pts_node_affinity_policy ||
+                 !d->pts_node_taints_policy)) ||
+      (nsents && !d->aterm_ns))
+    return bad("NULL array with a non-zero count");
+  // ---- status 2: sizes, from the counts and offsets alone ----
+  const int64_t NV = (int64_t)nh.num_values + nv, NNS = (int64_t)ph.num_namespaces + nns, NL = (int64_t)nh.num_labelsets + nl;
+  const int64_t NSEL = (int64_t)ph.num_selectors + nsel, NNF = (int64_t)ph.num_naff + nnf;
+  const int64_t NTL = (int64_t)ph.num_tol_lists + ntol, NPL = (int64_t)ph.port_off.size() - 1 + npl;
+  const int64_t NPTS = (int64_t)ph.pts_off.size() - 1 + npts, NAL = (int64_t)ph.aff_off.size() - 1 + nal, S = (int64_t)S0 + nsp;
+  if (NV > INT32_MAX || NNS > INT32_MAX || NL >= INT32_MAX || (int64_t)nh.ls_off.back() + pairs > INT32_MAX ||
+      (int64_t)ph.num_reqs + nrq >= INT32_MAX || (int64_t)ph.req_vals + rvals > INT32_MAX || NSEL >= INT32_MAX || NNF >= INT32_MAX ||
+      (int64_t)ph.num_naff_terms + ntm >= INT32_MAX || (int64_t)ph.fields + fields > INT32_MAX || NTL >= INT32_MAX ||
+      (int64_t)ph.tol_entries + tents > INT32_MAX || NPL >= INT32_MAX || (int64_t)ph.port_off.back() + pents > INT32_MAX ||
+      NPTS >= INT32_MAX || (int64_t)ph.pts_off.back() + cents > INT32_MAX || NAL >= INT32_MAX ||
+      (int64_t)ph.num_aterms + nat >= INT32_MAX || (int64_t)ph.aterm_ns + nsents > INT32_MAX || S > INT32_MAX / R)
+  { set_error("cae_load_pods: a table would pass 2^31 - 1 entries"); return 2; }
+  // ---- ids and enums ----
+  auto in = [](int64_t v, int64_t lo, int64_t hi) { return v >= lo && v < hi; };
+  for (int i = 0; i < nns; ++i) if (!in(d->ns_labelset[i], 0, NL) || d->ns_exists[i] > 1) return bad("namespace tail out of range");
+  for (int j = 0; j < nl; ++j)
+    for (int q = d->ls_off[j]; q < d->ls_off[j + 1]; ++q) {
+      if (d->ls_key[q] < 0 || (q > d->ls_off[j] && d->ls_key[q] <= d->ls_key[q - 1])) return bad("label pairs not sorted by key id");
+      if (!in(d->ls_val[q], 0, NV)) return bad("label value id out of range");
+    }
+  for (int i = 0; i < nrq; ++i) if (d->req_key[i] < 0 || !in(d->req_op[i], CAE_OP_IN, CAE_OP_LT + 1)) return bad("requirement out of range");
+  for (int64_t q = 0; q < rvals; ++q) if (!in(d->req_vals[q], 0, NV)) return bad("requirement value id out of range");
+  for (int i = 0; i < nsel; ++i) if (!in(d->sel_kind[i], CAE_SEL_NOTHING, CAE_SEL_REQS + 1)) return bad("selector kind out of range");
+  for (int i = 0; i < nnf; ++i)
+    if (!in(d->naff_nodesel[i], -1, NSEL) || d->naff_has_required[i] > 1) return bad("node-affinity record out of range");
+  for (int i = 0; i < ntm; ++i) if (!in(d->term_expr_sel[i], -1, NSEL)) return bad("node-affinity term selector out of range");
+  for (int64_t q = 0; q < fields; ++q)
+    if (!in(d->field_op[q], CAE_OP_IN, CAE_OP_NOT_IN + 1) || d->field_node_name[q] < 0) return bad("matchFields entry out of range");
+  for (int64_t q = 0; q < tents; ++q)
+    if (d->tol_key[q] < -1 || !in(d->tol_op[q], CAE_TOL_EQUAL, CAE_TOL_INVALID + 1) || !in(d->tol_val[q], -1, NV) ||
+        !in(d->tol_effect[q], CAE_EFFECT_NONE, CAE_EFFECT_NO_EXECUTE + 1))
+      return bad("toleration out of range");
+  for (int64_t q = 0; q < pents; ++q)
+    if (d->port_ip[q] < 0 || !in(d->port_proto[q], CAE_PROTO_TCP, CAE_PROTO_SCTP + 1) || d->port_num[q] <= 0) return bad("host port out of range");
+  for (int64_t q = 0; q < cents; ++q)
+    if (d->pts_key[q] < 0 || !in(d->pts_selector[q], 0, NSEL) || !in(d->pts_node_affinity_policy[q], 0, 2) ||
+        !in(d->pts_node_taints_policy[q], 0, 2))
+      return bad("topology spread constraint out of range");
+  for (int i = 0; i < nat; ++i)
+    if (!in(d->aterm_selector[i], 0, NSEL) || d->aterm_key[i] < 0 || !in(d->aterm_ns_selector[i], 0, NSEL)) return bad("affinity term out of range");
+  for (int64_t q = 0; q < nsents; ++q) if (!in(d->aterm_ns[q], 0, NNS)) return bad("affinity term namespace out of range");
+  for (int i = 0; i < nsp; ++i) {
+    if (!in(d->ps_namespace[i], 0, NNS) || !in(d->ps_labelset[i], 0, NL) || !in(d->ps_tol_list[i], 0, NTL) ||
+        !in(d->ps_naff[i], -1, NNF) || d->ps_node_name[i] < -1 || !in(d->ps_port_list[i], 0, NPL) || !in(d->ps_pts_list[i], 0, NPTS) ||
+        !in(d->ps_aff_list[i], 0, NAL) || !in(d->ps_anti_list[i], 0, NAL) || d->ps_terminating[i] > 1 || d->ps_hostname_spread[i] > 1)
+      return bad("pod-spec id out of range");
+    for (int r = 0; r < R; ++r)
+      if (d->ps_req[(size_t)i * R + r] < 0) return bad("pod-spec request negative");
+  }
+  for (int p = 0; p < P; ++p) if (!in(d->pend_spec[p], 0, S)) return bad("pending pod-spec id out of range");
+  for (int i = 0; i < nsp; ++i)   // a new resource dimension changes num_res: a full load
+    for (int r = ph.num_res; r < R; ++r)
+      if (d->ps_req[(size_t)i * R + r] != 0) { set_error("cae_load_pods: a request in a dim past the load's num_res"); return 2; }
+  e->stats.h2d_bytes = 0;
+  // ---- the node side the derivation reads on the host: the specs of the resident pods, each row's label set ----
+  std::vector<uint8_t> resident(S, 0);
+  std::vector<int32_t> row_ls((size_t)e->N + e->T);
+  if (pd_resident_specs(e, S0, resident.data(), row_ls.data())) { e->loaded = false; return -1; }
+
+  // ---- the host mirrors the derivation reads, with the tails appended (taken back if a limit refuses the delta) ----
+  const size_t ls0 = nh.ls_off.size(), lp0 = nh.ls_key.size(), po0 = ph.port_off.size(), co0 = ph.pts_off.size(), ck0 = ph.pts_key.size();
+  const size_t ao0 = ph.aff_off.size(), ak0 = ph.aterm_key.size();
+  const int32_t old_pairs = nh.ls_off.back(), old_pents = ph.port_off.back(), old_cents = ph.pts_off.back();
+  for (int j = 0; j < nl; ++j) nh.ls_off.push_back(old_pairs + d->ls_off[j + 1]);
+  nh.ls_key.insert(nh.ls_key.end(), d->ls_key, d->ls_key + pairs);
+  nh.ls_val.insert(nh.ls_val.end(), d->ls_val, d->ls_val + pairs);
+  for (int j = 0; j < npl; ++j) ph.port_off.push_back(old_pents + d->port_off[j + 1]);
+  for (int j = 0; j < npts; ++j) ph.pts_off.push_back(old_cents + d->pts_off[j + 1]);
+  ph.pts_key.insert(ph.pts_key.end(), d->pts_key, d->pts_key + cents);
+  for (int j = 0; j < nal; ++j) ph.aff_off.push_back(ph.num_aterms + d->aff_off[j + 1]);
+  ph.aterm_key.insert(ph.aterm_key.end(), d->aterm_key, d->aterm_key + nat);
+  std::vector<int32_t>* cols[9] = {&ph.ps_namespace, &ph.ps_labelset, &ph.ps_tol_list, &ph.ps_naff, &ph.ps_node_name, &ph.ps_port_list,
+                                    &ph.ps_pts_list, &ph.ps_aff_list, &ph.ps_anti_list};
+  const int32_t* tails[9] = {d->ps_namespace, d->ps_labelset, d->ps_tol_list, d->ps_naff, d->ps_node_name, d->ps_port_list,
+                             d->ps_pts_list, d->ps_aff_list, d->ps_anti_list};
+  for (int c = 0; c < 9; ++c) cols[c]->insert(cols[c]->end(), tails[c], tails[c] + nsp);
+  e->h_spec_req.insert(e->h_spec_req.end(), d->ps_req, d->ps_req + (size_t)nsp * R);
+  auto take_back = [&]() {
+    nh.ls_off.resize(ls0); nh.ls_key.resize(lp0); nh.ls_val.resize(lp0); ph.port_off.resize(po0); ph.pts_off.resize(co0);
+    ph.pts_key.resize(ck0); ph.aff_off.resize(ao0); ph.aterm_key.resize(ak0);
+    for (int c = 0; c < 9; ++c) cols[c]->resize(S0);
+    e->h_spec_req.resize((size_t)S0 * R);
+  };
+  cae_objects v{};
+  v.abi_version = CAE_ABI_VERSION; v.num_res = ph.num_res; v.num_values = (int32_t)NV; v.hostname_key = ph.hostname_key;
+  v.num_labelsets = (int32_t)NL; v.ls_off = nh.ls_off.data(); v.ls_key = nh.ls_key.data(); v.ls_val = nh.ls_val.data();
+  v.num_port_lists = (int32_t)NPL; v.port_off = ph.port_off.data();
+  v.num_pts_lists = (int32_t)NPTS; v.pts_off = ph.pts_off.data(); v.pts_key = ph.pts_key.data();
+  v.num_aff_lists = (int32_t)NAL; v.aff_off = ph.aff_off.data(); v.aterm_key = ph.aterm_key.data(); v.num_aterms = ph.num_aterms + nat;
+  v.num_podspecs = (int32_t)S; v.ps_namespace = ph.ps_namespace.data(); v.ps_labelset = ph.ps_labelset.data();
+  v.ps_req = e->h_spec_req.data(); v.ps_tol_list = ph.ps_tol_list.data(); v.ps_naff = ph.ps_naff.data();
+  v.ps_node_name = ph.ps_node_name.data(); v.ps_port_list = ph.ps_port_list.data(); v.ps_pts_list = ph.ps_pts_list.data();
+  v.ps_aff_list = ph.ps_aff_list.data(); v.ps_anti_list = ph.ps_anti_list.data();
+  v.num_cluster_nodes = e->N; v.num_templates = e->T; v.node_labelset = row_ls.data();
+  v.num_groups = E; v.num_pending = P; v.group_off = d->group_off; v.pend_spec = d->pend_spec;
+
+  // ---- commit: one pinned blob and one H2D copy of every tail (offsets made absolute), then the device tables grow ----
+  DevObjects& o = e->dobj;
+  struct Col { Engine::DevBuf* buf; const void** cur; size_t elem, n_old; const void* src; size_t n; int64_t base; bool off; };
+  auto C_ = [](Engine::DevBuf& b, const void* field_addr, size_t elem, size_t n_old, const void* src, size_t n) {
+    return Col{&b, (const void**)field_addr, elem, n_old, src, n, 0, false};
+  };
+  auto O_ = [](Engine::DevBuf& b, const void* field_addr, size_t n_old, const int32_t* rel, size_t n, int64_t base) {
+    return Col{&b, (const void**)field_addr, 4, n_old, rel, n, base, true};
+  };
+  Engine::DevBuf* t = e->pd_tab;
+  const Col col[] = {
+      C_(e->nd_tab[0], &o.value_is_int, 1, nh.num_values, d->value_is_int, nv), C_(e->nd_tab[1], &o.value_int, 8, nh.num_values, d->value_int, nv),
+      C_(t[0], &o.ns_labelset, 4, ph.num_namespaces, d->ns_labelset, nns), C_(t[1], &o.ns_exists, 1, ph.num_namespaces, d->ns_exists, nns),
+      O_(e->nd_tab[2], &o.ls_off, (size_t)nh.num_labelsets + 1, d->ls_off, nl, old_pairs),
+      C_(e->nd_tab[3], &o.ls_key, 4, old_pairs, d->ls_key, pairs), C_(e->nd_tab[4], &o.ls_val, 4, old_pairs, d->ls_val, pairs),
+      C_(t[2], &o.req_key, 4, ph.num_reqs, d->req_key, nrq), C_(t[3], &o.req_op, 4, ph.num_reqs, d->req_op, nrq),
+      O_(t[4], &o.req_val_off, (size_t)ph.num_reqs + 1, d->req_val_off, nrq, ph.req_vals), C_(t[5], &o.req_vals, 4, ph.req_vals, d->req_vals, rvals),
+      C_(t[6], &o.sel_kind, 4, ph.num_selectors, d->sel_kind, nsel),
+      O_(t[7], &o.sel_req_off, (size_t)ph.num_selectors + 1, d->sel_req_off, nsel, ph.num_reqs),
+      C_(t[8], &o.naff_nodesel, 4, ph.num_naff, d->naff_nodesel, nnf), C_(t[9], &o.naff_has_required, 1, ph.num_naff, d->naff_has_required, nnf),
+      O_(t[10], &o.naff_term_off, (size_t)ph.num_naff + 1, d->naff_term_off, nnf, ph.num_naff_terms),
+      C_(t[11], &o.term_expr_sel, 4, ph.num_naff_terms, d->term_expr_sel, ntm),
+      O_(t[12], &o.term_field_off, (size_t)ph.num_naff_terms + 1, d->term_field_off, ntm, ph.fields),
+      C_(t[13], &o.field_op, 4, ph.fields, d->field_op, fields), C_(t[14], &o.field_node_name, 4, ph.fields, d->field_node_name, fields),
+      O_(t[15], &o.tol_off, (size_t)ph.num_tol_lists + 1, d->tol_off, ntol, ph.tol_entries),
+      C_(t[16], &o.tol_key, 4, ph.tol_entries, d->tol_key, tents), C_(t[17], &o.tol_op, 4, ph.tol_entries, d->tol_op, tents),
+      C_(t[18], &o.tol_val, 4, ph.tol_entries, d->tol_val, tents), C_(t[19], &o.tol_effect, 4, ph.tol_entries, d->tol_effect, tents),
+      O_(t[20], &o.port_off, po0, d->port_off, npl, old_pents),
+      C_(t[21], &o.port_ip, 4, old_pents, d->port_ip, pents), C_(t[22], &o.port_proto, 4, old_pents, d->port_proto, pents),
+      C_(t[23], &o.port_num, 4, old_pents, d->port_num, pents),
+      O_(t[24], &o.pts_off, co0, d->pts_off, npts, old_cents),
+      C_(t[25], &o.pts_max_skew, 4, old_cents, d->pts_max_skew, cents), C_(t[26], &o.pts_key, 4, old_cents, d->pts_key, cents),
+      C_(t[27], &o.pts_selector, 4, old_cents, d->pts_selector, cents), C_(t[28], &o.pts_min_domains, 4, old_cents, d->pts_min_domains, cents),
+      C_(t[29], &o.pts_node_affinity_policy, 4, old_cents, d->pts_node_affinity_policy, cents),
+      C_(t[30], &o.pts_node_taints_policy, 4, old_cents, d->pts_node_taints_policy, cents),
+      O_(t[31], &o.aff_off, ao0, d->aff_off, nal, ph.num_aterms),
+      C_(t[32], &o.aterm_selector, 4, ph.num_aterms, d->aterm_selector, nat), C_(t[33], &o.aterm_key, 4, ph.num_aterms, d->aterm_key, nat),
+      O_(t[34], &o.aterm_ns_off, (size_t)ph.num_aterms + 1, d->aterm_ns_off, nat, ph.aterm_ns),
+      C_(t[35], &o.aterm_ns, 4, ph.aterm_ns, d->aterm_ns, nsents), C_(t[36], &o.aterm_ns_selector, 4, ph.num_aterms, d->aterm_ns_selector, nat),
+      C_(t[37], &o.ps_namespace, 4, S0, d->ps_namespace, nsp), C_(t[38], &o.ps_labelset, 4, S0, d->ps_labelset, nsp),
+      C_(t[39], &o.ps_req, 8 * R, S0, d->ps_req, nsp), C_(t[40], &o.ps_tol_list, 4, S0, d->ps_tol_list, nsp),
+      C_(t[41], &o.ps_naff, 4, S0, d->ps_naff, nsp), C_(t[42], &o.ps_node_name, 4, S0, d->ps_node_name, nsp),
+      C_(t[43], &o.ps_port_list, 4, S0, d->ps_port_list, nsp), C_(t[44], &o.ps_pts_list, 4, S0, d->ps_pts_list, nsp),
+      C_(t[45], &o.ps_aff_list, 4, S0, d->ps_aff_list, nsp), C_(t[46], &o.ps_anti_list, 4, S0, d->ps_anti_list, nsp),
+      C_(t[47], &o.ps_terminating, 1, S0, d->ps_terminating, nsp), C_(t[48], &o.ps_hostname_spread, 1, S0, d->ps_hostname_spread, nsp),
+  };
+  auto commit = [&]() -> int {
+    size_t bytes = 0;
+    std::vector<size_t> at;
+    for (const Col& c : col) { at.push_back(bytes); bytes = (bytes + c.n * c.elem + 7) & ~(size_t)7; }
+    if (pinned_reserve(e, e->pd_stage, std::max<size_t>(bytes, 8))) return -1;
+    char* h = static_cast<char*>(e->pd_stage.p);
+    for (size_t i = 0; i < sizeof(col) / sizeof(col[0]); ++i) {
+      const Col& c = col[i];
+      if (!c.n) continue;
+      if (c.off) for (size_t j = 0; j < c.n; ++j) reinterpret_cast<int32_t*>(h + at[i])[j] = (int32_t)(c.base + static_cast<const int32_t*>(c.src)[j + 1]);
+      else memcpy(h + at[i], c.src, c.n * c.elem);
+    }
+    if (devbuf_reserve(e, e->pd_blob, std::max<size_t>(bytes, 8))) return -1;
+    char* dv = static_cast<char*>(e->pd_blob.p);
+    if (bytes) CAE_CUDA(cudaMemcpyAsync(dv, h, bytes, cudaMemcpyHostToDevice, e->stream));
+    CAE_CUDA(cudaEventRecord(e->pd_stage.ev, e->stream));
+    e->stats.h2d_bytes += (int64_t)bytes;
+    for (size_t i = 0; i < sizeof(col) / sizeof(col[0]); ++i)
+      if (grow_bytes(e, *col[i].buf, *col[i].cur, col[i].elem, col[i].n_old, dv + at[i], col[i].n)) return -1;
+    // host counts and per-spec state of the grown tables
+    o.num_values = (int32_t)NV;
+    nh.num_values = (int32_t)NV; nh.num_labelsets = (int32_t)NL;
+    ph.num_namespaces = (int32_t)NNS; ph.num_reqs += nrq; ph.req_vals += (int32_t)rvals; ph.num_selectors = (int32_t)NSEL;
+    ph.num_naff = (int32_t)NNF; ph.num_naff_terms += ntm; ph.fields += (int32_t)fields; ph.num_tol_lists = (int32_t)NTL;
+    ph.tol_entries += (int32_t)tents; ph.num_aterms += nat; ph.aterm_ns += (int32_t)nsents;
+    nh.spec_anti.resize(S);
+    for (int64_t s = S0; s < S; ++s) nh.spec_anti[s] = ph.aff_off[ph.ps_anti_list[s] + 1] > ph.aff_off[ph.ps_anti_list[s]];
+    return 0;
+  };
+  const int rc = derive_pending(e, &v, lt, &resident, commit);
+  if (rc > 0 || rc == -2) take_back();
+  else if (rc) e->loaded = false;   // a CUDA error part way: the engine needs a cae_load
+  return rc;
+}
+
 }  // namespace cae
 
 using cae::Engine;
@@ -1078,6 +1427,7 @@ void cae_destroy(cae_engine* h) {
   Engine* e = reinterpret_cast<Engine*>(h);
   cudaSetDevice(e->cfg.device);
   e->up.release();
+  e->pup.release();
   e->scratch.release();
   for (int r = 0; r < Engine::PEER_MAX; ++r)   // the other ranks' exchange buffers, opened by cae_peer_attach
     if (r != e->cfg.rank && e->peer_base[r]) cudaIpcCloseMemHandle(e->peer_base[r]);
@@ -1143,6 +1493,14 @@ int32_t cae_load_node_churn(cae_engine* h, const cae_node_churn* c) {
   if (!c) { cae::set_error("cae_load_node_churn: no churn"); return -2; }
   cudaSetDevice(e->cfg.device);
   return cae::do_load_node_churn(e, c);
+}
+
+int32_t cae_load_pods(cae_engine* h, const cae_pod_delta* d) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_load_pods before cae_load"); return -2; }
+  if (!d) { cae::set_error("cae_load_pods: no delta"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_load_pods(e, d);
 }
 
 int32_t cae_feasibility(cae_engine* h, uint32_t* fit_bits, uint8_t* reasons, int32_t* fit_count) {

@@ -99,9 +99,10 @@ struct Engine {
   cae_config cfg{};
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
-  Arena up;         // uploaded tables (pinned mirror), reset per load
-  Arena scratch;    // device-only tables of the current load
-  Engine() { up.mirrored = true; }
+  Arena up;         // uploaded object tables (pinned mirror), reset per load
+  Arena pup;        // uploaded tables of the pending-side derivation (pinned mirror), reset per cae_load / cae_load_pods
+  Arena scratch;    // device-only tables of the pending-side derivation, reset with pup
+  Engine() { up.mirrored = true; pup.mirrored = true; }
   DynTables dyn;    // PodTopologySpread / InterPodAffinity tables (dyn.cuh)
   const uint8_t* d_spec_used = nullptr;
   const int32_t* d_dc_ngroups = nullptr;
@@ -229,6 +230,20 @@ struct Engine {
     std::vector<int32_t> q_k;                      // [Q] topology key of each counter (its pool segment has Dc[q_k] entries)
     std::vector<int32_t> dom_scratch;              // value id -> domain while the domains are assigned (all -1 in between)
   } nh;
+  // host mirrors of the spec-side tables the pending-side derivation reads (derive_pending in api.cu), so that
+  // cae_load_pods can rerun it without the caller's cae_objects (the node side it reads from the device)
+  struct PodHost {
+    int32_t hostname_key = -1, num_res = 0;
+    int32_t num_namespaces = 0, num_reqs = 0, req_vals = 0, num_selectors = 0, num_naff = 0, num_naff_terms = 0, fields = 0;
+    int32_t num_tol_lists = 0, tol_entries = 0, num_aterms = 0, aterm_ns = 0;
+    std::vector<int32_t> ps_namespace, ps_labelset, ps_tol_list, ps_naff, ps_node_name, ps_port_list, ps_pts_list, ps_aff_list,
+        ps_anti_list;                              // [S] spec columns (requests: h_spec_req)
+    std::vector<int32_t> port_off, pts_off, pts_key, aff_off, aterm_key;
+  } ph;
+  DevBuf pd_tab[49];                      // spec-side dictionary tables and spec columns grown by cae_load_pods
+  PinnedBuf pd_stage;                     // cae_load_pods' tails, source of its one H2D copy
+  DevBuf pd_blob;                         // device copy of the tails
+  DevBuf pd_used;                         // [S] specs of the resident pods (pod_delta.cu)
   // buffers of cae_load_nodes (a cae_load points DevObjects back at its arena)
   DevBuf nd_tab[9];                       // grown dictionary tables: value_is_int, value_int, ls_off|key|val, taint_off|key|val|effect
   DevBuf nd_off[2], nd_spec[2];           // double-buffered resident CSR (node_pod_off / node_pod_spec)
@@ -308,6 +323,18 @@ struct RemovalState {
   GroupRecSrc grs;
 };
 int launch_removals(Engine* e, const RemovalLaunch& r);
+// pod_delta.cu: the T x ranks and N x R part of the pending-side derivation, shared by cae_load and cae_load_pods
+struct RankArgs {
+  int A, N, T, Tw, Twp, W, lut_rows, feas_B, Bpad;
+  int act[CAE_MAX_RES], f_word[CAE_MAX_RES], f_shift[CAE_MAX_RES], f_bits[CAE_MAX_RES], lut_base[CAE_MAX_RES];
+  uint32_t lut_mask[CAE_MAX_RES];
+  int rv_off[CAE_MAX_RES + 1];            // the distinct requests of active dim k: rvals[rv_off[k], rv_off[k + 1]), ascending
+  uint8_t sword[32], sshift[32];
+};
+// c_free [A][N], tmpl_free [A][T], tmpl_w [W][T] (scratch), rlut and (when e->d_tslice is set) tslice
+int launch_rank_tables(Engine* e, const RankArgs& a, const int64_t* d_rvals, uint32_t* d_tmpl_w);
+// cae_load_pods: the specs the resident pods use ([S] flags) and the rows' label sets ([N + T]), on the host
+int pd_resident_specs(Engine* e, int S, uint8_t* h_used, int32_t* h_labelset);
 int launch_price(Engine* e, const cae_price_inputs& in_dev, const int32_t* d_node_count, const int32_t* d_sched, const int32_t* d_order,
                  double* d_score);
 int launch_waste(Engine* e, const int32_t* d_node_count, const int32_t* d_sched, double* d_waste);

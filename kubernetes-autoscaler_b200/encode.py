@@ -501,6 +501,68 @@ class EncodedObjects:
         res.struct = out._restruct(a, num_cluster_nodes=len(keep) + na)
         return res
 
+    def apply_pod_delta(self, delta: "PodDelta") -> "EncodedObjects":
+        """The objects after cae_load_pods(delta), stated on the host: every dictionary tail and the new specs appended
+        (tail offsets made absolute) and the pending list replaced.  A cae_load of the result must answer like the engine
+        after the delta."""
+        import copy
+        a, d, s = dict(self.arrays), delta.arrays, self.struct
+
+        def cat(nm, n_old, tail, dtype=np.int32):
+            return np.ascontiguousarray(np.concatenate([a[nm][:n_old], np.asarray(tail, dtype)]).astype(dtype))
+
+        def csr(off_nm, n_lists, child_nms, dtypes=None):
+            """an offsets table of n_lists resident lists and its child columns"""
+            c0 = int(a[off_nm][n_lists])
+            a[off_nm] = cat(off_nm, n_lists + 1, c0 + d[off_nm][1:])
+            for nm in child_nms:
+                a[nm] = cat(nm, c0, d[nm], (dtypes or {}).get(nm, np.int32))
+
+        nv, nns = s.num_values, s.num_namespaces
+        a["value_is_int"] = cat("value_is_int", nv, d["value_is_int"], np.uint8)
+        a["value_int"] = cat("value_int", nv, d["value_int"], np.int64)
+        a["ns_labelset"] = cat("ns_labelset", nns, d["ns_labelset"])
+        a["ns_exists"] = cat("ns_exists", nns, d["ns_exists"], np.uint8)
+        csr("ls_off", s.num_labelsets, ("ls_key", "ls_val"))
+        # requirements and their values, then the selectors over the requirements
+        a["req_key"] = cat("req_key", s.num_reqs, d["req_key"])
+        a["req_op"] = cat("req_op", s.num_reqs, d["req_op"])
+        csr("req_val_off", s.num_reqs, ("req_vals",))
+        a["sel_kind"] = cat("sel_kind", s.num_selectors, d["sel_kind"])
+        a["sel_req_off"] = cat("sel_req_off", s.num_selectors + 1, s.num_reqs + d["sel_req_off"][1:])
+        a["naff_nodesel"] = cat("naff_nodesel", s.num_naff, d["naff_nodesel"])
+        a["naff_has_required"] = cat("naff_has_required", s.num_naff, d["naff_has_required"], np.uint8)
+        a["naff_term_off"] = cat("naff_term_off", s.num_naff + 1, s.num_naff_terms + d["naff_term_off"][1:])
+        a["term_expr_sel"] = cat("term_expr_sel", s.num_naff_terms, d["term_expr_sel"])
+        csr("term_field_off", s.num_naff_terms, ("field_op", "field_node_name"))
+        csr("tol_off", s.num_tol_lists, ("tol_key", "tol_op", "tol_val", "tol_effect"))
+        csr("port_off", s.num_port_lists, ("port_ip", "port_proto", "port_num"))
+        csr("pts_off", s.num_pts_lists, ("pts_max_skew", "pts_key", "pts_selector", "pts_min_domains",
+                                         "pts_node_affinity_policy", "pts_node_taints_policy"))
+        a["aff_off"] = cat("aff_off", s.num_aff_lists + 1, s.num_aterms + d["aff_off"][1:])
+        a["aterm_selector"] = cat("aterm_selector", s.num_aterms, d["aterm_selector"])
+        a["aterm_key"] = cat("aterm_key", s.num_aterms, d["aterm_key"])
+        a["aterm_ns_selector"] = cat("aterm_ns_selector", s.num_aterms, d["aterm_ns_selector"])
+        csr("aterm_ns_off", s.num_aterms, ("aterm_ns",))
+        S = s.num_podspecs
+        for nm in ("ps_namespace", "ps_labelset", "ps_tol_list", "ps_naff", "ps_node_name", "ps_port_list", "ps_pts_list",
+                   "ps_aff_list", "ps_anti_list"):
+            a[nm] = cat(nm, S, d[nm])
+        a["ps_terminating"] = cat("ps_terminating", S, d["ps_terminating"], np.uint8)
+        a["ps_hostname_spread"] = cat("ps_hostname_spread", S, d["ps_hostname_spread"], np.uint8)
+        a["ps_req"] = np.ascontiguousarray(np.concatenate([a["ps_req"][:S], d["ps_req"]]).astype(np.int64))
+        a["pend_spec"] = np.ascontiguousarray(d["pend_spec"], np.int32)
+        a["group_off"] = np.ascontiguousarray(d["group_off"], np.int32)
+        out = copy.copy(self)
+        out.arrays = a
+        out.struct = self._restruct(
+            a, num_values=len(a["value_is_int"]), num_namespaces=len(a["ns_labelset"]), num_labelsets=len(a["ls_off"]) - 1,
+            num_reqs=len(a["req_key"]), num_selectors=len(a["sel_kind"]), num_naff=len(a["naff_nodesel"]),
+            num_naff_terms=len(a["term_expr_sel"]), num_tol_lists=len(a["tol_off"]) - 1, num_port_lists=len(a["port_off"]) - 1,
+            num_pts_lists=len(a["pts_off"]) - 1, num_aff_lists=len(a["aff_off"]) - 1, num_aterms=len(a["aterm_selector"]),
+            num_podspecs=len(a["ps_namespace"]), num_pending=len(a["pend_spec"]), num_groups=len(a["group_off"]) - 1)
+        return out
+
     def _restruct(self, arrays, **counts) -> "capi.cae_objects":
         s = capi.cae_objects()
         C.memmove(C.byref(s), C.byref(self.struct), C.sizeof(s))
@@ -607,6 +669,49 @@ class NodeChurn:
     @property
     def num_added(self) -> int:
         return self.struct.num_added
+
+    def ptr(self):
+        return C.byref(self.struct)
+
+
+class PodDelta:
+    """Owns the numpy arrays behind one ``cae_pod_delta`` struct: the dictionary tails and new pod specs (continuing the
+    resident tables; offsets relative to the tail) and the complete new pending list.  Field names are the header's."""
+
+    # count field -> the array whose length gives it (minus one for an offsets array)
+    _COUNTS = {"num_new_values": "value_is_int", "num_new_namespaces": "ns_labelset", "num_new_labelsets": "ls_off",
+               "num_new_reqs": "req_key", "num_new_selectors": "sel_kind", "num_new_naff": "naff_nodesel",
+               "num_new_naff_terms": "term_expr_sel", "num_new_tol_lists": "tol_off", "num_new_port_lists": "port_off",
+               "num_new_pts_lists": "pts_off", "num_new_aff_lists": "aff_off", "num_new_aterms": "aterm_selector",
+               "num_new_specs": "ps_namespace", "num_groups": "group_off", "num_pending": "pend_spec"}
+    _OFFSETS = ("ls_off", "req_val_off", "sel_req_off", "naff_term_off", "term_field_off", "tol_off", "port_off", "pts_off",
+                "aff_off", "aterm_ns_off", "group_off")
+
+    def __init__(self, **arrays) -> None:
+        a: Dict[str, np.ndarray] = {}
+        for name, ctype in capi.cae_pod_delta._fields_:
+            if not hasattr(ctype, "contents"):
+                continue
+            dt = {C.c_uint8: np.uint8, C.c_int64: np.int64}.get(ctype._type_, np.int32)
+            a[name] = np.ascontiguousarray(arrays.get(name, [0] if name in self._OFFSETS else []), dt)
+        a["ps_req"] = np.ascontiguousarray(a["ps_req"].reshape(len(a["ps_namespace"]), MAX_RES))
+        self.arrays = a
+        s = capi.cae_pod_delta()
+        s.abi_version = capi.CONST["CAE_ABI_VERSION"]
+        for cnt, nm in self._COUNTS.items():
+            setattr(s, cnt, len(a[nm]) - (nm in self._OFFSETS))
+        for name, ctype in capi.cae_pod_delta._fields_:
+            if name in a:
+                setattr(s, name, a[name].ctypes.data_as(ctype))
+        self.struct = s
+
+    def replace(self, **arrays) -> "PodDelta":
+        """A copy with some arrays replaced (the counts follow the arrays)."""
+        return PodDelta(**{**self.arrays, **arrays})
+
+    @property
+    def num_new_specs(self) -> int:
+        return self.struct.num_new_specs
 
     def ptr(self):
         return C.byref(self.struct)
@@ -791,6 +896,10 @@ class Encoder:
         enc = self.b.finish()
         # what the engine holds after a load of `enc`: node_delta() emits what the interner adds beyond it as tails
         self._emitted = (enc.struct.num_values, enc.struct.num_labelsets, enc.struct.num_taint_lists)
+        s = enc.struct   # the spec-side tables the engine holds: pod_delta() emits what the interner adds beyond them
+        self._pods_emitted = dict(ns=s.num_namespaces, reqs=s.num_reqs, sel=s.num_selectors, naff=s.num_naff,
+                                  terms=s.num_naff_terms, tols=s.num_tol_lists, ports=s.num_port_lists, pts=s.num_pts_lists,
+                                  aff=s.num_aff_lists, aterms=s.num_aterms, specs=s.num_podspecs, num_res=s.num_res)
         self._delta_ok = True
         self._spec_wo_name: Optional[Dict[tuple, int]] = None
         # the cluster rows the engine holds: (node-name id, row state) per row, kept current by node_delta / node_churn
@@ -800,10 +909,10 @@ class Encoder:
                          for r in range(b.num_cluster_nodes)]
         return enc
 
-    def _resident_spec(self, pod: Pod) -> int:
+    def _resident_spec(self, pod: Pod, allow_new: bool = False) -> int:
         """Spec id of a resident pod of a changed node, among the specs of the last load.  No filter reads a resident pod's
         spec.nodeName (only the incoming pod's), so the lookup ignores it: a pod bound since the last tick finds its
-        pending spec.  No match: Unsupported (the tick needs a full load)."""
+        pending spec.  No match: Unsupported (the tick needs a full load), or with `allow_new` (pod_delta) a new spec."""
         b = self.b
         n = len(b.ps_rows)
         saved, self._podspec_cache = self._podspec_cache, {}
@@ -816,6 +925,11 @@ class Encoder:
         key = b.ps_rows.pop()           # the interner added a row: take it back and look for the same spec without nodeName
         del b.ps_ids[key]
         hit = b.ps_ids.get(key[:5] + (-1,) + key[6:])
+        if hit is None and allow_new:   # the first pod of a new spec: keep the row
+            b.ps_ids[key] = sid
+            b.ps_rows.append(key)
+            self._spec_wo_name = None
+            return sid
         if hit is None:
             if self._spec_wo_name is None:
                 self._spec_wo_name = {}
@@ -935,6 +1049,67 @@ class Encoder:
                           allowed_pods=[st[4] for _, st in added], pod_off=po, pod_spec=[x for _, st in added for x in st[5]])
         self._cluster = new_list + added
         return churn
+
+    def pod_delta(self, groups: Sequence[PodEquivalenceGroup], residents: Sequence[NodeInfo] = ()) -> "PodDelta":
+        """The shim's side of cae_load_pods: `groups` become the complete new pending list, and every spec and dictionary
+        entry interned since the last load or delta becomes a tail.  The pods of `residents` (the changed or added nodes
+        of this tick) are interned first, so that the node_delta / node_churn that follows finds their specs; the tick
+        is load_pods, then the node call.  Unsupported: a resource dimension the last load did not have (a full load)."""
+        self._check_resident()
+        b, em = self.b, self._pods_emitted
+        for ni in residents:
+            for p in ni.pods:
+                self._resident_spec(p, allow_new=True)
+        pend, off = [], [0]
+        for g in groups:
+            pend.extend(self.podspec(p) for p in g.pods)
+            off.append(len(pend))
+        if len(self.resources) > em["num_res"]:
+            self._delta_ok = False
+            raise Unsupported("a pod requests a resource the last load did not have")
+        if len(b.ns_labelset) < em["ns"]:
+            self._delta_ok = False
+            raise Unsupported("the namespace table of the last load was padded")
+        nv0, nl0, nt0 = self._emitted
+        L = b.labelsets
+        lp0, r0, s0, f0, t0 = L.off[nl0], em["reqs"], em["sel"], em["naff"], em["terms"]
+        rv0, fd0, a0 = b.reqs_val_off[r0], b.term_field_off[t0], em["aterms"]
+        ns0 = b.aterm_ns_off[a0]
+
+        def tail(csr, n0, names):
+            c0 = csr.off[n0]
+            return dict([(names[0], [o - c0 for o in csr.off[n0:]])] + [(nm, csr.cols[i][c0:]) for i, nm in enumerate(names[1:])])
+
+        rows = b.ps_rows[em["specs"]:]
+        cols = list(zip(*rows)) if rows else [[] for _ in range(12)]
+        delta = PodDelta(
+            value_is_int=b.value_is_int[nv0:], value_int=b.value_int[nv0:],
+            ns_labelset=b.ns_labelset[em["ns"]:], ns_exists=b.ns_exists[em["ns"]:],
+            ls_off=[o - lp0 for o in L.off[nl0:]], ls_key=L.cols[0][lp0:], ls_val=L.cols[1][lp0:],
+            req_key=b.reqs_key[r0:], req_op=b.reqs_op[r0:], req_val_off=[o - rv0 for o in b.reqs_val_off[r0:]],
+            req_vals=b.reqs_vals[rv0:], sel_kind=b.sel_kind[s0:], sel_req_off=[o - r0 for o in b.sel_req_off[s0:]],
+            naff_nodesel=b.naff_nodesel[f0:], naff_has_required=b.naff_has_required[f0:],
+            naff_term_off=[o - t0 for o in b.naff_term_off[f0:]], term_expr_sel=b.term_expr_sel[t0:],
+            term_field_off=[o - fd0 for o in b.term_field_off[t0:]], field_op=b.field_op[fd0:],
+            field_node_name=b.field_node_name[fd0:],
+            **tail(b.tols, em["tols"], ("tol_off", "tol_key", "tol_op", "tol_val", "tol_effect")),
+            **tail(b.ports, em["ports"], ("port_off", "port_ip", "port_proto", "port_num")),
+            **tail(b.pts, em["pts"], ("pts_off", "pts_max_skew", "pts_key", "pts_selector", "pts_min_domains",
+                                      "pts_node_affinity_policy", "pts_node_taints_policy")),
+            aff_off=[o - a0 for o in b.aff_off[em["aff"]:]],
+            aterm_selector=b.aterm_selector[a0:], aterm_key=b.aterm_key[a0:],
+            aterm_ns_off=[o - ns0 for o in b.aterm_ns_off[a0:]], aterm_ns=b.aterm_ns[ns0:],
+            aterm_ns_selector=b.aterm_ns_selector[a0:],
+            ps_namespace=cols[0], ps_labelset=cols[1], ps_req=np.asarray(cols[2], np.int64).reshape(len(rows), MAX_RES),
+            ps_tol_list=cols[3], ps_naff=cols[4], ps_node_name=cols[5], ps_port_list=cols[6], ps_pts_list=cols[7],
+            ps_aff_list=cols[8], ps_anti_list=cols[9], ps_terminating=cols[10], ps_hostname_spread=cols[11],
+            group_off=off, pend_spec=pend)
+        self._emitted = (len(b.value_is_int), L.n, nt0)
+        self._pods_emitted = dict(ns=len(b.ns_labelset), reqs=len(b.reqs_key), sel=len(b.sel_kind), naff=len(b.naff_nodesel),
+                                  terms=len(b.term_expr_sel), tols=b.tols.n, ports=b.ports.n, pts=b.pts.n,
+                                  aff=len(b.aff_off) - 1, aterms=len(b.aterm_selector), specs=len(b.ps_rows),
+                                  num_res=em["num_res"])
+        return delta
 
 
 def encode(cluster: Sequence[NodeInfo], templates: Sequence[NodeInfo],

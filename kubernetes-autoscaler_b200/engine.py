@@ -164,6 +164,19 @@ class Engine:
         self._check(rc)
         return True
 
+    def load_pods(self, delta, enc: Optional[EncodedObjects] = None) -> int:
+        """The per-tick delta of the pod specs (cae_load_pods): new pod specs with the dictionary tails they need and the
+        complete new pending list (encode.PodDelta).  Returns the status: 0 applied, 1 a limit of the engine (use the stock
+        path), 2 a table would overflow (use a full load); the engine is unchanged unless 0.  `enc`: the objects the engine
+        now holds (EncodedObjects.apply_pod_delta), kept as this engine's shapes."""
+        rc = self.lib.cae_load_pods(self.h, delta.ptr())
+        if rc in (1, 2):
+            return rc
+        self._check(rc)
+        if enc is not None:
+            self.enc = enc
+        return 0
+
     def feasibility(self, want_bits: bool = True):
         """Dense pods x templates pass. Returns (fit_bits [T][ceil(Pl/32)] uint32 | None,
         reasons [T][Pl] uint8 | None, fit_count [T] int32) for this rank's pod shard."""

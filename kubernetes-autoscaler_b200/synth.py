@@ -452,3 +452,28 @@ def node_scale(enc: EncodedObjects, seed: int, n_remove: int, n_add: int, n_dirt
                       unschedulable=np.zeros(n_add, np.uint8), alloc=alloc, allowed_pods=allowed, pod_off=pod_off,
                       pod_spec=pod_spec)
     return churn, pending
+
+
+def pod_churn(enc: EncodedObjects, seed: int, arrive: int, leave: int):
+    """A deterministic random tick of workload churn against a snapshot of ``generate``: ``leave`` random pending groups
+    finish, and ``arrive`` new workloads come, each a new spec copied from a random pending spec with a new cpu request
+    (every third one also a new memory request) and 1..8 pending pods.  Returns the encode.PodDelta (no new dictionary
+    entries: the copies reuse the label sets, constraints and lists of their originals)."""
+    from .encode import PodDelta
+    rng = SplitMix64(0x90D5 ^ (seed * 0x9E3779B9))
+    a, S = enc.arrays, enc.struct.num_podspecs
+    go = a["group_off"]
+    E = len(go) - 1
+    gone = set(int(x) for x in rng.randint(leave, max(E, 1))) if E else set()
+    groups = [a["pend_spec"][go[g]:go[g + 1]] for g in range(E) if g not in gone]
+    pending = np.unique(a["pend_spec"]) if len(a["pend_spec"]) else np.arange(S)
+    src = pending[rng.randint(arrive, len(pending))] if len(pending) else np.zeros(arrive, np.int64)
+    cols = {nm: a[nm][src] for nm in ("ps_namespace", "ps_labelset", "ps_tol_list", "ps_naff", "ps_node_name", "ps_port_list",
+                                      "ps_pts_list", "ps_aff_list", "ps_anti_list", "ps_terminating", "ps_hostname_spread")}
+    req = a["ps_req"][src].copy()
+    req[:, 0] += 1 + rng.randint(arrive, 997)
+    req[::3, 1] += 1 << 20
+    sizes = 1 + rng.randint(arrive, 8)
+    groups += [np.full(int(sizes[i]), S + i, np.int32) for i in range(arrive)]
+    off = np.concatenate([[0], np.cumsum([len(g) for g in groups])]).astype(np.int32)
+    return PodDelta(ps_req=req, group_off=off, pend_spec=np.concatenate(groups) if groups else [], **cols)
