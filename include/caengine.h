@@ -624,6 +624,48 @@ int32_t cae_expander_chain_ex(const int32_t* chain, int32_t chain_len, int32_t n
                               const int32_t* pod_count, const double* waste_score, const double* price_score,
                               const uint8_t* price_error, const int32_t* priority, uint8_t* best_mask /* [T] */);
 
+/* Similar node groups of every loaded template and the similar-groups limiter cap, in one call.
+ * Replaces, with --balance-similar-node-groups: ComputeSimilarNodeGroups (core/scaleup/orchestrator/orchestrator.go:757-812)
+ * over FindSimilarNodeGroups with the generic comparator (processors/nodegroupset/balancing_processor.go:44-77,
+ * compare_nodegroups.go:88-163) for every template, and SngCapacityThreshold.NodeLimit (estimator/sng_capacity_threshold.go)
+ * on the result.  The candidates are the loaded templates: exact when they are the valid node groups (a group outside them
+ * has no schedulablePodGroups entry in Go, so it never passes the subset test).
+ * Group s is in row t iff s != t, eligible[t], safe[s], t's schedulable set {g : group reason[t][g] == CAE_R_OK} is
+ * non-empty and a subset of s's, and the comparator accepts the pair: equal res_sig, equal label sets once the ignored
+ * keys are removed, memory capacity within max_capacity_memory_difference_ratio, every allocatable dim and `pods`
+ * within max_allocatable_difference_ratio (a dim absent on both sides is 0 on both), cpu / memory / ephemeral-storage /
+ * `pods` and the dims in free_dims of allocatable minus the requests of the template's pods within
+ * max_free_difference_ratio.  A tolerance test is resourceListWithinTolerance (compare_nodegroups.go:57-64) on
+ * float64(Quantity.MilliValue()): larger - smaller <= larger * ratio, without fused multiply-add.
+ *   similar_bits [T][ceil(T/32)]  bit s%32 of word s/32 of row t: s is similar to t (the caller lists a row in its own
+ *                                 template order).  May be NULL.
+ *   similar_count [T]             groups in row t.  May be NULL.
+ *   sng_limit [T]                 max(max_size - target_size, 0) of t plus that of every group in row t, summed in int64;
+ *                                 -1 when the sum is <= 0.  May be NULL.
+ * Every rank computes all T rows (the group reasons cover every template); no collective is needed.
+ * Status -2 (nothing done): before a load, a NULL required array, an ignored key id < 0, a flag byte > 1.
+ * Status 1 (no output written): a memory, ephemeral-storage or scalar value the comparator reads has a magnitude past
+ *   INT64_MAX / 1000, where the exact milli conversion is impossible: use the stock path. */
+typedef struct cae_similarity_inputs {
+  int32_t abi_version; /* CAE_ABI_VERSION */
+  int32_t num_ignored_keys;
+  const int32_t* ignored_keys; /* label key ids: BasicIgnoredLabels + --balancing-ignore-label + provider extras; ids the
+                                  interner never gave out may be left out */
+  double max_allocatable_difference_ratio;
+  double max_free_difference_ratio;
+  double max_capacity_memory_difference_ratio;
+  const int32_t* res_sig;    /* [T] caller-interned: equal ids <=> same Allocatable key set, same Requested key set and the
+                                same Capacity map apart from memory's VALUE (memory's presence included) */
+  const uint32_t* free_dims; /* [T] bit r: dim r is a key of ResourceToResourceList(Requested); cpu, memory and
+                                ephemeral-storage always are */
+  const uint8_t* eligible;   /* [T] 0 = the group has ZeroOrMaxNodeScaling: it gets no similar groups */
+  const uint8_t* safe;       /* [T] NodeGroupScaleUpSafety(t).SafeToScale as a candidate; NULL = all */
+  const int32_t* max_size;   /* [T] */
+  const int32_t* target_size; /* [T] */
+} cae_similarity_inputs;
+int32_t cae_similar_node_groups(cae_engine* e, const cae_similarity_inputs* in, uint32_t* similar_bits, int32_t* similar_count,
+                                int64_t* sng_limit);
+
 int32_t cae_get_stats(cae_engine* e, cae_stats* out);
 
 /* Raw device pointers of the engine's result buffers, for zero-copy collectives (torch.distributed

@@ -104,6 +104,10 @@ class cae_pod_delta(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_pod_delta")
 
 
+class cae_similarity_inputs(C.Structure):
+    _fields_ = _parse_struct(_SRC, "cae_similarity_inputs")
+
+
 def declared_functions() -> List[str]:
     """Names of every function the header declares (used by the symbol-export test)."""
     return sorted(set(re.findall(r"\b(cae_\w+)\s*\(", _SRC)))
@@ -192,6 +196,8 @@ def load_engine_lib() -> C.CDLL:
     lib.cae_waste_scores.restype = C.c_int32
     lib.cae_expander_chain.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.cae_expander_chain.restype = C.c_int32
+    lib.cae_similar_node_groups.argtypes = [C.c_void_p, P(cae_similarity_inputs), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.cae_similar_node_groups.restype = C.c_int32
     lib.cae_stream.argtypes = [C.c_void_p]
     lib.cae_stream.restype = C.c_void_p
     _engine_lib = lib

@@ -688,6 +688,7 @@ static int do_load(Engine* e, const cae_objects* o) {
     nh.pod_cnt.resize(N);
     for (int n = 0; n < N; ++n) nh.pod_cnt[n] = o->node_pod_off[n + 1] - o->node_pod_off[n];
     nh.pod_total = o->node_pod_off[NT];
+    nh.tmpl_ls.assign(o->node_labelset + N, o->node_labelset + NT);
     nh.spec_anti.resize(S);
     for (int s = 0; s < S; ++s) nh.spec_anti[s] = o->aff_off[o->ps_anti_list[s] + 1] > o->aff_off[o->ps_anti_list[s]];
     e->h_spec_req.assign(o->ps_req, o->ps_req + (size_t)S * R);
@@ -1320,6 +1321,96 @@ static int do_load_pods(Engine* e, const cae_pod_delta* d) {
   return rc;
 }
 
+// cae_similar_node_groups.  The label signatures are built here from the host mirror of the label-set table: dense ids of
+// the templates' label-pair lists with the ignored keys removed (pairs are sorted by key id, so equal lists <=> equal maps).
+// Inputs travel in one H2D copy, outputs in one D2H copy; nothing is written to the caller's buffers unless the status is 0.
+static int do_similar(Engine* e, const cae_similarity_inputs* in, uint32_t* bits_out, int32_t* count_out, int64_t* limit_out) {
+  if (in->abi_version != CAE_ABI_VERSION) { set_error("cae_similarity_inputs.abi_version mismatch"); return -2; }
+  const int T = e->T, Tw = e->Tw, Ew = (e->E + 31) / 32;
+  const int nk = in->num_ignored_keys;
+  if (nk < 0 || (nk && !in->ignored_keys) ||
+      (T && (!in->res_sig || !in->free_dims || !in->eligible || !in->max_size || !in->target_size))) {
+    set_error("cae_similar_node_groups: a required array is NULL");
+    return -2;
+  }
+  std::vector<int32_t> ign(in->ignored_keys, in->ignored_keys + nk);
+  for (int32_t k : ign)
+    if (k < 0) { set_error("cae_similar_node_groups: ignored key id < 0"); return -2; }
+  for (int t = 0; t < T; ++t)
+    if (in->eligible[t] > 1 || (in->safe && in->safe[t] > 1)) { set_error("cae_similar_node_groups: flag byte > 1"); return -2; }
+  if (T == 0) return 0;
+  std::sort(ign.begin(), ign.end());
+
+  // layout (the same offsets on the device and in the pinned stage): inputs | outputs, then device-only scratch
+  const int K = 2 * e->dobj.num_res + 3;
+  size_t off = 0;
+  auto take = [&](size_t b) { const size_t o = off; off += (std::max<size_t>(b, 1) + 255) & ~(size_t)255; return o; };
+  const size_t o_i32 = take((size_t)16 * T), o_cap = take((size_t)8 * T), in_end = off;
+  const size_t o_status = take(8 + (size_t)12 * T), o_bits = take((size_t)4 * T * Tw), out_end = off;
+  const size_t o_x = take((size_t)8 * T * K), o_sched = take((size_t)4 * T * Ew);
+  if (pinned_reserve(e, e->sim_stage, out_end) || devbuf_reserve(e, e->sim_dev, off)) return -1;
+  char* h = static_cast<char*>(e->sim_stage.p);
+  char* d = static_cast<char*>(e->sim_dev.p);
+  int32_t* h_res = reinterpret_cast<int32_t*>(h + o_i32);
+  int32_t *h_lab = h_res + T, *h_fd = h_res + 2 * T, *h_fl = h_res + 3 * T;
+  int64_t* h_cap = reinterpret_cast<int64_t*>(h + o_cap);
+  const Engine::NodeHost& nh = e->nh;
+  std::unordered_map<std::string, int32_t> lab_id;
+  lab_id.reserve((size_t)T * 2);
+  std::string key;
+  for (int t = 0; t < T; ++t) {
+    key.clear();
+    const int ls = nh.tmpl_ls[t];
+    for (int i = nh.ls_off[ls]; i < nh.ls_off[ls + 1]; ++i) {
+      if (std::binary_search(ign.begin(), ign.end(), nh.ls_key[i])) continue;
+      const int32_t kv[2] = {nh.ls_key[i], nh.ls_val[i]};
+      key.append(reinterpret_cast<const char*>(kv), sizeof(kv));
+    }
+    h_lab[t] = lab_id.emplace(key, (int32_t)lab_id.size()).first->second;
+    h_res[t] = in->res_sig[t];
+    h_fd[t] = (int32_t)in->free_dims[t];
+    h_fl[t] = (in->eligible[t] ? 1 : 0) | (!in->safe || in->safe[t] ? 2 : 0);
+    h_cap[t] = std::max<int64_t>((int64_t)in->max_size[t] - in->target_size[t], 0);
+  }
+  CAE_CUDA(cudaMemcpyAsync(d, h, in_end, cudaMemcpyHostToDevice, e->stream));
+  CAE_CUDA(cudaEventRecord(e->sim_stage.ev, e->stream));
+  CAE_CUDA(cudaMemsetAsync(d + o_status, 0, 8 + (size_t)12 * T, e->stream));
+  SimLaunch s{};
+  s.ratio[0] = in->max_allocatable_difference_ratio;
+  s.ratio[1] = in->max_free_difference_ratio;
+  s.ratio[2] = in->max_capacity_memory_difference_ratio;
+  s.res_sig = reinterpret_cast<const int32_t*>(d + o_i32);
+  s.lab_sig = s.res_sig + T;
+  s.free_dims = s.res_sig + 2 * T;
+  s.flags = reinterpret_cast<int32_t*>(d + o_i32) + 3 * T;
+  s.cap = reinterpret_cast<const int64_t*>(d + o_cap);
+  s.status = reinterpret_cast<int32_t*>(d + o_status);
+  s.sum = reinterpret_cast<unsigned long long*>(d + o_status + 8);
+  s.count = reinterpret_cast<int32_t*>(d + o_status + 8 + (size_t)8 * T);
+  s.bits = reinterpret_cast<uint32_t*>(d + o_bits);
+  s.x = reinterpret_cast<double*>(d + o_x);
+  s.sched = reinterpret_cast<uint32_t*>(d + o_sched);
+  if (launch_similar(e, s)) return -1;
+  const size_t d2h = (bits_out ? out_end : o_bits) - o_status;
+  CAE_CUDA(cudaMemcpyAsync(h + o_status, d + o_status, d2h, cudaMemcpyDeviceToHost, e->stream));
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
+  e->stats.h2d_bytes = (int64_t)in_end;
+  e->stats.d2h_bytes = (int64_t)d2h;
+  if (*reinterpret_cast<const int32_t*>(h + o_status)) {
+    set_error("cae_similar_node_groups: a quantity past INT64_MAX / 1000 has no exact milli value: use the stock path");
+    return 1;
+  }
+  const int64_t* sum = reinterpret_cast<const int64_t*>(h + o_status + 8);
+  if (count_out) memcpy(count_out, h + o_status + 8 + (size_t)8 * T, (size_t)4 * T);
+  if (bits_out) memcpy(bits_out, h + o_bits, (size_t)4 * T * Tw);
+  if (limit_out)
+    for (int t = 0; t < T; ++t) {
+      const int64_t total = h_cap[t] + sum[t];
+      limit_out[t] = total <= 0 ? -1 : total;
+    }
+  return 0;
+}
+
 }  // namespace cae
 
 using cae::Engine;
@@ -1718,6 +1809,15 @@ int32_t cae_expander_chain_ex(const int32_t* chain, int32_t chain_len, int32_t n
   for (int c = 0; c < chain_len; ++c)
     if (chain[c] == CAE_EXP_LEAST_WASTE && !waste_score) { cae::set_error("least-waste filter without waste scores"); return -2; }
   return run_expander_chain(chain, chain_len, num_templates, node_count, pod_count, waste_score, best_mask, price_score, price_error, priority);
+}
+
+int32_t cae_similar_node_groups(cae_engine* h, const cae_similarity_inputs* in, uint32_t* similar_bits, int32_t* similar_count,
+                                int64_t* sng_limit) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_similar_node_groups before cae_load"); return -2; }
+  if (!in) { cae::set_error("cae_similar_node_groups: no inputs"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_similar(e, in, similar_bits, similar_count, sng_limit);
 }
 
 int32_t cae_get_stats(cae_engine* h, cae_stats* out) {

@@ -229,6 +229,7 @@ struct Engine {
     std::vector<int32_t> tkey_val;                 // [K][T] the same on the templates (domain rebuild of a churn)
     std::vector<int32_t> q_k;                      // [Q] topology key of each counter (its pool segment has Dc[q_k] entries)
     std::vector<int32_t> dom_scratch;              // value id -> domain while the domains are assigned (all -1 in between)
+    std::vector<int32_t> tmpl_ls;                  // [T] label set of each template (no delta changes a template)
   } nh;
   // host mirrors of the spec-side tables the pending-side derivation reads (derive_pending in api.cu), so that
   // cae_load_pods can rerun it without the caller's cae_objects (the node side it reads from the device)
@@ -253,6 +254,9 @@ struct Engine {
   DevBuf ch_nodes[2];                     // double-buffered node columns [N+T] + c_free [A][N] + c_slots [N] (node_delta.cu)
   DevBuf ch_pre;                          // pre_code [SC][U]
   DevBuf ch_dyn;                          // dom [K][N+T] | q_base_off [Q+1] | base_cnt, base_pres [pool] | elig [Q][U]
+  // buffers of cae_similar_node_groups (similar.cu)
+  DevBuf sim_dev;                         // inputs | outputs | operand rows | schedulable bit rows
+  PinnedBuf sim_stage;                    // inputs (one H2D copy) | outputs (one D2H copy)
   int sm_count = 132;
   int smem_optin = 227 * 1024;             // opt-in shared memory per thread block
   size_t hbm_bytes = (size_t)80 << 30;     // device memory (sizes the estimator's global slabs)
@@ -338,5 +342,23 @@ int pd_resident_specs(Engine* e, int S, uint8_t* h_used, int32_t* h_labelset);
 int launch_price(Engine* e, const cae_price_inputs& in_dev, const int32_t* d_node_count, const int32_t* d_sched, const int32_t* d_order,
                  double* d_score);
 int launch_waste(Engine* e, const int32_t* d_node_count, const int32_t* d_sched, double* d_waste);
+// similar.cu: cae_similar_node_groups.  In (device, uploaded by api.cu): res_sig, lab_sig, free_dims, flags [T] int32 (bit 0
+// eligible, bit 1 safe; the launch adds bit 2: non-empty schedulable set) and cap [T] int64 = max(max_size - target_size, 0).
+// Out (device; api.cu zeroes status, sum and count): status (1 = a value past INT64_MAX / 1000), sum [T] of the similar groups' caps,
+// count [T], bits [T][Tw].
+constexpr int SIM_KMAX = 2 * CAE_MAX_RES + 3;   // operand columns: alloc [num_res] | pods | free [num_res] | pods | memory capacity
+struct SimLaunch {
+  double ratio[3];                        // allocatable, free, memory capacity
+  const int32_t *res_sig, *lab_sig, *free_dims;
+  int32_t* flags;
+  const int64_t* cap;
+  int32_t* status;
+  unsigned long long* sum;
+  int32_t* count;
+  uint32_t* bits;
+  double* x;                              // scratch [T][K]
+  uint32_t* sched;                        // scratch [T][ceil(E/32)]
+};
+int launch_similar(Engine* e, const SimLaunch& s);
 
 }  // namespace cae

@@ -889,6 +889,29 @@ class Encoder:
     def add_group(self, g: PodEquivalenceGroup) -> int:
         return self.b.group([self.podspec(p) for p in g.pods])
 
+    # ---- inputs of cae_similar_node_groups ------------------------------------------------------
+    def similarity_signatures(self, templates: Sequence[NodeInfo]) -> Tuple[np.ndarray, np.ndarray]:
+        """(res_sig [T] int32, free_dims [T] uint32) of the encoded templates, in their order.  res_sig interns what the
+        comparator (compare_nodegroups.go:104-163) compares exactly: the Allocatable key set, the key set of
+        ResourceToResourceList(Requested) (cpu, memory, pods, ephemeral-storage always, plus every resource a pod of the
+        template requests) and the Capacity map with memory's value left out.  free_dims: bit r = dim r is such a key."""
+        sigs: Dict[tuple, int] = {}
+        res_sig = np.zeros(len(templates), np.int32)
+        free_dims = np.zeros(len(templates), np.uint32)
+        for t, ni in enumerate(templates):
+            requested = {"cpu", "memory", "pods", "ephemeral-storage"}
+            for p in ni.pods:
+                requested.update(p.requests)
+            cap = tuple(sorted((k, None if k == "memory" else int(v)) for k, v in ni.node.capacity.items()))
+            key = (frozenset(ni.node.allocatable), frozenset(requested), cap)
+            res_sig[t] = sigs.setdefault(key, len(sigs))
+            free_dims[t] = sum(1 << self.resources.ids[r] for r in requested if r != "pods")
+        return res_sig, free_dims
+
+    def label_key_ids(self, keys: Iterable[str]) -> np.ndarray:
+        """Key ids of label keys; a key the interner never saw is on no template and is left out."""
+        return np.asarray(sorted({self.keys.ids[k] for k in keys if k in self.keys.ids}), np.int32)
+
     def finish(self) -> EncodedObjects:
         self._key(LABEL_HOSTNAME)
         self._key(TAINT_NODE_UNSCHEDULABLE)
@@ -1114,8 +1137,9 @@ class Encoder:
 
 def encode(cluster: Sequence[NodeInfo], templates: Sequence[NodeInfo],
            groups: Sequence[PodEquivalenceGroup],
-           namespaces: Sequence[Namespace] = ()) -> EncodedObjects:
-    enc = Encoder()
+           namespaces: Sequence[Namespace] = (), encoder: Optional[Encoder] = None) -> EncodedObjects:
+    """encoder: the Encoder to intern with (a fresh one by default), for a caller that needs its dictionaries afterwards."""
+    enc = encoder or Encoder()
     for ns in namespaces:
         enc.add_namespace(ns)
     for ni in cluster:

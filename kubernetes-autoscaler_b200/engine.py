@@ -337,6 +337,38 @@ class Engine:
             return rc, None, None, np.zeros((int(n[0]), 3), np.int32)
         return rc, res[:len(cn)], int(li[0]), log[:int(n[0])]
 
+    def similar_node_groups(self, res_sig, free_dims, eligible, max_size, target_size, ignored_keys=(), safe=None,
+                            ratios=(0.05, 0.05, 0.015)):
+        """cae_similar_node_groups over the loaded templates.  ratios = (allocatable, free, memory capacity).  Returns
+        (bits [T, ceil(T/32)] uint32: bit s of row t = s is similar to t, count [T] int32, sng_limit [T] int64).  Raises
+        EngineUnsupported on status 1 (a quantity past INT64_MAX / 1000)."""
+        T = self.enc.T
+        keep = []
+
+        def arr(a, dt, ctype):
+            a = np.ascontiguousarray(a, dt)
+            keep.append(a)
+            return a.ctypes.data_as(C.POINTER(ctype))
+        si = capi.cae_similarity_inputs()
+        si.abi_version = capi.CONST["CAE_ABI_VERSION"]
+        ign = np.ascontiguousarray(list(ignored_keys), np.int32)
+        si.num_ignored_keys = len(ign)
+        si.ignored_keys = arr(ign, np.int32, C.c_int32)
+        si.max_allocatable_difference_ratio, si.max_free_difference_ratio, si.max_capacity_memory_difference_ratio = \
+            (float(r) for r in ratios)
+        si.res_sig = arr(res_sig, np.int32, C.c_int32)
+        si.free_dims = arr(free_dims, np.uint32, C.c_uint32)
+        si.eligible = arr(eligible, np.uint8, C.c_uint8)
+        si.safe = None if safe is None else arr(safe, np.uint8, C.c_uint8)
+        si.max_size = arr(max_size, np.int32, C.c_int32)
+        si.target_size = arr(target_size, np.int32, C.c_int32)
+        bits = np.zeros((T, (T + 31) // 32), np.uint32)
+        count = np.zeros(T, np.int32)
+        limit = np.zeros(T, np.int64)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        self._check(self.lib.cae_similar_node_groups(self.h, C.byref(si), vp(bits), vp(count), vp(limit)))
+        return bits, count, limit
+
     # ---- fused histogram exchange over peer memory (multi-GPU dense pass) -------------------------
     def peer_handle(self) -> bytes:
         buf = C.create_string_buffer(capi.CONST["CAE_PEER_HANDLE_BYTES"])

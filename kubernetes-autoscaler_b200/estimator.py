@@ -22,7 +22,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import capi
-from .encode import EncodedObjects, encode
+from .encode import EncodedObjects, Encoder, encode
 from .engine import Engine
 from .objects import NodeInfo, Pod, PodEquivalenceGroup
 
@@ -102,6 +102,36 @@ class ThresholdBasedEstimationLimiter:
 NewThresholdBasedEstimationLimiter = ThresholdBasedEstimationLimiter
 
 
+def limiter_caps(node_groups: Sequence[NodeGroupInfo], sng_limit: Optional[Sequence[int]], max_nodes_per_scaleup: int,
+                 max_nodes_total: int = 0, current_node_count: int = 0) -> Dict[str, int]:
+    """The max_nodes of every node group as estimator.NewDefaultEstimationLimiter folds it (threshold_based_limiter.go:34-53):
+    getMinLimit over the static threshold, the cluster-capacity threshold and SngCapacityThreshold.  sng_limit[i]: that
+    threshold's NodeLimit for node_groups[i] (cae_similar_node_groups); None = no similar groups (the group's own headroom)."""
+    ctx = EstimationContext([], max_nodes_total, current_node_count)
+    cluster = ClusterCapacityThreshold().NodeLimit(None, ctx)
+    out: Dict[str, int] = {}
+    for i, ng in enumerate(node_groups):
+        sng = SngCapacityThreshold().NodeLimit(ng, ctx) if sng_limit is None else int(sng_limit[i])
+        out[ng.id] = getMinLimit(getMinLimit(getMinLimit(0, max_nodes_per_scaleup), cluster), sng)
+    return out
+
+
+# ---- FindSimilarNodeGroups' generic comparator (processors/nodegroupset/compare_nodegroups.go) ------------------------------
+BasicIgnoredLabels = frozenset({
+    "kubernetes.io/hostname", "failure-domain.beta.kubernetes.io/zone", "failure-domain.beta.kubernetes.io/region",
+    "topology.kubernetes.io/zone", "topology.kubernetes.io/region", "beta.kubernetes.io/fluentd-ds-ready",
+    "kops.k8s.io/instancegroup",
+})
+
+
+@dataclass
+class NodeGroupDifferenceRatios:
+    """config/autoscaling_options.go:79-104 (NewDefaultNodeGroupDifferenceRatios)."""
+    max_allocatable_difference_ratio: float = 0.05
+    max_free_difference_ratio: float = 0.05
+    max_capacity_memory_difference_ratio: float = 0.015
+
+
 # ---- single-call estimator (reference shape) ---------------------------------------------------
 _shared_engine: Optional[Engine] = None
 
@@ -169,8 +199,11 @@ class ScaleUpSimulation:
     def __init__(self, cluster: Sequence[NodeInfo], templates: Dict[str, NodeInfo],
                  groups: Sequence[PodEquivalenceGroup], engine: Optional[Engine] = None, namespaces=()) -> None:
         self.ids = list(templates.keys())
+        self.templates = [templates[i] for i in self.ids]
         self.groups = list(groups)
-        self.enc: EncodedObjects = encode(cluster, [templates[i] for i in self.ids], groups, namespaces)
+        self.encoder = Encoder()
+        self.enc: EncodedObjects = encode(cluster, self.templates, groups, namespaces, encoder=self.encoder)
+        self.sng_limit: Optional[np.ndarray] = None
         self.engine = engine or shared_engine()
         self.engine.load(self.enc)
 
@@ -178,6 +211,35 @@ class ScaleUpSimulation:
         """orchestrator.go:603-638 for every node group: indices of the groups whose exemplar fits."""
         reasons = self.engine.feasibility_groups()
         return {ng: [g for g in range(len(self.groups)) if reasons[t][g] == 0] for t, ng in enumerate(self.ids)}
+
+    def similar_node_groups(self, node_groups: Sequence[NodeGroupInfo], extra_ignored_labels: Sequence[str] = (),
+                            ratios: NodeGroupDifferenceRatios = NodeGroupDifferenceRatios(), safe=None,
+                            zero_or_max=None) -> Dict[str, List[str]]:
+        """ComputeSimilarNodeGroups over FindSimilarNodeGroups with the generic comparator for every node group, on the
+        engine (cae_similar_node_groups); lists follow the template order.  node_groups: max / target size of every loaded
+        template.  safe: ids that pass NodeGroupScaleUpSafety (None = all); zero_or_max: ids with ZeroOrMaxNodeScaling.
+        Keeps the similar-groups limiter cap of every node group for limiter_caps."""
+        by_id = {ng.id: ng for ng in node_groups}
+        ngs = [by_id[i] for i in self.ids]
+        res_sig, free_dims = self.encoder.similarity_signatures(self.templates)
+        ignored = self.encoder.label_key_ids(BasicIgnoredLabels | frozenset(extra_ignored_labels))
+        bits, _, self.sng_limit = self.engine.similar_node_groups(
+            res_sig, free_dims, [0 if zero_or_max and i in zero_or_max else 1 for i in self.ids],
+            [ng.max_size for ng in ngs], [ng.target_size for ng in ngs], ignored,
+            None if safe is None else [1 if i in safe else 0 for i in self.ids],
+            (ratios.max_allocatable_difference_ratio, ratios.max_free_difference_ratio,
+             ratios.max_capacity_memory_difference_ratio))
+        T = len(self.ids)
+        member = np.unpackbits(bits.view(np.uint8), axis=1, bitorder="little")[:, :T]
+        return {ng: [self.ids[s] for s in np.flatnonzero(member[t])] for t, ng in enumerate(self.ids)}
+
+    def limiter_caps(self, node_groups: Sequence[NodeGroupInfo], max_nodes_per_scaleup: int, max_nodes_total: int = 0,
+                     current_node_count: int = 0) -> Dict[str, int]:
+        """max_nodes of every node group for compute_expansion_options: limiter_caps with the similar-groups caps of the
+        last similar_node_groups call (none: no similar groups)."""
+        by_id = {ng.id: ng for ng in node_groups}
+        return limiter_caps([by_id[i] for i in self.ids], self.sng_limit, max_nodes_per_scaleup, max_nodes_total,
+                            current_node_count)
 
     def compute_expansion_options(self, max_nodes: Optional[Dict[str, int]] = None,
                                   zero_or_max: Optional[Dict[str, int]] = None, all_or_nothing: bool = False) -> List[Option]:

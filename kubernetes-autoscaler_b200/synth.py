@@ -477,3 +477,82 @@ def pod_churn(enc: EncodedObjects, seed: int, arrive: int, leave: int):
     groups += [np.full(int(sizes[i]), S + i, np.int32) for i in range(arrive)]
     off = np.concatenate([[0], np.cumsum([len(g) for g in groups])]).astype(np.int32)
     return PodDelta(ps_req=req, group_off=off, pend_spec=np.concatenate(groups) if groups else [], **cols)
+
+
+def node_group_families(config: int, templates: int, family: int, seed: int = 0, groups: Optional[int] = None):
+    """Object-level node groups for cae_similar_node_groups: ``templates`` node groups in families of ``family`` zones of
+    one instance type (the usual layout under --balance-similar-node-groups), and the pending groups of config ``config``'s
+    pod shapes (E = pods / 100 groups unless ``groups`` is given, one pod each: only the exemplars matter here).
+    Inside a family the allocatable cpu / memory carry a small jitter, and one member in six a jitter past the 5 % ratios;
+    memory capacity varies within, and one member in eight past, the 1.5 % ratio; one member in five carries an extra
+    taint, so that similar groups differ in schedulable sets, as they do for the pods (5 %) that select one zone.  Families
+    differ in instance type, pool and DaemonSet requests.  Returns (templates {id: NodeInfo}, pod groups,
+    [NodeGroupInfo])."""
+    from .estimator import NodeGroupInfo
+    from .objects import LABEL_ZONE, LABEL_HOSTNAME, Node, NodeInfo, Pod, PodEquivalenceGroup, Taint, Toleration
+    cfg = CONFIGS[config]
+    E = max(1, cfg.pods // 100) if groups is None else groups
+    rng = SplitMix64(0x51A11A ^ (seed * 0x9E3779B9) ^ config)
+    nfam = (templates + family - 1) // family
+    f_vcpu = rng.choice(nfam, [2, 4, 8, 16, 32, 64, 96], [1] * 7)
+    f_mem = rng.choice(nfam, [2, 4, 8], [1, 1, 1])
+    f_gpu = np.where(rng.uniform(nfam) < 0.15, rng.choice(nfam, [1, 4, 8], [1, 1, 1]), 0)
+    f_pool, f_ds, f_taint = rng.randint(nfam, 8), rng.randint(nfam, 5), rng.randint(nfam, 6)
+    u_far, u_cap, u_taint = rng.uniform(templates), rng.uniform(templates), rng.uniform(templates)
+    jit, mem_jit = rng.randint(templates, 1000), rng.randint(templates, 1000)
+    mx = 1 + rng.randint(templates, 20)
+    size = (rng.uniform(templates) * (mx + 1)).astype(np.int64).clip(0, mx)
+    infos: dict = {}
+    ngs = []
+    for t in range(templates):
+        f, z = t // family, t % family
+        v, gpu = int(f_vcpu[f]), int(f_gpu[f])
+        cap_cpu, cap_mem = v * 1000, v * int(f_mem[f]) * GiB
+        far = u_far[t] < 1 / 6
+        scale = (0.08 + 0.04 * jit[t] / 1000) if far else 0.02 * jit[t] / 1000       # fraction of the allocatable taken off
+        alloc_cpu = int((cap_cpu - RESERVED[v]) * (1 - scale))
+        alloc_mem = int((cap_mem - cap_mem // 20) * (1 - scale))
+        if u_cap[t] < 1 / 8:
+            cap_mem = int(cap_mem * (1.02 + 0.01 * mem_jit[t] / 1000))
+        else:
+            cap_mem = int(cap_mem * (1 - 0.01 * mem_jit[t] / 1000))
+        alloc = {"cpu": alloc_cpu, "memory": alloc_mem, "pods": 110}
+        cap = {"cpu": cap_cpu, "memory": cap_mem, "pods": 110}
+        if gpu:
+            alloc["nvidia.com/gpu"] = cap["nvidia.com/gpu"] = gpu
+        taints = []
+        if f_taint[f] < 2:
+            taints.append(Taint("dedicated", "team-%d" % f_taint[f]))
+        if u_taint[t] < 0.2:
+            taints.append(Taint("maintenance", "soon"))
+        name = "ng-%05d" % t
+        node = Node(name + "-template", labels={LABEL_HOSTNAME: name + "-template", LABEL_ZONE: "zone-%d" % z,
+                                                "pool": "pool-%d" % f_pool[f], "instance-type": "it-%d-%d-%d" % (v, f_mem[f], gpu)},
+                    taints=taints, allocatable=alloc, capacity=cap)
+        ds = [Pod("%s-ds-%d" % (name, i), namespace="kube-system",
+                  requests={"cpu": 100 + 20 * int(f_ds[f]), "memory": (200 + 50 * int(f_ds[f])) * MiB},
+                  tolerations=[Toleration(operator="Exists")]) for i in range(2)]
+        infos[name] = NodeInfo(node, ds)
+        ngs.append(NodeGroupInfo(name, int(mx[t]), int(size[t])))
+    cpu = rng.choice(E, [50, 100, 250, 500, 1000, 2000, 4000], [20, 25, 20, 15, 10, 7, 3]).astype(np.int64)
+    mem = cpu * rng.choice(E, [1, 2, 4, 8], [1, 1, 1, 1]).astype(np.int64) * MiB
+    gpu = np.where(rng.uniform(E) < 0.10, rng.choice(E, [1, 2, 4, 8], [1, 1, 1, 1]), 0)
+    u_tol, u_sel, sel = rng.uniform(E), rng.uniform(E), rng.randint(E, 16)
+    pgs = []
+    for g in range(E):
+        req = {"cpu": int(cpu[g]), "memory": int(mem[g])}
+        if gpu[g]:
+            req["nvidia.com/gpu"] = int(gpu[g])
+        tols = []
+        if u_tol[g] < 0.3:
+            tols.append(Toleration("dedicated", "Equal", "team-%d" % (g % 2), "NoSchedule"))
+        if u_tol[g] < 0.1:
+            tols.append(Toleration("maintenance", "Exists"))
+        node_sel = {}
+        if u_sel[g] < 0.05:
+            node_sel[LABEL_ZONE] = "zone-%d" % (sel[g] % family)
+        elif u_sel[g] < 0.15:
+            node_sel["pool"] = "pool-%d" % (sel[g] % 8)
+        pgs.append(PodEquivalenceGroup([Pod("p-%d" % g, namespace="ns-%d" % (g % 32), labels={"app": "a%d" % g}, requests=req,
+                                            tolerations=tols, node_selector=node_sel)]))
+    return infos, pgs, ngs

@@ -7,12 +7,13 @@ self-cleaning accumulators, last-block election, shared-memory state and block-w
 
 Dense pass (K1, both variants), Estimate() of every template (K0 + K3: plain closed form, capacity form with the cluster
 fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals), a cluster-node delta
-(cae_load_nodes) and a cluster-node churn (cae_load_node_churn) — on miniatures of C2, C3 and C4 — each checked
+(cae_load_nodes), a cluster-node churn (cae_load_node_churn) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
 against the CPU oracle so that a "clean" run also means "correct results under the tool"."""
 import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 import numpy as np  # noqa: E402
 
 
@@ -21,6 +22,8 @@ def main():
     ge.build()
     from kubernetes_autoscaler_b200 import synth
     from kubernetes_autoscaler_b200.engine import Engine, unpack_bits
+    from kubernetes_autoscaler_b200.estimator import ScaleUpSimulation
+    import nodegroupset_harness as h
     from oracle import pyoracle
     eng = Engine(device=0, want_reasons=True)
     for cfg, kw in ((2, dict(pods=3000, templates=40)), (3, dict(pods=2500, templates=24, cluster_nodes=48)),
@@ -77,6 +80,12 @@ def main():
             got = eng.filter_schedulable(order_p)
             ref = pyoracle.filter_schedulable(after, order_p)
             assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
+        # similar node groups (cae_similar_node_groups: operand / bit-row prep, the pair kernel's staged tiles and ballots)
+        infos, groups, ngs = synth.node_group_families(cfg, 45, 4, seed=cfg, groups=40)
+        sim = ScaleUpSimulation([], infos, groups, eng)
+        got = sim.similar_node_groups(ngs)
+        sched, cmp = sim.schedulable_pod_groups(), h.CreateGenericNodeInfoComparator()
+        assert got == {t: h.ComputeSimilarNodeGroups(t, h.FindSimilarNodeGroups(t, infos, cmp), sched) for t in sim.ids}
         print("config", cfg, "ok: nodes", int(nc.sum()), "pods", int(pc.sum()), flush=True)
     eng.close()
     print("sanitize workload ok")
