@@ -11,10 +11,12 @@
 #include <algorithm>
 #include <chrono>
 #include <cstdio>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <map>
 #include <tuple>
+#include <type_traits>
 #include <unordered_map>
 
 #include "engine.h"
@@ -611,6 +613,220 @@ static int derive_pending(Engine* e, const cae_objects* o, LoadTimer& lt, const 
   return 0;
 }
 
+// ---- the dictionary tables (CAE_DICT_TABLES in engine.h): uploaded by cae_load, continued by the deltas' tails ----
+constexpr size_t ABSENT = ~(size_t)0;
+#define CAE_IN_NODE_BOTH(f) offsetof(cae_node_delta, f)
+#define CAE_IN_NODE_NODE(f) offsetof(cae_node_delta, f)
+#define CAE_IN_NODE_POD(f) ABSENT
+#define CAE_IN_POD_BOTH(f) offsetof(cae_pod_delta, f)
+#define CAE_IN_POD_POD(f) offsetof(cae_pod_delta, f)
+#define CAE_IN_POD_NODE(f) ABSENT
+struct DictTab {
+  size_t dev, obj, node, pod;   // offset of the field in DevObjects, cae_objects, cae_node_delta, cae_pod_delta (ABSENT: none)
+  size_t esz;                   // bytes per entry
+  int per, cnt, child;          // elements per entry, the count that sizes the table, the child count of an offsets table
+  bool host;                    // a host mirror is kept
+};
+#define CAE_DICT_ENTRY(f, type, per, cnt, child, by, host)                                                         \
+  {offsetof(DevObjects, f), offsetof(cae_objects, f), CAE_IN_NODE_##by(f), CAE_IN_POD_##by(f), sizeof(type) * (per), \
+   per, CNT_##cnt, CNT_##child, host},
+static const DictTab kDict[NUM_DICT_TABLES] = {CAE_DICT_TABLES(CAE_DICT_ENTRY)};
+#undef CAE_DICT_ENTRY
+// every entry's element type is the type of its field in DevObjects, cae_objects and the delta structs that carry it
+template <class F, class T>
+constexpr bool is_col = std::is_same<F, const T*>::value;
+#define CAE_TYPE_NODE_BOTH(f, type) is_col<decltype(cae_node_delta::f), type>
+#define CAE_TYPE_NODE_NODE(f, type) is_col<decltype(cae_node_delta::f), type>
+#define CAE_TYPE_NODE_POD(f, type) true
+#define CAE_TYPE_POD_BOTH(f, type) is_col<decltype(cae_pod_delta::f), type>
+#define CAE_TYPE_POD_POD(f, type) is_col<decltype(cae_pod_delta::f), type>
+#define CAE_TYPE_POD_NODE(f, type) true
+#define CAE_DICT_TYPE(f, type, per, cnt, child, by, host)                                                       \
+  static_assert(is_col<decltype(DevObjects::f), type> && is_col<decltype(cae_objects::f), type> &&                \
+                    CAE_TYPE_NODE_##by(f, type) && CAE_TYPE_POD_##by(f, type) && (CNT_##child == CNT_NONE || (per) == 1), \
+                "CAE_DICT_TABLES entry " #f " does not match the field");
+CAE_DICT_TABLES(CAE_DICT_TYPE)
+#undef CAE_DICT_TYPE
+
+static const void*& dev_table(DevObjects& d, int t) { return *reinterpret_cast<const void**>(reinterpret_cast<char*>(&d) + kDict[t].dev); }
+// entries (of kDict[t].esz bytes) of table t at the given counts
+static size_t table_len(const int64_t* cnt, int t) { return (size_t)cnt[kDict[t].cnt] + (kDict[t].child >= 0); }
+
+// The tables of a cae_objects, or the tails a delta carries: the entries of each count and the caller's array of each
+// table.  A tail's offsets are relative to the tail.  Counts the struct does not carry stay 0.
+struct Tails {
+  int64_t n[NUM_DICT_COUNTS] = {};
+  bool carried[NUM_DICT_COUNTS] = {};
+  const void* src[NUM_DICT_TABLES] = {};
+};
+static Tails arrays_of(const void* s, size_t DictTab::*at) {
+  Tails v;
+  for (int t = 0; t < NUM_DICT_TABLES; ++t)
+    if (kDict[t].*at != ABSENT) {
+      v.src[t] = *reinterpret_cast<const void* const*>(static_cast<const char*>(s) + kDict[t].*at);
+      v.carried[kDict[t].cnt] = true;
+    }
+  return v;
+}
+// the last offset of an offsets table: the entries of its child
+static int64_t child_len(const Tails& v, int t) {
+  const int64_t n = v.n[kDict[t].cnt];
+  return n ? static_cast<const int32_t*>(v.src[t])[n] : 0;
+}
+static Tails object_tables(const cae_objects* o) {
+  Tails v = arrays_of(o, &DictTab::obj);
+  int64_t* n = v.n;
+  n[CNT_VALUES] = o->num_values; n[CNT_NAMESPACES] = o->num_namespaces; n[CNT_LABELSETS] = o->num_labelsets; n[CNT_REQS] = o->num_reqs;
+  n[CNT_SELECTORS] = o->num_selectors; n[CNT_NAFF] = o->num_naff; n[CNT_NAFF_TERMS] = o->num_naff_terms;
+  n[CNT_TOL_LISTS] = o->num_tol_lists; n[CNT_TAINT_LISTS] = o->num_taint_lists; n[CNT_PORT_LISTS] = o->num_port_lists;
+  n[CNT_PTS_LISTS] = o->num_pts_lists; n[CNT_AFF_LISTS] = o->num_aff_lists; n[CNT_ATERMS] = o->num_aterms; n[CNT_SPECS] = o->num_podspecs;
+  for (int t = 0; t < NUM_DICT_TABLES; ++t)
+    if (kDict[t].child >= CNT_ROOTS) n[kDict[t].child] = child_len(v, t);
+  return v;
+}
+static Tails node_tails(const cae_node_delta* d) {
+  Tails v = arrays_of(d, &DictTab::node);
+  v.n[CNT_VALUES] = d->num_new_values; v.n[CNT_LABELSETS] = d->num_new_labelsets; v.n[CNT_TAINT_LISTS] = d->num_new_taint_lists;
+  return v;
+}
+static Tails pod_tails(const cae_pod_delta* d) {
+  Tails v = arrays_of(d, &DictTab::pod);
+  int64_t* n = v.n;
+  n[CNT_VALUES] = d->num_new_values; n[CNT_NAMESPACES] = d->num_new_namespaces; n[CNT_LABELSETS] = d->num_new_labelsets;
+  n[CNT_REQS] = d->num_new_reqs; n[CNT_SELECTORS] = d->num_new_selectors; n[CNT_NAFF] = d->num_new_naff;
+  n[CNT_NAFF_TERMS] = d->num_new_naff_terms; n[CNT_TOL_LISTS] = d->num_new_tol_lists; n[CNT_PORT_LISTS] = d->num_new_port_lists;
+  n[CNT_PTS_LISTS] = d->num_new_pts_lists; n[CNT_AFF_LISTS] = d->num_new_aff_lists; n[CNT_ATERMS] = d->num_new_aterms;
+  n[CNT_SPECS] = d->num_new_specs;
+  return v;
+}
+
+// The checks of a delta's tails, in the order the statuses are decided: the stated counts and their arrays (-2), the
+// offsets and the child tails they size or must stay within (-2), the 2^31 - 1 limits from counts and offsets alone (2),
+// then every id and enum (-2).  The node calls check their rows between these steps.
+template <class Bad>
+static int tails_present(const Tails& v, Bad bad) {
+  for (int c = 0; c < CNT_ROOTS; ++c) if (v.n[c] < 0) return bad("negative count");
+  for (int t = 0; t < NUM_DICT_TABLES; ++t)
+    if (kDict[t].cnt < CNT_ROOTS && v.n[kDict[t].cnt] && !v.src[t]) return bad("NULL array with a non-zero count");
+  return 0;
+}
+// offsets [n + 1] that start at 0 and do not decrease
+static bool offsets_ok(const int32_t* off, int64_t n) {
+  if (off[0] != 0) return false;
+  for (int64_t i = 0; i < n; ++i) if (off[i + 1] < off[i]) return false;
+  return true;
+}
+template <class Bad>
+static int tails_offsets(Tails& v, Bad bad) {
+  for (int t = 0; t < NUM_DICT_TABLES; ++t) {
+    const int ch = kDict[t].child;
+    if (ch < 0) continue;
+    const int64_t n = v.n[kDict[t].cnt];
+    if (n && !offsets_ok(static_cast<const int32_t*>(v.src[t]), n)) return bad("offsets that do not start at 0 or decrease");
+    if (ch >= CNT_ROOTS) v.n[ch] = child_len(v, t);
+    else if (child_len(v, t) > v.n[ch]) return bad("a tail's offsets run past its child tail");
+  }
+  for (int t = 0; t < NUM_DICT_TABLES; ++t)
+    if (kDict[t].cnt >= CNT_ROOTS && v.n[kDict[t].cnt] && !v.src[t]) return bad("NULL array with a non-zero count");
+  return 0;
+}
+static bool tails_fit(const Engine* e, const Tails& v) {
+  for (int t = 0; t < NUM_DICT_TABLES; ++t) {
+    const int c = kDict[t].cnt;
+    if (v.carried[c] && (e->dict_cnt[c] + v.n[c]) * kDict[t].per + (kDict[t].child >= 0) > INT32_MAX) return false;
+  }
+  return true;
+}
+template <class Bad>
+static int tails_ids(const Engine* e, const Tails& v, Bad bad) {
+  auto tot = [&](int c) { return e->dict_cnt[c] + v.n[c]; };
+  auto in = [](int64_t x, int64_t lo, int64_t hi) { return x >= lo && x < hi; };
+  const int64_t NV = tot(CNT_VALUES), NNS = tot(CNT_NAMESPACES), NL = tot(CNT_LABELSETS), NSEL = tot(CNT_SELECTORS);
+  const int64_t NNF = tot(CNT_NAFF), NTL = tot(CNT_TOL_LISTS), NPL = tot(CNT_PORT_LISTS), NPTS = tot(CNT_PTS_LISTS), NAL = tot(CNT_AFF_LISTS);
+#define TAIL(f) static_cast<const int32_t*>(v.src[TAB_##f])
+#define TAIL8(f) static_cast<const uint8_t*>(v.src[TAB_##f])
+  for (int64_t i = 0; i < v.n[CNT_NAMESPACES]; ++i)
+    if (!in(TAIL(ns_labelset)[i], 0, NL) || TAIL8(ns_exists)[i] > 1) return bad("namespace tail out of range");
+  for (int64_t j = 0; j < v.n[CNT_LABELSETS]; ++j)
+    for (int q = TAIL(ls_off)[j]; q < TAIL(ls_off)[j + 1]; ++q) {
+      if (TAIL(ls_key)[q] < 0 || (q > TAIL(ls_off)[j] && TAIL(ls_key)[q] <= TAIL(ls_key)[q - 1])) return bad("label pairs not sorted by key id");
+      if (!in(TAIL(ls_val)[q], 0, NV)) return bad("label value id out of range");
+    }
+  for (int64_t i = 0; i < v.n[CNT_REQS]; ++i)
+    if (TAIL(req_key)[i] < 0 || !in(TAIL(req_op)[i], CAE_OP_IN, CAE_OP_LT + 1)) return bad("requirement out of range");
+  for (int64_t q = 0; q < v.n[CNT_REQ_VALS]; ++q) if (!in(TAIL(req_vals)[q], 0, NV)) return bad("requirement value id out of range");
+  for (int64_t i = 0; i < v.n[CNT_SELECTORS]; ++i)
+    if (!in(TAIL(sel_kind)[i], CAE_SEL_NOTHING, CAE_SEL_REQS + 1)) return bad("selector kind out of range");
+  for (int64_t i = 0; i < v.n[CNT_NAFF]; ++i)
+    if (!in(TAIL(naff_nodesel)[i], -1, NSEL) || TAIL8(naff_has_required)[i] > 1) return bad("node-affinity record out of range");
+  for (int64_t i = 0; i < v.n[CNT_NAFF_TERMS]; ++i)
+    if (!in(TAIL(term_expr_sel)[i], -1, NSEL)) return bad("node-affinity term selector out of range");
+  for (int64_t q = 0; q < v.n[CNT_FIELDS]; ++q)
+    if (!in(TAIL(field_op)[q], CAE_OP_IN, CAE_OP_NOT_IN + 1) || TAIL(field_node_name)[q] < 0) return bad("matchFields entry out of range");
+  for (int64_t q = 0; q < v.n[CNT_TOLS]; ++q)
+    if (TAIL(tol_key)[q] < -1 || !in(TAIL(tol_op)[q], CAE_TOL_EQUAL, CAE_TOL_INVALID + 1) || !in(TAIL(tol_val)[q], -1, NV) ||
+        !in(TAIL(tol_effect)[q], CAE_EFFECT_NONE, CAE_EFFECT_NO_EXECUTE + 1))
+      return bad("toleration out of range");
+  for (int64_t q = 0; q < v.n[CNT_TAINTS]; ++q)
+    if (TAIL(taint_key)[q] < 0 || !in(TAIL(taint_val)[q], -1, NV) || !in(TAIL(taint_effect)[q], CAE_EFFECT_NONE, CAE_EFFECT_NO_EXECUTE + 1))
+      return bad("taint out of range");
+  for (int64_t q = 0; q < v.n[CNT_PORTS]; ++q)
+    if (TAIL(port_ip)[q] < 0 || !in(TAIL(port_proto)[q], CAE_PROTO_TCP, CAE_PROTO_SCTP + 1) || TAIL(port_num)[q] <= 0)
+      return bad("host port out of range");
+  for (int64_t q = 0; q < v.n[CNT_PTS]; ++q)
+    if (TAIL(pts_key)[q] < 0 || !in(TAIL(pts_selector)[q], 0, NSEL) || !in(TAIL(pts_node_affinity_policy)[q], 0, 2) ||
+        !in(TAIL(pts_node_taints_policy)[q], 0, 2))
+      return bad("topology spread constraint out of range");
+  for (int64_t i = 0; i < v.n[CNT_ATERMS]; ++i)
+    if (!in(TAIL(aterm_selector)[i], 0, NSEL) || TAIL(aterm_key)[i] < 0 || !in(TAIL(aterm_ns_selector)[i], 0, NSEL))
+      return bad("affinity term out of range");
+  for (int64_t q = 0; q < v.n[CNT_ATERM_NS]; ++q) if (!in(TAIL(aterm_ns)[q], 0, NNS)) return bad("affinity term namespace out of range");
+  for (int64_t i = 0; i < v.n[CNT_SPECS]; ++i) {
+    if (!in(TAIL(ps_namespace)[i], 0, NNS) || !in(TAIL(ps_labelset)[i], 0, NL) || !in(TAIL(ps_tol_list)[i], 0, NTL) ||
+        !in(TAIL(ps_naff)[i], -1, NNF) || TAIL(ps_node_name)[i] < -1 || !in(TAIL(ps_port_list)[i], 0, NPL) ||
+        !in(TAIL(ps_pts_list)[i], 0, NPTS) || !in(TAIL(ps_aff_list)[i], 0, NAL) || !in(TAIL(ps_anti_list)[i], 0, NAL) ||
+        TAIL8(ps_terminating)[i] > 1 || TAIL8(ps_hostname_spread)[i] > 1)
+      return bad("pod-spec id out of range");
+    for (int r = 0; r < R; ++r)
+      if (static_cast<const int64_t*>(v.src[TAB_ps_req])[(size_t)i * R + r] < 0) return bad("pod-spec request negative");
+  }
+#undef TAIL
+#undef TAIL8
+  return 0;
+}
+
+// Appending tails: tails_layout places them in the caller's pinned blob (8-byte aligned segments from `bytes` on, returns the
+// end); tails_put writes them there with the offsets made absolute and appends them to the host mirrors; after the blob's
+// H2D copy, tails_grow grows the device tables from its device copy and advances the counts.  Until then
+// take_back_mirrors undoes tails_put.
+static size_t tails_layout(const Tails& v, size_t at[NUM_DICT_TABLES], size_t bytes) {
+  for (int t = 0; t < NUM_DICT_TABLES; ++t) {
+    at[t] = bytes;
+    bytes = (bytes + (size_t)v.n[kDict[t].cnt] * kDict[t].esz + 7) & ~(size_t)7;
+  }
+  return bytes;
+}
+static void tails_put(Engine* e, const Tails& v, const size_t at[NUM_DICT_TABLES], char* h) {
+  for (int t = 0; t < NUM_DICT_TABLES; ++t) {
+    const DictTab& d = kDict[t];
+    const size_t n = (size_t)v.n[d.cnt];
+    if (!n) continue;
+    char* dst = h + at[t];
+    if (d.child >= 0) {
+      const int32_t* rel = static_cast<const int32_t*>(v.src[t]);
+      const int32_t base = (int32_t)e->dict_cnt[d.child];
+      for (size_t j = 0; j < n; ++j) reinterpret_cast<int32_t*>(dst)[j] = base + rel[j + 1];
+    } else {
+      memcpy(dst, v.src[t], n * d.esz);
+    }
+    if (d.host) e->dict_host[t].insert(e->dict_host[t].end(), dst, dst + n * d.esz);
+  }
+}
+static void take_back_mirrors(Engine* e) {
+  for (int t = 0; t < NUM_DICT_TABLES; ++t)
+    if (kDict[t].host) e->dict_host[t].resize(table_len(e->dict_cnt, t) * kDict[t].esz);
+}
+
 static int do_load(Engine* e, const cae_objects* o) {
   LoadTimer lt;
   if (o->abi_version != CAE_ABI_VERSION) { set_error("cae_objects.abi_version mismatch"); return -2; }
@@ -631,25 +847,18 @@ static int do_load(Engine* e, const cae_objects* o) {
   DevObjects& d = e->dobj;
   d.num_res = o->num_res; d.num_values = o->num_values; d.hostname_key = o->hostname_key;
   d.unschedulable_taint_key = o->unschedulable_taint_key; d.N = N; d.T = T;
-  UP(value_is_int, o->num_values); UP(value_int, o->num_values);
-  UP(ns_labelset, o->num_namespaces); UP(ns_exists, o->num_namespaces);
-  UP(ls_off, o->num_labelsets + 1); UP(ls_key, o->ls_off[o->num_labelsets]); UP(ls_val, o->ls_off[o->num_labelsets]);
-  UP(req_key, o->num_reqs); UP(req_op, o->num_reqs); UP(req_val_off, o->num_reqs + 1);
-  UP(req_vals, o->num_reqs ? o->req_val_off[o->num_reqs] : 0);
-  UP(sel_kind, o->num_selectors); UP(sel_req_off, o->num_selectors + 1);
-  UP(naff_nodesel, o->num_naff); UP(naff_has_required, o->num_naff); UP(naff_term_off, o->num_naff + 1);
-  UP(term_expr_sel, o->num_naff_terms); UP(term_field_off, o->num_naff_terms + 1);
-  { int nf = o->term_field_off[o->num_naff_terms]; UP(field_op, nf); UP(field_node_name, nf); }
-  { int n = o->tol_off[o->num_tol_lists]; UP(tol_off, o->num_tol_lists + 1); UP(tol_key, n); UP(tol_op, n); UP(tol_val, n); UP(tol_effect, n); }
-  { int n = o->taint_off[o->num_taint_lists]; UP(taint_off, o->num_taint_lists + 1); UP(taint_key, n); UP(taint_val, n); UP(taint_effect, n); }
-  { int n = o->port_off[o->num_port_lists]; UP(port_off, o->num_port_lists + 1); UP(port_ip, n); UP(port_proto, n); UP(port_num, n); }
-  { int n = o->pts_off[o->num_pts_lists]; UP(pts_off, o->num_pts_lists + 1); UP(pts_max_skew, n); UP(pts_key, n); UP(pts_selector, n);
-    UP(pts_min_domains, n); UP(pts_node_affinity_policy, n); UP(pts_node_taints_policy, n); }
-  { int n = o->num_aterms; UP(aff_off, o->num_aff_lists + 1); UP(aterm_selector, n); UP(aterm_key, n); UP(aterm_ns_off, n + 1);
-    UP(aterm_ns, o->aterm_ns_off[n]); UP(aterm_ns_selector, n); }
-  { int n = o->num_podspecs; UP(ps_namespace, n); UP(ps_labelset, n); UP(ps_req, (size_t)n * R); UP(ps_tol_list, n); UP(ps_naff, n);
-    UP(ps_node_name, n); UP(ps_port_list, n); UP(ps_pts_list, n); UP(ps_aff_list, n); UP(ps_anti_list, n); UP(ps_terminating, n);
-    UP(ps_hostname_spread, n); }
+  {   // the dictionary tables, their counts and host mirrors
+    const Tails ob = object_tables(o);
+    for (int t = 0; t < NUM_DICT_TABLES; ++t) {
+      const char* src = static_cast<const char*>(ob.src[t]);
+      const size_t bytes = table_len(ob.n, t) * kDict[t].esz;
+      const char* p = nullptr;
+      if (upload(e->up, src, bytes, &p)) return -1;
+      dev_table(d, t) = p;
+      if (kDict[t].host) e->dict_host[t].assign(src, src + bytes);
+    }
+    std::copy(ob.n, ob.n + NUM_DICT_COUNTS, e->dict_cnt);
+  }
   UP(node_name, NT); UP(node_labelset, NT); UP(node_taint_list, NT); UP(node_unschedulable, NT);
   UP(node_alloc, (size_t)NT * R); UP(node_allowed_pods, NT); UP(node_cap_cpu, NT); UP(node_cap_mem, NT);
   UP(node_has_alloc_cpu, NT); UP(node_has_alloc_mem, NT);
@@ -657,7 +866,6 @@ static int do_load(Engine* e, const cae_objects* o) {
 
   // node side: free capacity of the templates over all R dims, free pod slots of every row
   const int S = o->num_podspecs;
-  Engine::PodHost& ph = e->ph;
   std::vector<int64_t> free_all((size_t)R * T);
   std::vector<int32_t> slots(T), cslots(std::max(N, 1));
   for (int row = 0; row < NT; ++row) {
@@ -677,50 +885,19 @@ static int do_load(Engine* e, const cae_objects* o) {
   // host state the per-tick deltas validate against and update (cae_load_pending, cae_load_nodes, cae_load_pods)
   {
     Engine::NodeHost& nh = e->nh;   // spec_used and key_val come from the derivation
-    nh.num_values = o->num_values;
-    nh.num_labelsets = o->num_labelsets;
-    nh.num_taint_lists = o->num_taint_lists;
-    nh.taint_entries = o->taint_off[o->num_taint_lists];
-    const int np = o->ls_off[o->num_labelsets];
-    nh.ls_off.assign(o->ls_off, o->ls_off + o->num_labelsets + 1);
-    nh.ls_key.assign(o->ls_key, o->ls_key + np);
-    nh.ls_val.assign(o->ls_val, o->ls_val + np);
     nh.pod_cnt.resize(N);
     for (int n = 0; n < N; ++n) nh.pod_cnt[n] = o->node_pod_off[n + 1] - o->node_pod_off[n];
     nh.pod_total = o->node_pod_off[NT];
     nh.tmpl_ls.assign(o->node_labelset + N, o->node_labelset + NT);
     nh.spec_anti.resize(S);
     for (int s = 0; s < S; ++s) nh.spec_anti[s] = o->aff_off[o->ps_anti_list[s] + 1] > o->aff_off[o->ps_anti_list[s]];
-    e->h_spec_req.assign(o->ps_req, o->ps_req + (size_t)S * R);
-    ph.hostname_key = o->hostname_key;
-    ph.num_res = o->num_res;
-    ph.num_namespaces = o->num_namespaces;
-    ph.num_reqs = o->num_reqs;
-    ph.req_vals = o->num_reqs ? o->req_val_off[o->num_reqs] : 0;
-    ph.num_selectors = o->num_selectors;
-    ph.num_naff = o->num_naff;
-    ph.num_naff_terms = o->num_naff_terms;
-    ph.fields = o->term_field_off[o->num_naff_terms];
-    ph.num_tol_lists = o->num_tol_lists;
-    ph.tol_entries = o->tol_off[o->num_tol_lists];
-    ph.num_aterms = o->num_aterms;
-    ph.aterm_ns = o->aterm_ns_off[o->num_aterms];
-    auto col = [S](std::vector<int32_t>& v, const int32_t* src) { v.assign(src, src + S); };
-    col(ph.ps_namespace, o->ps_namespace); col(ph.ps_labelset, o->ps_labelset); col(ph.ps_tol_list, o->ps_tol_list);
-    col(ph.ps_naff, o->ps_naff); col(ph.ps_node_name, o->ps_node_name); col(ph.ps_port_list, o->ps_port_list);
-    col(ph.ps_pts_list, o->ps_pts_list); col(ph.ps_aff_list, o->ps_aff_list); col(ph.ps_anti_list, o->ps_anti_list);
-    ph.port_off.assign(o->port_off, o->port_off + o->num_port_lists + 1);
-    ph.pts_off.assign(o->pts_off, o->pts_off + o->num_pts_lists + 1);
-    ph.pts_key.assign(o->pts_key, o->pts_key + o->pts_off[o->num_pts_lists]);
-    ph.aff_off.assign(o->aff_off, o->aff_off + o->num_aff_lists + 1);
-    ph.aterm_key.assign(o->aterm_key, o->aterm_key + o->num_aterms);
   }
   { const int rc = derive_pending(e, o, lt, nullptr, [] { return 0; }); if (rc) return rc; }
   e->loaded = true;
   return 0;
 }
 
-// Append a dictionary tail (already on the device, in the staged delta) to a DevObjects table.  The grown table lives in an
+// Append a tail (already on the device, in the staged delta) to a DevObjects table.  The grown table lives in an
 // engine-owned buffer: the first delta after a load copies the arena's contents there once, later deltas append in place
 // while the headroom lasts.
 static int grow_bytes(Engine* e, Engine::DevBuf& b, const void*& cur, size_t elem, size_t n_old, const void* d_tail, size_t n_tail) {
@@ -743,12 +920,13 @@ static int grow_bytes(Engine* e, Engine::DevBuf& b, const void*& cur, size_t ele
   return 0;
 }
 
-template <class T>
-static int grow_table(Engine* e, Engine::DevBuf& b, const T*& cur, size_t n_old, const void* d_tail, size_t n_tail) {
-  const void* c = cur;
-  const int rc = grow_bytes(e, b, c, sizeof(T), n_old, d_tail, n_tail);
-  cur = static_cast<const T*>(c);
-  return rc;
+static int tails_grow(Engine* e, const Tails& v, const size_t at[NUM_DICT_TABLES], const char* dv) {
+  for (int t = 0; t < NUM_DICT_TABLES; ++t)
+    if (grow_bytes(e, e->dict_tab[t], dev_table(e->dobj, t), kDict[t].esz, table_len(e->dict_cnt, t), dv + at[t], (size_t)v.n[kDict[t].cnt]))
+      return -1;
+  for (int c = 0; c < NUM_DICT_COUNTS; ++c) e->dict_cnt[c] += v.n[c];
+  e->dobj.num_values = (int32_t)e->dict_cnt[CNT_VALUES];
+  return 0;
 }
 
 // The new state of cluster rows a node delta carries: the dirty rows of a cae_node_delta, the added nodes of a churn
@@ -762,11 +940,11 @@ struct RowsIn {
 // One cae_load_nodes or cae_load_node_churn call: its input, then what check_nodes derived from it
 struct NodePlan {
   const cae_node_delta* dl = nullptr;   // dictionary tails and dirty rows (row numbers before the call)
+  Tails tails;
   RowsIn dirty, added;
   const int32_t *removed = nullptr, *name = nullptr;   // churn: removed rows, node names of the added rows
   int nr = 0;
-  int64_t pairs = 0, tents = 0, npods_d = 0, npods_a = 0, NV = 0, NL = 0, NTL = 0, total = 0;
-  int32_t old_nv = 0, old_nl = 0, old_ntl = 0, old_tents = 0, old_pairs = 0;
+  int64_t npods_d = 0, npods_a = 0, total = 0;
 };
 
 static RowsIn dirty_rows(const cae_node_delta* dl) {
@@ -777,10 +955,13 @@ static RowsIn dirty_rows(const cae_node_delta* dl) {
 }
 
 // value id of `key` in label set ls of the resident table or of the delta's tail, -1 absent
-static int label_of(const Engine::NodeHost& nh, const cae_node_delta* dl, int ls, int key) {
-  const bool tail = ls >= nh.num_labelsets;
-  const int32_t *off = tail ? dl->ls_off : nh.ls_off.data(), *k = tail ? dl->ls_key : nh.ls_key.data(), *v = tail ? dl->ls_val : nh.ls_val.data();
-  const int j = tail ? ls - nh.num_labelsets : ls;   // a tail's offsets and pairs are numbered from 0
+static int label_of(const Engine* e, const cae_node_delta* dl, int ls, int key) {
+  const int64_t nl = e->dict_cnt[CNT_LABELSETS];
+  const bool tail = ls >= nl;
+  const int32_t* off = tail ? dl->ls_off : e->host_tab<int32_t>(TAB_ls_off);
+  const int32_t* k = tail ? dl->ls_key : e->host_tab<int32_t>(TAB_ls_key);
+  const int32_t* v = tail ? dl->ls_val : e->host_tab<int32_t>(TAB_ls_val);
+  const int j = tail ? (int)(ls - nl) : ls;   // a tail's offsets and pairs are numbered from 0
   for (int p = off[j]; p < off[j + 1]; ++p) if (k[p] == key) return v[p];
   return -1;
 }
@@ -795,12 +976,11 @@ static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed)
   if (dl->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
   const Engine::NodeHost& nh = e->nh;
   const int N = e->N, S = e->num_podspecs;
-  const int nv = dl->num_new_values, nl = dl->num_new_labelsets, ntl = dl->num_new_taint_lists, nd = dl->num_dirty;
-  const int na = p.added.n, nr = p.nr;
-  if (nv < 0 || nl < 0 || ntl < 0 || nd < 0 || na < 0 || nr < 0) return bad("negative count");
-  if (nv && (!dl->value_is_int || !dl->value_int)) return bad("value tail without arrays");
-  if (nl && !dl->ls_off) return bad("label-set tail without offsets");
-  if (ntl && !dl->taint_off) return bad("taint-list tail without offsets");
+  const int nd = dl->num_dirty, na = p.added.n, nr = p.nr;
+  Tails& v = p.tails;
+  v = node_tails(dl);
+  if (nd < 0 || na < 0 || nr < 0) return bad("negative count");
+  { const int rc = tails_present(v, bad); if (rc) return rc; }
   auto rows_null = [](const RowsIn& r) {
     return r.n && (!r.labelset || !r.taint_list || !r.unsched || !r.alloc || !r.allowed || !r.pod_off);
   };
@@ -808,33 +988,20 @@ static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed)
   if (nr && !p.removed) return bad("removed rows without an array");
   if (rows_null(p.added) || (na && !p.name)) return bad("added rows without arrays");
   if ((int64_t)N - nr + na + 2 * (int64_t)e->T > INT32_MAX) return refuse("the node rows and template copies would pass 2^31 - 1");
-  auto offsets_ok = [](const int32_t* off, int n) {
-    if (off[0] != 0) return false;
-    for (int i = 0; i < n; ++i) if (off[i + 1] < off[i]) return false;
-    return true;
-  };
-  if (nl && !offsets_ok(dl->ls_off, nl)) return bad("label-set offsets");
-  if (ntl && !offsets_ok(dl->taint_off, ntl)) return bad("taint-list offsets");
+  { const int rc = tails_offsets(v, bad); if (rc) return rc; }
   if (nd && !offsets_ok(dl->pod_off, nd)) return bad("resident-pod offsets");
   if (na && !offsets_ok(p.added.pod_off, na)) return bad("resident-pod offsets of the added rows");
-  p.pairs = nl ? dl->ls_off[nl] : 0;
-  p.tents = ntl ? dl->taint_off[ntl] : 0;
   p.npods_d = nd ? dl->pod_off[nd] : 0;
   p.npods_a = na ? p.added.pod_off[na] : 0;
-  if (p.pairs && (!dl->ls_key || !dl->ls_val)) return bad("label pairs without arrays");
-  if (p.tents && (!dl->taint_key || !dl->taint_val || !dl->taint_effect)) return bad("taints without arrays");
   if ((p.npods_d && !dl->pod_spec) || (p.npods_a && !p.added.pod_spec)) return bad("resident pods without pod_spec");
-  p.NV = (int64_t)nh.num_values + nv; p.NL = (int64_t)nh.num_labelsets + nl; p.NTL = (int64_t)nh.num_taint_lists + ntl;
-  const int64_t old_pairs = nh.ls_off.back();
-  if (p.NV > INT32_MAX || p.NL >= INT32_MAX || p.NTL >= INT32_MAX || old_pairs + p.pairs > INT32_MAX ||
-      (int64_t)nh.taint_entries + p.tents > INT32_MAX)
-    return refuse("a dictionary table would pass 2^31 - 1 entries");
+  if (!tails_fit(e, v)) return refuse("a dictionary table would pass 2^31 - 1 entries");
+  const int64_t NL = e->dict_cnt[CNT_LABELSETS] + v.n[CNT_LABELSETS], NTL = e->dict_cnt[CNT_TAINT_LISTS] + v.n[CNT_TAINT_LISTS];
   int64_t total = nh.pod_total;
   for (int i = 0; i < nd; ++i) {
     const int r = dl->row[i];
     if (r < 0 || r >= N || (i > 0 && r <= dl->row[i - 1])) return bad("rows out of range or not strictly increasing");
-    if (dl->labelset[i] < 0 || dl->labelset[i] >= p.NL) return bad("label-set id out of range");
-    if (dl->taint_list[i] < 0 || dl->taint_list[i] >= p.NTL) return bad("taint-list id out of range");
+    if (dl->labelset[i] < 0 || dl->labelset[i] >= NL) return bad("label-set id out of range");
+    if (dl->taint_list[i] < 0 || dl->taint_list[i] >= NTL) return bad("taint-list id out of range");
     total += (int64_t)(dl->pod_off[i + 1] - dl->pod_off[i]) - nh.pod_cnt[r];
   }
   for (int i = 0, j = 0; i < nr; ++i) {   // j walks the dirty rows alongside
@@ -846,21 +1013,12 @@ static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed)
   }
   for (int i = 0; i < na; ++i) {
     if (p.name[i] < 0) return bad("node-name id of an added row out of range");
-    if (p.added.labelset[i] < 0 || p.added.labelset[i] >= p.NL) return bad("label-set id of an added row out of range");
-    if (p.added.taint_list[i] < 0 || p.added.taint_list[i] >= p.NTL) return bad("taint-list id of an added row out of range");
+    if (p.added.labelset[i] < 0 || p.added.labelset[i] >= NL) return bad("label-set id of an added row out of range");
+    if (p.added.taint_list[i] < 0 || p.added.taint_list[i] >= NTL) return bad("taint-list id of an added row out of range");
   }
   total += p.npods_a;
   if (total > INT32_MAX) return refuse("more than 2^31 - 1 resident pods");
-  for (int j = 0; j < nl; ++j)
-    for (int q = dl->ls_off[j]; q < dl->ls_off[j + 1]; ++q) {
-      if (dl->ls_key[q] < 0 || (q > dl->ls_off[j] && dl->ls_key[q] <= dl->ls_key[q - 1])) return bad("label pairs not sorted by key id");
-      if (dl->ls_val[q] < 0 || dl->ls_val[q] >= p.NV) return bad("label value id out of range");
-    }
-  for (int64_t q = 0; q < p.tents; ++q) {
-    if (dl->taint_key[q] < 0) return bad("taint key id out of range");
-    if (dl->taint_val[q] < -1 || dl->taint_val[q] >= p.NV) return bad("taint value id out of range");
-    if (dl->taint_effect[q] < CAE_EFFECT_NONE || dl->taint_effect[q] > CAE_EFFECT_NO_EXECUTE) return bad("taint effect out of range");
-  }
+  { const int rc = tails_ids(e, v, bad); if (rc) return rc; }
   for (int64_t q = 0; q < p.npods_d; ++q)
     if (dl->pod_spec[q] < 0 || dl->pod_spec[q] >= S) return bad("pod-spec id out of range");
   for (int64_t q = 0; q < p.npods_a; ++q)
@@ -874,24 +1032,16 @@ static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed)
   if (topo_fixed)
     for (int k = 0; k < (e->has_dynamic ? dy.K : 0); ++k)
       for (int i = 0; i < nd; ++i)
-        if (label_of(nh, dl, dl->labelset[i], dy.key_id[k]) != nh.key_val[(size_t)k * N + dl->row[i]])
+        if (label_of(e, dl, dl->labelset[i], dy.key_id[k]) != nh.key_val[(size_t)k * N + dl->row[i]])
           return refuse("a dirty node changes the value of a topology key the counters use");
   p.total = total;
   return 0;
 }
 
-// The host state every applied delta updates: the dictionary tails, the specs in the snapshot, the resident total
+// The host state every applied delta updates besides the dictionary tables: the specs in the snapshot, the resident total
 static void commit_nodes(Engine* e, NodePlan& p) {
   Engine::NodeHost& nh = e->nh;
   const cae_node_delta* dl = p.dl;
-  p.old_nv = nh.num_values; p.old_nl = nh.num_labelsets; p.old_ntl = nh.num_taint_lists; p.old_tents = nh.taint_entries;
-  p.old_pairs = nh.ls_off.back();
-  for (int j = 0; j < dl->num_new_labelsets; ++j) nh.ls_off.push_back((int32_t)(p.old_pairs + dl->ls_off[j + 1]));
-  if (p.pairs) {
-    nh.ls_key.insert(nh.ls_key.end(), dl->ls_key, dl->ls_key + p.pairs);
-    nh.ls_val.insert(nh.ls_val.end(), dl->ls_val, dl->ls_val + p.pairs);
-  }
-  nh.num_values = (int32_t)p.NV; nh.num_labelsets = (int32_t)p.NL; nh.num_taint_lists = (int32_t)p.NTL; nh.taint_entries += (int32_t)p.tents;
   nh.pod_total = p.total;
   for (int64_t q = 0; q < p.npods_d; ++q) nh.spec_used[dl->pod_spec[q]] = 1;
   for (int64_t q = 0; q < p.npods_a; ++q) nh.spec_used[p.added.pod_spec[q]] = 1;
@@ -904,30 +1054,20 @@ static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<std::pair
                        std::vector<const char*>* xdev) {
   const cae_node_delta* dl = p.dl;
   const int A = e->A;
-  const int nv = dl->num_new_values, nl = dl->num_new_labelsets, ntl = dl->num_new_taint_lists;
   const int nd = p.dirty.n, na = p.added.n, ns = nd + na;
-  const int64_t pairs = p.pairs, tents = p.tents, npods = p.npods_d + p.npods_a;
-  size_t bytes = 0;
-  auto seg = [&](size_t n, size_t elem) { const size_t at = bytes; bytes = (bytes + n * elem + 7) & ~(size_t)7; return at; };
-  const size_t o_vint = seg(nv, 8), o_alloc = seg((size_t)ns * R, 8), o_cfree = seg((size_t)ns * A, 8);
-  const size_t o_lsoff = seg(nl, 4), o_lskey = seg(pairs, 4), o_lsval = seg(pairs, 4);
-  const size_t o_toff = seg(ntl, 4), o_tkey = seg(tents, 4), o_tval = seg(tents, 4), o_teff = seg(tents, 4);
+  const int64_t npods = p.npods_d + p.npods_a;
+  size_t at[NUM_DICT_TABLES];
+  size_t bytes = tails_layout(p.tails, at, 0);
+  auto seg = [&](size_t n, size_t elem) { const size_t o = bytes; bytes = (bytes + n * elem + 7) & ~(size_t)7; return o; };
+  const size_t o_alloc = seg((size_t)ns * R, 8), o_cfree = seg((size_t)ns * A, 8);
   const size_t o_row = seg(nd, 4), o_name = seg(na, 4), o_ls = seg(ns, 4), o_tl = seg(ns, 4), o_allowed = seg(ns, 4), o_slots = seg(ns, 4);
-  const size_t o_poff = seg((size_t)ns + 1, 4), o_pspec = seg(npods, 4), o_visint = seg(nv, 1), o_unsched = seg(ns, 1);
+  const size_t o_poff = seg((size_t)ns + 1, 4), o_pspec = seg(npods, 4), o_unsched = seg(ns, 1);
   std::vector<size_t> o_extra;
   for (const auto& x : extra) o_extra.push_back(seg(x.second, 1));
   if (pinned_reserve(e, e->nd_stage, bytes)) return -1;
   char* h = static_cast<char*>(e->nd_stage.p);
   auto put = [&](size_t at, const void* src, size_t n) { if (n) memcpy(h + at, src, n); };
-  put(o_vint, dl->value_int, (size_t)nv * 8);
-  put(o_visint, dl->value_is_int, (size_t)nv);
-  for (int j = 0; j < nl; ++j) reinterpret_cast<int32_t*>(h + o_lsoff)[j] = (int32_t)(p.old_pairs + dl->ls_off[j + 1]);   // absolute
-  put(o_lskey, dl->ls_key, (size_t)pairs * 4);
-  put(o_lsval, dl->ls_val, (size_t)pairs * 4);
-  for (int j = 0; j < ntl; ++j) reinterpret_cast<int32_t*>(h + o_toff)[j] = p.old_tents + dl->taint_off[j + 1];
-  put(o_tkey, dl->taint_key, (size_t)tents * 4);
-  put(o_tval, dl->taint_val, (size_t)tents * 4);
-  put(o_teff, dl->taint_effect, (size_t)tents * 4);
+  tails_put(e, p.tails, at, h);
   put(o_row, dl->row, (size_t)nd * 4);
   put(o_name, p.name, (size_t)na * 4);
   int32_t* poff = reinterpret_cast<int32_t*>(h + o_poff);
@@ -945,7 +1085,7 @@ static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<std::pair
     for (int i = 0; i < r.n; ++i) {
       poff[i0 + i + 1] = poff[i0] + r.pod_off[i + 1];
       cluster_row_state(e, r.alloc + (size_t)i * R, r.allowed[i], r.pod_spec + r.pod_off[i], r.pod_off[i + 1] - r.pod_off[i],
-                        e->h_spec_req.data(), cfree + (size_t)(i0 + i) * A, 1, cslots + i0 + i);
+                        e->host_tab<int64_t>(TAB_ps_req), cfree + (size_t)(i0 + i) * A, 1, cslots + i0 + i);
     }
     i0 += r.n;
   }
@@ -955,20 +1095,8 @@ static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<std::pair
   CAE_CUDA(cudaMemcpyAsync(dv, h, bytes, cudaMemcpyHostToDevice, e->stream));
   CAE_CUDA(cudaEventRecord(e->nd_stage.ev, e->stream));
   e->stats.h2d_bytes = (int64_t)bytes;
-  if (xdev) for (size_t at : o_extra) xdev->push_back(dv + at);
-
-  // ---- dictionary tails ----
-  DevObjects& d = e->dobj;
-  if (grow_table(e, e->nd_tab[0], d.value_is_int, p.old_nv, dv + o_visint, nv) || grow_table(e, e->nd_tab[1], d.value_int, p.old_nv, dv + o_vint, nv) ||
-      grow_table(e, e->nd_tab[2], d.ls_off, (size_t)p.old_nl + 1, dv + o_lsoff, nl) ||
-      grow_table(e, e->nd_tab[3], d.ls_key, (size_t)p.old_pairs, dv + o_lskey, pairs) ||
-      grow_table(e, e->nd_tab[4], d.ls_val, (size_t)p.old_pairs, dv + o_lsval, pairs) ||
-      grow_table(e, e->nd_tab[5], d.taint_off, (size_t)p.old_ntl + 1, dv + o_toff, ntl) ||
-      grow_table(e, e->nd_tab[6], d.taint_key, (size_t)p.old_tents, dv + o_tkey, tents) ||
-      grow_table(e, e->nd_tab[7], d.taint_val, (size_t)p.old_tents, dv + o_tval, tents) ||
-      grow_table(e, e->nd_tab[8], d.taint_effect, (size_t)p.old_tents, dv + o_teff, tents))
-    return -1;
-  d.num_values = (int32_t)p.NV;
+  if (xdev) for (size_t o : o_extra) xdev->push_back(dv + o);
+  if (tails_grow(e, p.tails, at, dv)) return -1;
   e->group_reason_valid = false;
   if (dd) {
     *dd = NodeDeltaDev{};
@@ -1045,14 +1173,14 @@ static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
     src[r] = dirty ? -1 - id : o;
     pod_cnt[r] = dirty ? dl->pod_off[id + 1] - dl->pod_off[id] : nh.pod_cnt[o];
     for (int k = 0; k < K; ++k)
-      key_val[(size_t)k * N + r] = dirty ? label_of(nh, dl, dl->labelset[id], dy.key_id[k]) : nh.key_val[(size_t)k * oldN + o];
+      key_val[(size_t)k * N + r] = dirty ? label_of(e, dl, dl->labelset[id], dy.key_id[k]) : nh.key_val[(size_t)k * oldN + o];
     id += dirty;
     ++r;
   }
   for (int j = 0; j < na; ++j, ++r) {
     src[r] = -1 - (nd + j);
     pod_cnt[r] = p.added.pod_off[j + 1] - p.added.pod_off[j];
-    for (int k = 0; k < K; ++k) key_val[(size_t)k * N + r] = label_of(nh, dl, p.added.labelset[j], dy.key_id[k]);
+    for (int k = 0; k < K; ++k) key_val[(size_t)k * N + r] = label_of(e, dl, p.added.labelset[j], dy.key_id[k]);
   }
   for (int t = 0; t < T; ++t) src[N + t] = oldN + t;
   // topology domains of the new list, and the counter pool they size
@@ -1105,97 +1233,19 @@ static int do_load_pods(Engine* e, const cae_pod_delta* d) {
   LoadTimer lt("cae_load_pods");
   auto bad = [](const char* m) { set_error(std::string("cae_load_pods: ") + m); return -2; };
   if (d->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
-  Engine::NodeHost& nh = e->nh;
-  Engine::PodHost& ph = e->ph;
-  const int S0 = e->num_podspecs;
-  const int nv = d->num_new_values, nns = d->num_new_namespaces, nl = d->num_new_labelsets, nrq = d->num_new_reqs;
-  const int nsel = d->num_new_selectors, nnf = d->num_new_naff, ntm = d->num_new_naff_terms, ntol = d->num_new_tol_lists;
-  const int npl = d->num_new_port_lists, npts = d->num_new_pts_lists, nal = d->num_new_aff_lists, nat = d->num_new_aterms;
-  const int nsp = d->num_new_specs, P = d->num_pending, E = d->num_groups;
-  if ((nv | nns | nl | nrq | nsel | nnf | ntm | ntol | npl | npts | nal | nat | nsp | P | E) < 0) return bad("negative count");
-  if ((nv && (!d->value_is_int || !d->value_int)) || (nns && (!d->ns_labelset || !d->ns_exists)) || (nl && !d->ls_off) ||
-      (nrq && (!d->req_key || !d->req_op || !d->req_val_off)) || (nsel && (!d->sel_kind || !d->sel_req_off)) ||
-      (nnf && (!d->naff_nodesel || !d->naff_has_required || !d->naff_term_off)) || (ntm && (!d->term_expr_sel || !d->term_field_off)) ||
-      (ntol && !d->tol_off) || (npl && !d->port_off) || (npts && !d->pts_off) || (nal && !d->aff_off) ||
-      (nat && (!d->aterm_selector || !d->aterm_key || !d->aterm_ns_off || !d->aterm_ns_selector)) ||
-      (nsp && (!d->ps_namespace || !d->ps_labelset || !d->ps_req || !d->ps_tol_list || !d->ps_naff || !d->ps_node_name ||
-               !d->ps_port_list || !d->ps_pts_list || !d->ps_aff_list || !d->ps_anti_list || !d->ps_terminating || !d->ps_hostname_spread)) ||
-      !d->group_off || (P && !d->pend_spec))
-    return bad("NULL array with a non-zero count");
-  auto offsets_ok = [](const int32_t* off, int n) {
-    if (n == 0) return true;
-    if (off[0] != 0) return false;
-    for (int i = 0; i < n; ++i) if (off[i + 1] < off[i]) return false;
-    return true;
-  };
-  if (!offsets_ok(d->ls_off, nl) || !offsets_ok(d->req_val_off, nrq) || !offsets_ok(d->sel_req_off, nsel) ||
-      !offsets_ok(d->naff_term_off, nnf) || !offsets_ok(d->term_field_off, ntm) || !offsets_ok(d->tol_off, ntol) ||
-      !offsets_ok(d->port_off, npl) || !offsets_ok(d->pts_off, npts) || !offsets_ok(d->aff_off, nal) ||
-      !offsets_ok(d->aterm_ns_off, nat) || d->group_off[0] != 0 || !offsets_ok(d->group_off, E) || d->group_off[E] != P)
-    return bad("offsets that do not start at 0, decrease, or group_off not covering pend_spec");
-  auto end = [](const int32_t* off, int n) -> int64_t { return n ? off[n] : 0; };
-  const int64_t pairs = end(d->ls_off, nl), rvals = end(d->req_val_off, nrq), fields = end(d->term_field_off, ntm);
-  const int64_t tents = end(d->tol_off, ntol), pents = end(d->port_off, npl), cents = end(d->pts_off, npts), nsents = end(d->aterm_ns_off, nat);
-  if (end(d->sel_req_off, nsel) > nrq || end(d->naff_term_off, nnf) > ntm || end(d->aff_off, nal) > nat)
-    return bad("a tail's offsets run past its child tail");
-  if ((pairs && (!d->ls_key || !d->ls_val)) || (rvals && !d->req_vals) || (fields && (!d->field_op || !d->field_node_name)) ||
-      (tents && (!d->tol_key || !d->tol_op || !d->tol_val || !d->tol_effect)) || (pents && (!d->port_ip || !d->port_proto || !d->port_num)) ||
-      (cents && (!d->pts_max_skew || !d->pts_key || !d->pts_selector || !d->pts_min_domains || !d->pts_node_affinity_policy ||
-                 !d->pts_node_taints_policy)) ||
-      (nsents && !d->aterm_ns))
-    return bad("NULL array with a non-zero count");
-  // ---- status 2: sizes, from the counts and offsets alone ----
-  const int64_t NV = (int64_t)nh.num_values + nv, NNS = (int64_t)ph.num_namespaces + nns, NL = (int64_t)nh.num_labelsets + nl;
-  const int64_t NSEL = (int64_t)ph.num_selectors + nsel, NNF = (int64_t)ph.num_naff + nnf;
-  const int64_t NTL = (int64_t)ph.num_tol_lists + ntol, NPL = (int64_t)ph.port_off.size() - 1 + npl;
-  const int64_t NPTS = (int64_t)ph.pts_off.size() - 1 + npts, NAL = (int64_t)ph.aff_off.size() - 1 + nal, S = (int64_t)S0 + nsp;
-  if (NV > INT32_MAX || NNS > INT32_MAX || NL >= INT32_MAX || (int64_t)nh.ls_off.back() + pairs > INT32_MAX ||
-      (int64_t)ph.num_reqs + nrq >= INT32_MAX || (int64_t)ph.req_vals + rvals > INT32_MAX || NSEL >= INT32_MAX || NNF >= INT32_MAX ||
-      (int64_t)ph.num_naff_terms + ntm >= INT32_MAX || (int64_t)ph.fields + fields > INT32_MAX || NTL >= INT32_MAX ||
-      (int64_t)ph.tol_entries + tents > INT32_MAX || NPL >= INT32_MAX || (int64_t)ph.port_off.back() + pents > INT32_MAX ||
-      NPTS >= INT32_MAX || (int64_t)ph.pts_off.back() + cents > INT32_MAX || NAL >= INT32_MAX ||
-      (int64_t)ph.num_aterms + nat >= INT32_MAX || (int64_t)ph.aterm_ns + nsents > INT32_MAX || S > INT32_MAX / R)
-  { set_error("cae_load_pods: a table would pass 2^31 - 1 entries"); return 2; }
-  // ---- ids and enums ----
-  auto in = [](int64_t v, int64_t lo, int64_t hi) { return v >= lo && v < hi; };
-  for (int i = 0; i < nns; ++i) if (!in(d->ns_labelset[i], 0, NL) || d->ns_exists[i] > 1) return bad("namespace tail out of range");
-  for (int j = 0; j < nl; ++j)
-    for (int q = d->ls_off[j]; q < d->ls_off[j + 1]; ++q) {
-      if (d->ls_key[q] < 0 || (q > d->ls_off[j] && d->ls_key[q] <= d->ls_key[q - 1])) return bad("label pairs not sorted by key id");
-      if (!in(d->ls_val[q], 0, NV)) return bad("label value id out of range");
-    }
-  for (int i = 0; i < nrq; ++i) if (d->req_key[i] < 0 || !in(d->req_op[i], CAE_OP_IN, CAE_OP_LT + 1)) return bad("requirement out of range");
-  for (int64_t q = 0; q < rvals; ++q) if (!in(d->req_vals[q], 0, NV)) return bad("requirement value id out of range");
-  for (int i = 0; i < nsel; ++i) if (!in(d->sel_kind[i], CAE_SEL_NOTHING, CAE_SEL_REQS + 1)) return bad("selector kind out of range");
-  for (int i = 0; i < nnf; ++i)
-    if (!in(d->naff_nodesel[i], -1, NSEL) || d->naff_has_required[i] > 1) return bad("node-affinity record out of range");
-  for (int i = 0; i < ntm; ++i) if (!in(d->term_expr_sel[i], -1, NSEL)) return bad("node-affinity term selector out of range");
-  for (int64_t q = 0; q < fields; ++q)
-    if (!in(d->field_op[q], CAE_OP_IN, CAE_OP_NOT_IN + 1) || d->field_node_name[q] < 0) return bad("matchFields entry out of range");
-  for (int64_t q = 0; q < tents; ++q)
-    if (d->tol_key[q] < -1 || !in(d->tol_op[q], CAE_TOL_EQUAL, CAE_TOL_INVALID + 1) || !in(d->tol_val[q], -1, NV) ||
-        !in(d->tol_effect[q], CAE_EFFECT_NONE, CAE_EFFECT_NO_EXECUTE + 1))
-      return bad("toleration out of range");
-  for (int64_t q = 0; q < pents; ++q)
-    if (d->port_ip[q] < 0 || !in(d->port_proto[q], CAE_PROTO_TCP, CAE_PROTO_SCTP + 1) || d->port_num[q] <= 0) return bad("host port out of range");
-  for (int64_t q = 0; q < cents; ++q)
-    if (d->pts_key[q] < 0 || !in(d->pts_selector[q], 0, NSEL) || !in(d->pts_node_affinity_policy[q], 0, 2) ||
-        !in(d->pts_node_taints_policy[q], 0, 2))
-      return bad("topology spread constraint out of range");
-  for (int i = 0; i < nat; ++i)
-    if (!in(d->aterm_selector[i], 0, NSEL) || d->aterm_key[i] < 0 || !in(d->aterm_ns_selector[i], 0, NSEL)) return bad("affinity term out of range");
-  for (int64_t q = 0; q < nsents; ++q) if (!in(d->aterm_ns[q], 0, NNS)) return bad("affinity term namespace out of range");
-  for (int i = 0; i < nsp; ++i) {
-    if (!in(d->ps_namespace[i], 0, NNS) || !in(d->ps_labelset[i], 0, NL) || !in(d->ps_tol_list[i], 0, NTL) ||
-        !in(d->ps_naff[i], -1, NNF) || d->ps_node_name[i] < -1 || !in(d->ps_port_list[i], 0, NPL) || !in(d->ps_pts_list[i], 0, NPTS) ||
-        !in(d->ps_aff_list[i], 0, NAL) || !in(d->ps_anti_list[i], 0, NAL) || d->ps_terminating[i] > 1 || d->ps_hostname_spread[i] > 1)
-      return bad("pod-spec id out of range");
-    for (int r = 0; r < R; ++r)
-      if (d->ps_req[(size_t)i * R + r] < 0) return bad("pod-spec request negative");
-  }
-  for (int p = 0; p < P; ++p) if (!in(d->pend_spec[p], 0, S)) return bad("pending pod-spec id out of range");
+  const int P = d->num_pending, E = d->num_groups;
+  Tails v = pod_tails(d);
+  if (P < 0 || E < 0) return bad("negative count");
+  { const int rc = tails_present(v, bad); if (rc) return rc; }
+  if (!d->group_off || (P && !d->pend_spec)) return bad("NULL array with a non-zero count");
+  { const int rc = tails_offsets(v, bad); if (rc) return rc; }
+  if (!offsets_ok(d->group_off, E) || d->group_off[E] != P) return bad("group_off not covering pend_spec");
+  if (!tails_fit(e, v)) { set_error("cae_load_pods: a table would pass 2^31 - 1 entries"); return 2; }
+  { const int rc = tails_ids(e, v, bad); if (rc) return rc; }
+  const int S0 = e->num_podspecs, nsp = (int)v.n[CNT_SPECS], S = S0 + nsp;
+  for (int p = 0; p < P; ++p) if (d->pend_spec[p] < 0 || d->pend_spec[p] >= S) return bad("pending pod-spec id out of range");
   for (int i = 0; i < nsp; ++i)   // a new resource dimension changes num_res: a full load
-    for (int r = ph.num_res; r < R; ++r)
+    for (int r = e->dobj.num_res; r < R; ++r)
       if (d->ps_req[(size_t)i * R + r] != 0) { set_error("cae_load_pods: a request in a dim past the load's num_res"); return 2; }
   e->stats.h2d_bytes = 0;
   // ---- the node side the derivation reads on the host: the specs of the resident pods, each row's label set ----
@@ -1203,120 +1253,37 @@ static int do_load_pods(Engine* e, const cae_pod_delta* d) {
   std::vector<int32_t> row_ls((size_t)e->N + e->T);
   if (pd_resident_specs(e, S0, resident.data(), row_ls.data())) { e->loaded = false; return -1; }
 
-  // ---- the host mirrors the derivation reads, with the tails appended (taken back if a limit refuses the delta) ----
-  const size_t ls0 = nh.ls_off.size(), lp0 = nh.ls_key.size(), po0 = ph.port_off.size(), co0 = ph.pts_off.size(), ck0 = ph.pts_key.size();
-  const size_t ao0 = ph.aff_off.size(), ak0 = ph.aterm_key.size();
-  const int32_t old_pairs = nh.ls_off.back(), old_pents = ph.port_off.back(), old_cents = ph.pts_off.back();
-  for (int j = 0; j < nl; ++j) nh.ls_off.push_back(old_pairs + d->ls_off[j + 1]);
-  nh.ls_key.insert(nh.ls_key.end(), d->ls_key, d->ls_key + pairs);
-  nh.ls_val.insert(nh.ls_val.end(), d->ls_val, d->ls_val + pairs);
-  for (int j = 0; j < npl; ++j) ph.port_off.push_back(old_pents + d->port_off[j + 1]);
-  for (int j = 0; j < npts; ++j) ph.pts_off.push_back(old_cents + d->pts_off[j + 1]);
-  ph.pts_key.insert(ph.pts_key.end(), d->pts_key, d->pts_key + cents);
-  for (int j = 0; j < nal; ++j) ph.aff_off.push_back(ph.num_aterms + d->aff_off[j + 1]);
-  ph.aterm_key.insert(ph.aterm_key.end(), d->aterm_key, d->aterm_key + nat);
-  std::vector<int32_t>* cols[9] = {&ph.ps_namespace, &ph.ps_labelset, &ph.ps_tol_list, &ph.ps_naff, &ph.ps_node_name, &ph.ps_port_list,
-                                    &ph.ps_pts_list, &ph.ps_aff_list, &ph.ps_anti_list};
-  const int32_t* tails[9] = {d->ps_namespace, d->ps_labelset, d->ps_tol_list, d->ps_naff, d->ps_node_name, d->ps_port_list,
-                             d->ps_pts_list, d->ps_aff_list, d->ps_anti_list};
-  for (int c = 0; c < 9; ++c) cols[c]->insert(cols[c]->end(), tails[c], tails[c] + nsp);
-  e->h_spec_req.insert(e->h_spec_req.end(), d->ps_req, d->ps_req + (size_t)nsp * R);
-  auto take_back = [&]() {
-    nh.ls_off.resize(ls0); nh.ls_key.resize(lp0); nh.ls_val.resize(lp0); ph.port_off.resize(po0); ph.pts_off.resize(co0);
-    ph.pts_key.resize(ck0); ph.aff_off.resize(ao0); ph.aterm_key.resize(ak0);
-    for (int c = 0; c < 9; ++c) cols[c]->resize(S0);
-    e->h_spec_req.resize((size_t)S0 * R);
-  };
-  cae_objects v{};
-  v.abi_version = CAE_ABI_VERSION; v.num_res = ph.num_res; v.num_values = (int32_t)NV; v.hostname_key = ph.hostname_key;
-  v.num_labelsets = (int32_t)NL; v.ls_off = nh.ls_off.data(); v.ls_key = nh.ls_key.data(); v.ls_val = nh.ls_val.data();
-  v.num_port_lists = (int32_t)NPL; v.port_off = ph.port_off.data();
-  v.num_pts_lists = (int32_t)NPTS; v.pts_off = ph.pts_off.data(); v.pts_key = ph.pts_key.data();
-  v.num_aff_lists = (int32_t)NAL; v.aff_off = ph.aff_off.data(); v.aterm_key = ph.aterm_key.data(); v.num_aterms = ph.num_aterms + nat;
-  v.num_podspecs = (int32_t)S; v.ps_namespace = ph.ps_namespace.data(); v.ps_labelset = ph.ps_labelset.data();
-  v.ps_req = e->h_spec_req.data(); v.ps_tol_list = ph.ps_tol_list.data(); v.ps_naff = ph.ps_naff.data();
-  v.ps_node_name = ph.ps_node_name.data(); v.ps_port_list = ph.ps_port_list.data(); v.ps_pts_list = ph.ps_pts_list.data();
-  v.ps_aff_list = ph.ps_aff_list.data(); v.ps_anti_list = ph.ps_anti_list.data();
-  v.num_cluster_nodes = e->N; v.num_templates = e->T; v.node_labelset = row_ls.data();
-  v.num_groups = E; v.num_pending = P; v.group_off = d->group_off; v.pend_spec = d->pend_spec;
+  // ---- the tails in one pinned blob and in the host mirrors the derivation reads (taken back if a limit refuses) ----
+  size_t at[NUM_DICT_TABLES];
+  const size_t bytes = tails_layout(v, at, 0);
+  // the blob is written before the status-1 limits are planned because the host mirrors the plan reads are appended from
+  // it; a refused delta leaves only this engine-internal staging buffer (possibly grown) behind
+  if (pinned_reserve(e, e->pd_stage, std::max<size_t>(bytes, 8))) { e->loaded = false; return -1; }
+  tails_put(e, v, at, static_cast<char*>(e->pd_stage.p));
+  cae_objects o{};
+  for (int t = 0; t < NUM_DICT_TABLES; ++t)
+    if (kDict[t].host) *reinterpret_cast<const void**>(reinterpret_cast<char*>(&o) + kDict[t].obj) = e->dict_host[t].data();
+  auto tot = [&](int c) { return (int32_t)(e->dict_cnt[c] + v.n[c]); };
+  o.abi_version = CAE_ABI_VERSION; o.num_res = e->dobj.num_res; o.hostname_key = e->dobj.hostname_key;
+  o.num_values = tot(CNT_VALUES); o.num_labelsets = tot(CNT_LABELSETS); o.num_port_lists = tot(CNT_PORT_LISTS);
+  o.num_pts_lists = tot(CNT_PTS_LISTS); o.num_aff_lists = tot(CNT_AFF_LISTS); o.num_aterms = tot(CNT_ATERMS); o.num_podspecs = S;
+  o.num_cluster_nodes = e->N; o.num_templates = e->T; o.node_labelset = row_ls.data();
+  o.num_groups = E; o.num_pending = P; o.group_off = d->group_off; o.pend_spec = d->pend_spec;
 
-  // ---- commit: one pinned blob and one H2D copy of every tail (offsets made absolute), then the device tables grow ----
-  DevObjects& o = e->dobj;
-  struct Col { Engine::DevBuf* buf; const void** cur; size_t elem, n_old; const void* src; size_t n; int64_t base; bool off; };
-  auto C_ = [](Engine::DevBuf& b, const void* field_addr, size_t elem, size_t n_old, const void* src, size_t n) {
-    return Col{&b, (const void**)field_addr, elem, n_old, src, n, 0, false};
-  };
-  auto O_ = [](Engine::DevBuf& b, const void* field_addr, size_t n_old, const int32_t* rel, size_t n, int64_t base) {
-    return Col{&b, (const void**)field_addr, 4, n_old, rel, n, base, true};
-  };
-  Engine::DevBuf* t = e->pd_tab;
-  const Col col[] = {
-      C_(e->nd_tab[0], &o.value_is_int, 1, nh.num_values, d->value_is_int, nv), C_(e->nd_tab[1], &o.value_int, 8, nh.num_values, d->value_int, nv),
-      C_(t[0], &o.ns_labelset, 4, ph.num_namespaces, d->ns_labelset, nns), C_(t[1], &o.ns_exists, 1, ph.num_namespaces, d->ns_exists, nns),
-      O_(e->nd_tab[2], &o.ls_off, (size_t)nh.num_labelsets + 1, d->ls_off, nl, old_pairs),
-      C_(e->nd_tab[3], &o.ls_key, 4, old_pairs, d->ls_key, pairs), C_(e->nd_tab[4], &o.ls_val, 4, old_pairs, d->ls_val, pairs),
-      C_(t[2], &o.req_key, 4, ph.num_reqs, d->req_key, nrq), C_(t[3], &o.req_op, 4, ph.num_reqs, d->req_op, nrq),
-      O_(t[4], &o.req_val_off, (size_t)ph.num_reqs + 1, d->req_val_off, nrq, ph.req_vals), C_(t[5], &o.req_vals, 4, ph.req_vals, d->req_vals, rvals),
-      C_(t[6], &o.sel_kind, 4, ph.num_selectors, d->sel_kind, nsel),
-      O_(t[7], &o.sel_req_off, (size_t)ph.num_selectors + 1, d->sel_req_off, nsel, ph.num_reqs),
-      C_(t[8], &o.naff_nodesel, 4, ph.num_naff, d->naff_nodesel, nnf), C_(t[9], &o.naff_has_required, 1, ph.num_naff, d->naff_has_required, nnf),
-      O_(t[10], &o.naff_term_off, (size_t)ph.num_naff + 1, d->naff_term_off, nnf, ph.num_naff_terms),
-      C_(t[11], &o.term_expr_sel, 4, ph.num_naff_terms, d->term_expr_sel, ntm),
-      O_(t[12], &o.term_field_off, (size_t)ph.num_naff_terms + 1, d->term_field_off, ntm, ph.fields),
-      C_(t[13], &o.field_op, 4, ph.fields, d->field_op, fields), C_(t[14], &o.field_node_name, 4, ph.fields, d->field_node_name, fields),
-      O_(t[15], &o.tol_off, (size_t)ph.num_tol_lists + 1, d->tol_off, ntol, ph.tol_entries),
-      C_(t[16], &o.tol_key, 4, ph.tol_entries, d->tol_key, tents), C_(t[17], &o.tol_op, 4, ph.tol_entries, d->tol_op, tents),
-      C_(t[18], &o.tol_val, 4, ph.tol_entries, d->tol_val, tents), C_(t[19], &o.tol_effect, 4, ph.tol_entries, d->tol_effect, tents),
-      O_(t[20], &o.port_off, po0, d->port_off, npl, old_pents),
-      C_(t[21], &o.port_ip, 4, old_pents, d->port_ip, pents), C_(t[22], &o.port_proto, 4, old_pents, d->port_proto, pents),
-      C_(t[23], &o.port_num, 4, old_pents, d->port_num, pents),
-      O_(t[24], &o.pts_off, co0, d->pts_off, npts, old_cents),
-      C_(t[25], &o.pts_max_skew, 4, old_cents, d->pts_max_skew, cents), C_(t[26], &o.pts_key, 4, old_cents, d->pts_key, cents),
-      C_(t[27], &o.pts_selector, 4, old_cents, d->pts_selector, cents), C_(t[28], &o.pts_min_domains, 4, old_cents, d->pts_min_domains, cents),
-      C_(t[29], &o.pts_node_affinity_policy, 4, old_cents, d->pts_node_affinity_policy, cents),
-      C_(t[30], &o.pts_node_taints_policy, 4, old_cents, d->pts_node_taints_policy, cents),
-      O_(t[31], &o.aff_off, ao0, d->aff_off, nal, ph.num_aterms),
-      C_(t[32], &o.aterm_selector, 4, ph.num_aterms, d->aterm_selector, nat), C_(t[33], &o.aterm_key, 4, ph.num_aterms, d->aterm_key, nat),
-      O_(t[34], &o.aterm_ns_off, (size_t)ph.num_aterms + 1, d->aterm_ns_off, nat, ph.aterm_ns),
-      C_(t[35], &o.aterm_ns, 4, ph.aterm_ns, d->aterm_ns, nsents), C_(t[36], &o.aterm_ns_selector, 4, ph.num_aterms, d->aterm_ns_selector, nat),
-      C_(t[37], &o.ps_namespace, 4, S0, d->ps_namespace, nsp), C_(t[38], &o.ps_labelset, 4, S0, d->ps_labelset, nsp),
-      C_(t[39], &o.ps_req, 8 * R, S0, d->ps_req, nsp), C_(t[40], &o.ps_tol_list, 4, S0, d->ps_tol_list, nsp),
-      C_(t[41], &o.ps_naff, 4, S0, d->ps_naff, nsp), C_(t[42], &o.ps_node_name, 4, S0, d->ps_node_name, nsp),
-      C_(t[43], &o.ps_port_list, 4, S0, d->ps_port_list, nsp), C_(t[44], &o.ps_pts_list, 4, S0, d->ps_pts_list, nsp),
-      C_(t[45], &o.ps_aff_list, 4, S0, d->ps_aff_list, nsp), C_(t[46], &o.ps_anti_list, 4, S0, d->ps_anti_list, nsp),
-      C_(t[47], &o.ps_terminating, 1, S0, d->ps_terminating, nsp), C_(t[48], &o.ps_hostname_spread, 1, S0, d->ps_hostname_spread, nsp),
-  };
+  // ---- commit: the H2D copy of the blob, then the device tables grow ----
   auto commit = [&]() -> int {
-    size_t bytes = 0;
-    std::vector<size_t> at;
-    for (const Col& c : col) { at.push_back(bytes); bytes = (bytes + c.n * c.elem + 7) & ~(size_t)7; }
-    if (pinned_reserve(e, e->pd_stage, std::max<size_t>(bytes, 8))) return -1;
-    char* h = static_cast<char*>(e->pd_stage.p);
-    for (size_t i = 0; i < sizeof(col) / sizeof(col[0]); ++i) {
-      const Col& c = col[i];
-      if (!c.n) continue;
-      if (c.off) for (size_t j = 0; j < c.n; ++j) reinterpret_cast<int32_t*>(h + at[i])[j] = (int32_t)(c.base + static_cast<const int32_t*>(c.src)[j + 1]);
-      else memcpy(h + at[i], c.src, c.n * c.elem);
-    }
     if (devbuf_reserve(e, e->pd_blob, std::max<size_t>(bytes, 8))) return -1;
     char* dv = static_cast<char*>(e->pd_blob.p);
-    if (bytes) CAE_CUDA(cudaMemcpyAsync(dv, h, bytes, cudaMemcpyHostToDevice, e->stream));
+    if (bytes) CAE_CUDA(cudaMemcpyAsync(dv, e->pd_stage.p, bytes, cudaMemcpyHostToDevice, e->stream));
     CAE_CUDA(cudaEventRecord(e->pd_stage.ev, e->stream));
     e->stats.h2d_bytes += (int64_t)bytes;
-    for (size_t i = 0; i < sizeof(col) / sizeof(col[0]); ++i)
-      if (grow_bytes(e, *col[i].buf, *col[i].cur, col[i].elem, col[i].n_old, dv + at[i], col[i].n)) return -1;
-    // host counts and per-spec state of the grown tables
-    o.num_values = (int32_t)NV;
-    nh.num_values = (int32_t)NV; nh.num_labelsets = (int32_t)NL;
-    ph.num_namespaces = (int32_t)NNS; ph.num_reqs += nrq; ph.req_vals += (int32_t)rvals; ph.num_selectors = (int32_t)NSEL;
-    ph.num_naff = (int32_t)NNF; ph.num_naff_terms += ntm; ph.fields += (int32_t)fields; ph.num_tol_lists = (int32_t)NTL;
-    ph.tol_entries += (int32_t)tents; ph.num_aterms += nat; ph.aterm_ns += (int32_t)nsents;
-    nh.spec_anti.resize(S);
-    for (int64_t s = S0; s < S; ++s) nh.spec_anti[s] = ph.aff_off[ph.ps_anti_list[s] + 1] > ph.aff_off[ph.ps_anti_list[s]];
+    if (tails_grow(e, v, at, dv)) return -1;
+    e->nh.spec_anti.resize(S);
+    for (int s = S0; s < S; ++s) e->nh.spec_anti[s] = o.aff_off[o.ps_anti_list[s] + 1] > o.aff_off[o.ps_anti_list[s]];
     return 0;
   };
-  const int rc = derive_pending(e, &v, lt, &resident, commit);
-  if (rc > 0 || rc == -2) take_back();
+  const int rc = derive_pending(e, &o, lt, &resident, commit);
+  if (rc > 0 || rc == -2) take_back_mirrors(e);
   else if (rc) e->loaded = false;   // a CUDA error part way: the engine needs a cae_load
   return rc;
 }
@@ -1354,16 +1321,17 @@ static int do_similar(Engine* e, const cae_similarity_inputs* in, uint32_t* bits
   int32_t* h_res = reinterpret_cast<int32_t*>(h + o_i32);
   int32_t *h_lab = h_res + T, *h_fd = h_res + 2 * T, *h_fl = h_res + 3 * T;
   int64_t* h_cap = reinterpret_cast<int64_t*>(h + o_cap);
-  const Engine::NodeHost& nh = e->nh;
+  const int32_t *ls_off = e->host_tab<int32_t>(TAB_ls_off), *ls_key = e->host_tab<int32_t>(TAB_ls_key),
+                *ls_val = e->host_tab<int32_t>(TAB_ls_val);
   std::unordered_map<std::string, int32_t> lab_id;
   lab_id.reserve((size_t)T * 2);
   std::string key;
   for (int t = 0; t < T; ++t) {
     key.clear();
-    const int ls = nh.tmpl_ls[t];
-    for (int i = nh.ls_off[ls]; i < nh.ls_off[ls + 1]; ++i) {
-      if (std::binary_search(ign.begin(), ign.end(), nh.ls_key[i])) continue;
-      const int32_t kv[2] = {nh.ls_key[i], nh.ls_val[i]};
+    const int ls = e->nh.tmpl_ls[t];
+    for (int i = ls_off[ls]; i < ls_off[ls + 1]; ++i) {
+      if (std::binary_search(ign.begin(), ign.end(), ls_key[i])) continue;
+      const int32_t kv[2] = {ls_key[i], ls_val[i]};
       key.append(reinterpret_cast<const char*>(kv), sizeof(kv));
     }
     h_lab[t] = lab_id.emplace(key, (int32_t)lab_id.size()).first->second;

@@ -19,6 +19,84 @@ constexpr int FEAS_TW = 16;                // template words per thread block of
 
 void set_error(const std::string& msg);
 
+// The counts that size the dictionary tables.  The first CNT_ROOTS are stated by cae_objects and the delta structs; each of
+// the others is the last offset of the offsets table that indexes it.
+enum DictCount : int {
+  CNT_NONE = -1,
+  CNT_VALUES, CNT_NAMESPACES, CNT_LABELSETS, CNT_REQS, CNT_SELECTORS, CNT_NAFF, CNT_NAFF_TERMS, CNT_TOL_LISTS, CNT_TAINT_LISTS,
+  CNT_PORT_LISTS, CNT_PTS_LISTS, CNT_AFF_LISTS, CNT_ATERMS, CNT_SPECS,
+  CNT_PAIRS, CNT_REQ_VALS, CNT_FIELDS, CNT_TOLS, CNT_TAINTS, CNT_PORTS, CNT_PTS, CNT_ATERM_NS,
+  NUM_DICT_COUNTS,
+  CNT_ROOTS = CNT_PAIRS
+};
+// The dictionary tables of cae_objects that the deltas continue with tails, in upload order (api.cu uploads, checks and
+// appends them from this list).  X(field, element type, elements per entry, count, child count, carried by, host mirror):
+// an offsets table has count + 1 entries and indexes the tables of its child count (NONE: not an offsets table); "carried
+// by" names the delta structs with the field (NODE: cae_node_delta, POD: cae_pod_delta, BOTH); a host mirror is kept for
+// the pending-side derivation, which cae_load_pods reruns without the caller's cae_objects.
+#define CAE_DICT_TABLES(X)                                         \
+  X(value_is_int, uint8_t, 1, VALUES, NONE, BOTH, 0)               \
+  X(value_int, int64_t, 1, VALUES, NONE, BOTH, 0)                  \
+  X(ns_labelset, int32_t, 1, NAMESPACES, NONE, POD, 0)             \
+  X(ns_exists, uint8_t, 1, NAMESPACES, NONE, POD, 0)               \
+  X(ls_off, int32_t, 1, LABELSETS, PAIRS, BOTH, 1)                 \
+  X(ls_key, int32_t, 1, PAIRS, NONE, BOTH, 1)                      \
+  X(ls_val, int32_t, 1, PAIRS, NONE, BOTH, 1)                      \
+  X(req_key, int32_t, 1, REQS, NONE, POD, 0)                       \
+  X(req_op, int32_t, 1, REQS, NONE, POD, 0)                        \
+  X(req_val_off, int32_t, 1, REQS, REQ_VALS, POD, 0)               \
+  X(req_vals, int32_t, 1, REQ_VALS, NONE, POD, 0)                  \
+  X(sel_kind, int32_t, 1, SELECTORS, NONE, POD, 0)                 \
+  X(sel_req_off, int32_t, 1, SELECTORS, REQS, POD, 0)              \
+  X(naff_nodesel, int32_t, 1, NAFF, NONE, POD, 0)                  \
+  X(naff_has_required, uint8_t, 1, NAFF, NONE, POD, 0)             \
+  X(naff_term_off, int32_t, 1, NAFF, NAFF_TERMS, POD, 0)           \
+  X(term_expr_sel, int32_t, 1, NAFF_TERMS, NONE, POD, 0)           \
+  X(term_field_off, int32_t, 1, NAFF_TERMS, FIELDS, POD, 0)        \
+  X(field_op, int32_t, 1, FIELDS, NONE, POD, 0)                    \
+  X(field_node_name, int32_t, 1, FIELDS, NONE, POD, 0)             \
+  X(tol_off, int32_t, 1, TOL_LISTS, TOLS, POD, 0)                  \
+  X(tol_key, int32_t, 1, TOLS, NONE, POD, 0)                       \
+  X(tol_op, int32_t, 1, TOLS, NONE, POD, 0)                        \
+  X(tol_val, int32_t, 1, TOLS, NONE, POD, 0)                       \
+  X(tol_effect, int32_t, 1, TOLS, NONE, POD, 0)                    \
+  X(taint_off, int32_t, 1, TAINT_LISTS, TAINTS, NODE, 0)           \
+  X(taint_key, int32_t, 1, TAINTS, NONE, NODE, 0)                  \
+  X(taint_val, int32_t, 1, TAINTS, NONE, NODE, 0)                  \
+  X(taint_effect, int32_t, 1, TAINTS, NONE, NODE, 0)               \
+  X(port_off, int32_t, 1, PORT_LISTS, PORTS, POD, 1)               \
+  X(port_ip, int32_t, 1, PORTS, NONE, POD, 0)                      \
+  X(port_proto, int32_t, 1, PORTS, NONE, POD, 0)                   \
+  X(port_num, int32_t, 1, PORTS, NONE, POD, 0)                     \
+  X(pts_off, int32_t, 1, PTS_LISTS, PTS, POD, 1)                   \
+  X(pts_max_skew, int32_t, 1, PTS, NONE, POD, 0)                   \
+  X(pts_key, int32_t, 1, PTS, NONE, POD, 1)                        \
+  X(pts_selector, int32_t, 1, PTS, NONE, POD, 0)                   \
+  X(pts_min_domains, int32_t, 1, PTS, NONE, POD, 0)                \
+  X(pts_node_affinity_policy, int32_t, 1, PTS, NONE, POD, 0)       \
+  X(pts_node_taints_policy, int32_t, 1, PTS, NONE, POD, 0)         \
+  X(aff_off, int32_t, 1, AFF_LISTS, ATERMS, POD, 1)                \
+  X(aterm_selector, int32_t, 1, ATERMS, NONE, POD, 0)              \
+  X(aterm_key, int32_t, 1, ATERMS, NONE, POD, 1)                   \
+  X(aterm_ns_off, int32_t, 1, ATERMS, ATERM_NS, POD, 0)            \
+  X(aterm_ns, int32_t, 1, ATERM_NS, NONE, POD, 0)                  \
+  X(aterm_ns_selector, int32_t, 1, ATERMS, NONE, POD, 0)           \
+  X(ps_namespace, int32_t, 1, SPECS, NONE, POD, 1)                 \
+  X(ps_labelset, int32_t, 1, SPECS, NONE, POD, 1)                  \
+  X(ps_req, int64_t, CAE_MAX_RES, SPECS, NONE, POD, 1)             \
+  X(ps_tol_list, int32_t, 1, SPECS, NONE, POD, 1)                  \
+  X(ps_naff, int32_t, 1, SPECS, NONE, POD, 1)                      \
+  X(ps_node_name, int32_t, 1, SPECS, NONE, POD, 1)                 \
+  X(ps_port_list, int32_t, 1, SPECS, NONE, POD, 1)                 \
+  X(ps_pts_list, int32_t, 1, SPECS, NONE, POD, 1)                  \
+  X(ps_aff_list, int32_t, 1, SPECS, NONE, POD, 1)                  \
+  X(ps_anti_list, int32_t, 1, SPECS, NONE, POD, 1)                 \
+  X(ps_terminating, uint8_t, 1, SPECS, NONE, POD, 0)               \
+  X(ps_hostname_spread, uint8_t, 1, SPECS, NONE, POD, 0)
+#define CAE_DICT_ID(field, type, per, cnt, child, by, host) TAB_##field,
+enum DictTable : int { CAE_DICT_TABLES(CAE_DICT_ID) NUM_DICT_TABLES };
+#undef CAE_DICT_ID
+
 // Everything the estimator needs to know about a pending pod group, gathered once per load so that a thread block
 // fetches ONE contiguous record per group (cp.async, one group ahead) instead of chasing five dependent tables.
 struct alignas(16) GroupRec {
@@ -215,12 +293,15 @@ struct Engine {
   std::vector<uint8_t> h_spec_pending;    // [num_podspecs] spec carried by a pending pod at the last full load
   int cap_P = 0, cap_E = 0, cap_Pl = 0;   // capacities of the resident per-pod / per-group buffers (cae_load_pending)
   PinnedBuf pending_stage;                // pend_spec | group_off, source of cae_load_pending's H2D copy
-  std::vector<int64_t> h_spec_req;        // [num_podspecs][R]
   int num_podspecs = 0;
+  // the resident dictionary tables (CAE_DICT_TABLES): set by cae_load, grown by every delta's tails (api.cu)
+  int64_t dict_cnt[NUM_DICT_COUNTS] = {0};   // entries of each count (DevObjects::num_values is set from CNT_VALUES)
+  DevBuf dict_tab[NUM_DICT_TABLES];          // engine-owned device copies of the tables a delta grew
+  std::vector<char> dict_host[NUM_DICT_TABLES];   // host mirrors of the tables marked so, tails appended
+  template <class T>
+  const T* host_tab(int t) const { return reinterpret_cast<const T*>(dict_host[t].data()); }
   // host state of the last load that cae_load_nodes / cae_load_node_churn validate against and update (api.cu)
   struct NodeHost {
-    int32_t num_values = 0, num_labelsets = 0, num_taint_lists = 0, taint_entries = 0;
-    std::vector<int32_t> ls_off, ls_key, ls_val;   // resident label-set table, tails appended
     std::vector<int32_t> pod_cnt;                  // [N] resident pods per cluster row
     int64_t pod_total = 0;                         // node_pod_off[N + T]
     std::vector<uint8_t> spec_used;                // [S] spec pending or resident (only grows between loads)
@@ -231,22 +312,10 @@ struct Engine {
     std::vector<int32_t> dom_scratch;              // value id -> domain while the domains are assigned (all -1 in between)
     std::vector<int32_t> tmpl_ls;                  // [T] label set of each template (no delta changes a template)
   } nh;
-  // host mirrors of the spec-side tables the pending-side derivation reads (derive_pending in api.cu), so that
-  // cae_load_pods can rerun it without the caller's cae_objects (the node side it reads from the device)
-  struct PodHost {
-    int32_t hostname_key = -1, num_res = 0;
-    int32_t num_namespaces = 0, num_reqs = 0, req_vals = 0, num_selectors = 0, num_naff = 0, num_naff_terms = 0, fields = 0;
-    int32_t num_tol_lists = 0, tol_entries = 0, num_aterms = 0, aterm_ns = 0;
-    std::vector<int32_t> ps_namespace, ps_labelset, ps_tol_list, ps_naff, ps_node_name, ps_port_list, ps_pts_list, ps_aff_list,
-        ps_anti_list;                              // [S] spec columns (requests: h_spec_req)
-    std::vector<int32_t> port_off, pts_off, pts_key, aff_off, aterm_key;
-  } ph;
-  DevBuf pd_tab[49];                      // spec-side dictionary tables and spec columns grown by cae_load_pods
   PinnedBuf pd_stage;                     // cae_load_pods' tails, source of its one H2D copy
   DevBuf pd_blob;                         // device copy of the tails
   DevBuf pd_used;                         // [S] specs of the resident pods (pod_delta.cu)
   // buffers of cae_load_nodes (a cae_load points DevObjects back at its arena)
-  DevBuf nd_tab[9];                       // grown dictionary tables: value_is_int, value_int, ls_off|key|val, taint_off|key|val|effect
   DevBuf nd_off[2], nd_spec[2];           // double-buffered resident CSR (node_pod_off / node_pod_spec)
   DevBuf nd_cnt, nd_didx, nd_cub, nd_blob;  // per-row counts / source rows, scan temp storage, device copy of the delta
   PinnedBuf nd_stage;                     // the delta, source of its one H2D copy

@@ -290,70 +290,144 @@ def _parse_int64(s: str) -> Tuple[bool, int]:
     return True, v
 
 
+# The dictionary tables of cae_objects that the deltas continue with tails (the engine states the same list in
+# csrc/engine.h, CAE_DICT_TABLES): (ABI array, the count that sizes it, the child count an offsets array indexes,
+# dtype, the builder storage behind it, the column of a row tuple or None).  An offsets array has count + 1 entries.
+_DICT = tuple((nm, cnt, child, dt, get, col) for nm, cnt, child, dt, get, col in (
+    ("value_is_int", "values", None, np.uint8, lambda b: b.value_is_int, None),
+    ("value_int", "values", None, np.int64, lambda b: b.value_int, None),
+    ("ns_labelset", "namespaces", None, np.int32, lambda b: b.ns_labelset, None),
+    ("ns_exists", "namespaces", None, np.uint8, lambda b: b.ns_exists, None),
+    ("ls_off", "labelsets", "pairs", np.int32, lambda b: b.labelsets.off, None),
+    ("ls_key", "pairs", None, np.int32, lambda b: b.labelsets.cols[0], None),
+    ("ls_val", "pairs", None, np.int32, lambda b: b.labelsets.cols[1], None),
+    ("req_key", "reqs", None, np.int32, lambda b: b.reqs_key, None),
+    ("req_op", "reqs", None, np.int32, lambda b: b.reqs_op, None),
+    ("req_val_off", "reqs", "req_vals", np.int32, lambda b: b.reqs_val_off, None),
+    ("req_vals", "req_vals", None, np.int32, lambda b: b.reqs_vals, None),
+    ("sel_kind", "selectors", None, np.int32, lambda b: b.sel_kind, None),
+    ("sel_req_off", "selectors", "reqs", np.int32, lambda b: b.sel_req_off, None),
+    ("naff_nodesel", "naff", None, np.int32, lambda b: b.naff_nodesel, None),
+    ("naff_has_required", "naff", None, np.uint8, lambda b: b.naff_has_required, None),
+    ("naff_term_off", "naff", "naff_terms", np.int32, lambda b: b.naff_term_off, None),
+    ("term_expr_sel", "naff_terms", None, np.int32, lambda b: b.term_expr_sel, None),
+    ("term_field_off", "naff_terms", "fields", np.int32, lambda b: b.term_field_off, None),
+    ("field_op", "fields", None, np.int32, lambda b: b.field_op, None),
+    ("field_node_name", "fields", None, np.int32, lambda b: b.field_node_name, None),
+    ("tol_off", "tol_lists", "tols", np.int32, lambda b: b.tols.off, None),
+    ("tol_key", "tols", None, np.int32, lambda b: b.tols.cols[0], None),
+    ("tol_op", "tols", None, np.int32, lambda b: b.tols.cols[1], None),
+    ("tol_val", "tols", None, np.int32, lambda b: b.tols.cols[2], None),
+    ("tol_effect", "tols", None, np.int32, lambda b: b.tols.cols[3], None),
+    ("taint_off", "taint_lists", "taints", np.int32, lambda b: b.taints.off, None),
+    ("taint_key", "taints", None, np.int32, lambda b: b.taints.cols[0], None),
+    ("taint_val", "taints", None, np.int32, lambda b: b.taints.cols[1], None),
+    ("taint_effect", "taints", None, np.int32, lambda b: b.taints.cols[2], None),
+    ("port_off", "port_lists", "ports", np.int32, lambda b: b.ports.off, None),
+    ("port_ip", "ports", None, np.int32, lambda b: b.ports.cols[0], None),
+    ("port_proto", "ports", None, np.int32, lambda b: b.ports.cols[1], None),
+    ("port_num", "ports", None, np.int32, lambda b: b.ports.cols[2], None),
+    ("pts_off", "pts_lists", "pts", np.int32, lambda b: b.pts.off, None),
+    ("pts_max_skew", "pts", None, np.int32, lambda b: b.pts.cols[0], None),
+    ("pts_key", "pts", None, np.int32, lambda b: b.pts.cols[1], None),
+    ("pts_selector", "pts", None, np.int32, lambda b: b.pts.cols[2], None),
+    ("pts_min_domains", "pts", None, np.int32, lambda b: b.pts.cols[3], None),
+    ("pts_node_affinity_policy", "pts", None, np.int32, lambda b: b.pts.cols[4], None),
+    ("pts_node_taints_policy", "pts", None, np.int32, lambda b: b.pts.cols[5], None),
+    ("aff_off", "aff_lists", "aterms", np.int32, lambda b: b.aff_off, None),
+    ("aterm_selector", "aterms", None, np.int32, lambda b: b.aterm_selector, None),
+    ("aterm_key", "aterms", None, np.int32, lambda b: b.aterm_key, None),
+    ("aterm_ns_off", "aterms", "aterm_ns", np.int32, lambda b: b.aterm_ns_off, None),
+    ("aterm_ns", "aterm_ns", None, np.int32, lambda b: b.aterm_ns, None),
+    ("aterm_ns_selector", "aterms", None, np.int32, lambda b: b.aterm_ns_selector, None),
+    ("ps_namespace", "specs", None, np.int32, lambda b: b.ps_rows, 0),
+    ("ps_labelset", "specs", None, np.int32, lambda b: b.ps_rows, 1),
+    ("ps_req", "specs", None, np.int64, lambda b: b.ps_rows, 2),
+    ("ps_tol_list", "specs", None, np.int32, lambda b: b.ps_rows, 3),
+    ("ps_naff", "specs", None, np.int32, lambda b: b.ps_rows, 4),
+    ("ps_node_name", "specs", None, np.int32, lambda b: b.ps_rows, 5),
+    ("ps_port_list", "specs", None, np.int32, lambda b: b.ps_rows, 6),
+    ("ps_pts_list", "specs", None, np.int32, lambda b: b.ps_rows, 7),
+    ("ps_aff_list", "specs", None, np.int32, lambda b: b.ps_rows, 8),
+    ("ps_anti_list", "specs", None, np.int32, lambda b: b.ps_rows, 9),
+    ("ps_terminating", "specs", None, np.uint8, lambda b: b.ps_rows, 10),
+    ("ps_hostname_spread", "specs", None, np.uint8, lambda b: b.ps_rows, 11),
+))
+# cae_objects' field for each count it states; the other counts are the last offset of the offsets array that indexes them
+_COUNT_FIELD = {"values": "num_values", "namespaces": "num_namespaces", "labelsets": "num_labelsets", "reqs": "num_reqs",
+                "selectors": "num_selectors", "naff": "num_naff", "naff_terms": "num_naff_terms", "tol_lists": "num_tol_lists",
+                "taint_lists": "num_taint_lists", "port_lists": "num_port_lists", "pts_lists": "num_pts_lists",
+                "aff_lists": "num_aff_lists", "aterms": "num_aterms", "specs": "num_podspecs"}
+
+
+def _dict_array(nm: str, dt, x) -> np.ndarray:
+    if nm == "ps_req":
+        return np.ascontiguousarray(np.asarray(x, np.int64).reshape(len(x), MAX_RES))
+    return _i32(x) if dt is np.int32 else np.ascontiguousarray(x, dt)
+
+
+def _cut(b: "TableBuilder", start: Dict[str, int], tables) -> Dict[str, np.ndarray]:
+    """The dictionary tables `tables` of builder b from the entries `start` of each count on (offsets relative to the
+    start of their child), as ABI arrays.  Costs what the cut holds, not the table."""
+    out = {}
+    for nm, cnt, child, dt, get, col in _DICT:
+        if nm in tables:
+            x = get(b)[start.get(cnt, 0):]
+            if col is not None:
+                x = [r[col] for r in x]
+            if child is not None and start.get(child, 0):
+                x = [o - start[child] for o in x]
+            out[nm] = _dict_array(nm, dt, x)
+    return out
+
+
+def _dict_sizes(b: "TableBuilder", counts) -> Dict[str, int]:
+    """The entries of each of `counts` in builder b."""
+    return {cnt: len(get(b)) - (child is not None) for nm, cnt, child, dt, get, col in _DICT if cnt in counts}
+
+
+def _dict_counts(s, a: Dict[str, np.ndarray]) -> Dict[str, int]:
+    """The entries of every count in the tables of cae_objects `s` with arrays `a`."""
+    n = {cnt: getattr(s, f) for cnt, f in _COUNT_FIELD.items()}
+    for nm, cnt, child, *_ in _DICT:
+        if child is not None and child not in _COUNT_FIELD:
+            n[child] = int(a[nm][n[cnt]])
+    return n
+
+
+def _root_counts(a: Dict[str, np.ndarray]) -> Dict[str, int]:
+    """cae_objects' count fields, from the lengths of the dictionary arrays `a`."""
+    out = {}
+    for nm, cnt, child, *_ in _DICT:
+        if cnt in _COUNT_FIELD and _COUNT_FIELD[cnt] not in out:
+            out[_COUNT_FIELD[cnt]] = len(a[nm]) - (child is not None)
+    return out
+
+
+def _table_names(struct_cls) -> set:
+    """The dictionary tables a delta struct carries."""
+    fields = {f for f, _ in struct_cls._fields_}
+    return {nm for nm, *_ in _DICT if nm in fields}
+
+
+def _families(tables) -> set:
+    """The counts that size `tables`."""
+    return {cnt for nm, cnt, *_ in _DICT if nm in tables}
+
+
+_ALL_TABLES = {nm for nm, *_ in _DICT}
+_NODE_TABLES = _table_names(capi.cae_node_delta)   # values, label sets, taint lists
+_POD_TABLES = _table_names(capi.cae_pod_delta)     # every family but the taint lists
+
+
 class EncodedObjects:
     """Owns the numpy arrays behind one ``cae_objects`` struct."""
 
     def __init__(self, b: TableBuilder) -> None:
-        a: Dict[str, np.ndarray] = {}
-        nvals = max(len(b.value_is_int), 1)
-        a["value_is_int"] = np.zeros(nvals, np.uint8)
-        a["value_int"] = np.zeros(nvals, np.int64)
-        a["value_is_int"][:len(b.value_is_int)] = b.value_is_int
-        a["value_int"][:len(b.value_int)] = b.value_int
-        nns = max(len(b.ns_labelset), 1)
-        a["ns_labelset"] = np.zeros(nns, np.int32)
-        a["ns_exists"] = np.zeros(nns, np.uint8)
-        a["ns_labelset"][:len(b.ns_labelset)] = b.ns_labelset
-        a["ns_exists"][:len(b.ns_exists)] = b.ns_exists
-        a["ls_off"] = _i32(b.labelsets.off)
-        a["ls_key"] = _i32(b.labelsets.cols[0])
-        a["ls_val"] = _i32(b.labelsets.cols[1])
-        a["req_key"] = _i32(b.reqs_key)
-        a["req_op"] = _i32(b.reqs_op)
-        a["req_val_off"] = _i32(b.reqs_val_off)
-        a["req_vals"] = _i32(b.reqs_vals)
-        a["sel_kind"] = _i32(b.sel_kind)
-        a["sel_req_off"] = _i32(b.sel_req_off)
-        a["naff_nodesel"] = _i32(b.naff_nodesel)
-        a["naff_has_required"] = np.asarray(b.naff_has_required, np.uint8)
-        a["naff_term_off"] = _i32(b.naff_term_off)
-        a["term_expr_sel"] = _i32(b.term_expr_sel)
-        a["term_field_off"] = _i32(b.term_field_off)
-        a["field_op"] = _i32(b.field_op)
-        a["field_node_name"] = _i32(b.field_node_name)
-        a["tol_off"] = _i32(b.tols.off)
-        for i, nm in enumerate(("tol_key", "tol_op", "tol_val", "tol_effect")):
-            a[nm] = _i32(b.tols.cols[i])
-        a["taint_off"] = _i32(b.taints.off)
-        for i, nm in enumerate(("taint_key", "taint_val", "taint_effect")):
-            a[nm] = _i32(b.taints.cols[i])
-        a["port_off"] = _i32(b.ports.off)
-        for i, nm in enumerate(("port_ip", "port_proto", "port_num")):
-            a[nm] = _i32(b.ports.cols[i])
-        a["pts_off"] = _i32(b.pts.off)
-        for i, nm in enumerate(("pts_max_skew", "pts_key", "pts_selector", "pts_min_domains",
-                                "pts_node_affinity_policy", "pts_node_taints_policy")):
-            a[nm] = _i32(b.pts.cols[i])
-        a["aff_off"] = _i32(b.aff_off)
-        a["aterm_selector"] = _i32(b.aterm_selector)
-        a["aterm_key"] = _i32(b.aterm_key)
-        a["aterm_ns_off"] = _i32(b.aterm_ns_off)
-        a["aterm_ns"] = _i32(b.aterm_ns)
-        a["aterm_ns_selector"] = _i32(b.aterm_ns_selector)
-        nps = len(b.ps_rows)
-        cols = list(zip(*b.ps_rows)) if nps else [[] for _ in range(12)]
-        a["ps_namespace"] = _i32(cols[0])
-        a["ps_labelset"] = _i32(cols[1])
-        a["ps_req"] = np.ascontiguousarray(np.asarray(cols[2], dtype=np.int64).reshape(nps, MAX_RES))
-        a["ps_tol_list"] = _i32(cols[3])
-        a["ps_naff"] = _i32(cols[4])
-        a["ps_node_name"] = _i32(cols[5])
-        a["ps_port_list"] = _i32(cols[6])
-        a["ps_pts_list"] = _i32(cols[7])
-        a["ps_aff_list"] = _i32(cols[8])
-        a["ps_anti_list"] = _i32(cols[9])
-        a["ps_terminating"] = np.asarray(cols[10], dtype=np.uint8)
-        a["ps_hostname_spread"] = np.asarray(cols[11], dtype=np.uint8)
+        a: Dict[str, np.ndarray] = _cut(b, {}, _ALL_TABLES)
+        for nm in ("value_is_int", "value_int", "ns_labelset", "ns_exists"):   # the value and namespace tables hold one entry at least
+            if not len(a[nm]):
+                a[nm] = np.zeros(1, a[nm].dtype)
         nn = len(b.node_rows)
         ncols = list(zip(*b.node_rows)) if nn else [[] for _ in range(9)]
         a["node_name"] = _i32(ncols[0])
@@ -375,22 +449,10 @@ class EncodedObjects:
         s = capi.cae_objects()
         s.abi_version = capi.CONST["CAE_ABI_VERSION"]
         s.num_res = b.num_res
-        s.num_values = nvals
         s.hostname_key = b.hostname_key
         s.unschedulable_taint_key = b.unschedulable_taint_key
-        s.num_namespaces = nns
-        s.num_labelsets = b.labelsets.n
-        s.num_reqs = len(b.reqs_key)
-        s.num_selectors = len(b.sel_kind)
-        s.num_naff = len(b.naff_nodesel)
-        s.num_naff_terms = len(b.term_expr_sel)
-        s.num_tol_lists = b.tols.n
-        s.num_taint_lists = b.taints.n
-        s.num_port_lists = b.ports.n
-        s.num_pts_lists = b.pts.n
-        s.num_aff_lists = len(b.aff_off) - 1
-        s.num_aterms = len(b.aterm_selector)
-        s.num_podspecs = nps
+        for f, v in _root_counts(a).items():
+            setattr(s, f, v)
         s.num_cluster_nodes = b.num_cluster_nodes
         s.num_templates = b.num_templates
         s.num_groups = len(b.group_off) - 1
@@ -439,18 +501,7 @@ class EncodedObjects:
         rows rewritten and the resident-pod CSR rebuilt.  A cae_load of the result must answer like the engine after the
         delta."""
         import copy
-        a, d, s = dict(self.arrays), delta.arrays, self.struct
-        nv, nl, nt = s.num_values, s.num_labelsets, s.num_taint_lists
-        a["value_is_int"] = np.concatenate([a["value_is_int"][:nv], d["value_is_int"]]).astype(np.uint8)
-        a["value_int"] = np.concatenate([a["value_int"][:nv], d["value_int"]]).astype(np.int64)
-        p0 = int(a["ls_off"][nl])
-        a["ls_off"] = _i32(np.concatenate([a["ls_off"][:nl + 1], p0 + d["ls_off"][1:]]))
-        a["ls_key"] = _i32(np.concatenate([a["ls_key"][:p0], d["ls_key"]]))
-        a["ls_val"] = _i32(np.concatenate([a["ls_val"][:p0], d["ls_val"]]))
-        t0 = int(a["taint_off"][nt])
-        a["taint_off"] = _i32(np.concatenate([a["taint_off"][:nt + 1], t0 + d["taint_off"][1:]]))
-        for nm in ("taint_key", "taint_val", "taint_effect"):
-            a[nm] = _i32(np.concatenate([a[nm][:t0], d[nm]]))
+        a, d = self._with_tails(delta.arrays, _NODE_TABLES), delta.arrays
         rows = d["row"]
         for nm, src in (("node_labelset", "labelset"), ("node_taint_list", "taint_list"),
                         ("node_unschedulable", "unschedulable"), ("node_allowed_pods", "allowed_pods")):
@@ -469,8 +520,7 @@ class EncodedObjects:
         a["node_pod_spec"] = _i32(np.concatenate(pieces) if pieces else [])
         out = copy.copy(self)
         out.arrays = a
-        out.struct = self._restruct(a, num_values=len(a["value_is_int"]), num_labelsets=len(a["ls_off"]) - 1,
-                                    num_taint_lists=len(a["taint_off"]) - 1)
+        out.struct = self._restruct(a, **_root_counts(a))
         return out
 
     def apply_node_churn(self, churn: "NodeChurn") -> "EncodedObjects":
@@ -506,62 +556,22 @@ class EncodedObjects:
         (tail offsets made absolute) and the pending list replaced.  A cae_load of the result must answer like the engine
         after the delta."""
         import copy
-        a, d, s = dict(self.arrays), delta.arrays, self.struct
-
-        def cat(nm, n_old, tail, dtype=np.int32):
-            return np.ascontiguousarray(np.concatenate([a[nm][:n_old], np.asarray(tail, dtype)]).astype(dtype))
-
-        def csr(off_nm, n_lists, child_nms, dtypes=None):
-            """an offsets table of n_lists resident lists and its child columns"""
-            c0 = int(a[off_nm][n_lists])
-            a[off_nm] = cat(off_nm, n_lists + 1, c0 + d[off_nm][1:])
-            for nm in child_nms:
-                a[nm] = cat(nm, c0, d[nm], (dtypes or {}).get(nm, np.int32))
-
-        nv, nns = s.num_values, s.num_namespaces
-        a["value_is_int"] = cat("value_is_int", nv, d["value_is_int"], np.uint8)
-        a["value_int"] = cat("value_int", nv, d["value_int"], np.int64)
-        a["ns_labelset"] = cat("ns_labelset", nns, d["ns_labelset"])
-        a["ns_exists"] = cat("ns_exists", nns, d["ns_exists"], np.uint8)
-        csr("ls_off", s.num_labelsets, ("ls_key", "ls_val"))
-        # requirements and their values, then the selectors over the requirements
-        a["req_key"] = cat("req_key", s.num_reqs, d["req_key"])
-        a["req_op"] = cat("req_op", s.num_reqs, d["req_op"])
-        csr("req_val_off", s.num_reqs, ("req_vals",))
-        a["sel_kind"] = cat("sel_kind", s.num_selectors, d["sel_kind"])
-        a["sel_req_off"] = cat("sel_req_off", s.num_selectors + 1, s.num_reqs + d["sel_req_off"][1:])
-        a["naff_nodesel"] = cat("naff_nodesel", s.num_naff, d["naff_nodesel"])
-        a["naff_has_required"] = cat("naff_has_required", s.num_naff, d["naff_has_required"], np.uint8)
-        a["naff_term_off"] = cat("naff_term_off", s.num_naff + 1, s.num_naff_terms + d["naff_term_off"][1:])
-        a["term_expr_sel"] = cat("term_expr_sel", s.num_naff_terms, d["term_expr_sel"])
-        csr("term_field_off", s.num_naff_terms, ("field_op", "field_node_name"))
-        csr("tol_off", s.num_tol_lists, ("tol_key", "tol_op", "tol_val", "tol_effect"))
-        csr("port_off", s.num_port_lists, ("port_ip", "port_proto", "port_num"))
-        csr("pts_off", s.num_pts_lists, ("pts_max_skew", "pts_key", "pts_selector", "pts_min_domains",
-                                         "pts_node_affinity_policy", "pts_node_taints_policy"))
-        a["aff_off"] = cat("aff_off", s.num_aff_lists + 1, s.num_aterms + d["aff_off"][1:])
-        a["aterm_selector"] = cat("aterm_selector", s.num_aterms, d["aterm_selector"])
-        a["aterm_key"] = cat("aterm_key", s.num_aterms, d["aterm_key"])
-        a["aterm_ns_selector"] = cat("aterm_ns_selector", s.num_aterms, d["aterm_ns_selector"])
-        csr("aterm_ns_off", s.num_aterms, ("aterm_ns",))
-        S = s.num_podspecs
-        for nm in ("ps_namespace", "ps_labelset", "ps_tol_list", "ps_naff", "ps_node_name", "ps_port_list", "ps_pts_list",
-                   "ps_aff_list", "ps_anti_list"):
-            a[nm] = cat(nm, S, d[nm])
-        a["ps_terminating"] = cat("ps_terminating", S, d["ps_terminating"], np.uint8)
-        a["ps_hostname_spread"] = cat("ps_hostname_spread", S, d["ps_hostname_spread"], np.uint8)
-        a["ps_req"] = np.ascontiguousarray(np.concatenate([a["ps_req"][:S], d["ps_req"]]).astype(np.int64))
+        a, d = self._with_tails(delta.arrays, _POD_TABLES), delta.arrays
         a["pend_spec"] = np.ascontiguousarray(d["pend_spec"], np.int32)
         a["group_off"] = np.ascontiguousarray(d["group_off"], np.int32)
         out = copy.copy(self)
         out.arrays = a
-        out.struct = self._restruct(
-            a, num_values=len(a["value_is_int"]), num_namespaces=len(a["ns_labelset"]), num_labelsets=len(a["ls_off"]) - 1,
-            num_reqs=len(a["req_key"]), num_selectors=len(a["sel_kind"]), num_naff=len(a["naff_nodesel"]),
-            num_naff_terms=len(a["term_expr_sel"]), num_tol_lists=len(a["tol_off"]) - 1, num_port_lists=len(a["port_off"]) - 1,
-            num_pts_lists=len(a["pts_off"]) - 1, num_aff_lists=len(a["aff_off"]) - 1, num_aterms=len(a["aterm_selector"]),
-            num_podspecs=len(a["ps_namespace"]), num_pending=len(a["pend_spec"]), num_groups=len(a["group_off"]) - 1)
+        out.struct = self._restruct(a, num_pending=len(a["pend_spec"]), num_groups=len(a["group_off"]) - 1, **_root_counts(a))
         return out
+
+    def _with_tails(self, d: Dict[str, np.ndarray], tables) -> Dict[str, np.ndarray]:
+        """A copy of the arrays with the tails `d` of the dictionary tables `tables` appended (tail offsets made absolute)."""
+        a, n = dict(self.arrays), _dict_counts(self.struct, self.arrays)
+        for nm, cnt, child, dt, *_ in _DICT:
+            if nm in tables:
+                tail = np.asarray(d[nm] if child is None else n[child] + d[nm][1:], dt)
+                a[nm] = np.ascontiguousarray(np.concatenate([a[nm][:n[cnt] + (child is not None)], tail]).astype(dt))
+        return a
 
     def _restruct(self, arrays, **counts) -> "capi.cae_objects":
         s = capi.cae_objects()
@@ -917,12 +927,10 @@ class Encoder:
         self._key(TAINT_NODE_UNSCHEDULABLE)
         self.b.num_res = max(3, len(self.resources))
         enc = self.b.finish()
-        # what the engine holds after a load of `enc`: node_delta() emits what the interner adds beyond it as tails
-        self._emitted = (enc.struct.num_values, enc.struct.num_labelsets, enc.struct.num_taint_lists)
-        s = enc.struct   # the spec-side tables the engine holds: pod_delta() emits what the interner adds beyond them
-        self._pods_emitted = dict(ns=s.num_namespaces, reqs=s.num_reqs, sel=s.num_selectors, naff=s.num_naff,
-                                  terms=s.num_naff_terms, tols=s.num_tol_lists, ports=s.num_port_lists, pts=s.num_pts_lists,
-                                  aff=s.num_aff_lists, aterms=s.num_aterms, specs=s.num_podspecs, num_res=s.num_res)
+        # what the engine holds after a load of `enc`, per count: node_delta() / pod_delta() emit what the interner adds
+        # beyond it as tails (the value and namespace tables of a load may be padded)
+        self._emitted = _dict_counts(enc.struct, enc.arrays)
+        self._num_res = enc.struct.num_res
         self._delta_ok = True
         self._spec_wo_name: Optional[Dict[tuple, int]] = None
         # the cluster rows the engine holds: (node-name id, row state) per row, kept current by node_delta / node_churn
@@ -990,7 +998,7 @@ class Encoder:
         """Unsupported unless the interner still matches what the engine holds."""
         if not getattr(self, "_delta_ok", False):
             raise Unsupported("no load to apply a node delta to, or an earlier delta was refused")
-        if len(self.b.value_is_int) < self._emitted[0]:
+        if len(self.b.value_is_int) < self._emitted["values"]:
             self._delta_ok = False
             raise Unsupported("the value table of the last load was padded")
 
@@ -1011,23 +1019,23 @@ class Encoder:
     def _tails_and_rows(self, rows: Sequence[int], states: Sequence[tuple]) -> NodeDelta:
         """The NodeDelta of dirty rows `rows` with row states `states`, carrying as tails what the interner added since the
         last load or delta."""
-        b = self.b
-        nv0, nl0, nt0 = self._emitted
         pod_off, pod_spec = [0], []
         for st in states:
             pod_spec.extend(st[5])
             pod_off.append(len(pod_spec))
-        L, Tn = b.labelsets, b.taints
-        lp0, tp0 = L.off[nl0], Tn.off[nt0]
         delta = NodeDelta(
-            value_is_int=b.value_is_int[nv0:], value_int=b.value_int[nv0:],
-            ls_off=[o - lp0 for o in L.off[nl0:]], ls_key=L.cols[0][lp0:], ls_val=L.cols[1][lp0:],
-            taint_off=[o - tp0 for o in Tn.off[nt0:]], taint_key=Tn.cols[0][tp0:], taint_val=Tn.cols[1][tp0:],
-            taint_effect=Tn.cols[2][tp0:], row=rows, labelset=[st[0] for st in states], taint_list=[st[1] for st in states],
+            **self._tails(_NODE_TABLES), row=rows, labelset=[st[0] for st in states], taint_list=[st[1] for st in states],
             unschedulable=[st[2] for st in states], alloc=np.asarray([st[3] for st in states], np.int64).reshape(len(rows), MAX_RES),
             allowed_pods=[st[4] for st in states], pod_off=pod_off, pod_spec=pod_spec)
-        self._emitted = (len(b.value_is_int), L.n, Tn.n)
         return delta
+
+    def _tails(self, tables) -> Dict[str, np.ndarray]:
+        """The tails of the dictionary tables `tables`: what the interner added since they were last emitted.  Their
+        families are emitted and advance."""
+        counts = _families(tables)
+        out = _cut(self.b, self._emitted, tables)
+        self._emitted.update(_dict_sizes(self.b, counts))
+        return out
 
     def node_churn(self, new_cluster: Sequence[NodeInfo]) -> "NodeChurn":
         """The shim's side of cae_load_node_churn: the complete new cluster-node list as a NodeChurn against what the engine
@@ -1079,7 +1087,6 @@ class Encoder:
         of this tick) are interned first, so that the node_delta / node_churn that follows finds their specs; the tick
         is load_pods, then the node call.  Unsupported: a resource dimension the last load did not have (a full load)."""
         self._check_resident()
-        b, em = self.b, self._pods_emitted
         for ni in residents:
             for p in ni.pods:
                 self._resident_spec(p, allow_new=True)
@@ -1087,52 +1094,13 @@ class Encoder:
         for g in groups:
             pend.extend(self.podspec(p) for p in g.pods)
             off.append(len(pend))
-        if len(self.resources) > em["num_res"]:
+        if len(self.resources) > self._num_res:
             self._delta_ok = False
             raise Unsupported("a pod requests a resource the last load did not have")
-        if len(b.ns_labelset) < em["ns"]:
+        if len(self.b.ns_labelset) < self._emitted["namespaces"]:
             self._delta_ok = False
             raise Unsupported("the namespace table of the last load was padded")
-        nv0, nl0, nt0 = self._emitted
-        L = b.labelsets
-        lp0, r0, s0, f0, t0 = L.off[nl0], em["reqs"], em["sel"], em["naff"], em["terms"]
-        rv0, fd0, a0 = b.reqs_val_off[r0], b.term_field_off[t0], em["aterms"]
-        ns0 = b.aterm_ns_off[a0]
-
-        def tail(csr, n0, names):
-            c0 = csr.off[n0]
-            return dict([(names[0], [o - c0 for o in csr.off[n0:]])] + [(nm, csr.cols[i][c0:]) for i, nm in enumerate(names[1:])])
-
-        rows = b.ps_rows[em["specs"]:]
-        cols = list(zip(*rows)) if rows else [[] for _ in range(12)]
-        delta = PodDelta(
-            value_is_int=b.value_is_int[nv0:], value_int=b.value_int[nv0:],
-            ns_labelset=b.ns_labelset[em["ns"]:], ns_exists=b.ns_exists[em["ns"]:],
-            ls_off=[o - lp0 for o in L.off[nl0:]], ls_key=L.cols[0][lp0:], ls_val=L.cols[1][lp0:],
-            req_key=b.reqs_key[r0:], req_op=b.reqs_op[r0:], req_val_off=[o - rv0 for o in b.reqs_val_off[r0:]],
-            req_vals=b.reqs_vals[rv0:], sel_kind=b.sel_kind[s0:], sel_req_off=[o - r0 for o in b.sel_req_off[s0:]],
-            naff_nodesel=b.naff_nodesel[f0:], naff_has_required=b.naff_has_required[f0:],
-            naff_term_off=[o - t0 for o in b.naff_term_off[f0:]], term_expr_sel=b.term_expr_sel[t0:],
-            term_field_off=[o - fd0 for o in b.term_field_off[t0:]], field_op=b.field_op[fd0:],
-            field_node_name=b.field_node_name[fd0:],
-            **tail(b.tols, em["tols"], ("tol_off", "tol_key", "tol_op", "tol_val", "tol_effect")),
-            **tail(b.ports, em["ports"], ("port_off", "port_ip", "port_proto", "port_num")),
-            **tail(b.pts, em["pts"], ("pts_off", "pts_max_skew", "pts_key", "pts_selector", "pts_min_domains",
-                                      "pts_node_affinity_policy", "pts_node_taints_policy")),
-            aff_off=[o - a0 for o in b.aff_off[em["aff"]:]],
-            aterm_selector=b.aterm_selector[a0:], aterm_key=b.aterm_key[a0:],
-            aterm_ns_off=[o - ns0 for o in b.aterm_ns_off[a0:]], aterm_ns=b.aterm_ns[ns0:],
-            aterm_ns_selector=b.aterm_ns_selector[a0:],
-            ps_namespace=cols[0], ps_labelset=cols[1], ps_req=np.asarray(cols[2], np.int64).reshape(len(rows), MAX_RES),
-            ps_tol_list=cols[3], ps_naff=cols[4], ps_node_name=cols[5], ps_port_list=cols[6], ps_pts_list=cols[7],
-            ps_aff_list=cols[8], ps_anti_list=cols[9], ps_terminating=cols[10], ps_hostname_spread=cols[11],
-            group_off=off, pend_spec=pend)
-        self._emitted = (len(b.value_is_int), L.n, nt0)
-        self._pods_emitted = dict(ns=len(b.ns_labelset), reqs=len(b.reqs_key), sel=len(b.sel_kind), naff=len(b.naff_nodesel),
-                                  terms=len(b.term_expr_sel), tols=b.tols.n, ports=b.ports.n, pts=b.pts.n,
-                                  aff=len(b.aff_off) - 1, aterms=len(b.aterm_selector), specs=len(b.ps_rows),
-                                  num_res=em["num_res"])
-        return delta
+        return PodDelta(**self._tails(_POD_TABLES), group_off=off, pend_spec=pend)
 
 
 def encode(cluster: Sequence[NodeInfo], templates: Sequence[NodeInfo],

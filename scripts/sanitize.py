@@ -7,7 +7,7 @@ self-cleaning accumulators, last-block election, shared-memory state and block-w
 
 Dense pass (K1, both variants), Estimate() of every template (K0 + K3: plain closed form, capacity form with the cluster
 fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals), a cluster-node delta
-(cae_load_nodes), a cluster-node churn (cae_load_node_churn) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
+(cae_load_nodes), a cluster-node churn (cae_load_node_churn), new pod specs (cae_load_pods) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
 against the CPU oracle so that a "clean" run also means "correct results under the tool"."""
 import os
 import sys
@@ -77,6 +77,19 @@ def main():
             caps = np.full(after.T, 30, np.int32)
             got_e, ref_e = eng.estimate_all(caps), pyoracle.estimate_all(after, caps)
             assert all(np.array_equal(x, y) for x, y in zip(got_e, ref_e[:4]))
+            got = eng.filter_schedulable(order_p)
+            ref = pyoracle.filter_schedulable(after, order_p)
+            assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
+            # new pod specs and a new pending list (cae_load_pods: spec tails appended, the pending-side derivation rerun)
+            pdelta = synth.pod_churn(after, cfg, 3, 3)
+            after = after.apply_pod_delta(pdelta)
+            assert eng.load_pods(pdelta, after) == 0
+            _, reasons, _ = eng.feasibility()
+            assert np.array_equal(reasons, pyoracle.feasibility_dense(after)[0])
+            caps = np.full(after.T, 30, np.int32)
+            got_e, ref_e = eng.estimate_all(caps), pyoracle.estimate_all(after, caps)
+            assert all(np.array_equal(x, y) for x, y in zip(got_e, ref_e[:4]))
+            order_p = np.arange(min(after.P, 600), dtype=np.int32)
             got = eng.filter_schedulable(order_p)
             ref = pyoracle.filter_schedulable(after, order_p)
             assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]

@@ -6,128 +6,13 @@ Chained deltas, both orders with cae_load_pending, boundary deltas, and every re
 import numpy as np
 import pytest
 
+from delta_harness import SHAPES, _assert_same, _check, _gen, _results, engines  # noqa: F401  (engines: fixture)
 from kubernetes_autoscaler_b200 import synth
 from kubernetes_autoscaler_b200.encode import Encoder, NodeDelta
 from kubernetes_autoscaler_b200.objects import (LABEL_HOSTNAME, BuildTestPod, LabelSelector, PodAffinityTerm, WithLabels,
                                                 WithNamespace, WithPodAntiAffinity)
 
 pytestmark = pytest.mark.gpu
-
-SHAPES = {
-    "c2": (2, dict(pods=3000, templates=40, cluster_nodes=48)),      # taints, tolerations, nodeSelectors
-    "c3": (3, dict(pods=2500, templates=24, cluster_nodes=48)),      # zone / hostname spread, minDomains
-    "c4": (4, dict(pods=3000, templates=20, cluster_nodes=40)),      # + anti-affinity and affinity
-}
-
-
-@pytest.fixture(scope="module")
-def engines():
-    import __graft_entry__ as g
-    g.build()
-    from kubernetes_autoscaler_b200.engine import Engine
-    made = {}
-
-    def get(reasons: bool):
-        if reasons not in made:
-            made[reasons] = (Engine(device=0, want_reasons=reasons), Engine(device=0, want_reasons=reasons))
-        return made[reasons]
-    yield get
-    for a, b in made.values():
-        a.close()
-        b.close()
-
-
-def _gen(shape):
-    cfg, kw = SHAPES[shape]
-    return synth.generate(cfg, **kw)
-
-
-def _results(eng, enc, oracle_side=None):
-    """Everything the entry points answer for the loaded snapshot (engine `eng`, shapes of `enc`)."""
-    from kubernetes_autoscaler_b200.engine import unpack_bits
-    out = {}
-    bits, reasons, count = eng.feasibility()
-    out["bits"] = unpack_bits(bits, enc.P).copy()
-    out["count"] = count.copy()
-    if reasons is not None:
-        out["reasons"] = reasons.copy()
-    out["groups"] = eng.feasibility_groups()
-    T, N = enc.T, enc.struct.num_cluster_nodes
-    for cap in (40, 0):
-        caps = np.full(T, cap, np.int32)
-        nc, pc, sched, order = eng.estimate_all(caps)
-        out["est%d" % cap] = (nc, pc, sched, order)
-        out["waste%d" % cap] = eng.waste_scores()
-        mask, waste = eng.expander_best([0, 1, 2], nc, pc)
-        out["best%d" % cap] = (mask, waste)
-        node_price = 1.0 + np.arange(T, dtype=np.float64) * 0.37
-        pod_price = 0.01 + (np.arange(enc.struct.num_podspecs, dtype=np.float64) % 13) * 0.003
-        out["price%d" % cap] = eng.price_scores(node_price, pod_price, 0.5, 1500)
-    li = (np.arange(T, dtype=np.int32) * 37 + 3 * N + 5).astype(np.int32)     # RAW: larger than the node list
-    out["li"] = eng.estimate_all_li(np.full(T, 25, np.int32), li)
-    out["filter"] = eng.filter_schedulable(*_filter_args(enc))
-    return out
-
-
-def _filter_args(enc):
-    P, N = enc.P, enc.struct.num_cluster_nodes
-    n = min(P, 700)
-    order = np.arange(n, dtype=np.int32)[::-1].copy()
-    rng = synth.SplitMix64(0xF17E)
-    hint = np.where(rng.uniform(P) < 0.1, rng.randint(P, max(N, 1)), -1).astype(np.int32)
-    cls = np.where(rng.uniform(P) < 0.5, rng.randint(P, 6), -1).astype(np.int32)
-    ctrl = np.array([0, 1, 1, 2, 3, 3], np.int32)
-    return order, hint, cls, ctrl, None, 11
-
-
-def _oracle_results(oracle, enc, want_reasons):
-    out = {}
-    reasons, _ = oracle.feasibility_dense(enc)
-    out["bits"] = reasons == 0
-    out["count"] = (reasons == 0).sum(axis=1).astype(np.int32)
-    if want_reasons:
-        out["reasons"] = reasons
-    out["groups"] = oracle.feasibility_groups(enc)
-    T = enc.T
-    for cap in (40, 0):
-        caps = np.full(T, cap, np.int32)
-        nc, pc, sched, order, _ = oracle.estimate_all(enc, caps)
-        out["est%d" % cap] = (nc, pc, sched, order)
-        mask, waste = oracle.expander(enc, [0, 1, 2], nc, pc, sched)
-        out["waste%d" % cap] = waste
-        out["best%d" % cap] = (mask, waste)
-        node_price = 1.0 + np.arange(T, dtype=np.float64) * 0.37
-        pod_price = 0.01 + (np.arange(enc.struct.num_podspecs, dtype=np.float64) % 13) * 0.003
-        out["price%d" % cap] = oracle.price_scores(enc, node_price, pod_price, 0.5, 1500, node_count=nc, sched=sched, order=order)
-    N = enc.struct.num_cluster_nodes
-    li = (np.arange(T, dtype=np.int32) * 37 + 3 * N + 5).astype(np.int32)
-    out["li"] = oracle.estimate_all_li(enc, np.full(T, 25, np.int32), li)
-    order, hint, cls, ctrl, ok, last = _filter_args(enc)
-    out["filter"] = oracle.filter_schedulable(enc, order, hint, cls, ctrl, ok, last)
-    return out
-
-
-def _equal(x, y):
-    if isinstance(x, tuple):
-        return len(x) == len(y) and all(_equal(a, b) for a, b in zip(x, y))
-    if isinstance(x, np.ndarray) or isinstance(y, np.ndarray):
-        return np.array_equal(np.asarray(x), np.asarray(y))
-    return x == y
-
-
-def _assert_same(got, want, what):
-    for k in want:
-        assert _equal(got[k], want[k]), "%s: %s differs" % (what, k)
-
-
-def _check(eng, fresh, oracle, after, want_reasons):
-    """`eng` holds `after` through deltas: compare with a fresh cae_load of `after` and with the oracle."""
-    eng.enc = after
-    got = _results(eng, after)
-    fresh.load(after)
-    _assert_same(got, _results(fresh, after), "fresh load")
-    _assert_same(got, _oracle_results(oracle, after, want_reasons), "oracle")
-    return got
 
 
 @pytest.mark.parametrize("want_reasons", [False, True], ids=["bits", "reasons"])
@@ -208,11 +93,6 @@ def test_boundary_deltas(engines, oracle):
     _check(eng, fresh, oracle, p3.apply_node_delta(d3), False)
 
 
-def _snapshot(eng, enc):
-    eng.enc = enc
-    return _results(eng, enc)
-
-
 def _label_delta(enc, row, change):
     """Row `row` switched to a new label set: its labels with `change` applied (value None = label removed)."""
     a = enc.arrays
@@ -251,7 +131,7 @@ def test_refusals_leave_the_engine_unchanged(engines):
     enc = _gen("c3")
     N = enc.struct.num_cluster_nodes
     eng.load(enc)
-    before = _snapshot(eng, enc)
+    before = _results(eng, enc)
     zone_other = (int(enc.arrays["ls_val"][enc.arrays["ls_off"][enc.arrays["node_labelset"][2]] + 1]) + 1) % 16
     refused = [
         _label_delta(enc, 2, {synth.K_ZONE: zone_other}),              # a topology value changes
@@ -269,15 +149,15 @@ def test_refusals_leave_the_engine_unchanged(engines):
                                                          both.arrays["labelset"][1:]])))
     for d in refused:
         assert not eng.load_nodes(d)
-        _assert_same(_snapshot(eng, enc), before, "after a refused delta")
+        _assert_same(_results(eng, enc), before, "after a refused delta")
     # a resident pod whose anti-affinity spec was in no pod of the last load
     eng_enc, enc2, cluster, lonely = _anti_world()
     eng.load(enc2)
-    before2 = _snapshot(eng, enc2)
+    before2 = _results(eng, enc2)
     cluster[1].pods.append(lonely)
     d = eng_enc.node_delta([(1, cluster[1])])
     assert not eng.load_nodes(d)
-    _assert_same(_snapshot(eng, enc2), before2, "after a refused anti-affinity resident")
+    _assert_same(_results(eng, enc2), before2, "after a refused anti-affinity resident")
 
 
 def test_malformed_deltas(engines):
@@ -286,7 +166,7 @@ def test_malformed_deltas(engines):
     enc = _gen("c2")
     N, S = enc.struct.num_cluster_nodes, enc.struct.num_podspecs
     eng.load(enc)
-    before = _snapshot(eng, enc)
+    before = _results(eng, enc)
     ok = synth.node_churn(enc, 4, 6)[0]
     ok_tail = _label_delta(enc, 2, {synth.K_POOL: 17})
     nl, nv = enc.struct.num_labelsets, enc.struct.num_values
@@ -317,4 +197,4 @@ def test_malformed_deltas(engines):
         with pytest.raises(EngineError, match="status -2"):
             eng.load_nodes(d)
         assert eng.load_nodes(NodeDelta()), what
-    _assert_same(_snapshot(eng, enc), before, "after malformed deltas")
+    _assert_same(_results(eng, enc), before, "after malformed deltas")

@@ -1,6 +1,6 @@
 """cae_load_pods on the GPU: after new pod specs arrive and the pending list is replaced, every entry point answers
 bit-identically to a second engine freshly loaded with EncodedObjects.apply_pod_delta(...), and to the oracle where that
-is affordable (the _results pattern of test_gpu_node_churn: dense bits / reasons / counts, group reasons, Estimate()
+is affordable (the results of tests/delta_harness.py: dense bits / reasons / counts, group reasons, Estimate()
 capped and unlimited, RAW lastIndex, waste and price scores, the filter pass).  Chained deltas interleaved with
 cae_load_pending, cae_load_nodes and cae_load_node_churn (node calls naming the new specs as residents), boundaries, and
 refusals / malformed input with the engine left as it was."""
@@ -10,7 +10,7 @@ import pytest
 from kubernetes_autoscaler_b200 import synth
 from kubernetes_autoscaler_b200.encode import PodDelta
 
-from test_gpu_node_churn import SHAPES, _check, _gen, _results, _assert_same, engines  # noqa: F401  (engines: fixture)
+from delta_harness import SHAPES, _assert_same, _check, _gen, _results, engines  # noqa: F401  (engines: fixture)
 from test_node_delta_host import _encoder, _world
 from test_pod_delta_host import new_workloads
 from test_node_churn_host import _new_node
@@ -186,7 +186,7 @@ def test_c1_shape_and_boundaries(engines, oracle):
 
 def test_scale_down_batch_after_pod_delta(engines):
     """cae_simulate_removals and the filter pass with non-zero lastIndex after cae_load_pods, against a fresh load"""
-    from test_gpu_node_churn import _equal, _filter_args
+    from delta_harness import _equal, _filter_args
     eng, fresh = engines(False)
     enc = _gen("c4", templates=0, pods=600)
     eng.load(enc)
