@@ -45,25 +45,34 @@ def _outcome(results, sim, cluster, persist):
     return out
 
 
-def oracle_loop(cluster, candidates, dest, persist, last_index=0, hints=None, pods_to_move=None):
+def oracle_loop(cluster, candidates, dest, persist, last_index=0, hints=None, pods_to_move=None, namespaces=()):
+    """An explicit pods_to_move[i] lists candidate i's pods in the snapshot as it is now; the pods earlier persisted
+    simulations moved onto it are appended, as SimulateNodeRemovals documents."""
     cluster = copy.deepcopy(cluster)
     sim = OracleSimulator()
     sim.last_index = last_index
     if hints:
         sim.hints.current.update(hints)
     r = RemovalSimulator(cluster, persist, schedulingSimulator=sim)
-    results = [r.SimulateNodeRemoval(n, dest, None if pods_to_move is None else pods_to_move[i]) for i, n in enumerate(candidates)]
+    copied = {id(p) for ni in cluster for p in ni.pods}
+    results = []
+    for i, n in enumerate(candidates):
+        explicit = None if pods_to_move is None else pods_to_move[i]
+        if explicit is not None:
+            moved_in = [p for ni in cluster if ni.node.name == n for p in ni.pods if id(p) not in copied]
+            explicit = list(explicit) + moved_in
+        results.append(r.SimulateNodeRemoval(n, dest, explicit, namespaces))
     return _outcome(results, sim, cluster, persist)
 
 
-def batch(make_sim, cluster, candidates, dest, persist, last_index=0, hints=None, pods_to_move=None):
+def batch(make_sim, cluster, candidates, dest, persist, last_index=0, hints=None, pods_to_move=None, namespaces=()):
     cluster = copy.deepcopy(cluster)
     sim = make_sim()
     sim.last_index = last_index
     if hints:
         sim.hints.current.update(hints)
     r = RemovalSimulator(cluster, persist, schedulingSimulator=sim)
-    results = r.SimulateNodeRemovals(candidates, dest, pods_to_move)
+    results = r.SimulateNodeRemovals(candidates, dest, pods_to_move, namespaces)
     return _outcome(results, sim, cluster, persist)
 
 
