@@ -546,11 +546,41 @@ int32_t cae_expander_best(cae_engine* e, const int32_t* chain, int32_t chain_len
  *   last_index_in          SchedulerPluginRunner.lastIndex before the call (0 for a fresh runner)
  * Outputs: assigned_node [num_pending] = cluster node index, -1 = stays unschedulable (also for pods not in
  * pod_order); the runner's lastIndex afterwards; SimilarPodsScheduling.OverflowingControllerCount().
- * Uses the tables of the last cae_load (its templates are ignored); does not change the estimator's results. */
+ * Uses the tables of the last cae_load (its templates are ignored).  The placements are made on a working copy that ends
+ * with the call: the resident snapshot and the estimator's results change only when the caller hands them back through
+ * cae_force_add_pods. */
 int32_t cae_filter_schedulable(cae_engine* e, const int32_t* pod_order, int32_t n_pods, const int32_t* hint_node,
                                const int32_t* sim_class, const int32_t* class_ctrl, int32_t n_classes, const uint8_t* node_ok,
                                int32_t last_index_in, int32_t break_on_failure, int32_t* assigned_node,
                                int32_t* last_index_out, int32_t* overflowing_controllers);
+
+/* ClusterSnapshot.ForceAddPod for a list of pending pods (what HintingSimulator.TrySchedulePods leaves behind,
+ * hinting_simulator.go:53-135): pending pod pod[i] becomes a resident of cluster row node[i], appended to that row's pods in
+ * list order, and leaves the pending list.  No predicate is checked (ForceAddPod checks none), so a row may end up with
+ * negative free resources or pod slots.  ScaleUp then sees the placed pods as residents: in the PodTopologySpread /
+ * InterPodAffinity counts, in the free resources, pod slots and host ports of the cluster rows, and in the pending groups.
+ *   pod  [n]  pending-pod indices (each at most once), node [n] cluster rows
+ *   new_index [num_pending before the call] or NULL: the index of each pod afterwards, -1 for a moved one
+ * The remaining pending pods keep their relative order and their groups; num_groups and every group index are unchanged,
+ * so a group may become empty.  Afterwards every entry point answers bit-identically to a cae_load of the same objects with
+ * those pods appended to node_pod_spec of their rows (spec ids unchanged) and pend_spec / group_off compacted.  Templates,
+ * node columns and dictionaries are not touched.  The call combines with cae_load_pending, cae_load_nodes,
+ * cae_load_node_churn and cae_load_pods in any order; the rules those state relative to the last cae_load hold as before,
+ * and for cae_load_pending's group -> spec sequence an emptied group is an empty group.  The pending and group indices a
+ * caller holds (hints, sim_class) follow new_index.
+ * Besides the compacted pending rows only the arrivals travel to the device (4 B per placed pod, 8 B per receiving row);
+ * the resident lists stay there.  Every check runs on the host before any device write.  n == 0 is a valid call that changes nothing.
+ * Status -2 (nothing changed): before cae_load, n < 0, a NULL array with n > 0, a pod index out of range or listed twice,
+ * a node outside [0, num_cluster_nodes).
+ * Status 2 (nothing changed): the resident pods of all rows would pass 2^31 - 1; the engine was created with
+ * CAE_CFG_PODS_PRESHARDED: a rank then holds only its own pending pods and cannot express the placements of the other
+ * ranks' pods; or, at world_size > 1, this rank's pod shard of the shorter list would hold more pods than its shard at the
+ * last cae_load (shard starts are multiples of 32, so a shard can grow when the list shrinks by a few pods): call cae_load
+ * with the objects after the placements instead, on every rank.  At world_size > 1 without presharding every rank applies
+ * the same list.
+ * Status -1 (a CUDA error part way): the engine needs a cae_load. */
+int32_t cae_force_add_pods(cae_engine* e, int32_t n, const int32_t* pod, const int32_t* node,
+                           int32_t* new_index /* [num_pending before the call] or NULL */);
 
 /* The scale-down removal simulation: RemovalSimulator.SimulateNodeRemoval(candidate, destinationMap) called on every
  * candidate in order, on ONE RemovalSimulator (one HintingSimulator: hints and lastIndex carried from call to call)

@@ -163,6 +163,8 @@ def load_engine_lib() -> C.CDLL:
     lib.cae_load_node_churn.restype = C.c_int32
     lib.cae_load_pods.argtypes = [C.c_void_p, P(cae_pod_delta)]
     lib.cae_load_pods.restype = C.c_int32
+    lib.cae_force_add_pods.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.cae_force_add_pods.restype = C.c_int32
     lib.cae_feasibility.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.cae_feasibility.restype = C.c_int32
     lib.cae_feasibility_groups.argtypes = [C.c_void_p, C.c_void_p]

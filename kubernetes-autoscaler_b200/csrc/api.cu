@@ -348,6 +348,21 @@ static void pod_shard(const Engine* e, int P, int* pb, int* pe) {
   if (e->cfg.flags & CAE_CFG_PODS_PRESHARDED) { *pb = 0; *pe = P; }
 }
 
+// The staged pending rows (stage_pending) into the resident device rows, and the sizes that follow from them; the per-pod
+// rows and the group records are for the caller to re-derive (launch_expand_pods, launch_group_records)
+static int upload_pending(Engine* e, int P, int E) {
+  if (P) CAE_CUDA(cudaMemcpyAsync(const_cast<int32_t*>(e->dobj.pend_spec), e->h_pend_spec, sizeof(int32_t) * P, cudaMemcpyHostToDevice, e->stream));
+  CAE_CUDA(cudaMemcpyAsync(const_cast<int32_t*>(e->dobj.group_off), e->h_group_off, sizeof(int32_t) * (E + 1), cudaMemcpyHostToDevice, e->stream));
+  CAE_CUDA(cudaEventRecord(e->pending_stage.ev, e->stream));
+  e->stats.h2d_bytes += (int64_t)((size_t)P + E + 1) * 4;
+  e->P = P; e->E = E;
+  pod_shard(e, P, &e->p_begin, &e->p_end);
+  e->Pl = e->p_end - e->p_begin;
+  e->Plw = (e->Pl + 31) / 32;
+  e->group_reason_valid = false;
+  return 0;
+}
+
 // Requests of a row's resident pods, summed per resource dim
 static void resident_req(const int64_t* spec_req, const int32_t* pod_spec, int npods, int64_t reqd[R]) {
   for (int r = 0; r < R; ++r) reqd[r] = 0;
@@ -1288,6 +1303,93 @@ static int do_load_pods(Engine* e, const cae_pod_delta* d) {
   return rc;
 }
 
+// cae_force_add_pods: every check on the host first, then one pinned H2D copy of the arrivals grouped by receiving row (a
+// stable counting sort of the (pod, node) list by node) and one of the compacted pending rows, and the device work in
+// stream order without a host synchronisation (force_add.cu).  The pending rows are compacted here, on the host mirror,
+// and travel like cae_load_pending's: the mirrors end up as stage_pending builds them for the compacted list.
+static int do_force_add(Engine* e, int n, const int32_t* pod, const int32_t* node, int32_t* new_index) {
+  auto bad = [](const char* m) { set_error(std::string("cae_force_add_pods: ") + m); return -2; };
+  auto refuse = [](const char* m) { set_error(std::string("cae_force_add_pods: ") + m); return 2; };
+  if (n < 0 || (n > 0 && (!pod || !node))) return bad("negative count or NULL array");
+  const int P = e->P, E = e->E, N = e->N;
+  std::vector<int32_t> to(P, 0), arr_cnt(N, 0);   // to[p]: -1 moved, then the new index; arrivals per row
+  for (int i = 0; i < n; ++i) {
+    if (pod[i] < 0 || pod[i] >= P) return bad("pod index out of range");
+    if (to[pod[i]] < 0) return bad("a pod is listed twice");
+    if (node[i] < 0 || node[i] >= N) return bad("node outside the cluster rows");
+    to[pod[i]] = -1;
+    ++arr_cnt[node[i]];
+  }
+  if (e->cfg.flags & CAE_CFG_PODS_PRESHARDED) return refuse("the pending pods are presharded: a rank cannot place the other ranks' pods");
+  const int64_t total = e->nh.pod_total + n;
+  if (total > INT32_MAX) return refuse("more than 2^31 - 1 resident pods");
+  {   // shard starts are rounded down to multiples of 32, so fewer pods can give a rank a LARGER shard than its buffers hold
+    int pb = 0, pe = 0;
+    pod_shard(e, P - n, &pb, &pe);
+    if (pe - pb > e->cap_Pl) return refuse("this rank's pod shard would outgrow the resident buffers");
+  }
+  e->stats.h2d_bytes = 0;
+  if (n == 0) {
+    if (new_index) for (int p = 0; p < P; ++p) new_index[p] = p;
+    return 0;
+  }
+  // ---- the arrivals per receiving row: rows ascending | offsets | specs in list order ----
+  int nrows = 0;
+  for (int r = 0; r < N; ++r) nrows += arr_cnt[r] > 0;
+  const size_t o_row = 0, o_off = (size_t)nrows, o_spec = o_off + nrows + 1, words = o_spec + n;
+  if (pinned_reserve(e, e->nd_stage, words * 4) || devbuf_reserve(e, e->nd_blob, words * 4)) return -1;
+  int32_t* h = static_cast<int32_t*>(e->nd_stage.p);
+  std::vector<int32_t> at(N, 0);                 // where the next arrival of a row goes
+  bool ports = false;
+  {
+    int i = 0, off = 0;
+    for (int r = 0; r < N; ++r) {
+      if (!arr_cnt[r]) continue;
+      h[o_row + i] = r;
+      h[o_off + i] = off;
+      at[r] = off;
+      off += arr_cnt[r];
+      ++i;
+    }
+    h[o_off + nrows] = off;
+    const int32_t* port_off = e->host_tab<int32_t>(TAB_port_off);
+    const int32_t* ps_port_list = e->host_tab<int32_t>(TAB_ps_port_list);
+    for (int k = 0; k < n; ++k) {
+      const int s = e->h_pend_spec[pod[k]];
+      h[o_spec + at[node[k]]++] = s;
+      ports |= port_off[ps_port_list[s] + 1] > port_off[ps_port_list[s]];
+    }
+  }
+  // ---- the pending rows without the moved pods: same groups, same order ----
+  std::vector<int32_t> pend((size_t)P - n), goff(E + 1, 0);
+  for (int g = 0, k = 0; g < E; ++g) {
+    for (int p = e->h_group_off[g]; p < e->h_group_off[g + 1]; ++p)
+      if (to[p] == 0) { pend[k] = e->h_pend_spec[p]; to[p] = k++; }
+    goff[g + 1] = k;
+  }
+  { const int rc = stage_pending(e, P - n, pend.data(), E, goff.data(), false); if (rc) return rc; }
+  if (new_index) std::copy(to.begin(), to.end(), new_index);
+  for (int i = 0; i < nrows; ++i) e->nh.pod_cnt[h[o_row + i]] += arr_cnt[h[o_row + i]];
+  e->nh.pod_total = total;
+  // ---- device: the host mirrors are ahead of it from here on, so a CUDA error leaves an engine that needs a cae_load ----
+  auto device = [&]() -> int {
+    int32_t* dv = static_cast<int32_t*>(e->nd_blob.p);
+    CAE_CUDA(cudaMemcpyAsync(dv, h, words * 4, cudaMemcpyHostToDevice, e->stream));
+    CAE_CUDA(cudaEventRecord(e->nd_stage.ev, e->stream));
+    e->stats.h2d_bytes += (int64_t)words * 4;
+    if (upload_pending(e, P - n, E)) return -1;
+    NodeDeltaDev dd{};
+    dd.nd = nrows;
+    dd.row = dv + o_row; dd.pod_off = dv + o_off; dd.pod_spec = dv + o_spec;
+    if (launch_force_add(e, dd, total, ports)) return -1;
+    if (launch_expand_pods(e)) return -1;
+    return launch_group_records(e);
+  };
+  const int rc = device();
+  if (rc) e->loaded = false;
+  return rc;
+}
+
 // cae_similar_node_groups.  The label signatures are built here from the host mirror of the label-set table: dense ids of
 // the templates' label-pair lists with the ignored keys removed (pairs are sorted by key id, so equal lists <=> equal maps).
 // Inputs travel in one H2D copy, outputs in one D2H copy; nothing is written to the caller's buffers unless the status is 0.
@@ -1572,13 +1674,8 @@ int32_t cae_load_pending(cae_engine* h, int32_t num_pending, const int32_t* pend
     if (!same) { cae::set_error("cae_load_pending: the group -> spec sequence changed under topology counters"); return 2; }
   }
   { int rc = cae::stage_pending(e, P, pend_spec, E, group_off, true); if (rc) return rc; }
-  const size_t words = (size_t)P + E + 1;
-  if (P) CAE_CUDA(cudaMemcpyAsync(const_cast<int32_t*>(e->dobj.pend_spec), e->h_pend_spec, sizeof(int32_t) * P, cudaMemcpyHostToDevice, e->stream));
-  CAE_CUDA(cudaMemcpyAsync(const_cast<int32_t*>(e->dobj.group_off), e->h_group_off, sizeof(int32_t) * (E + 1), cudaMemcpyHostToDevice, e->stream));
-  CAE_CUDA(cudaEventRecord(e->pending_stage.ev, e->stream));
-  e->stats.h2d_bytes = (int64_t)words * 4;
-  e->P = P; e->E = E; e->p_begin = pb; e->p_end = pe; e->Pl = Pl; e->Plw = (Pl + 31) / 32;
-  e->group_reason_valid = false;
+  e->stats.h2d_bytes = 0;
+  if (cae::upload_pending(e, P, E)) return -1;
   if (cae::launch_expand_pods(e)) return -1;
   if (cae::launch_group_records(e)) return -1;
   // no synchronize: the stream orders the copies and the two kernels before whatever the caller launches next
@@ -1607,6 +1704,13 @@ int32_t cae_load_pods(cae_engine* h, const cae_pod_delta* d) {
   if (!d) { cae::set_error("cae_load_pods: no delta"); return -2; }
   cudaSetDevice(e->cfg.device);
   return cae::do_load_pods(e, d);
+}
+
+int32_t cae_force_add_pods(cae_engine* h, int32_t n, const int32_t* pod, const int32_t* node, int32_t* new_index) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_force_add_pods before cae_load"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_force_add(e, n, pod, node, new_index);
 }
 
 int32_t cae_feasibility(cae_engine* h, uint32_t* fit_bits, uint8_t* reasons, int32_t* fit_count) {

@@ -168,6 +168,13 @@ __global__ void dyn_feed_kernel(DevObjects o, DynTables d, int E, const int32_t*
   if (d.q_dc[q] != mine || dc_ngroups[mine] > 1) d.group_feeds[g] = 1;
 }
 
+// non-empty pending groups per dynamic class (plan_dynamic counts the same on the host at a load)
+__global__ void dyn_ngroups_kernel(DevObjects o, int E, const int32_t* __restrict__ spec_dc, int32_t* __restrict__ dc_ngroups) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= E || o.group_off[g + 1] == o.group_off[g]) return;
+  atomicAdd(&dc_ngroups[spec_dc[o.pend_spec[o.group_off[g]]]], 1);
+}
+
 // reason of the PodTopologySpread / InterPodAffinity filters for class dc on the EMPTY template t,
 // with the template node added to the cluster snapshot (SchedulablePodGroups, orchestrator.go:608-620)
 __global__ void dyn_post_code_kernel(DevObjects o, DynTables d, int U, uint8_t* __restrict__ post_code) {
@@ -247,6 +254,27 @@ int launch_dynamic_tables(Engine* e, const uint8_t* d_spec_used, const int32_t* 
   if (e->T > 0) dyn_post_code_kernel<<<dim3((e->T + 127) / 128, d.DC), 128, 0, e->stream>>>(e->dobj, d, U, e->d_post_code);
   dyn_qrec_kernel<<<(Q + 127) / 128, 128, 0, e->stream>>>(e->dobj, d);
   e->stats.kernel_launches += 10;
+  CAE_KERNEL_OK();
+  return 0;
+}
+
+// After cae_force_add_pods emptied pending groups: which groups feed which counters, from the resident pending rows, as a
+// load of those rows counts them.  spec_dc is the folded table here (a load counts before it folds the inactive classes into
+// class 0); that changes nothing: every counter of a folded class is an inactive Q_EXIST counter, for which no spec in the
+// snapshot has a weight, so its groups feed exactly the counters of other classes either way, and no class that keeps its
+// counters loses or gains a group.  launch_dynamic_recount, which the caller runs next, carries q_nfeed into qrec.
+int launch_dynamic_feeds(Engine* e) {
+  DynTables& d = e->dyn;
+  if (d.Q == 0) return 0;
+  int32_t* ngroups = const_cast<int32_t*>(e->d_dc_ngroups);
+  CAE_CUDA(cudaMemsetAsync(ngroups, 0, sizeof(int32_t) * d.DC, e->stream));
+  CAE_CUDA(cudaMemsetAsync(d.q_nfeed, 0, sizeof(int32_t) * d.Q, e->stream));
+  CAE_CUDA(cudaMemsetAsync(d.group_feeds, 0, std::max(e->E, 1), e->stream));
+  if (e->E > 0) {
+    dyn_ngroups_kernel<<<(e->E + 127) / 128, 128, 0, e->stream>>>(e->dobj, e->E, e->d_spec_dc, ngroups);
+    dyn_feed_kernel<<<dim3((e->E + 127) / 128, d.Q), 128, 0, e->stream>>>(e->dobj, d, e->E, e->d_spec_dc, ngroups);
+    e->stats.kernel_launches += 2;
+  }
   CAE_KERNEL_OK();
   return 0;
 }

@@ -347,11 +347,18 @@ struct NodeDeltaDev {                    // device views into the staged rows of
   const int64_t *alloc, *cfree;          // [nd + na][R], [nd + na][A]
 };
 int launch_node_rows(Engine* e, const NodeDeltaDev& d, int64_t total);   // rows in place + resident CSR rebuilt into the spare buffer
+// cae_force_add_pods: d.row [nd] receiving rows, d.pod_off / d.pod_spec their arrivals (nothing else of d is read); the
+// resident CSR with each arrival list appended to its row's old list
+int launch_node_arrivals(Engine* e, const NodeDeltaDev& d, int64_t total);
+// force_add.cu: everything on the device that follows from the arrivals of launch_node_arrivals' `d`: the resident CSR, the
+// receiving rows' run state, their pre_code when an arrival holds host ports (`ports`), the topology counters
+int launch_force_add(Engine* e, const NodeDeltaDev& d, int64_t total, bool ports);
 // cae_load_node_churn: node columns, run state and resident CSR of the new row list; src [N'+T] = old row, or -1 - staged row
 int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int N_new, int64_t total);
 int launch_pre_ok_bits(Engine* e);       // pre_ok[SC][Twp]: needs pre_code and the templates' pod slots
 int launch_post_bits(Engine* e);
 int launch_dynamic_tables(Engine* e, const uint8_t* d_spec_used, const int32_t* d_dc_ngroups);
+int launch_dynamic_feeds(Engine* e);     // dc_ngroups, q_nfeed and group_feeds of the resident pending rows (groups emptied since the load)
 int launch_expand_pods(Engine* e);
 int launch_port_conflicts(Engine* e, int num_port_lists);
 int launch_feasibility(Engine* e, bool want_reasons);

@@ -1,4 +1,5 @@
-// node_delta.cu — device half of cae_load_nodes and cae_load_node_churn (api.cu).
+// node_delta.cu — device half of cae_load_nodes and cae_load_node_churn (api.cu), and the resident CSR of
+// cae_force_add_pods (force_add.cu).
 //
 // cae_load_nodes: the dirty cluster-node rows are written in place, and the resident pod CSR (node_pod_off /
 // node_pod_spec) is rebuilt on the device — per-row counts, an exclusive scan, a gather of the clean rows' old lists and
@@ -7,6 +8,8 @@
 // new row -> source (an old row: a clean survivor or a shifted template; or a staged row: a dirty or an added node),
 // and the CSR is rebuilt through the same map.  Only the staged rows travel over PCIe; everything else is read where it
 // already is.
+// cae_force_add_pods: the rows stay as they are and the receiving rows' lists grow: the same counts, scan and gather, with
+// the staged lists (the arrivals per receiving row) appended to the rows' old lists instead of replacing them.
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
@@ -42,16 +45,34 @@ __global__ void nd_rows_kernel(DevObjects o, NodeDeltaDev d, int A, int N, int64
   src[r] = -1 - i;
 }
 
-// one warp per new row: its list from the old CSR (src >= 0: old row) or from the staged rows (src < 0: row -1 - src)
+// the receiving rows of a force-add: their resident count grows by their arrivals, their source is the staged arrival list
+__global__ void nd_arrive_kernel(NodeDeltaDev d, int32_t* __restrict__ cnt, int32_t* __restrict__ src) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= d.nd) return;
+  const int r = d.row[i];
+  cnt[r] += d.pod_off[i + 1] - d.pod_off[i];
+  src[r] = -1 - i;
+}
+
+// one warp per new row: its list from the old CSR (src >= 0: old row) or from the staged rows (src < 0: row -1 - src);
+// `append`: a staged list follows the old list of the row (which keeps its place) instead of replacing it
 __global__ void nd_gather_kernel(const int32_t* __restrict__ old_off, const int32_t* __restrict__ old_spec,
                                  const int32_t* __restrict__ new_off, int NT, const int32_t* __restrict__ src, NodeDeltaDev d,
-                                 int32_t* __restrict__ new_spec) {
+                                 bool append, int32_t* __restrict__ new_spec) {
   const int r = (int)(((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (r >= NT) return;
   const int s = src[r];
-  const int32_t* from = s >= 0 ? old_spec + old_off[s] : d.pod_spec + d.pod_off[-1 - s];
   const int b = new_off[r], n = new_off[r + 1] - b;
-  for (int j = lane; j < n; j += 32) new_spec[b + j] = from[j];
+  const int32_t *old = nullptr, *staged = nullptr;
+  int n_old = n;
+  if (s >= 0) {
+    old = old_spec + old_off[s];
+  } else {
+    staged = d.pod_spec + d.pod_off[-1 - s];
+    n_old = append ? n - (d.pod_off[-s] - d.pod_off[-1 - s]) : 0;
+    if (append) old = old_spec + old_off[r];
+  }
+  for (int j = lane; j < n; j += 32) new_spec[b + j] = j < n_old ? old[j] : staged[j - n_old];
 }
 
 // Where the churn's node columns live: one engine-owned buffer per half, sub-arrays 256-byte aligned, node_name first
@@ -131,7 +152,9 @@ static int spare_csr(Engine* e, int NT, int64_t total, int32_t** new_off, int32_
   return 0;
 }
 
-int launch_node_rows(Engine* e, const NodeDeltaDev& d, int64_t total) {
+// The resident CSR after the staged rows of `d`: dirty rows (their node columns and run state written in place, their lists
+// replaced) or, with `append`, the arrivals of receiving rows
+static int rebuild_csr(Engine* e, const NodeDeltaDev& d, int64_t total, bool append) {
   const int N = e->N, NT = e->N + e->T;
   int32_t *new_off = nullptr, *new_spec = nullptr;
   if (spare_csr(e, NT, total, &new_off, &new_spec) ||
@@ -143,18 +166,23 @@ int launch_node_rows(Engine* e, const NodeDeltaDev& d, int64_t total) {
   CAE_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp, cnt, new_off, NT + 1, e->stream));
   if (devbuf_reserve(e, e->nd_cub, tmp)) return -1;
   nd_count_kernel<<<(NT + 256) / 256, 256, 0, e->stream>>>(e->dobj.node_pod_off, NT, cnt, src);
-  if (d.nd > 0)
+  if (d.nd > 0 && append)
+    nd_arrive_kernel<<<(d.nd + 127) / 128, 128, 0, e->stream>>>(d, cnt, src);
+  else if (d.nd > 0)
     nd_rows_kernel<<<(d.nd + 127) / 128, 128, 0, e->stream>>>(e->dobj, d, e->A, N, e->d_c_free, e->d_c_slots, cnt, src);
   CAE_CUDA(cub::DeviceScan::ExclusiveSum(e->nd_cub.p, tmp, cnt, new_off, NT + 1, e->stream));
   if (NT > 0)
     nd_gather_kernel<<<(unsigned)(((size_t)NT * 32 + 255) / 256), 256, 0, e->stream>>>(e->dobj.node_pod_off, e->dobj.node_pod_spec, new_off,
-                                                                                      NT, src, d, new_spec);
+                                                                                      NT, src, d, append, new_spec);
   e->stats.kernel_launches += 4;
   CAE_KERNEL_OK();
   e->dobj.node_pod_off = new_off;
   e->dobj.node_pod_spec = new_spec;
   return 0;
 }
+
+int launch_node_rows(Engine* e, const NodeDeltaDev& d, int64_t total) { return rebuild_csr(e, d, total, false); }
+int launch_node_arrivals(Engine* e, const NodeDeltaDev& d, int64_t total) { return rebuild_csr(e, d, total, true); }
 
 int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int N, int64_t total) {
   const int NT = N + e->T, A1 = std::max(e->A, 1);
@@ -174,7 +202,7 @@ int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int 
   CAE_CUDA(cub::DeviceScan::ExclusiveSum(e->nd_cub.p, tmp, cnt, new_off, NT + 1, e->stream));
   if (NT > 0)
     nd_gather_kernel<<<(unsigned)(((size_t)NT * 32 + 255) / 256), 256, 0, e->stream>>>(e->dobj.node_pod_off, e->dobj.node_pod_spec, new_off,
-                                                                                      NT, src, d, new_spec);
+                                                                                      NT, src, d, false, new_spec);
   e->stats.kernel_launches += 3;
   CAE_KERNEL_OK();
   DevObjects& o = e->dobj;

@@ -564,6 +564,48 @@ class EncodedObjects:
         out.struct = self._restruct(a, num_pending=len(a["pend_spec"]), num_groups=len(a["group_off"]) - 1, **_root_counts(a))
         return out
 
+    def apply_force_add(self, pods, nodes) -> Tuple["EncodedObjects", np.ndarray]:
+        """The objects after cae_force_add_pods(pods, nodes), stated on the host, and the new_index map: pending pod
+        pods[i] is appended to the resident pods of cluster row nodes[i] in list order (its spec id unchanged) and leaves
+        the pending list; the other pods keep their order and groups, so a group may become empty.  new_index [P] is
+        each pod's index afterwards, -1 for a moved one.  A cae_load of the result must answer like the engine after
+        the call.  ValueError: what the engine answers with status -2."""
+        import copy
+        pods, nodes = np.asarray(pods, np.int64).reshape(-1), np.asarray(nodes, np.int64).reshape(-1)
+        P, N = self.P, self.struct.num_cluster_nodes
+        if len(pods) != len(nodes):
+            raise ValueError("force add: pods and nodes differ in length")
+        if len(pods) and (pods.min() < 0 or pods.max() >= P or len(np.unique(pods)) != len(pods)):
+            raise ValueError("force add: a pod index is out of range or listed twice")
+        if len(nodes) and (nodes.min() < 0 or nodes.max() >= N):
+            raise ValueError("force add: a node is not a cluster row")
+        a = dict(self.arrays)
+        keep = np.ones(P, bool)
+        keep[pods] = False
+        new_index = np.where(keep, np.cumsum(keep) - 1, -1).astype(np.int32)
+        kept_before = np.concatenate([[0], np.cumsum(keep)])
+        a["pend_spec"] = np.ascontiguousarray(a["pend_spec"][keep])
+        a["group_off"] = _i32(kept_before[a["group_off"]])
+        off, spec = a["node_pod_off"], a["node_pod_spec"]
+        by_row = np.argsort(nodes, kind="stable")                     # arrivals grouped by row, list order kept
+        arrivals = np.bincount(nodes, minlength=len(off) - 1)
+        new_off = np.concatenate([[0], np.cumsum((off[1:] - off[:-1]) + arrivals)])
+        out_spec = np.empty(int(new_off[-1]), np.int32)
+        is_old = np.ones(len(out_spec), bool)
+        first_new = new_off[1:] - arrivals                            # where each row's arrivals start
+        rows_sorted = nodes[by_row]
+        rank = np.arange(len(pods)) - np.searchsorted(rows_sorted, rows_sorted, side="left")
+        dst = first_new[rows_sorted] + rank
+        is_old[dst] = False
+        out_spec[is_old] = spec[:off[-1]]
+        out_spec[dst] = self.arrays["pend_spec"][pods[by_row]]
+        a["node_pod_off"] = _i32(new_off)
+        a["node_pod_spec"] = out_spec
+        out = copy.copy(self)
+        out.arrays = a
+        out.struct = self._restruct(a, num_pending=int(keep.sum()))
+        return out, new_index
+
     def _with_tails(self, d: Dict[str, np.ndarray], tables) -> Dict[str, np.ndarray]:
         """A copy of the arrays with the tails `d` of the dictionary tables `tables` appended (tail offsets made absolute)."""
         a, n = dict(self.arrays), _dict_counts(self.struct, self.arrays)

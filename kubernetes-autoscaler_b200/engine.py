@@ -177,6 +177,29 @@ class Engine:
             self.enc = enc
         return 0
 
+    def force_add_pods(self, pods: Sequence[int], nodes: Sequence[int], enc: Optional[EncodedObjects] = None):
+        """ClusterSnapshot.ForceAddPod for a list of pending pods (cae_force_add_pods): pending pod pods[i] becomes a
+        resident of cluster row nodes[i] and leaves the pending list, e.g. what filter_schedulable assigned.  Returns
+        new_index [P before the call] int32 (-1 = moved), or False when the engine answers "use a full load" (status 2);
+        the engine is unchanged then.  `enc`: the objects the engine now holds (EncodedObjects.apply_force_add), kept as
+        this engine's shapes."""
+        pd, nd = np.ascontiguousarray(pods, np.int32), np.ascontiguousarray(nodes, np.int32)
+        if pd.ndim != 1 or pd.shape != nd.shape:
+            raise ValueError("force_add_pods: pods and nodes must be two lists of one length")
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        # new_index is worked out here, not asked of the library: the library writes one entry per pending pod IT holds, and
+        # this object's shapes (self.enc) are only as current as the caller kept them
+        rc = self.lib.cae_force_add_pods(self.h, len(pd), vp(pd), vp(nd), None)
+        if rc == 2:
+            return False
+        self._check(rc)
+        keep = np.ones(self.enc.P, bool)
+        keep[pd] = False
+        new_index = np.where(keep, np.cumsum(keep) - 1, -1).astype(np.int32)
+        if enc is not None:
+            self.enc = enc
+        return new_index
+
     def feasibility(self, want_bits: bool = True):
         """Dense pods x templates pass. Returns (fit_bits [T][ceil(Pl/32)] uint32 | None,
         reasons [T][Pl] uint8 | None, fit_count [T] int32) for this rank's pod shard."""

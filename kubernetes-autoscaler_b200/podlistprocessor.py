@@ -72,11 +72,13 @@ class TryScheduleInputs:
     node_ok: Optional[np.ndarray]
 
 
-def _encode_pending(cluster: List[NodeInfo], pods: List[Pod], hints: Optional[Hints], namespaces: Sequence[Namespace]):
+def _encode_pending(cluster: List[NodeInfo], pods: List[Pod], hints: Optional[Hints], namespaces: Sequence[Namespace],
+                    templates: Sequence[NodeInfo] = ()):
     """The snapshot with `pods` as the pending pods: (enc, id(pod) -> pending index, hinted row per pending pod,
-    SimilarPodsScheduling class per pending pod, controller per class)."""
+    SimilarPodsScheduling class per pending pod, controller per class).  `templates`: the node-group templates of a
+    scale-up that is to run on the same snapshot (the placement loop ignores them)."""
     groups = build_pod_groups(pods)
-    enc = encode(cluster, [], groups, namespaces)
+    enc = encode(cluster, list(templates), groups, namespaces)
     index_of: Dict[int, int] = {}
     k = 0
     for g in groups:
@@ -109,10 +111,10 @@ def _encode_pending(cluster: List[NodeInfo], pods: List[Pod], hints: Optional[Hi
 
 def prepare_try_schedule(cluster_snapshot: Sequence[NodeInfo], pods: Sequence[Pod], hints: Optional[Hints] = None,
                          isNodeAcceptable: Callable[[NodeInfo], bool] = ScheduleAnywhere,
-                         namespaces: Sequence[Namespace] = ()) -> TryScheduleInputs:
+                         namespaces: Sequence[Namespace] = (), templates: Sequence[NodeInfo] = ()) -> TryScheduleInputs:
     pods = list(pods)
     cluster = list(cluster_snapshot)
-    enc, index_of, hint, sim, class_ctrl = _encode_pending(cluster, pods, hints, namespaces)
+    enc, index_of, hint, sim, class_ctrl = _encode_pending(cluster, pods, hints, namespaces, templates)
     order = [index_of[id(p)] for p in pods]
     ok = None
     if isNodeAcceptable is not ScheduleAnywhere:
@@ -195,6 +197,7 @@ class HintingSimulator:
         self.hints = Hints()
         self.engine = engine
         self.last_index = 0   # SchedulerPluginRunner.lastIndex of the snapshot the pods are tried on
+        self.committed = None   # after TrySchedulePods(commit=True): (the objects the engine holds, new_index [P])
 
     def _run(self, x: TryScheduleInputs, breakOnFailure: bool):
         eng = self.engine or shared_engine()
@@ -203,19 +206,35 @@ class HintingSimulator:
 
     def TrySchedulePods(self, cluster_snapshot: Sequence[NodeInfo], pods: Sequence[Pod],
                         isNodeAcceptable: Callable[[NodeInfo], bool] = ScheduleAnywhere, breakOnFailure: bool = False,
-                        namespaces: Sequence[Namespace] = ()) -> Tuple[List[Status], int]:
+                        namespaces: Sequence[Namespace] = (), commit: bool = False,
+                        templates: Sequence[NodeInfo] = ()) -> Tuple[List[Status], int]:
         """Returns (statuses of the pods that were placed, in processing order; overflowing controller count).
-        The pods are placed in the engine's copy of the snapshot only (the caller's NodeInfos are not modified)."""
+        The caller's NodeInfos are not modified.  Without `commit` the pods are placed in a working copy of the engine's
+        snapshot that ends with the call.  With `commit` the placed pods become residents of their nodes in the
+        engine's snapshot, in processing order (ClusterSnapshot.ForceAddPod), and leave its pending pods, so that a
+        scale-up on the same engine sees what the reference's ScaleUp sees; `templates` puts the node-group templates
+        of that scale-up into the snapshot.  ``self.committed`` then holds the objects the engine holds
+        (``engine.enc``) and the new index of every pending pod (-1 = placed)."""
+        self.committed = None
         if not pods:
             return [], 0
-        x = prepare_try_schedule(cluster_snapshot, pods, self.hints, isNodeAcceptable, namespaces)
+        x = prepare_try_schedule(cluster_snapshot, pods, self.hints, isNodeAcceptable, namespaces, templates)
         assigned, self.last_index, overflowing = self._run(x, breakOnFailure)
-        statuses = []
+        statuses, placed, rows = [], [], []
         for p in x.pods:
-            n = int(assigned[x.index_of[id(p)]])
+            i = x.index_of[id(p)]
+            n = int(assigned[i])
             if n >= 0:
                 statuses.append(Status(p, x.cluster[n].node.name))
                 self.hints.Set(HintKeyFromPod(p), x.cluster[n].node.name)
+                placed.append(i)
+                rows.append(n)
+        if commit:
+            eng = self.engine or shared_engine()
+            after, new_index = x.enc.apply_force_add(placed, rows)
+            if eng.force_add_pods(placed, rows, after) is False:   # the resident lists would overflow: a full load
+                eng.load(after)
+            self.committed = (after, new_index)
         return statuses, overflowing
 
     def DropOldHints(self) -> None:
@@ -234,11 +253,12 @@ class FilterOutSchedulablePodListProcessor:
         self.overflowing_controllers = 0
 
     def Process(self, cluster_snapshot: Sequence[NodeInfo], unschedulablePods: Sequence[Pod],
-                namespaces: Sequence[Namespace] = ()) -> List[Pod]:
-        """Returns the pods that remain unschedulable (filterOutSchedulableByPacking, :96-126)."""
+                namespaces: Sequence[Namespace] = (), commit: bool = False, templates: Sequence[NodeInfo] = ()) -> List[Pod]:
+        """Returns the pods that remain unschedulable (filterOutSchedulableByPacking, :96-126).  `commit`, `templates`:
+        as for HintingSimulator.TrySchedulePods."""
         candidates = sorted(unschedulablePods, key=lambda p: -p.priority)   # :98-100 (stable here)
         statuses, self.overflowing_controllers = self.schedulingSimulator.TrySchedulePods(
-            cluster_snapshot, candidates, self.nodeFilter, False, namespaces)
+            cluster_snapshot, candidates, self.nodeFilter, False, namespaces, commit, templates)
         scheduled = {id(s.pod) for s in statuses}
         self.schedulingSimulator.DropOldHints()
         return [p for p in candidates if id(p) not in scheduled]

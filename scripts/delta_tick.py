@@ -7,6 +7,7 @@
     python scripts/delta_tick.py --kind nodes --config 3 --scale 1,20,200,2000 --reps 5 [--check]
     python scripts/delta_tick.py --kind churn --config 3 --scale 1,10,100 --dirty 20 --reps 5 [--check]
     python scripts/delta_tick.py --kind pods --config 3 --scale 1,10,100 --reps 5 [--check]
+    python scripts/delta_tick.py --kind placed --config 3 --reps 5 [--check]
 
 Kinds, with the change `scale` stands for and the delta call:
   nodes  synth.node_churn on `scale` dirty nodes (binds, evictions, moves, cordons, taints, allocatable, relabels):
@@ -15,6 +16,13 @@ Kinds, with the change `scale` stands for and the delta call:
          cae_load_node_churn(removed, added and dirty rows) + cae_load_pending(pending rows);
   pods   synth.pod_churn: `scale` new workloads arrive, `scale` pending groups finish: cae_load_pods(new specs + the new
          pending list).  The caller-side encode is not part of either tick (synth builds tables, not objects).
+  placed the reference's tick, filter pass then scale-up on ONE snapshot, three ways (`scale` is not used): every tick is
+         cae_load + cae_filter_schedulable over all pending pods, then the placements become residents, then estimate_all +
+         expander_best.  Tick A: cae_force_add_pods(what the pass assigned).  Tick B: the same placements as host-built
+         deltas, cae_load_nodes(the complete new resident lists of the receiving rows) + cae_load_pods(the compacted
+         pending list).  Tick C: a second cae_load of the objects after the placements.  Only the step that makes the
+         placements resident is timed per tick, beside the tick; array work that builds B's deltas and C's objects is
+         inside their ticks, since A needs none of it.
 Also reported: the delta call's host wall time (cae_load_nodes and cae_load_node_churn return without a device
 synchronise, cae_load_pods synchronises), its device time (CUDA events on the engine's stream) and the bytes it uploaded,
 with the device name and power limit.  --check: both ticks' node counts, pod counts, sched, order and dense fit counts must
@@ -29,7 +37,7 @@ import time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 
-SCALES = {"nodes": "1,20,200,2000", "churn": "1,10,100", "pods": "1,10,100"}
+SCALES = {"nodes": "1,20,200,2000", "churn": "1,10,100", "pods": "1,10,100", "placed": "0"}
 
 
 def _card():
@@ -63,6 +71,100 @@ def _change(synth, kind, enc, seed, scale, dirty):
     return after, lambda eng: eng.load_pods(delta, after) == 0, None
 
 
+def _placed_as_deltas(enc, pods, nodes):
+    """The placements as the deltas a caller without cae_force_add_pods sends: the receiving rows as dirty rows with their
+    unchanged node columns and complete new resident lists, and the pending list without the placed pods."""
+    from kubernetes_autoscaler_b200.encode import NodeDelta, PodDelta
+    after, _ = enc.apply_force_add(pods, nodes)
+    a, b = enc.arrays, after.arrays
+    rows = np.unique(nodes)
+    off = b["node_pod_off"]
+    lists = [b["node_pod_spec"][off[r]:off[r + 1]] for r in rows]
+    nd = NodeDelta(row=rows, labelset=a["node_labelset"][rows], taint_list=a["node_taint_list"][rows],
+                   unschedulable=a["node_unschedulable"][rows], alloc=a["node_alloc"][rows], allowed_pods=a["node_allowed_pods"][rows],
+                   pod_off=np.concatenate([[0], np.cumsum([len(x) for x in lists])]), pod_spec=np.concatenate(lists))
+    return after, nd, PodDelta(group_off=b["group_off"], pend_spec=b["pend_spec"])
+
+
+def _placed(args):
+    """--kind placed: ticks A, B and C of the module docstring, alternating, on three engines."""
+    import __graft_entry__ as ge
+    ge.build()
+    import torch
+    from kubernetes_autoscaler_b200 import synth
+    from kubernetes_autoscaler_b200.engine import Engine
+    enc = synth.generate(args.config, pods=args.pods, templates=args.templates, cluster_nodes=args.cluster_nodes)
+    caps = np.full(enc.T, args.cap, np.int32)
+    chain = [0, 1, 2]
+    order = np.arange(enc.P, dtype=np.int32)[::-1].copy()
+    engs = {k: Engine(device=0) for k in "ABC"}
+    sa = torch.cuda.ExternalStream(engs["A"].stream(), device=torch.device("cuda", 0))
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+
+    def tick(kind):
+        eng = engs[kind]
+        r = {}
+        t0 = time.perf_counter()
+        eng.load(enc)
+        assigned, _, _ = eng.filter_schedulable(order)
+        placed = np.ascontiguousarray(order[assigned[order] >= 0], np.int32)
+        nodes = np.ascontiguousarray(assigned[placed], np.int32)
+        t1 = time.perf_counter()
+        if kind == "A":
+            e0.record(sa)
+            # the ABI call itself (the binding's force_add_pods also builds the new_index map in numpy)
+            assert eng.lib.cae_force_add_pods(eng.h, len(placed), placed.ctypes.data, nodes.ctypes.data, None) == 0
+            e1.record(sa)
+            r["A_call_host_ms"] = 1e3 * (time.perf_counter() - t1)
+            r["A_h2d_bytes"] = int(eng.stats().h2d_bytes)
+        elif kind == "B":
+            after, nd, pd = _placed_as_deltas(enc, placed, nodes)
+            assert eng.load_nodes(nd)
+            nbytes = int(eng.stats().h2d_bytes)
+            assert eng.load_pods(pd, after) == 0
+            r["B_h2d_bytes"] = nbytes + int(eng.stats().h2d_bytes)
+        else:
+            eng.load(enc.apply_force_add(placed, nodes)[0])
+        t2 = time.perf_counter()
+        nc, pc, sched, order_t = eng.estimate_all(caps, copy=False)
+        eng.expander_best(chain, nc, pc)
+        t3 = time.perf_counter()
+        r["%s_tick_ms" % kind] = 1e3 * (t3 - t0)
+        r["%s_placements_ms" % kind] = 1e3 * (t2 - t1)
+        if kind == "A":
+            e1.synchronize()
+            r["A_call_dev_ms"] = e0.elapsed_time(e1)
+            eng.enc = enc.apply_force_add(placed, nodes)[0]   # untimed: the binding's shapes (P changed) for the check below
+        out = [x.copy() for x in (nc, pc, sched, order_t)] + [eng.feasibility(want_bits=False)[2].copy()] if args.check else None
+        return r, out, len(placed)
+
+    for k in "ABC":   # warm every shape the timed window uses
+        tick(k)
+    out = {"kind": "placed", "config": args.config, "pods": enc.P, "templates": enc.T,
+           "cluster_nodes": enc.struct.num_cluster_nodes, "cap": args.cap, **_card()}
+    rows, ok_all = [], True
+    for rep in range(args.reps):
+        r, outs = {}, {}
+        for k in ("ABC", "BCA", "CAB")[rep % 3]:
+            rk, outs[k], r["placed_pods"] = tick(k)
+            r.update(rk)
+        if args.check:
+            r["same"] = all(np.array_equal(x, y) and np.array_equal(x, z) for x, y, z in zip(outs["A"], outs["B"], outs["C"]))
+            ok_all &= r["same"]
+        rows.append(r)
+    run = {"reps": args.reps, "placed_pods": rows[0]["placed_pods"]}
+    for k in rows[0]:
+        if k not in ("same", "placed_pods"):
+            run[k] = _stats([r[k] for r in rows])
+    out["run"] = run
+    out["check"] = ok_all if args.check else None
+    print(json.dumps(out))
+    for e in engs.values():
+        e.close()
+    if args.check and not ok_all:
+        sys.exit(1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--kind", choices=sorted(SCALES), required=True)
@@ -76,6 +178,8 @@ def main():
     ap.add_argument("--cluster-nodes", type=int, default=None)
     ap.add_argument("--check", action="store_true")
     args = ap.parse_args()
+    if args.kind == "placed":
+        return _placed(args)
     import __graft_entry__ as ge
     ge.build()
     import torch
