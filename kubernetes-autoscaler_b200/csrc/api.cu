@@ -87,6 +87,16 @@ int pinned_reserve(Engine* e, Engine::PinnedBuf& b, size_t bytes) {
   b.cap = cap;
   return 0;
 }
+int stage_reserve(Engine* e, Engine::Staging& s, size_t bytes, size_t pinned) {
+  return devbuf_reserve(e, s.dev, bytes) || pinned_reserve(e, s.host, pinned) ? -1 : 0;
+}
+// Without the event record the next call's host writes would race this copy
+int stage_upload(Engine* e, Engine::Staging& s, size_t in) {
+  if (in) CAE_CUDA(cudaMemcpyAsync(s.dev.p, s.host.p, in, cudaMemcpyHostToDevice, e->stream));
+  CAE_CUDA(cudaEventRecord(s.host.ev, e->stream));
+  e->stats.h2d_bytes += (int64_t)in;
+  return 0;
+}
 
 template <class T>
 static int upload(Arena& a, const T* host, size_t n, const T** dev) {
@@ -810,23 +820,19 @@ static int tails_ids(const Engine* e, const Tails& v, Bad bad) {
   return 0;
 }
 
-// Appending tails: tails_layout places them in the caller's pinned blob (8-byte aligned segments from `bytes` on, returns the
-// end); tails_put writes them there with the offsets made absolute and appends them to the host mirrors; after the blob's
-// H2D copy, tails_grow grows the device tables from its device copy and advances the counts.  Until then
+// Appending tails: tails_layout places them in the caller's staged blob (tab[t]: the device copy of table t's tail);
+// tails_put writes them to its host copy with the offsets made absolute and appends them to the host mirrors; after the
+// blob's H2D copy, tails_grow grows the device tables from the device copy and advances the counts.  Until then
 // take_back_mirrors undoes tails_put.
-static size_t tails_layout(const Tails& v, size_t at[NUM_DICT_TABLES], size_t bytes) {
-  for (int t = 0; t < NUM_DICT_TABLES; ++t) {
-    at[t] = bytes;
-    bytes = (bytes + (size_t)v.n[kDict[t].cnt] * kDict[t].esz + 7) & ~(size_t)7;
-  }
-  return bytes;
+static void tails_layout(Layout& l, const Tails& v, char* tab[NUM_DICT_TABLES]) {
+  for (int t = 0; t < NUM_DICT_TABLES; ++t) l.add(tab[t], (size_t)v.n[kDict[t].cnt] * kDict[t].esz);
 }
-static void tails_put(Engine* e, const Tails& v, const size_t at[NUM_DICT_TABLES], char* h) {
+static void tails_put(Engine* e, const Tails& v, char* const tab[NUM_DICT_TABLES], const Engine::Staging& s) {
   for (int t = 0; t < NUM_DICT_TABLES; ++t) {
     const DictTab& d = kDict[t];
     const size_t n = (size_t)v.n[d.cnt];
     if (!n) continue;
-    char* dst = h + at[t];
+    char* dst = s.host_of(tab[t]);
     if (d.child >= 0) {
       const int32_t* rel = static_cast<const int32_t*>(v.src[t]);
       const int32_t base = (int32_t)e->dict_cnt[d.child];
@@ -935,9 +941,9 @@ static int grow_bytes(Engine* e, Engine::DevBuf& b, const void*& cur, size_t ele
   return 0;
 }
 
-static int tails_grow(Engine* e, const Tails& v, const size_t at[NUM_DICT_TABLES], const char* dv) {
+static int tails_grow(Engine* e, const Tails& v, char* const tab[NUM_DICT_TABLES]) {
   for (int t = 0; t < NUM_DICT_TABLES; ++t)
-    if (grow_bytes(e, e->dict_tab[t], dev_table(e->dobj, t), kDict[t].esz, table_len(e->dict_cnt, t), dv + at[t], (size_t)v.n[kDict[t].cnt]))
+    if (grow_bytes(e, e->dict_tab[t], dev_table(e->dobj, t), kDict[t].esz, table_len(e->dict_cnt, t), tab[t], (size_t)v.n[kDict[t].cnt]))
       return -1;
   for (int c = 0; c < NUM_DICT_COUNTS; ++c) e->dict_cnt[c] += v.n[c];
   e->dobj.num_values = (int32_t)e->dict_cnt[CNT_VALUES];
@@ -1062,67 +1068,56 @@ static void commit_nodes(Engine* e, NodePlan& p) {
   for (int64_t q = 0; q < p.npods_a; ++q) nh.spec_used[p.added.pod_spec[q]] = 1;
 }
 
-// One pinned staging blob and one H2D copy: the dictionary tails, the staged rows (dirty rows, then added ones) with their
-// run state (cluster_row_state), and the caller's `extra` segments (device addresses in xdev); then the dictionary tables
+// One staged blob and one H2D copy: the dictionary tails, the staged rows (dirty rows, then added ones) with their run
+// state (cluster_row_state), and the caller's `extra` arrays (their device copies in xdev); then the dictionary tables
 // grow on the device.  After commit_nodes.
-static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<std::pair<const void*, size_t>>& extra, NodeDeltaDev* dd,
-                       std::vector<const char*>* xdev) {
+static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<const std::vector<int32_t>*>& extra, NodeDeltaDev* dd,
+                       std::vector<const int32_t*>* xdev) {
   const cae_node_delta* dl = p.dl;
   const int A = e->A;
   const int nd = p.dirty.n, na = p.added.n, ns = nd + na;
   const int64_t npods = p.npods_d + p.npods_a;
-  size_t at[NUM_DICT_TABLES];
-  size_t bytes = tails_layout(p.tails, at, 0);
-  auto seg = [&](size_t n, size_t elem) { const size_t o = bytes; bytes = (bytes + n * elem + 7) & ~(size_t)7; return o; };
-  const size_t o_alloc = seg((size_t)ns * R, 8), o_cfree = seg((size_t)ns * A, 8);
-  const size_t o_row = seg(nd, 4), o_name = seg(na, 4), o_ls = seg(ns, 4), o_tl = seg(ns, 4), o_allowed = seg(ns, 4), o_slots = seg(ns, 4);
-  const size_t o_poff = seg((size_t)ns + 1, 4), o_pspec = seg(npods, 4), o_unsched = seg(ns, 1);
-  std::vector<size_t> o_extra;
-  for (const auto& x : extra) o_extra.push_back(seg(x.second, 1));
-  if (pinned_reserve(e, e->nd_stage, bytes)) return -1;
-  char* h = static_cast<char*>(e->nd_stage.p);
-  auto put = [&](size_t at, const void* src, size_t n) { if (n) memcpy(h + at, src, n); };
-  tails_put(e, p.tails, at, h);
-  put(o_row, dl->row, (size_t)nd * 4);
-  put(o_name, p.name, (size_t)na * 4);
-  int32_t* poff = reinterpret_cast<int32_t*>(h + o_poff);
+  Engine::Staging& s = e->nd;
+  char* tab[NUM_DICT_TABLES] = {};
+  NodeDeltaDev d{};
+  d.nd = nd; d.na = na;
+  std::vector<const int32_t*> xd(extra.size());
+  auto walk = [&](Layout& l) {
+    tails_layout(l, p.tails, tab);
+    l.add(d.alloc, (size_t)ns * R); l.add(d.cfree, (size_t)ns * A);
+    l.add(d.row, nd); l.add(d.name, na); l.add(d.labelset, ns); l.add(d.taint_list, ns); l.add(d.allowed, ns); l.add(d.cslots, ns);
+    l.add(d.pod_off, (size_t)ns + 1); l.add(d.pod_spec, npods); l.add(d.unsched, ns);
+    for (size_t x = 0; x < extra.size(); ++x) l.add(xd[x], extra[x]->size());
+  };
+  const size_t bytes = layout_bytes(walk);
+  if (stage_reserve(e, s, bytes, bytes)) return -1;
+  layout_bind(s.dev.p, walk);
+  tails_put(e, p.tails, tab, s);
+  std::copy(dl->row, dl->row + nd, s.host_of(d.row));
+  std::copy(p.name, p.name + na, s.host_of(d.name));
+  int32_t* poff = s.host_of(d.pod_off);
   poff[0] = 0;
-  int64_t* cfree = reinterpret_cast<int64_t*>(h + o_cfree);
-  int32_t* cslots = reinterpret_cast<int32_t*>(h + o_slots);
   for (int part = 0, i0 = 0; part < 2; ++part) {   // the dirty rows, then the added ones
     const RowsIn& r = part ? p.added : p.dirty;
-    put(o_ls + (size_t)i0 * 4, r.labelset, (size_t)r.n * 4);
-    put(o_tl + (size_t)i0 * 4, r.taint_list, (size_t)r.n * 4);
-    put(o_allowed + (size_t)i0 * 4, r.allowed, (size_t)r.n * 4);
-    put(o_unsched + (size_t)i0, r.unsched, (size_t)r.n);
-    put(o_alloc + (size_t)i0 * R * 8, r.alloc, (size_t)r.n * R * 8);
-    put(o_pspec + (size_t)poff[i0] * 4, r.pod_spec, (size_t)(r.n ? r.pod_off[r.n] : 0) * 4);
+    std::copy(r.labelset, r.labelset + r.n, s.host_of(d.labelset) + i0);
+    std::copy(r.taint_list, r.taint_list + r.n, s.host_of(d.taint_list) + i0);
+    std::copy(r.allowed, r.allowed + r.n, s.host_of(d.allowed) + i0);
+    std::copy(r.unsched, r.unsched + r.n, s.host_of(d.unsched) + i0);
+    std::copy(r.alloc, r.alloc + (size_t)r.n * R, s.host_of(d.alloc) + (size_t)i0 * R);
+    if (r.n) std::copy(r.pod_spec, r.pod_spec + r.pod_off[r.n], s.host_of(d.pod_spec) + poff[i0]);
     for (int i = 0; i < r.n; ++i) {
       poff[i0 + i + 1] = poff[i0] + r.pod_off[i + 1];
       cluster_row_state(e, r.alloc + (size_t)i * R, r.allowed[i], r.pod_spec + r.pod_off[i], r.pod_off[i + 1] - r.pod_off[i],
-                        e->host_tab<int64_t>(TAB_ps_req), cfree + (size_t)(i0 + i) * A, 1, cslots + i0 + i);
+                        e->host_tab<int64_t>(TAB_ps_req), s.host_of(d.cfree) + (size_t)(i0 + i) * A, 1, s.host_of(d.cslots) + i0 + i);
     }
     i0 += r.n;
   }
-  for (size_t x = 0; x < extra.size(); ++x) put(o_extra[x], extra[x].first, extra[x].second);
-  if (devbuf_reserve(e, e->nd_blob, bytes)) return -1;
-  char* dv = static_cast<char*>(e->nd_blob.p);
-  CAE_CUDA(cudaMemcpyAsync(dv, h, bytes, cudaMemcpyHostToDevice, e->stream));
-  CAE_CUDA(cudaEventRecord(e->nd_stage.ev, e->stream));
-  e->stats.h2d_bytes = (int64_t)bytes;
-  if (xdev) for (size_t o : o_extra) xdev->push_back(dv + o);
-  if (tails_grow(e, p.tails, at, dv)) return -1;
+  for (size_t x = 0; x < extra.size(); ++x) std::copy(extra[x]->begin(), extra[x]->end(), s.host_of(xd[x]));
+  if (stage_upload(e, s, bytes)) return -1;
+  if (xdev) *xdev = xd;
+  if (tails_grow(e, p.tails, tab)) return -1;
   e->group_reason_valid = false;
-  if (dd) {
-    *dd = NodeDeltaDev{};
-    dd->nd = nd; dd->na = na;
-    dd->row = reinterpret_cast<const int32_t*>(dv + o_row); dd->name = reinterpret_cast<const int32_t*>(dv + o_name);
-    dd->labelset = reinterpret_cast<const int32_t*>(dv + o_ls); dd->taint_list = reinterpret_cast<const int32_t*>(dv + o_tl);
-    dd->allowed = reinterpret_cast<const int32_t*>(dv + o_allowed); dd->cslots = reinterpret_cast<const int32_t*>(dv + o_slots);
-    dd->pod_off = reinterpret_cast<const int32_t*>(dv + o_poff); dd->pod_spec = reinterpret_cast<const int32_t*>(dv + o_pspec);
-    dd->unsched = reinterpret_cast<const uint8_t*>(dv + o_unsched);
-    dd->alloc = reinterpret_cast<const int64_t*>(dv + o_alloc); dd->cfree = reinterpret_cast<const int64_t*>(dv + o_cfree);
-  }
+  if (dd) *dd = d;
   return 0;
 }
 
@@ -1209,13 +1204,13 @@ static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
   if (e->has_dynamic)
     for (int q = 0; q < dy.Q; ++q) qbo.push_back(qbo.back() + Dc[nh.q_k[q]]);
   NodeDeltaDev dd{};
-  std::vector<const char*> xd;
-  if (stage_nodes(e, p, {{src.data(), 4 * src.size()}, {dom.data(), 4 * dom.size()}, {qbo.data(), 4 * qbo.size()}}, &dd, &xd)) return -1;
+  std::vector<const int32_t*> xd;
+  if (stage_nodes(e, p, {&src, &dom, &qbo}, &dd, &xd)) return -1;
   nh.pod_cnt.swap(pod_cnt);
   nh.key_val.swap(key_val);
 
   // ---- device: node columns + resident CSR, then everything a load derives from the node list ----
-  if (launch_node_churn(e, dd, reinterpret_cast<const int32_t*>(xd[0]), N, p.total)) return -1;
+  if (launch_node_churn(e, dd, xd[0], N, p.total)) return -1;
   e->N = N;
   e->U = N + 2 * T;
   if (devbuf_reserve(e, e->ch_pre, (size_t)std::max(e->SC, 1) * std::max(e->U, 1))) return -1;
@@ -1223,19 +1218,17 @@ static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
   if (launch_class_matrix(e) || launch_pre_ok_bits(e)) return -1;
   if (e->has_dynamic) {
     const size_t Q1 = std::max(dy.Q, 1), pool = std::max(qbo.back(), 1);
-    size_t off = 0;
-    auto take = [&](size_t b) { const size_t o = off; off += (std::max<size_t>(b, 1) + 255) & ~(size_t)255; return o; };
-    const size_t o_dom = take(4 * dom.size()), o_qbo = take(4 * qbo.size()), o_cnt = take(4 * pool), o_pres = take(4 * pool);
-    const size_t o_elig = take(Q1 * std::max(e->U, 1));
-    if (devbuf_reserve(e, e->ch_dyn, off)) return -1;
-    char* b = static_cast<char*>(e->ch_dyn.p);
-    if (!dom.empty()) CAE_CUDA(cudaMemcpyAsync(b + o_dom, xd[1], 4 * dom.size(), cudaMemcpyDeviceToDevice, e->stream));
-    CAE_CUDA(cudaMemcpyAsync(b + o_qbo, xd[2], 4 * qbo.size(), cudaMemcpyDeviceToDevice, e->stream));
-    dy.dom = reinterpret_cast<const int32_t*>(b + o_dom);
-    dy.q_base_off = reinterpret_cast<const int32_t*>(b + o_qbo);
-    dy.base_cnt = reinterpret_cast<int32_t*>(b + o_cnt);
-    dy.base_pres = reinterpret_cast<int32_t*>(b + o_pres);
-    dy.elig = reinterpret_cast<uint8_t*>(b + o_elig);
+    int32_t *d_dom = nullptr, *d_qbo = nullptr;
+    auto walk = [&](Layout& l) {
+      l.add(d_dom, dom.size()); l.add(d_qbo, qbo.size()); l.add(dy.base_cnt, pool); l.add(dy.base_pres, pool);
+      l.add(dy.elig, Q1 * std::max(e->U, 1));
+    };
+    if (devbuf_reserve(e, e->ch_dyn, layout_bytes(walk))) return -1;
+    layout_bind(e->ch_dyn.p, walk);
+    if (!dom.empty()) CAE_CUDA(cudaMemcpyAsync(d_dom, xd[1], 4 * dom.size(), cudaMemcpyDeviceToDevice, e->stream));
+    CAE_CUDA(cudaMemcpyAsync(d_qbo, xd[2], 4 * qbo.size(), cudaMemcpyDeviceToDevice, e->stream));
+    dy.dom = d_dom;
+    dy.q_base_off = d_qbo;
     dy.pool = qbo.back();
     for (int k = 0; k < K; ++k) { dy.Dc[k] = Dc[k]; dy.D[k] = D[k]; }
     if (launch_dynamic_recount(e, nullptr, e->U)) return -1;
@@ -1268,13 +1261,15 @@ static int do_load_pods(Engine* e, const cae_pod_delta* d) {
   std::vector<int32_t> row_ls((size_t)e->N + e->T);
   if (pd_resident_specs(e, S0, resident.data(), row_ls.data())) { e->loaded = false; return -1; }
 
-  // ---- the tails in one pinned blob and in the host mirrors the derivation reads (taken back if a limit refuses) ----
-  size_t at[NUM_DICT_TABLES];
-  const size_t bytes = tails_layout(v, at, 0);
+  // ---- the tails in one staged blob and in the host mirrors the derivation reads (taken back if a limit refuses) ----
+  char* tab[NUM_DICT_TABLES] = {};
+  auto walk = [&](Layout& l) { tails_layout(l, v, tab); };
+  const size_t bytes = layout_bytes(walk);
   // the blob is written before the status-1 limits are planned because the host mirrors the plan reads are appended from
-  // it; a refused delta leaves only this engine-internal staging buffer (possibly grown) behind
-  if (pinned_reserve(e, e->pd_stage, std::max<size_t>(bytes, 8))) { e->loaded = false; return -1; }
-  tails_put(e, v, at, static_cast<char*>(e->pd_stage.p));
+  // it; a refused delta leaves only this engine-internal staging (possibly grown) behind
+  if (stage_reserve(e, e->pd, bytes, bytes)) { e->loaded = false; return -1; }
+  layout_bind(e->pd.dev.p, walk);
+  tails_put(e, v, tab, e->pd);
   cae_objects o{};
   for (int t = 0; t < NUM_DICT_TABLES; ++t)
     if (kDict[t].host) *reinterpret_cast<const void**>(reinterpret_cast<char*>(&o) + kDict[t].obj) = e->dict_host[t].data();
@@ -1287,12 +1282,7 @@ static int do_load_pods(Engine* e, const cae_pod_delta* d) {
 
   // ---- commit: the H2D copy of the blob, then the device tables grow ----
   auto commit = [&]() -> int {
-    if (devbuf_reserve(e, e->pd_blob, std::max<size_t>(bytes, 8))) return -1;
-    char* dv = static_cast<char*>(e->pd_blob.p);
-    if (bytes) CAE_CUDA(cudaMemcpyAsync(dv, e->pd_stage.p, bytes, cudaMemcpyHostToDevice, e->stream));
-    CAE_CUDA(cudaEventRecord(e->pd_stage.ev, e->stream));
-    e->stats.h2d_bytes += (int64_t)bytes;
-    if (tails_grow(e, v, at, dv)) return -1;
+    if (stage_upload(e, e->pd, bytes) || tails_grow(e, v, tab)) return -1;
     e->nh.spec_anti.resize(S);
     for (int s = S0; s < S; ++s) e->nh.spec_anti[s] = o.aff_off[o.ps_anti_list[s] + 1] > o.aff_off[o.ps_anti_list[s]];
     return 0;
@@ -1336,27 +1326,32 @@ static int do_force_add(Engine* e, int n, const int32_t* pod, const int32_t* nod
   // ---- the arrivals per receiving row: rows ascending | offsets | specs in list order ----
   int nrows = 0;
   for (int r = 0; r < N; ++r) nrows += arr_cnt[r] > 0;
-  const size_t o_row = 0, o_off = (size_t)nrows, o_spec = o_off + nrows + 1, words = o_spec + n;
-  if (pinned_reserve(e, e->nd_stage, words * 4) || devbuf_reserve(e, e->nd_blob, words * 4)) return -1;
-  int32_t* h = static_cast<int32_t*>(e->nd_stage.p);
+  Engine::Staging& st = e->nd;
+  NodeDeltaDev dd{};
+  dd.nd = nrows;
+  auto walk = [&](Layout& l) { l.add(dd.row, nrows); l.add(dd.pod_off, (size_t)nrows + 1); l.add(dd.pod_spec, n); };
+  const size_t bytes = layout_bytes(walk);
+  if (stage_reserve(e, st, bytes, bytes)) return -1;
+  layout_bind(st.dev.p, walk);
+  int32_t *h_row = st.host_of(dd.row), *h_off = st.host_of(dd.pod_off), *h_spec = st.host_of(dd.pod_spec);
   std::vector<int32_t> at(N, 0);                 // where the next arrival of a row goes
   bool ports = false;
   {
     int i = 0, off = 0;
     for (int r = 0; r < N; ++r) {
       if (!arr_cnt[r]) continue;
-      h[o_row + i] = r;
-      h[o_off + i] = off;
+      h_row[i] = r;
+      h_off[i] = off;
       at[r] = off;
       off += arr_cnt[r];
       ++i;
     }
-    h[o_off + nrows] = off;
+    h_off[nrows] = off;
     const int32_t* port_off = e->host_tab<int32_t>(TAB_port_off);
     const int32_t* ps_port_list = e->host_tab<int32_t>(TAB_ps_port_list);
     for (int k = 0; k < n; ++k) {
       const int s = e->h_pend_spec[pod[k]];
-      h[o_spec + at[node[k]]++] = s;
+      h_spec[at[node[k]]++] = s;
       ports |= port_off[ps_port_list[s] + 1] > port_off[ps_port_list[s]];
     }
   }
@@ -1369,18 +1364,11 @@ static int do_force_add(Engine* e, int n, const int32_t* pod, const int32_t* nod
   }
   { const int rc = stage_pending(e, P - n, pend.data(), E, goff.data(), false); if (rc) return rc; }
   if (new_index) std::copy(to.begin(), to.end(), new_index);
-  for (int i = 0; i < nrows; ++i) e->nh.pod_cnt[h[o_row + i]] += arr_cnt[h[o_row + i]];
+  for (int i = 0; i < nrows; ++i) e->nh.pod_cnt[h_row[i]] += arr_cnt[h_row[i]];
   e->nh.pod_total = total;
   // ---- device: the host mirrors are ahead of it from here on, so a CUDA error leaves an engine that needs a cae_load ----
   auto device = [&]() -> int {
-    int32_t* dv = static_cast<int32_t*>(e->nd_blob.p);
-    CAE_CUDA(cudaMemcpyAsync(dv, h, words * 4, cudaMemcpyHostToDevice, e->stream));
-    CAE_CUDA(cudaEventRecord(e->nd_stage.ev, e->stream));
-    e->stats.h2d_bytes += (int64_t)words * 4;
-    if (upload_pending(e, P - n, E)) return -1;
-    NodeDeltaDev dd{};
-    dd.nd = nrows;
-    dd.row = dv + o_row; dd.pod_off = dv + o_off; dd.pod_spec = dv + o_spec;
+    if (stage_upload(e, st, bytes) || upload_pending(e, P - n, E)) return -1;
     if (launch_force_add(e, dd, total, ports)) return -1;
     if (launch_expand_pods(e)) return -1;
     return launch_group_records(e);
@@ -1407,22 +1395,29 @@ static int do_similar(Engine* e, const cae_similarity_inputs* in, uint32_t* bits
     if (k < 0) { set_error("cae_similar_node_groups: ignored key id < 0"); return -2; }
   for (int t = 0; t < T; ++t)
     if (in->eligible[t] > 1 || (in->safe && in->safe[t] > 1)) { set_error("cae_similar_node_groups: flag byte > 1"); return -2; }
+  e->stats.h2d_bytes = 0;
   if (T == 0) return 0;
   std::sort(ign.begin(), ign.end());
 
-  // layout (the same offsets on the device and in the pinned stage): inputs | outputs, then device-only scratch
+  // layout: inputs | outputs (staged), then device-only scratch
   const int K = 2 * e->dobj.num_res + 3;
-  size_t off = 0;
-  auto take = [&](size_t b) { const size_t o = off; off += (std::max<size_t>(b, 1) + 255) & ~(size_t)255; return o; };
-  const size_t o_i32 = take((size_t)16 * T), o_cap = take((size_t)8 * T), in_end = off;
-  const size_t o_status = take(8 + (size_t)12 * T), o_bits = take((size_t)4 * T * Tw), out_end = off;
-  const size_t o_x = take((size_t)8 * T * K), o_sched = take((size_t)4 * T * Ew);
-  if (pinned_reserve(e, e->sim_stage, out_end) || devbuf_reserve(e, e->sim_dev, off)) return -1;
-  char* h = static_cast<char*>(e->sim_stage.p);
-  char* d = static_cast<char*>(e->sim_dev.p);
-  int32_t* h_res = reinterpret_cast<int32_t*>(h + o_i32);
-  int32_t *h_lab = h_res + T, *h_fd = h_res + 2 * T, *h_fl = h_res + 3 * T;
-  int64_t* h_cap = reinterpret_cast<int64_t*>(h + o_cap);
+  Engine::Staging& st = e->sim;
+  SimLaunch s{};
+  size_t in_end = 0, o_bits = 0, out_end = 0;
+  auto walk = [&](Layout& l) {
+    l.add(s.res_sig, T); l.add(s.lab_sig, T); l.add(s.free_dims, T); l.add(s.flags, T); l.add(s.cap, T);
+    in_end = l.bytes;
+    l.add(s.status, 1); l.add(s.sum, T); l.add(s.count, T);
+    o_bits = l.bytes;
+    l.add(s.bits, (size_t)T * Tw);
+    out_end = l.bytes;
+    l.add(s.x, (size_t)T * K); l.add(s.sched, (size_t)T * Ew);
+  };
+  const size_t bytes = layout_bytes(walk);
+  if (stage_reserve(e, st, bytes, out_end)) return -1;
+  layout_bind(st.dev.p, walk);
+  int32_t *h_res = st.host_of(s.res_sig), *h_lab = st.host_of(s.lab_sig), *h_fd = st.host_of(s.free_dims), *h_fl = st.host_of(s.flags);
+  int64_t* h_cap = st.host_of(s.cap);
   const int32_t *ls_off = e->host_tab<int32_t>(TAB_ls_off), *ls_key = e->host_tab<int32_t>(TAB_ls_key),
                 *ls_val = e->host_tab<int32_t>(TAB_ls_val);
   std::unordered_map<std::string, int32_t> lab_id;
@@ -1442,40 +1437,26 @@ static int do_similar(Engine* e, const cae_similarity_inputs* in, uint32_t* bits
     h_fl[t] = (in->eligible[t] ? 1 : 0) | (!in->safe || in->safe[t] ? 2 : 0);
     h_cap[t] = std::max<int64_t>((int64_t)in->max_size[t] - in->target_size[t], 0);
   }
-  CAE_CUDA(cudaMemcpyAsync(d, h, in_end, cudaMemcpyHostToDevice, e->stream));
-  CAE_CUDA(cudaEventRecord(e->sim_stage.ev, e->stream));
-  CAE_CUDA(cudaMemsetAsync(d + o_status, 0, 8 + (size_t)12 * T, e->stream));
-  SimLaunch s{};
+  if (stage_upload(e, st, in_end)) return -1;
+  CAE_CUDA(cudaMemsetAsync(s.status, 0, o_bits - in_end, e->stream));   // status, sum, count
   s.ratio[0] = in->max_allocatable_difference_ratio;
   s.ratio[1] = in->max_free_difference_ratio;
   s.ratio[2] = in->max_capacity_memory_difference_ratio;
-  s.res_sig = reinterpret_cast<const int32_t*>(d + o_i32);
-  s.lab_sig = s.res_sig + T;
-  s.free_dims = s.res_sig + 2 * T;
-  s.flags = reinterpret_cast<int32_t*>(d + o_i32) + 3 * T;
-  s.cap = reinterpret_cast<const int64_t*>(d + o_cap);
-  s.status = reinterpret_cast<int32_t*>(d + o_status);
-  s.sum = reinterpret_cast<unsigned long long*>(d + o_status + 8);
-  s.count = reinterpret_cast<int32_t*>(d + o_status + 8 + (size_t)8 * T);
-  s.bits = reinterpret_cast<uint32_t*>(d + o_bits);
-  s.x = reinterpret_cast<double*>(d + o_x);
-  s.sched = reinterpret_cast<uint32_t*>(d + o_sched);
   if (launch_similar(e, s)) return -1;
-  const size_t d2h = (bits_out ? out_end : o_bits) - o_status;
-  CAE_CUDA(cudaMemcpyAsync(h + o_status, d + o_status, d2h, cudaMemcpyDeviceToHost, e->stream));
+  const size_t d2h = (bits_out ? out_end : o_bits) - in_end;
+  CAE_CUDA(cudaMemcpyAsync(st.host_of(s.status), s.status, d2h, cudaMemcpyDeviceToHost, e->stream));
   CAE_CUDA(cudaStreamSynchronize(e->stream));
-  e->stats.h2d_bytes = (int64_t)in_end;
   e->stats.d2h_bytes = (int64_t)d2h;
-  if (*reinterpret_cast<const int32_t*>(h + o_status)) {
+  if (*st.host_of(s.status)) {
     set_error("cae_similar_node_groups: a quantity past INT64_MAX / 1000 has no exact milli value: use the stock path");
     return 1;
   }
-  const int64_t* sum = reinterpret_cast<const int64_t*>(h + o_status + 8);
-  if (count_out) memcpy(count_out, h + o_status + 8 + (size_t)8 * T, (size_t)4 * T);
-  if (bits_out) memcpy(bits_out, h + o_bits, (size_t)4 * T * Tw);
+  const unsigned long long* sum = st.host_of(s.sum);
+  if (count_out) std::copy(st.host_of(s.count), st.host_of(s.count) + T, count_out);
+  if (bits_out) std::copy(st.host_of(s.bits), st.host_of(s.bits) + (size_t)T * Tw, bits_out);
   if (limit_out)
     for (int t = 0; t < T; ++t) {
-      const int64_t total = h_cap[t] + sum[t];
+      const int64_t total = h_cap[t] + (int64_t)sum[t];
       limit_out[t] = total <= 0 ? -1 : total;
     }
   return 0;
@@ -1557,25 +1538,6 @@ static int sim_class_check(const char* who, const int32_t* sim_class, const int3
     for (int i = 0; i < P; ++i)
       if (sim_class[i] < min_class || sim_class[i] >= n_classes) { cae::set_error(std::string(who) + ": similarity class out of range"); return -2; }
   return nctrl;
-}
-// Offsets, in int32 words, of the arrays of one device blob; byte arrays take whole words
-struct WordBlob {
-  size_t words = 0;
-  size_t add_words(size_t n) { const size_t o = words; words += n; return o; }
-  size_t add_bytes(size_t n) { return add_words((n + 3) / 4); }
-};
-// The device blob of `words` words and the pinned staging of its first `in_words` (the inputs), free for the host to fill:
-// pinned_reserve waits for the previous call's copy out of the staging, fm_blob_upload records the event it waits on.
-static int fm_blob_begin(Engine* e, size_t words, size_t in_words, int32_t** blob, int32_t** stage) {
-  if (cae::devbuf_reserve(e, e->fm_blob, words * 4) || cae::pinned_reserve(e, e->fm_stage, in_words * 4)) return -1;
-  *blob = static_cast<int32_t*>(e->fm_blob.p);
-  *stage = static_cast<int32_t*>(e->fm_stage.p);
-  return 0;
-}
-static int fm_blob_upload(Engine* e, size_t in_words) {
-  CAE_CUDA(cudaMemcpyAsync(e->fm_blob.p, e->fm_stage.p, in_words * 4, cudaMemcpyHostToDevice, e->stream));
-  CAE_CUDA(cudaEventRecord(e->fm_stage.ev, e->stream));
-  return 0;
 }
 // After the launch between ev0 and ev1: the kernel's n_out result words (d_out NULL: nothing ran) and the status word
 // (non-zero: placement log overflow) to the host, the stream drained, estimate_ms taken.
@@ -1988,42 +1950,42 @@ int32_t cae_filter_schedulable(cae_engine* h, const int32_t* pod_order, int32_t 
   if (!sim_class) n_classes = 0;
   const int nctrl = sim_class_check("cae_filter_schedulable", sim_class, class_ctrl, n_classes, P, INT_MIN);
   if (nctrl < 0) return -2;
-  // one blob: run_off | pods | hint | class | class_ctrl | node_ok (bytes), then assigned | out[4] | ctrl_cnt | class_mark,
-  // ctrl_over (bytes)
-  WordBlob wb;
-  const size_t o_run = wb.add_words(runs + 1), o_pods = wb.add_words(std::max(n_pods, 1));
-  const size_t o_hint = wb.add_words(hint_node ? P : 0), o_cls = wb.add_words(sim_class ? P : 0);
-  const size_t o_cc = wb.add_words(std::max(n_classes, 1)), o_nodeok = wb.add_bytes(node_ok ? N : 0);
-  const size_t in_words = wb.words;
-  const size_t o_asg = wb.add_words(std::max(P, 1)), o_out = wb.add_words(4), o_cnt = wb.add_words(std::max(nctrl, 1));
-  const size_t o_mark = wb.add_bytes(std::max(n_classes, 1)), o_over = wb.add_bytes(std::max(nctrl, 1));
-  int32_t *blob, *hb;
-  if (fm_blob_begin(e, wb.words, in_words, &blob, &hb)) return -1;
-  std::copy(run_off.begin(), run_off.end(), hb + o_run);
-  if (n_pods) std::copy(pod_order, pod_order + n_pods, hb + o_pods);
-  if (hint_node) std::copy(hint_node, hint_node + P, hb + o_hint);
-  if (sim_class) std::copy(sim_class, sim_class + P, hb + o_cls);
-  if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, hb + o_cc);
-  if (node_ok && N) memcpy(hb + o_nodeok, node_ok, N);
-  if (fm_blob_upload(e, in_words)) return -1;
-  CAE_CUDA(cudaMemsetAsync(blob + o_asg, 0xFF, (size_t)std::max(P, 1) * 4, e->stream));   // -1 = stays unschedulable
-  CAE_CUDA(cudaMemsetAsync(blob + o_out, 0, (wb.words - o_out) * 4, e->stream));
+  e->stats.h2d_bytes = 0;
+  // one staged blob: run_off | pods | hint | class | class_ctrl | node_ok, then the outputs assigned | out[4] | ctrl_cnt |
+  // class_mark | ctrl_over (device only); an absent hint, class or node_ok array stays NULL
+  Engine::Staging& st = e->fm;
   cae::FilterLaunch f{};
   f.runs = runs; f.n_pods = n_pods; f.last_index = last_index_in; f.break_on_failure = break_on_failure ? 1 : 0; f.nctrl = nctrl;
-  f.run_off = blob + o_run; f.pods = blob + o_pods;
-  f.hint = hint_node ? blob + o_hint : nullptr;
-  f.cls = sim_class ? blob + o_cls : nullptr;
-  f.class_ctrl = blob + o_cc;
-  f.node_ok = node_ok ? reinterpret_cast<const uint8_t*>(blob + o_nodeok) : nullptr;
-  f.assigned = blob + o_asg; f.out = blob + o_out; f.ctrl_cnt = blob + o_cnt;
-  f.class_mark = reinterpret_cast<uint8_t*>(blob + o_mark);
-  f.ctrl_over = reinterpret_cast<uint8_t*>(blob + o_over);
+  size_t in_end = 0, o_out = 0;
+  auto walk = [&](cae::Layout& l) {
+    l.add(f.run_off, runs + 1); l.add(f.pods, std::max(n_pods, 1));
+    if (hint_node) l.add(f.hint, P);
+    if (sim_class) l.add(f.cls, P);
+    l.add(f.class_ctrl, std::max(n_classes, 1));
+    if (node_ok) l.add(f.node_ok, N);
+    in_end = l.bytes;
+    l.add(f.assigned, std::max(P, 1));
+    o_out = l.bytes;
+    l.add(f.out, 4); l.add(f.ctrl_cnt, std::max(nctrl, 1)); l.add(f.class_mark, std::max(n_classes, 1)); l.add(f.ctrl_over, std::max(nctrl, 1));
+  };
+  const size_t bytes = cae::layout_bytes(walk);
+  if (cae::stage_reserve(e, st, bytes, in_end)) return -1;
+  cae::layout_bind(st.dev.p, walk);
+  std::copy(run_off.begin(), run_off.end(), st.host_of(f.run_off));
+  std::copy(pod_order, pod_order + n_pods, st.host_of(f.pods));
+  if (hint_node) std::copy(hint_node, hint_node + P, st.host_of(f.hint));
+  if (sim_class) std::copy(sim_class, sim_class + P, st.host_of(f.cls));
+  if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, st.host_of(f.class_ctrl));
+  if (node_ok) std::copy(node_ok, node_ok + N, st.host_of(f.node_ok));
+  if (cae::stage_upload(e, st, in_end)) return -1;
+  CAE_CUDA(cudaMemsetAsync(f.assigned, 0xFF, (size_t)std::max(P, 1) * 4, e->stream));   // -1 = stays unschedulable
+  CAE_CUDA(cudaMemsetAsync(f.out, 0, bytes - o_out, e->stream));
   cudaEventRecord(e->ev0, e->stream);
   if (runs > 0 && cae::launch_filter(e, f)) return -1;
   cudaEventRecord(e->ev1, e->stream);
   int32_t out[4] = {last_index_raw, 0, 0, 0}, status = 0;
-  if (P) CAE_CUDA(cudaMemcpyAsync(assigned_node, blob + o_asg, (size_t)P * 4, cudaMemcpyDeviceToHost, e->stream));
-  if (fm_finish(e, runs > 0 ? blob + o_out : nullptr, out, 4, &status)) return -1;
+  if (P) CAE_CUDA(cudaMemcpyAsync(assigned_node, f.assigned, (size_t)P * 4, cudaMemcpyDeviceToHost, e->stream));
+  if (fm_finish(e, runs > 0 ? f.out : nullptr, out, 4, &status)) return -1;
   if (status) { cae::set_error("placement log overflow in the filter pass"); return 1; }
   if (last_index_out) *last_index_out = out[3] ? out[0] : last_index_raw;
   if (overflowing_controllers) *overflowing_controllers = out[1];
@@ -2074,44 +2036,46 @@ int32_t cae_simulate_removals(cae_engine* h, int32_t n_cand, const int32_t* cand
       if (hint_node[i] < -1 || hint_node[i] >= N) { cae::set_error("cae_simulate_removals: hinted row out of range"); return -2; }
   const int nctrl = sim_class_check("cae_simulate_removals", sim_class, class_ctrl, n_classes, P, -1);
   if (nctrl < 0) return -2;
+  e->stats.h2d_bytes = 0;
   if (n_cand == 0) { *last_index_out = last_index_in; *log_len = 0; return 0; }
   cudaSetDevice(e->cfg.device);
-  // one blob: cand | move_off | move_pod | hint | class | class_ctrl | dest_ok (bytes), then result | out[2] | log
-  WordBlob wb;
-  const size_t o_cand = wb.add_words(n_cand), o_moff = wb.add_words(n_cand + 1), o_mpod = wb.add_words(std::max(M, 1));
-  const size_t o_hint = wb.add_words(hint_node ? P : 0), o_cls = wb.add_words(sim_class ? P : 0);
-  const size_t o_cc = wb.add_words(std::max(n_classes, 1)), o_dest = wb.add_bytes(dest_ok ? N : 0);
-  const size_t in_words = wb.words;
-  const size_t o_res = wb.add_words(n_cand), o_out = wb.add_words(2), o_log = wb.add_words((size_t)std::max(log_cap, 1) * 3);
-  int32_t *blob, *hb;
-  if (fm_blob_begin(e, wb.words, in_words, &blob, &hb)) return -1;
-  std::copy(cand_node, cand_node + n_cand, hb + o_cand);
-  std::copy(move_off, move_off + n_cand + 1, hb + o_moff);
-  if (M) std::copy(move_pod, move_pod + M, hb + o_mpod);
-  if (hint_node) std::copy(hint_node, hint_node + P, hb + o_hint);
-  if (sim_class) std::copy(sim_class, sim_class + P, hb + o_cls);
-  if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, hb + o_cc);
-  if (dest_ok && N) memcpy(hb + o_dest, dest_ok, N);
-  if (fm_blob_upload(e, in_words)) return -1;
+  // one staged blob: cand | move_off | move_pod | hint | class | class_ctrl | dest_ok, then the outputs result | out[2] | log
+  // (device only); an absent hint, class or dest_ok array stays NULL
+  Engine::Staging& st = e->fm;
   cae::RemovalLaunch r{};
   r.ncand = n_cand; r.persist = persist ? 1 : 0; r.ncls = n_classes; r.nctrl = nctrl; r.log_cap = log_cap;
   r.last_index = last_index_in;
-  r.cand = blob + o_cand; r.move_off = blob + o_moff; r.move_pod = blob + o_mpod;
-  r.hint = hint_node ? blob + o_hint : nullptr;
-  r.cls = sim_class ? blob + o_cls : nullptr;
-  r.class_ctrl = blob + o_cc;
-  r.dest_ok = dest_ok ? reinterpret_cast<const uint8_t*>(blob + o_dest) : nullptr;
-  r.result = blob + o_res; r.out = blob + o_out; r.log = blob + o_log;
+  size_t in_end = 0;
+  auto walk = [&](cae::Layout& l) {
+    l.add(r.cand, n_cand); l.add(r.move_off, n_cand + 1); l.add(r.move_pod, std::max(M, 1));
+    if (hint_node) l.add(r.hint, P);
+    if (sim_class) l.add(r.cls, P);
+    l.add(r.class_ctrl, std::max(n_classes, 1));
+    if (dest_ok) l.add(r.dest_ok, N);
+    in_end = l.bytes;
+    l.add(r.result, n_cand); l.add(r.out, 2); l.add(r.log, (size_t)std::max(log_cap, 1) * 3);
+  };
+  const size_t bytes = cae::layout_bytes(walk);
+  if (cae::stage_reserve(e, st, bytes, in_end)) return -1;
+  cae::layout_bind(st.dev.p, walk);
+  std::copy(cand_node, cand_node + n_cand, st.host_of(r.cand));
+  std::copy(move_off, move_off + n_cand + 1, st.host_of(r.move_off));
+  if (M) std::copy(move_pod, move_pod + M, st.host_of(r.move_pod));
+  if (hint_node) std::copy(hint_node, hint_node + P, st.host_of(r.hint));
+  if (sim_class) std::copy(sim_class, sim_class + P, st.host_of(r.cls));
+  if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, st.host_of(r.class_ctrl));
+  if (dest_ok) std::copy(dest_ok, dest_ok + N, st.host_of(r.dest_ok));
+  if (cae::stage_upload(e, st, in_end)) return -1;
   cudaEventRecord(e->ev0, e->stream);
   if (cae::launch_removals(e, r)) return -1;
   cudaEventRecord(e->ev1, e->stream);
   int32_t out[2] = {0, 0}, status = 0;
-  if (fm_finish(e, blob + o_out, out, 2, &status)) return -1;
+  if (fm_finish(e, r.out, out, 2, &status)) return -1;
   if (status) { cae::set_error("placement log overflow in the removal batch"); return -1; }
   *log_len = out[1];
   if (out[1] > log_cap) { cae::set_error("cae_simulate_removals: the log needs more entries than log_cap"); return 1; }
-  CAE_CUDA(cudaMemcpyAsync(result, blob + o_res, sizeof(int32_t) * n_cand, cudaMemcpyDeviceToHost, e->stream));
-  if (out[1]) CAE_CUDA(cudaMemcpyAsync(log, blob + o_log, sizeof(int32_t) * 3 * (size_t)out[1], cudaMemcpyDeviceToHost, e->stream));
+  CAE_CUDA(cudaMemcpyAsync(result, r.result, sizeof(int32_t) * n_cand, cudaMemcpyDeviceToHost, e->stream));
+  if (out[1]) CAE_CUDA(cudaMemcpyAsync(log, r.log, sizeof(int32_t) * 3 * (size_t)out[1], cudaMemcpyDeviceToHost, e->stream));
   CAE_CUDA(cudaStreamSynchronize(e->stream));
   *last_index_out = out[0];
   return 0;

@@ -1866,29 +1866,19 @@ int launch_removals(Engine* e, const RemovalLaunch& rl) {
   r.cand = rl.cand; r.move_off = rl.move_off; r.move_pod = rl.move_pod; r.dest_ok = rl.dest_ok;
   r.result = rl.result; r.log = rl.log; r.out = rl.out;
   r.grs = group_rec_src(e);
-  // batch state, one buffer, every array 256-byte aligned: walked once for the size, once more to bind the pointers
-  unsigned char* b = nullptr;
-  size_t off = 0;
-  auto carve = [&](auto*& ptr, size_t count) {
-    using T = std::remove_reference_t<decltype(*ptr)>;
-    if (b) ptr = reinterpret_cast<T*>(b + off);
-    off += (count * sizeof(T) + 255) & ~(size_t)255;
+  // batch state, one buffer
+  auto walk = [&](Layout& l) {
+    l.add(r.cfree, A1 * N); l.add(r.cslots, N); l.add(r.cports, N);
+    l.add(r.live, N); l.add(r.live_w, N); l.add(p.fm_node_ok, N); l.add(r.rank, N);
+    l.add(r.ccnt, pool); l.add(r.cpres, pool); l.add(r.wcnt, pool); l.add(r.wpres, pool);
+    l.add(r.ctot, Q); l.add(r.wtot, Q); l.add(r.stat, 3 * Q);
+    l.add(r.hint, P); l.add(p.fm_hint, P); l.add(p.fm_assigned, P); l.add(p.fm_pods, P);
+    l.add(r.head, N); l.add(r.tail, N); l.add(r.next, P); l.add(r.run_off, P + 1);
+    l.add(p.grec, P);
+    l.add(p.fm_class_mark, ncls); l.add(p.fm_ctrl_cnt, nctrl); l.add(p.fm_ctrl_over, nctrl);
   };
-  for (int pass = 0; pass < 2; ++pass) {
-    off = 0;
-    carve(r.cfree, A1 * N); carve(r.cslots, N); carve(r.cports, N);
-    carve(r.live, N); carve(r.live_w, N); carve(p.fm_node_ok, N); carve(r.rank, N);
-    carve(r.ccnt, pool); carve(r.cpres, pool); carve(r.wcnt, pool); carve(r.wpres, pool);
-    carve(r.ctot, Q); carve(r.wtot, Q); carve(r.stat, 3 * Q);
-    carve(r.hint, P); carve(p.fm_hint, P); carve(p.fm_assigned, P); carve(p.fm_pods, P);
-    carve(r.head, N); carve(r.tail, N); carve(r.next, P); carve(r.run_off, P + 1);
-    carve(p.grec, P);
-    carve(p.fm_class_mark, ncls); carve(p.fm_ctrl_cnt, nctrl); carve(p.fm_ctrl_over, nctrl);
-    if (pass == 0) {
-      if (devbuf_reserve(e, e->rm_state, off)) return -1;
-      b = static_cast<unsigned char*>(e->rm_state.p);
-    }
-  }
+  if (devbuf_reserve(e, e->rm_state, layout_bytes(walk))) return -1;
+  layout_bind(e->rm_state.p, walk);
   if (rl.hint) CAE_CUDA(cudaMemcpyAsync(r.hint, rl.hint, sizeof(int32_t) * e->P, cudaMemcpyDeviceToDevice, e->stream));
   else CAE_CUDA(cudaMemsetAsync(r.hint, 0xFF, sizeof(int32_t) * P, e->stream));
   // one placement log entry per pod of a candidate at most

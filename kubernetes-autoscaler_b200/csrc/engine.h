@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <climits>
+#include <cstddef>
 #include <cstdint>
 #include <string>
 #include <vector>
@@ -271,11 +272,21 @@ struct Engine {
     PinnedBuf& operator=(const PinnedBuf&) = delete;
     ~PinnedBuf() { if (p) cudaFreeHost(p); if (ev) cudaEventDestroy(ev); }
   };
+  // The device blob of one call and the pinned copy of its first bytes (the inputs, and the outputs a call copies back) at
+  // the same offsets (stage_reserve / stage_upload in api.cu).  One per kind of call: a call waits only for the copy out
+  // of its own staging.
+  struct Staging {
+    PinnedBuf host;
+    DevBuf dev;
+    template <class T>
+    T* host_of(const T* d) const {        // the host copy of device array d
+      return reinterpret_cast<T*>(static_cast<char*>(host.p) + (reinterpret_cast<const char*>(d) - static_cast<const char*>(dev.p)));
+    }
+  };
   struct Slab { DevBuf buf; size_t sig = 0, zeroed = 0; };   // estimator slab: layout signature, bytes zeroed under it
   Slab pack_slab, fm_slab;                // estimator / filter-out-schedulable pass (binpack.cu)
-  DevBuf fm_blob;                         // inputs and outputs of the filter pass / the scale-down batch
+  Staging fm;                             // inputs, then outputs of the filter pass / the scale-down batch
   DevBuf rm_state;                        // scale-down batch state (RemovalState)
-  PinnedBuf fm_stage;                     // host staging of the inputs of the filter pass / the scale-down batch
   std::vector<int32_t> rm_owner, rm_seen; // [P] argument checks of the scale-down batch (kept to avoid per-call allocation)
   DevBuf x_rows;                          // caller-supplied option rows: node_count | sched | order
   DevBuf x_price;                         // price inputs: node_price | pod_price | unfitness | score, then has_gpu | exists
@@ -312,20 +323,18 @@ struct Engine {
     std::vector<int32_t> dom_scratch;              // value id -> domain while the domains are assigned (all -1 in between)
     std::vector<int32_t> tmpl_ls;                  // [T] label set of each template (no delta changes a template)
   } nh;
-  PinnedBuf pd_stage;                     // cae_load_pods' tails, source of its one H2D copy
-  DevBuf pd_blob;                         // device copy of the tails
+  Staging pd;                             // cae_load_pods' tails
   DevBuf pd_used;                         // [S] specs of the resident pods (pod_delta.cu)
   // buffers of cae_load_nodes (a cae_load points DevObjects back at its arena)
   DevBuf nd_off[2], nd_spec[2];           // double-buffered resident CSR (node_pod_off / node_pod_spec)
-  DevBuf nd_cnt, nd_didx, nd_cub, nd_blob;  // per-row counts / source rows, scan temp storage, device copy of the delta
-  PinnedBuf nd_stage;                     // the delta, source of its one H2D copy
+  DevBuf nd_cnt, nd_didx, nd_cub;         // per-row counts / source rows, scan temp storage
+  Staging nd;                             // the delta, churn or force-add arrivals
   // buffers of cae_load_node_churn: the tables whose size follows the node count, until the next cae_load
   DevBuf ch_nodes[2];                     // double-buffered node columns [N+T] + c_free [A][N] + c_slots [N] (node_delta.cu)
   DevBuf ch_pre;                          // pre_code [SC][U]
   DevBuf ch_dyn;                          // dom [K][N+T] | q_base_off [Q+1] | base_cnt, base_pres [pool] | elig [Q][U]
   // buffers of cae_similar_node_groups (similar.cu)
-  DevBuf sim_dev;                         // inputs | outputs | operand rows | schedulable bit rows
-  PinnedBuf sim_stage;                    // inputs (one H2D copy) | outputs (one D2H copy)
+  Staging sim;                            // inputs | outputs (one D2H copy) | operand rows | schedulable bit rows (device only)
   int sm_count = 132;
   int smem_optin = 227 * 1024;             // opt-in shared memory per thread block
   size_t hbm_bytes = (size_t)80 << 30;     // device memory (sizes the estimator's global slabs)
@@ -334,6 +343,35 @@ struct Engine {
 // api.cu: growth of the engine-owned buffers; the contents are not kept
 int devbuf_reserve(Engine* e, Engine::DevBuf& b, size_t bytes);          // stream-ordered
 int pinned_reserve(Engine* e, Engine::PinnedBuf& b, size_t bytes);       // after the last copy out of b has finished
+// Before any host write: s.dev for the whole layout (`bytes`), s.host for the first `pinned` bytes
+int stage_reserve(Engine* e, Engine::Staging& s, size_t bytes, size_t pinned);
+// The one H2D copy of the first `in` bytes, the event the next stage_reserve waits on, and the bytes in stats.h2d_bytes
+int stage_upload(Engine* e, Engine::Staging& s, size_t in);
+
+// Typed arrays laid out in order in one buffer, each at a 256-byte boundary (the alignment of Arena::alloc); a
+// zero-length array takes no bytes.  A walk(Layout&) that calls add() for every array runs twice: layout_bytes sums the
+// sizes, layout_bind points each array into the buffer at `base`.
+struct Layout {
+  char* base = nullptr;                   // NULL: sizes only
+  size_t bytes = 0;                       // the end of the arrays added so far
+  template <class T>
+  void add(T*& p, size_t n) {
+    if (base) p = reinterpret_cast<T*>(base + bytes);
+    bytes += (n * sizeof(T) + 255) & ~(size_t)255;
+  }
+};
+template <class Walk>
+size_t layout_bytes(Walk&& walk) {
+  Layout l;
+  walk(l);
+  return l.bytes;
+}
+template <class Walk>
+void layout_bind(void* base, Walk&& walk) {
+  Layout l;
+  l.base = static_cast<char*>(base);
+  walk(l);
+}
 
 // kernels.cu
 int launch_class_matrix(Engine* e);      // pre_code[SC][U]: needs only the object tables + the static classes

@@ -75,33 +75,12 @@ __global__ void nd_gather_kernel(const int32_t* __restrict__ old_off, const int3
   for (int j = lane; j < n; j += 32) new_spec[b + j] = j < n_old ? old[j] : staged[j - n_old];
 }
 
-// Where the churn's node columns live: one engine-owned buffer per half, sub-arrays 256-byte aligned, node_name first
+// Where the churn's node columns live: one engine-owned buffer per half (launch_node_churn), node_name first
 struct NodeCols {
   int32_t *name, *labelset, *taint_list, *allowed, *c_slots;
   uint8_t *unsched, *has_cpu, *has_mem;
   int64_t *alloc, *cap_cpu, *cap_mem, *c_free;
 };
-static size_t node_cols_layout(int NT, int N, int A1, uintptr_t base, NodeCols* c) {   // base 0: sizes only
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    const size_t o = off;
-    off += (std::max<size_t>(bytes, 1) + 255) & ~(size_t)255;
-    return reinterpret_cast<unsigned char*>(base + o);
-  };
-  c->name = reinterpret_cast<int32_t*>(take(4 * (size_t)NT));
-  c->labelset = reinterpret_cast<int32_t*>(take(4 * (size_t)NT));
-  c->taint_list = reinterpret_cast<int32_t*>(take(4 * (size_t)NT));
-  c->allowed = reinterpret_cast<int32_t*>(take(4 * (size_t)NT));
-  c->unsched = take(NT);
-  c->has_cpu = take(NT);
-  c->has_mem = take(NT);
-  c->alloc = reinterpret_cast<int64_t*>(take(8 * (size_t)NT * R));
-  c->cap_cpu = reinterpret_cast<int64_t*>(take(8 * (size_t)NT));
-  c->cap_mem = reinterpret_cast<int64_t*>(take(8 * (size_t)NT));
-  c->c_free = reinterpret_cast<int64_t*>(take(8 * (size_t)A1 * std::max(N, 1)));
-  c->c_slots = reinterpret_cast<int32_t*>(take(4 * (size_t)std::max(N, 1)));
-  return off;
-}
 
 // one thread per new row: every node column, the run state of a cluster row and the resident count, from the row's source.
 // An added node has no capacity / has_alloc_* (read for templates only); a dirty row keeps those of its old row.
@@ -188,9 +167,14 @@ int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int 
   const int NT = N + e->T, A1 = std::max(e->A, 1);
   const int tgt = e->dobj.node_name == e->ch_nodes[0].p ? 1 : 0;   // the half the node columns are NOT in (or the arena's)
   NodeCols c{};
-  const size_t bytes = node_cols_layout(NT, N, A1, 0, &c);
-  if (devbuf_reserve(e, e->ch_nodes[tgt], bytes)) return -1;
-  node_cols_layout(NT, N, A1, reinterpret_cast<uintptr_t>(e->ch_nodes[tgt].p), &c);
+  auto walk = [&](Layout& l) {
+    l.add(c.name, NT); l.add(c.labelset, NT); l.add(c.taint_list, NT); l.add(c.allowed, NT);
+    l.add(c.unsched, NT); l.add(c.has_cpu, NT); l.add(c.has_mem, NT);
+    l.add(c.alloc, (size_t)NT * R); l.add(c.cap_cpu, NT); l.add(c.cap_mem, NT);
+    l.add(c.c_free, (size_t)A1 * std::max(N, 1)); l.add(c.c_slots, std::max(N, 1));
+  };
+  if (devbuf_reserve(e, e->ch_nodes[tgt], layout_bytes(walk))) return -1;
+  layout_bind(e->ch_nodes[tgt].p, walk);
   int32_t *new_off = nullptr, *new_spec = nullptr;
   if (spare_csr(e, NT, total, &new_off, &new_spec) || devbuf_reserve(e, e->nd_cnt, sizeof(int32_t) * ((size_t)NT + 1)))
     return -1;
