@@ -315,8 +315,8 @@ int32_t cae_load_pending(cae_engine* e, int32_t num_pending, const int32_t* pend
  *     resident) at the last cae_load — it could add an existing-anti-affinity counter;
  *   - the resident pods of all nodes, or the entries of a dictionary table, would pass 2^31 - 1 (checked from the counts
  *     and offsets alone, before any pod-spec id is read).
- * Adding or removing nodes: cae_load_node_churn.  New pod specs: cae_load_pods first.  Template changes cannot be
- * expressed: cae_load.
+ * Adding or removing nodes: cae_load_node_churn.  New pod specs: cae_load_pods first.  Template changes:
+ * cae_load_templates.
  * The interner is append-only across deltas: hostname_key and unschedulable_taint_key stay those of the last cae_load (a
  * caller that needs them to change does a full load). */
 typedef struct cae_node_delta {
@@ -386,6 +386,52 @@ typedef struct cae_node_churn {
 } cae_node_churn;
 int32_t cae_load_node_churn(cae_engine* e, const cae_node_churn* c);
 
+/* The per-tick delta of the node-group TEMPLATES: templates removed (a node group went away), changed (a DaemonSet rolled
+ * out, the template-from-real-node provider picked another sample node) and added (a new node group), against the
+ * snapshot that is already resident.  Replaces: the TemplateNodeInfoProvider refresh between two loops, which the other
+ * deltas cannot express.  A template's identity is its node group, not its node name, so a changed row carries its name.
+ * The new template list is the surviving templates in their old order (changed ones in place), then the added ones in the
+ * given order: template t' is row N + t', its sanitized copy universe column N + T' + t'.  Every template index the caller
+ * holds (max_nodes, similarity inputs, price inputs, expander rows) refers to the new list after the call.  After the call
+ * every entry point answers bit-identically to a cae_load of the objects with the new template rows.  Cluster rows and
+ * pending pods are not touched; the call combines with cae_load_pending, cae_load_nodes, cae_load_node_churn,
+ * cae_load_pods and cae_force_add_pods in any order.  At world_size > 1 every rank applies the same delta (the template
+ * shard bounds are re-derived; presharded pods are unaffected).  T' = 0 and growing from T = 0 are valid.  Every check runs
+ * on the host before any device write; a refused call changes nothing.
+ * Status -2 (malformed): before cae_load; every cause of cae_load_nodes on `tails` (whose num_dirty must be 0); removed or
+ *   changed indices out of range or not strictly increasing, or a changed index also removed; NULL arrays with non-zero
+ *   counts; ids outside the resident tables plus the tails (a name id must be >= 0); pod offsets that do not start at 0 or
+ *   decrease; a pod-spec id out of range.
+ * Status 1 (nothing changed): more templates than the fused histogram exchange holds (65536) while peers are attached
+ *   (cae_peer_attach), which the dense pass could not exchange: use the stock path.
+ * Status 2 (nothing changed: call cae_load): a template pod's spec has required anti-affinity terms and no pod of that
+ *   spec was in the snapshot; a non-zero allocatable at a dim at or past the load's num_res; the rows and template copies
+ *   (N + 2T'), the resident pods of all rows, or the entries of a dictionary table would pass 2^31 - 1 (checked from the
+ *   counts and offsets alone). */
+typedef struct cae_template_delta {
+  int32_t abi_version;           /* CAE_ABI_VERSION */
+  const cae_node_delta* tails;   /* the value, label-set and taint-list tails the new rows use (num_dirty == 0); NULL = none */
+  int32_t num_removed;
+  const int32_t* removed;        /* template indices before the call, strictly increasing */
+  int32_t num_changed;
+  const int32_t* changed;        /* template indices before the call, strictly increasing, none of them also removed */
+  int32_t num_added;             /* new templates, appended after the surviving ones in this order */
+  /* rows: the changed templates (in `changed` order), then the added ones; every column has its cae_objects meaning */
+  const int32_t* name;
+  const int32_t* labelset;
+  const int32_t* taint_list;
+  const uint8_t* unschedulable;
+  const int64_t* alloc;          /* [(num_changed + num_added) * CAE_MAX_RES] */
+  const int32_t* allowed_pods;
+  const int64_t* cap_cpu;
+  const int64_t* cap_mem;
+  const uint8_t* has_alloc_cpu;
+  const uint8_t* has_alloc_mem;
+  const int32_t* pod_off;        /* [num_changed + num_added + 1] */
+  const int32_t* pod_spec;       /* DaemonSet and mirror pods: spec ids of the resident table */
+} cae_template_delta;
+int32_t cae_load_templates(cae_engine* e, const cae_template_delta* d);
+
 /* The per-tick delta of the pod specs: new pod specs (a new Deployment, a rollout, a Job) and the complete new pending list
  * against the snapshot that is already resident.  The dictionary entries the new specs need arrive as TAILS that continue
  * the resident tables (ids [resident count, resident count + n)); the offsets of a tail start at 0 and index that
@@ -409,7 +455,7 @@ int32_t cae_load_node_churn(cae_engine* e, const cae_node_churn* c);
  * Status 2 (nothing changed): a table would pass 2^31 - 1 entries (checked from the counts and offsets alone), or a new
  *   spec requests a dim at or past the load's num_res (a new resource dimension): cae_load.
  * Node-name ids (ps_node_name, field_node_name) are an open id space, as in cae_objects: only -1 / >= 0 is checked.
- * Template changes and label changes of an existing Namespace: cae_load. */
+ * Template changes: cae_load_templates.  Label changes of an existing Namespace: cae_load. */
 typedef struct cae_pod_delta {
   int32_t abi_version; /* CAE_ABI_VERSION */
   int32_t num_new_values;

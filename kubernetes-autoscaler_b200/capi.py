@@ -100,6 +100,10 @@ class cae_node_churn(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_node_churn", {"cae_node_delta": cae_node_delta})
 
 
+class cae_template_delta(C.Structure):
+    _fields_ = _parse_struct(_SRC, "cae_template_delta", {"cae_node_delta": cae_node_delta})
+
+
 class cae_pod_delta(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_pod_delta")
 
@@ -161,6 +165,8 @@ def load_engine_lib() -> C.CDLL:
     lib.cae_load_nodes.restype = C.c_int32
     lib.cae_load_node_churn.argtypes = [C.c_void_p, P(cae_node_churn)]
     lib.cae_load_node_churn.restype = C.c_int32
+    lib.cae_load_templates.argtypes = [C.c_void_p, P(cae_template_delta)]
+    lib.cae_load_templates.restype = C.c_int32
     lib.cae_load_pods.argtypes = [C.c_void_p, P(cae_pod_delta)]
     lib.cae_load_pods.restype = C.c_int32
     lib.cae_force_add_pods.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]

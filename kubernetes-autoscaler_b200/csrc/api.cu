@@ -167,9 +167,6 @@ struct PendPlan {
   int A = 0, W = 0, act_dim[CAE_MAX_RES] = {0};   // rank encoding
   int f_word[CAE_MAX_RES] = {0}, f_shift[CAE_MAX_RES] = {0}, f_bits[CAE_MAX_RES] = {0};
   std::vector<std::vector<int64_t>> rvals;
-  RankArgs ra{};                                  // the device half (pod_delta.cu)
-  const int64_t* d_rvals = nullptr;
-  uint32_t* d_tmpl_w = nullptr;
 };
 
 // Interning for the pod-state dependent plugins (dyn.cuh): topology keys -> compact ids, label values
@@ -485,7 +482,8 @@ static int plan_ranks(const cae_objects* o, PendPlan& pl) {
 }
 
 // The rank fields of the specs, the layout of the template rank fields and threshold bitmaps, and the device buffers of
-// the free capacity over the active dims; launch_rank_tables (pod_delta.cu) fills the per-row tables after the flush
+// the free capacity over the active dims, and the engine's RankArgs (the device half, pod_delta.cu) with the distinct
+// requests it reads; launch_rank_tables fills the per-row tables after the flush
 static int apply_ranks(Engine* e, const cae_objects* o, PendPlan& pl) {
   const int S = o->num_podspecs, N = e->N, T = e->T;
   e->A = pl.A;
@@ -525,7 +523,7 @@ static int apply_ranks(Engine* e, const cae_objects* o, PendPlan& pl) {
     e->lut_shift[a] = (uint8_t)f_shift[a];
     e->lut_mask[a] = (1u << (f_bits[a] - 1)) - 1u;
   }
-  RankArgs& ra = pl.ra;
+  RankArgs& ra = e->ra;
   ra = RankArgs{};
   ra.A = e->A; ra.N = N; ra.T = T; ra.Tw = e->Tw; ra.Twp = e->Twp; ra.W = e->W; ra.lut_rows = e->lut_rows; ra.feas_B = e->feas_B;
   ra.Bpad = std::max(4, (e->feas_B + 3) / 4 * 4);
@@ -544,8 +542,8 @@ static int apply_ranks(Engine* e, const cae_objects* o, PendPlan& pl) {
     return -1;
   const int64_t* d_rv = nullptr;
   if (upload(e->pup, rv.data(), rv.size(), &d_rv)) return -1;
-  pl.d_rvals = d_rv;
-  if (dev_alloc(e, &pl.d_tmpl_w, (size_t)std::max(e->W, 1) * std::max(T, 1)) ||
+  e->d_rvals = d_rv;
+  if (dev_alloc(e, &e->d_tmpl_w, (size_t)std::max(e->W, 1) * std::max(T, 1)) ||
       dev_alloc(e, &e->d_rlut, (size_t)std::max(e->lut_rows, 1) * std::max(e->Twp, 1)) ||
       dev_alloc(e, &e->d_tmpl_free, (size_t)A1 * T) || dev_alloc(e, &e->d_c_free, (size_t)A1 * std::max(N, 1)))
     return -1;
@@ -611,7 +609,7 @@ static int derive_pending(Engine* e, const cae_objects* o, LoadTimer& lt, const 
 
   lt.mark("dev_alloc+memsets");
   if (e->pup.flush(e->stream, &e->stats.h2d_bytes)) return -1;   // ONE pinned H2D copy per arena chunk
-  if (launch_rank_tables(e, pl.ra, pl.d_rvals, pl.d_tmpl_w)) return -1;
+  if (launch_rank_tables(e, e->ra, e->d_rvals, e->d_tmpl_w)) return -1;
   if (launch_pre_ok_bits(e)) return -1;
   if (e->has_dynamic) {
     if (launch_dynamic_tables(e, e->d_spec_used, e->d_dc_ngroups)) return -1;
@@ -848,6 +846,17 @@ static void take_back_mirrors(Engine* e) {
     if (kDict[t].host) e->dict_host[t].resize(table_len(e->dict_cnt, t) * kDict[t].esz);
 }
 
+// The sizes that follow from the template count: universe columns, template words and their pitch, this rank's template shard
+static void set_template_count(Engine* e, int T) {
+  e->T = T;
+  e->U = e->N + 2 * T;
+  e->Tw = (T + 31) / 32;
+  e->Twp = (e->Tw + FEAS_TW - 1) / FEAS_TW * FEAS_TW;
+  const int W = std::max(1, e->cfg.world_size), rk = e->cfg.rank;
+  e->t_begin = (int)((int64_t)T * rk / W);
+  e->t_end = (int)((int64_t)T * (rk + 1) / W);
+}
+
 static int do_load(Engine* e, const cae_objects* o) {
   LoadTimer lt;
   if (o->abi_version != CAE_ABI_VERSION) { set_error("cae_objects.abi_version mismatch"); return -2; }
@@ -857,12 +866,8 @@ static int do_load(Engine* e, const cae_objects* o) {
   e->group_reason_valid = false;
   e->stats.h2d_bytes = 0;
   const int N = o->num_cluster_nodes, T = o->num_templates, NT = N + T;
-  e->N = N; e->T = T; e->U = N + 2 * T;
-  e->Tw = (T + 31) / 32;
-  e->Twp = (e->Tw + FEAS_TW - 1) / FEAS_TW * FEAS_TW;
-  const int W = std::max(1, e->cfg.world_size), rk = e->cfg.rank;
-  e->t_begin = (int)((int64_t)T * rk / W);
-  e->t_end = (int)((int64_t)T * (rk + 1) / W);
+  e->N = N;
+  set_template_count(e, T);
 
   cudaEventRecord(e->ev0, e->stream);
   DevObjects& d = e->dobj;
@@ -889,6 +894,9 @@ static int do_load(Engine* e, const cae_objects* o) {
   const int S = o->num_podspecs;
   std::vector<int64_t> free_all((size_t)R * T);
   std::vector<int32_t> slots(T), cslots(std::max(N, 1));
+  Engine::NodeHost& nh = e->nh;   // the template mirrors cae_load_templates continues from
+  nh.tmpl_pods.resize(T);
+  nh.tmpl_free.resize((size_t)T * R);
   for (int row = 0; row < NT; ++row) {
     const int npods = o->node_pod_off[row + 1] - o->node_pod_off[row];
     if (row < N) {
@@ -898,14 +906,15 @@ static int do_load(Engine* e, const cae_objects* o) {
     int64_t reqd[R];
     resident_req(o->ps_req, o->node_pod_spec + o->node_pod_off[row], npods, reqd);
     const int t = row - N;
-    for (int r = 0; r < R; ++r) free_all[(size_t)r * T + t] = o->node_alloc[(size_t)row * R + r] - reqd[r];
+    for (int r = 0; r < R; ++r) free_all[(size_t)r * T + t] = nh.tmpl_free[(size_t)t * R + r] = o->node_alloc[(size_t)row * R + r] - reqd[r];
     slots[t] = o->node_allowed_pods[row] - npods;
+    nh.tmpl_pods[t] = npods;
   }
+  nh.tmpl_slots = slots;
   if (upload_mut(e->up, slots, &e->d_tmpl_slots) || upload_mut(e->up, free_all, &e->d_tmpl_free_all) || upload_mut(e->up, cslots, &e->d_c_slots))
     return -1;
   // host state the per-tick deltas validate against and update (cae_load_pending, cae_load_nodes, cae_load_pods)
-  {
-    Engine::NodeHost& nh = e->nh;   // spec_used and key_val come from the derivation
+  {   // spec_used and key_val come from the derivation
     nh.pod_cnt.resize(N);
     for (int n = 0; n < N; ++n) nh.pod_cnt[n] = o->node_pod_off[n + 1] - o->node_pod_off[n];
     nh.pod_total = o->node_pod_off[NT];
@@ -966,6 +975,8 @@ struct NodePlan {
   const int32_t *removed = nullptr, *name = nullptr;   // churn: removed rows, node names of the added rows
   int nr = 0;
   int64_t npods_d = 0, npods_a = 0, total = 0;
+  int64_t rows_after = -1;   // cae_load_templates: the node rows and template copies after the call (-1: those of a churn)
+  int64_t drop = 0;          // cae_load_templates: the pods of the templates the call replaces or removes
 };
 
 static RowsIn dirty_rows(const cae_node_delta* dl) {
@@ -1008,7 +1019,8 @@ static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed)
   if (rows_null(p.dirty) || (nd && !dl->row)) return bad("dirty rows without arrays");
   if (nr && !p.removed) return bad("removed rows without an array");
   if (rows_null(p.added) || (na && !p.name)) return bad("added rows without arrays");
-  if ((int64_t)N - nr + na + 2 * (int64_t)e->T > INT32_MAX) return refuse("the node rows and template copies would pass 2^31 - 1");
+  const int64_t rows_after = p.rows_after >= 0 ? p.rows_after : (int64_t)N - nr + na + 2 * (int64_t)e->T;
+  if (rows_after > INT32_MAX) return refuse("the node rows and template copies would pass 2^31 - 1");
   { const int rc = tails_offsets(v, bad); if (rc) return rc; }
   if (nd && !offsets_ok(dl->pod_off, nd)) return bad("resident-pod offsets");
   if (na && !offsets_ok(p.added.pod_off, na)) return bad("resident-pod offsets of the added rows");
@@ -1017,7 +1029,7 @@ static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed)
   if ((p.npods_d && !dl->pod_spec) || (p.npods_a && !p.added.pod_spec)) return bad("resident pods without pod_spec");
   if (!tails_fit(e, v)) return refuse("a dictionary table would pass 2^31 - 1 entries");
   const int64_t NL = e->dict_cnt[CNT_LABELSETS] + v.n[CNT_LABELSETS], NTL = e->dict_cnt[CNT_TAINT_LISTS] + v.n[CNT_TAINT_LISTS];
-  int64_t total = nh.pod_total;
+  int64_t total = nh.pod_total - p.drop;
   for (int i = 0; i < nd; ++i) {
     const int r = dl->row[i];
     if (r < 0 || r >= N || (i > 0 && r <= dl->row[i - 1])) return bad("rows out of range or not strictly increasing");
@@ -1068,11 +1080,18 @@ static void commit_nodes(Engine* e, NodePlan& p) {
   for (int64_t q = 0; q < p.npods_a; ++q) nh.spec_used[p.added.pod_spec[q]] = 1;
 }
 
+// An array a node call stages beside its rows
+struct Extra {
+  const void* p;
+  size_t bytes;
+};
+template <class T>
+static Extra extra_of(const std::vector<T>& v) { return {v.data(), v.size() * sizeof(T)}; }
+
 // One staged blob and one H2D copy: the dictionary tails, the staged rows (dirty rows, then added ones) with their run
 // state (cluster_row_state), and the caller's `extra` arrays (their device copies in xdev); then the dictionary tables
 // grow on the device.  After commit_nodes.
-static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<const std::vector<int32_t>*>& extra, NodeDeltaDev* dd,
-                       std::vector<const int32_t*>* xdev) {
+static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<Extra>& extra, NodeDeltaDev* dd, std::vector<const void*>* xdev) {
   const cae_node_delta* dl = p.dl;
   const int A = e->A;
   const int nd = p.dirty.n, na = p.added.n, ns = nd + na;
@@ -1081,13 +1100,13 @@ static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<const std
   char* tab[NUM_DICT_TABLES] = {};
   NodeDeltaDev d{};
   d.nd = nd; d.na = na;
-  std::vector<const int32_t*> xd(extra.size());
+  std::vector<char*> xd(extra.size());
   auto walk = [&](Layout& l) {
     tails_layout(l, p.tails, tab);
     l.add(d.alloc, (size_t)ns * R); l.add(d.cfree, (size_t)ns * A);
     l.add(d.row, nd); l.add(d.name, na); l.add(d.labelset, ns); l.add(d.taint_list, ns); l.add(d.allowed, ns); l.add(d.cslots, ns);
     l.add(d.pod_off, (size_t)ns + 1); l.add(d.pod_spec, npods); l.add(d.unsched, ns);
-    for (size_t x = 0; x < extra.size(); ++x) l.add(xd[x], extra[x]->size());
+    for (size_t x = 0; x < extra.size(); ++x) l.add(xd[x], extra[x].bytes);
   };
   const size_t bytes = layout_bytes(walk);
   if (stage_reserve(e, s, bytes, bytes)) return -1;
@@ -1112,9 +1131,10 @@ static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<const std
     }
     i0 += r.n;
   }
-  for (size_t x = 0; x < extra.size(); ++x) std::copy(extra[x]->begin(), extra[x]->end(), s.host_of(xd[x]));
+  for (size_t x = 0; x < extra.size(); ++x)
+    if (extra[x].bytes) memcpy(s.host_of(xd[x]), extra[x].p, extra[x].bytes);
   if (stage_upload(e, s, bytes)) return -1;
-  if (xdev) *xdev = xd;
+  if (xdev) xdev->assign(xd.begin(), xd.end());
   if (tails_grow(e, p.tails, tab)) return -1;
   e->group_reason_valid = false;
   if (dd) *dd = d;
@@ -1204,13 +1224,13 @@ static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
   if (e->has_dynamic)
     for (int q = 0; q < dy.Q; ++q) qbo.push_back(qbo.back() + Dc[nh.q_k[q]]);
   NodeDeltaDev dd{};
-  std::vector<const int32_t*> xd;
-  if (stage_nodes(e, p, {&src, &dom, &qbo}, &dd, &xd)) return -1;
+  std::vector<const void*> xd;
+  if (stage_nodes(e, p, {extra_of(src), extra_of(dom), extra_of(qbo)}, &dd, &xd)) return -1;
   nh.pod_cnt.swap(pod_cnt);
   nh.key_val.swap(key_val);
 
   // ---- device: node columns + resident CSR, then everything a load derives from the node list ----
-  if (launch_node_churn(e, dd, xd[0], N, p.total)) return -1;
+  if (launch_node_churn(e, dd, static_cast<const int32_t*>(xd[0]), N, T, p.total)) return -1;
   e->N = N;
   e->U = N + 2 * T;
   if (devbuf_reserve(e, e->ch_pre, (size_t)std::max(e->SC, 1) * std::max(e->U, 1))) return -1;
@@ -1235,6 +1255,184 @@ static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
     if (launch_post_bits(e)) return -1;
   }
   return 0;
+}
+
+// The tables a load sizes by the template count (derive_pending and apply_dynamic allocate them in the arenas), laid out in
+// one engine-owned buffer for the sizes of the engine; the tables a load zeroes come first, `zeroed` bytes of them.  The
+// per-group and per-pod rows are sized by the resident capacities, as a load sizes them.
+static void tp_layout(Engine* e, Layout& l, size_t* zeroed) {
+  const size_t T1 = std::max(e->T, 1), E1 = std::max(e->cap_E, 1), Pl1 = std::max(e->cap_Pl, 1), Plw1 = (Pl1 + 31) / 32;
+  const size_t Twp1 = std::max(e->Twp, 1), A1 = std::max(e->A, 1), Q1 = std::max(e->dyn.Q, 1);
+  l.add(e->d_fit_count, T1); l.add(e->d_fit_acc, T1); l.add(e->d_chunk_done, std::max(e->Twp / FEAS_TW, 1));
+  l.add(e->d_counts2, 2 * T1); l.add(e->d_sched, T1 * E1); l.add(e->d_order_n, T1); l.add(e->d_max_nodes, T1);
+  l.add(e->d_last_index_buf, 2 * T1); l.add(e->d_tmpl_cost, T1); l.add(e->d_post_code, (size_t)e->DC * T1);
+  *zeroed = l.bytes;
+  l.add(e->d_fit_bits, T1 * Plw1);
+  if (e->cfg.want_reasons) l.add(e->d_reasons, T1 * Pl1);
+  l.add(e->d_group_reason, T1 * E1); l.add(e->d_order, T1 * E1); l.add(e->d_waste, T1); l.add(e->d_perm, T1);
+  l.add(e->d_pre_ok, (size_t)e->SC * Twp1); l.add(e->d_post_ok, (size_t)e->DC * Twp1);
+  l.add(e->d_rlut, (size_t)std::max(e->lut_rows, 1) * Twp1);
+  if (e->force_bitslice || e->lut_rows > FEAS_LUT_MAX_ROWS) l.add(e->d_tslice, (size_t)e->ra.Bpad * std::max(e->Tw, 1));
+  l.add(e->d_tmpl_free, A1 * e->T); l.add(e->d_tmpl_w, (size_t)std::max(e->W, 1) * T1);
+  l.add(e->d_tmpl_free_all, (size_t)R * e->T); l.add(e->d_tmpl_slots, e->T);
+  l.add(e->d_pre_code, (size_t)e->SC * e->U);
+  if (e->has_dynamic) l.add(e->dyn.ds_w, Q1 * T1);
+}
+
+// cae_load_templates: the checks of the node calls on the staged template rows (check_nodes) plus the template index lists,
+// then one staged blob (stage_nodes) with the new row -> source map, the template domains and the template run state.  The
+// host builds the new template list and its mirrors; the device gathers the node columns and the resident CSR through the
+// map (launch_node_churn) and reruns what a load derives from the templates: the rank tables, the class matrix over the
+// new universe, the template bits and, with topology counters, the template columns of the counter tables.  Nothing on the
+// pending side depends on the templates (DESIGN.md, "Template delta"), so derive_pending does not run.
+static int do_load_templates(Engine* e, const cae_template_delta* c) {
+  auto bad = [](const char* m) { set_error(std::string("cae_load_templates: ") + m); return -2; };
+  auto refuse = [](const char* m) { set_error(std::string("cae_load_templates: ") + m); return 2; };
+  if (c->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
+  if (c->tails && c->tails->num_dirty != 0) return bad("the tails carry dirty rows");
+  const int N = e->N, T = e->T, nr = c->num_removed, nc = c->num_changed, na = c->num_added;
+  if (nr < 0 || nc < 0 || na < 0) return bad("negative count");
+  if ((nr && !c->removed) || (nc && !c->changed)) return bad("an index list without its array");
+  if ((int64_t)nc + na > INT32_MAX) return refuse("the node rows and template copies would pass 2^31 - 1");
+  const int ns = nc + na;
+  if (ns && (!c->cap_cpu || !c->cap_mem || !c->has_alloc_cpu || !c->has_alloc_mem)) return bad("template rows without arrays");
+  Engine::NodeHost& nh = e->nh;
+  int64_t drop = 0;
+  for (int i = 0; i < nr; ++i) {
+    const int t = c->removed[i];
+    if (t < 0 || t >= T || (i > 0 && t <= c->removed[i - 1])) return bad("removed templates out of range or not strictly increasing");
+    drop += nh.tmpl_pods[t];
+  }
+  for (int i = 0, j = 0; i < nc; ++i) {   // j walks the removed list alongside
+    const int t = c->changed[i];
+    if (t < 0 || t >= T || (i > 0 && t <= c->changed[i - 1])) return bad("changed templates out of range or not strictly increasing");
+    while (j < nr && c->removed[j] < t) ++j;
+    if (j < nr && c->removed[j] == t) return bad("a changed template is also removed");
+    drop += nh.tmpl_pods[t];
+  }
+  const int Tn = T - nr + na;
+  cae_node_delta none{};
+  none.abi_version = CAE_ABI_VERSION;
+  NodePlan p;
+  p.dl = c->tails ? c->tails : &none;
+  p.dirty = dirty_rows(p.dl);
+  p.added.n = ns; p.added.labelset = c->labelset; p.added.taint_list = c->taint_list; p.added.allowed = c->allowed_pods;
+  p.added.pod_off = c->pod_off; p.added.pod_spec = c->pod_spec; p.added.unsched = c->unschedulable; p.added.alloc = c->alloc;
+  p.name = c->name;
+  p.rows_after = (int64_t)N + 2 * (int64_t)Tn;
+  p.drop = drop;
+  { const int rc = check_nodes(e, "cae_load_templates", p, false); if (rc) return rc; }
+  for (int i = 0; i < ns; ++i)   // a new resource dimension changes num_res: a full load
+    for (int r = e->dobj.num_res; r < R; ++r)
+      if (c->alloc[(size_t)i * R + r] != 0) return refuse("an allocatable in a dim past the load's num_res");
+  if (e->peer_world > 1 && Tn > Engine::PEER_CAP) {
+    set_error("cae_load_templates: more templates than the fused histogram exchange holds");
+    return 1;
+  }
+  e->stats.h2d_bytes = 0;
+  const cae_node_delta* dl = p.dl;
+  if (!dl->num_new_values && !dl->num_new_labelsets && !dl->num_new_taint_lists && !nr && !ns) return 0;
+
+  // ---- the new template list on the host: survivors in their old order (changed ones staged in place), then the added ----
+  DynTables& dy = e->dyn;
+  const int NT = N + Tn, K = e->has_dynamic ? dy.K : 0;
+  const int64_t* ps_req = e->host_tab<int64_t>(TAB_ps_req);
+  std::vector<int32_t> src(NT), tls(Tn), tpods(Tn), tslots(Tn), tkv((size_t)K * Tn);
+  std::vector<int64_t> tfree((size_t)Tn * R), free_all((size_t)R * Tn);
+  for (int r = 0; r < N; ++r) src[r] = r;
+  auto staged = [&](int i, int t) {   // staged row i becomes template t
+    const int npods = c->pod_off[i + 1] - c->pod_off[i];
+    int64_t reqd[R];
+    resident_req(ps_req, c->pod_spec + c->pod_off[i], npods, reqd);
+    for (int r = 0; r < R; ++r) tfree[(size_t)t * R + r] = c->alloc[(size_t)i * R + r] - reqd[r];
+    src[N + t] = -1 - i;
+    tls[t] = c->labelset[i];
+    tpods[t] = npods;
+    tslots[t] = c->allowed_pods[i] - npods;
+    for (int k = 0; k < K; ++k) tkv[(size_t)k * Tn + t] = label_of(e, dl, c->labelset[i], dy.key_id[k]);
+  };
+  int t = 0;
+  for (int o = 0, ir = 0, ic = 0; o < T; ++o) {
+    if (ir < nr && c->removed[ir] == o) { ++ir; continue; }
+    if (ic < nc && c->changed[ic] == o) {
+      staged(ic++, t++);
+      continue;
+    }
+    src[N + t] = N + o;
+    tls[t] = nh.tmpl_ls[o];
+    tpods[t] = nh.tmpl_pods[o];
+    tslots[t] = nh.tmpl_slots[o];
+    std::copy(nh.tmpl_free.begin() + (size_t)o * R, nh.tmpl_free.begin() + (size_t)(o + 1) * R, tfree.begin() + (size_t)t * R);
+    for (int k = 0; k < K; ++k) tkv[(size_t)k * Tn + t] = nh.tkey_val[(size_t)k * T + o];
+    ++t;
+  }
+  for (int j = 0; j < na; ++j) staged(nc + j, t++);
+  for (int x = 0; x < Tn; ++x)
+    for (int r = 0; r < R; ++r) free_all[(size_t)r * Tn + x] = tfree[(size_t)x * R + r];
+  // Topology domains of the new list.  assign_domains numbers the cluster rows first, so the domains of the cluster rows,
+  // Dc, the counter pool and the counts over the cluster stay what they are: only the template part of dom (and D) moves.
+  std::vector<int32_t> dom((size_t)K * NT), val(NT);
+  int D[DYN_MAX_KEYS] = {0};
+  for (int k = 0; k < K; ++k) {
+    std::copy(nh.key_val.begin() + (size_t)k * N, nh.key_val.begin() + (size_t)(k + 1) * N, val.begin());
+    std::copy(tkv.begin() + (size_t)k * Tn, tkv.begin() + (size_t)(k + 1) * Tn, val.begin() + N);
+    int Dc = 0;
+    assign_domains(val.data(), N, NT, nh.dom_scratch, dom.data() + (size_t)k * NT, &Dc, &D[k]);
+    if (Dc != dy.Dc[k]) { set_error("cae_load_templates: the cluster domains moved (internal error)"); return -1; }
+  }
+  std::vector<int64_t> cap_cpu(c->cap_cpu, c->cap_cpu + ns), cap_mem(c->cap_mem, c->cap_mem + ns);
+  std::vector<uint8_t> has_cpu(c->has_alloc_cpu, c->has_alloc_cpu + ns), has_mem(c->has_alloc_mem, c->has_alloc_mem + ns);
+
+  // ---- commit: host mirrors, one staged blob, then the device work in stream order ----
+  commit_nodes(e, p);
+  NodeDeltaDev dd{};
+  std::vector<const void*> xd;
+  if (stage_nodes(e, p, {extra_of(src), extra_of(dom), extra_of(free_all), extra_of(tslots), extra_of(cap_cpu), extra_of(cap_mem),
+                         extra_of(has_cpu), extra_of(has_mem)},
+                  &dd, &xd))
+    return -1;
+  nh.tmpl_ls.swap(tls);
+  nh.tmpl_pods.swap(tpods);
+  nh.tmpl_slots = tslots;
+  nh.tmpl_free.swap(tfree);
+  nh.tkey_val.swap(tkv);
+  if (!nr && !ns) return 0;
+  auto device = [&]() -> int {
+    dd.cap_cpu = static_cast<const int64_t*>(xd[4]); dd.cap_mem = static_cast<const int64_t*>(xd[5]);
+    dd.has_cpu = static_cast<const uint8_t*>(xd[6]); dd.has_mem = static_cast<const uint8_t*>(xd[7]);
+    if (launch_node_churn(e, dd, static_cast<const int32_t*>(xd[0]), N, Tn, p.total)) return -1;
+    set_template_count(e, Tn);
+    size_t zeroed = 0;
+    auto walk = [&](Layout& l) { tp_layout(e, l, &zeroed); };
+    if (devbuf_reserve(e, e->tp_buf, layout_bytes(walk))) return -1;
+    layout_bind(e->tp_buf.p, walk);
+    CAE_CUDA(cudaMemsetAsync(e->tp_buf.p, 0, zeroed, e->stream));
+    if (Tn) {
+      CAE_CUDA(cudaMemcpyAsync(e->d_tmpl_free_all, xd[2], sizeof(int64_t) * free_all.size(), cudaMemcpyDeviceToDevice, e->stream));
+      CAE_CUDA(cudaMemcpyAsync(e->d_tmpl_slots, xd[3], sizeof(int32_t) * Tn, cudaMemcpyDeviceToDevice, e->stream));
+    }
+    RankArgs& ra = e->ra;
+    ra.N = N; ra.T = Tn; ra.Tw = e->Tw; ra.Twp = e->Twp;
+    if (launch_rank_tables(e, ra, e->d_rvals, e->d_tmpl_w)) return -1;
+    if (launch_class_matrix(e) || launch_pre_ok_bits(e)) return -1;
+    if (e->has_dynamic) {
+      const size_t Q1 = std::max(dy.Q, 1);
+      int32_t* d_dom = nullptr;
+      auto dwalk = [&](Layout& l) { l.add(d_dom, dom.size()); l.add(dy.elig, Q1 * std::max(e->U, 1)); };
+      if (devbuf_reserve(e, e->tp_dyn, layout_bytes(dwalk))) return -1;
+      layout_bind(e->tp_dyn.p, dwalk);
+      if (!dom.empty()) CAE_CUDA(cudaMemcpyAsync(d_dom, xd[1], 4 * dom.size(), cudaMemcpyDeviceToDevice, e->stream));
+      dy.dom = d_dom;
+      for (int k = 0; k < K; ++k) dy.D[k] = D[k];
+      if (launch_template_dynamic(e)) return -1;
+    }
+    if (launch_post_bits(e)) return -1;
+    e->group_reason_valid = false;
+    return 0;
+  };
+  const int rc = device();
+  if (rc) e->loaded = false;   // the host mirrors are ahead of the device: the engine needs a cae_load
+  return rc;
 }
 
 static int do_load_pods(Engine* e, const cae_pod_delta* d) {
@@ -1658,6 +1856,14 @@ int32_t cae_load_node_churn(cae_engine* h, const cae_node_churn* c) {
   if (!c) { cae::set_error("cae_load_node_churn: no churn"); return -2; }
   cudaSetDevice(e->cfg.device);
   return cae::do_load_node_churn(e, c);
+}
+
+int32_t cae_load_templates(cae_engine* h, const cae_template_delta* d) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_load_templates before cae_load"); return -2; }
+  if (!d) { cae::set_error("cae_load_templates: no delta"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_load_templates(e, d);
 }
 
 int32_t cae_load_pods(cae_engine* h, const cae_pod_delta* d) {

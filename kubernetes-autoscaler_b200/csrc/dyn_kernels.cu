@@ -301,4 +301,22 @@ int launch_dynamic_recount(Engine* e, const int32_t* d_cols, int ncols) {
   return 0;
 }
 
+// After cae_load_templates rebuilt the template half of the domains (pre_code of the new universe already computed): the
+// eligibility of every column (the pitch U changed), the templates' DaemonSet weights and their post codes.  The counters
+// over the cluster (base_cnt, base_pres, base_tot, the min statistics, qrec) read cluster rows and cluster domains only,
+// which the call leaves as they are (assign_domains numbers cluster rows first), so they stay.
+int launch_template_dynamic(Engine* e) {
+  DynTables& d = e->dyn;
+  if (d.Q == 0) return 0;
+  const int Q = d.Q, U = e->U, T = e->T;
+  if (U > 0) dyn_elig_kernel<<<dim3((U + 127) / 128, Q), 128, 0, e->stream>>>(e->dobj, d, U, nullptr, U, e->d_pre_code);
+  if (T > 0) {
+    dyn_dsw_kernel<<<dim3((T + 127) / 128, Q), 128, 0, e->stream>>>(e->dobj, d);
+    dyn_post_code_kernel<<<dim3((T + 127) / 128, d.DC), 128, 0, e->stream>>>(e->dobj, d, U, e->d_post_code);
+  }
+  e->stats.kernel_launches += (U > 0) + 2 * (T > 0);
+  CAE_KERNEL_OK();
+  return 0;
+}
+
 }  // namespace cae

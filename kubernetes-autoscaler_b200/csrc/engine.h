@@ -142,6 +142,16 @@ __device__ __forceinline__ GroupRec build_group_rec(const DevObjects& o, const G
 }
 constexpr int ORDER_NOT_ON_FRESH = 1 << 30;   // order entry flag: the group's static filters fail on the SANITIZED template
 
+// pod_delta.cu: the T x ranks and N x R part of the pending-side derivation, shared by cae_load, cae_load_pods and
+// cae_load_templates
+struct RankArgs {
+  int A, N, T, Tw, Twp, W, lut_rows, feas_B, Bpad;
+  int act[CAE_MAX_RES], f_word[CAE_MAX_RES], f_shift[CAE_MAX_RES], f_bits[CAE_MAX_RES], lut_base[CAE_MAX_RES];
+  uint32_t lut_mask[CAE_MAX_RES];
+  int rv_off[CAE_MAX_RES + 1];            // the distinct requests of active dim k: rvals[rv_off[k], rv_off[k + 1]), ascending
+  uint8_t sword[32], sshift[32];
+};
+
 #define CAE_CUDA(expr)                                                                        \
   do {                                                                                        \
     cudaError_t _e = (expr);                                                                  \
@@ -225,6 +235,10 @@ struct Engine {
   uint8_t lut_word[CAE_MAX_RES] = {0}, lut_shift[CAE_MAX_RES] = {0};
   uint32_t lut_mask[CAE_MAX_RES] = {0};
   uint32_t* d_rlut = nullptr;             // [lut_rows][Twp]
+  // the rank encoding of the last derive_pending (cae_load_templates reruns launch_rank_tables over the new templates)
+  RankArgs ra{};
+  const int64_t* d_rvals = nullptr;       // distinct pending requests per active dim (RankArgs::rv_off)
+  uint32_t* d_tmpl_w = nullptr;           // [W][T] scratch of launch_rank_tables
   long long* d_tmpl_cost = nullptr;       // [T] pods in the schedulable groups of a template (order kernel)
   int32_t* d_perm = nullptr;              // [T] work order of the pack
   bool force_bitslice = false;            // CAE_K1_BITSLICE=1: always take the bit-sliced comparator (tests)
@@ -321,7 +335,10 @@ struct Engine {
     std::vector<int32_t> tkey_val;                 // [K][T] the same on the templates (domain rebuild of a churn)
     std::vector<int32_t> q_k;                      // [Q] topology key of each counter (its pool segment has Dc[q_k] entries)
     std::vector<int32_t> dom_scratch;              // value id -> domain while the domains are assigned (all -1 in between)
-    std::vector<int32_t> tmpl_ls;                  // [T] label set of each template (no delta changes a template)
+    std::vector<int32_t> tmpl_ls;                  // [T] label set of each template (cae_load_templates rewrites it)
+    std::vector<int32_t> tmpl_pods;                // [T] DaemonSet / mirror pods per template
+    std::vector<int64_t> tmpl_free;                // [T][R] allocatable - DaemonSet requested (columns of d_tmpl_free_all)
+    std::vector<int32_t> tmpl_slots;               // [T] allowed pods - DaemonSet pods
   } nh;
   Staging pd;                             // cae_load_pods' tails
   DevBuf pd_used;                         // [S] specs of the resident pods (pod_delta.cu)
@@ -333,6 +350,10 @@ struct Engine {
   DevBuf ch_nodes[2];                     // double-buffered node columns [N+T] + c_free [A][N] + c_slots [N] (node_delta.cu)
   DevBuf ch_pre;                          // pre_code [SC][U]
   DevBuf ch_dyn;                          // dom [K][N+T] | q_base_off [Q+1] | base_cnt, base_pres [pool] | elig [Q][U]
+  // buffers of cae_load_templates: every table whose size follows the template count, until the next cae_load or
+  // cae_load_pods (tp_layout in api.cu)
+  DevBuf tp_buf;                          // the [T]-, [Twp]- and [U]-shaped tables of a load
+  DevBuf tp_dyn;                          // dom [K][N+T] | elig [Q][U]
   // buffers of cae_similar_node_groups (similar.cu)
   Staging sim;                            // inputs | outputs (one D2H copy) | operand rows | schedulable bit rows (device only)
   int sm_count = 132;
@@ -383,6 +404,8 @@ struct NodeDeltaDev {                    // device views into the staged rows of
   const int32_t *labelset, *taint_list, *allowed, *cslots, *pod_off, *pod_spec;
   const uint8_t* unsched;
   const int64_t *alloc, *cfree;          // [nd + na][R], [nd + na][A]
+  const int64_t *cap_cpu, *cap_mem;      // [na] template rows of cae_load_templates (NULL: cluster rows carry none)
+  const uint8_t *has_cpu, *has_mem;
 };
 int launch_node_rows(Engine* e, const NodeDeltaDev& d, int64_t total);   // rows in place + resident CSR rebuilt into the spare buffer
 // cae_force_add_pods: d.row [nd] receiving rows, d.pod_off / d.pod_spec their arrivals (nothing else of d is read); the
@@ -391,8 +414,11 @@ int launch_node_arrivals(Engine* e, const NodeDeltaDev& d, int64_t total);
 // force_add.cu: everything on the device that follows from the arrivals of launch_node_arrivals' `d`: the resident CSR, the
 // receiving rows' run state, their pre_code when an arrival holds host ports (`ports`), the topology counters
 int launch_force_add(Engine* e, const NodeDeltaDev& d, int64_t total, bool ports);
-// cae_load_node_churn: node columns, run state and resident CSR of the new row list; src [N'+T] = old row, or -1 - staged row
-int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int N_new, int64_t total);
+// cae_load_node_churn and cae_load_templates: node columns, run state and resident CSR of the new row list of N' cluster rows
+// and T' templates; src [N'+T'] = old row, or -1 - staged row (staged rows are cluster rows of a churn or templates)
+int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int N_new, int T_new, int64_t total);
+// cae_load_templates, after the domains of the new templates: elig of every column, ds_w and post_code (dyn_kernels.cu)
+int launch_template_dynamic(Engine* e);
 int launch_pre_ok_bits(Engine* e);       // pre_ok[SC][Twp]: needs pre_code and the templates' pod slots
 int launch_post_bits(Engine* e);
 int launch_dynamic_tables(Engine* e, const uint8_t* d_spec_used, const int32_t* d_dc_ngroups);
@@ -441,14 +467,6 @@ struct RemovalState {
   GroupRecSrc grs;
 };
 int launch_removals(Engine* e, const RemovalLaunch& r);
-// pod_delta.cu: the T x ranks and N x R part of the pending-side derivation, shared by cae_load and cae_load_pods
-struct RankArgs {
-  int A, N, T, Tw, Twp, W, lut_rows, feas_B, Bpad;
-  int act[CAE_MAX_RES], f_word[CAE_MAX_RES], f_shift[CAE_MAX_RES], f_bits[CAE_MAX_RES], lut_base[CAE_MAX_RES];
-  uint32_t lut_mask[CAE_MAX_RES];
-  int rv_off[CAE_MAX_RES + 1];            // the distinct requests of active dim k: rvals[rv_off[k], rv_off[k + 1]), ascending
-  uint8_t sword[32], sshift[32];
-};
 // c_free [A][N], tmpl_free [A][T], tmpl_w [W][T] (scratch), rlut and (when e->d_tslice is set) tslice
 int launch_rank_tables(Engine* e, const RankArgs& a, const int64_t* d_rvals, uint32_t* d_tmpl_w);
 // cae_load_pods: the specs the resident pods use ([S] flags) and the rows' label sets ([N + T]), on the host

@@ -7,7 +7,8 @@
 // cae_load_node_churn: the row list itself changes, so every node column is gathered into a new buffer through a map
 // new row -> source (an old row: a clean survivor or a shifted template; or a staged row: a dirty or an added node),
 // and the CSR is rebuilt through the same map.  Only the staged rows travel over PCIe; everything else is read where it
-// already is.
+// already is.  cae_load_templates uses the same gather with the cluster rows as their own sources and the templates routed
+// through the map (a surviving old template, or a staged changed / added one that carries its capacity columns).
 // cae_force_add_pods: the rows stay as they are and the receiving rows' lists grow: the same counts, scan and gather, with
 // the staged lists (the arrivals per receiving row) appended to the rows' old lists instead of replacing them.
 #include <cub/device/device_scan.cuh>
@@ -83,7 +84,8 @@ struct NodeCols {
 };
 
 // one thread per new row: every node column, the run state of a cluster row and the resident count, from the row's source.
-// An added node has no capacity / has_alloc_* (read for templates only); a dirty row keeps those of its old row.
+// An added node has no capacity / has_alloc_* (read for templates only); a dirty row keeps those of its old row; a staged
+// template row (cae_load_templates: d.cap_cpu set) carries its own.
 __global__ void nc_columns_kernel(DevObjects o, NodeDeltaDev d, const int32_t* __restrict__ src, int NT, int N, int oldN, int A,
                                   const int64_t* __restrict__ old_cfree, const int32_t* __restrict__ old_cslots, NodeCols c,
                                   int32_t* __restrict__ cnt) {
@@ -106,17 +108,20 @@ __global__ void nc_columns_kernel(DevObjects o, NodeDeltaDev d, const int32_t* _
     return;
   }
   const int i = -1 - s;
-  const int old = i < d.nd ? d.row[i] : -1;
-  c.name[r] = old >= 0 ? o.node_name[old] : d.name[i - d.nd];
-  c.cap_cpu[r] = old >= 0 ? o.node_cap_cpu[old] : 0;
-  c.cap_mem[r] = old >= 0 ? o.node_cap_mem[old] : 0;
-  c.has_cpu[r] = old >= 0 ? o.node_has_alloc_cpu[old] : 0;
-  c.has_mem[r] = old >= 0 ? o.node_has_alloc_mem[old] : 0;
+  const int old = i < d.nd ? d.row[i] : -1, j = i - d.nd;
+  const bool tmpl = d.cap_cpu != nullptr;
+  c.name[r] = old >= 0 ? o.node_name[old] : d.name[j];
+  c.cap_cpu[r] = old >= 0 ? o.node_cap_cpu[old] : tmpl ? d.cap_cpu[j] : 0;
+  c.cap_mem[r] = old >= 0 ? o.node_cap_mem[old] : tmpl ? d.cap_mem[j] : 0;
+  c.has_cpu[r] = old >= 0 ? o.node_has_alloc_cpu[old] : tmpl ? d.has_cpu[j] : 0;
+  c.has_mem[r] = old >= 0 ? o.node_has_alloc_mem[old] : tmpl ? d.has_mem[j] : 0;
   c.labelset[r] = d.labelset[i]; c.taint_list[r] = d.taint_list[i]; c.unsched[r] = d.unsched[i]; c.allowed[r] = d.allowed[i];
 #pragma unroll
   for (int k = 0; k < R; ++k) c.alloc[(size_t)r * R + k] = d.alloc[(size_t)i * R + k];
-  for (int a = 0; a < A; ++a) c.c_free[(size_t)a * N + r] = d.cfree[(size_t)i * A + a];
-  c.c_slots[r] = d.cslots[i];
+  if (r < N) {   // a cluster row: its run state
+    for (int a = 0; a < A; ++a) c.c_free[(size_t)a * N + r] = d.cfree[(size_t)i * A + a];
+    c.c_slots[r] = d.cslots[i];
+  }
   cnt[r] = d.pod_off[i + 1] - d.pod_off[i];
 }
 
@@ -163,8 +168,8 @@ static int rebuild_csr(Engine* e, const NodeDeltaDev& d, int64_t total, bool app
 int launch_node_rows(Engine* e, const NodeDeltaDev& d, int64_t total) { return rebuild_csr(e, d, total, false); }
 int launch_node_arrivals(Engine* e, const NodeDeltaDev& d, int64_t total) { return rebuild_csr(e, d, total, true); }
 
-int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int N, int64_t total) {
-  const int NT = N + e->T, A1 = std::max(e->A, 1);
+int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int N, int T, int64_t total) {
+  const int NT = N + T, A1 = std::max(e->A, 1);
   const int tgt = e->dobj.node_name == e->ch_nodes[0].p ? 1 : 0;   // the half the node columns are NOT in (or the arena's)
   NodeCols c{};
   auto walk = [&](Layout& l) {
@@ -196,6 +201,7 @@ int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int 
   o.node_pod_off = new_off;
   o.node_pod_spec = new_spec;
   o.N = N;
+  o.T = T;
   e->d_c_free = c.c_free;
   e->d_c_slots = c.c_slots;
   return 0;

@@ -551,6 +551,41 @@ class EncodedObjects:
         res.struct = out._restruct(a, num_cluster_nodes=len(keep) + na)
         return res
 
+    def apply_template_delta(self, delta: "TemplateDelta") -> "EncodedObjects":
+        """The objects after cae_load_templates(delta), stated on the host: the tails of ``delta.tails`` appended, then the
+        template rows rebuilt: the surviving templates in their old order (a changed one replaced by its staged row in
+        place), then the added ones.  A cae_load of the result must answer like the engine after the delta."""
+        import copy
+        out = self.apply_node_delta(delta.tails) if delta.tails is not None else self
+        a, d = dict(out.arrays), delta.arrays
+        N, T = out.struct.num_cluster_nodes, out.struct.num_templates
+        removed = set(d["removed"].tolist())
+        changed = {int(t): i for i, t in enumerate(d["changed"])}
+        src = []                                      # per new template: ("old", row) or ("new", staged row)
+        for t in range(T):
+            if t in removed:
+                continue
+            src.append(("new", changed[t]) if t in changed else ("old", N + t))
+        src += [("new", len(changed) + j) for j in range(delta.num_added)]
+        staged = {"node_name": d["name"], "node_labelset": d["labelset"], "node_taint_list": d["taint_list"],
+                  "node_unschedulable": d["unschedulable"], "node_allowed_pods": d["allowed_pods"], "node_alloc": d["alloc"],
+                  "node_cap_cpu": d["cap_cpu"], "node_cap_mem": d["cap_mem"], "node_has_alloc_cpu": d["has_alloc_cpu"],
+                  "node_has_alloc_mem": d["has_alloc_mem"]}
+        for nm, new in staged.items():
+            col = a[nm]
+            rows = [col[r] if kind == "old" else np.asarray(new[r], col.dtype) for kind, r in src]
+            tail = np.asarray(rows, col.dtype).reshape((len(src),) + col.shape[1:])
+            a[nm] = np.ascontiguousarray(np.concatenate([col[:N], tail]))
+        off, spec, po = a["node_pod_off"], a["node_pod_spec"], d["pod_off"]
+        pieces = [spec[off[r]:off[r + 1]] for r in range(N)] + \
+                 [spec[off[r]:off[r + 1]] if kind == "old" else d["pod_spec"][po[r]:po[r + 1]] for kind, r in src]
+        a["node_pod_off"] = _i32(np.concatenate([[0], np.cumsum([len(p) for p in pieces], dtype=np.int64)]))
+        a["node_pod_spec"] = _i32(np.concatenate(pieces) if pieces else [])
+        res = copy.copy(out)
+        res.arrays = a
+        res.struct = out._restruct(a, num_templates=len(src))
+        return res
+
     def apply_pod_delta(self, delta: "PodDelta") -> "EncodedObjects":
         """The objects after cae_load_pods(delta), stated on the host: every dictionary tail and the new specs appended
         (tail offsets made absolute) and the pending list replaced.  A cae_load of the result must answer like the engine
@@ -726,6 +761,57 @@ class NodeChurn:
         return C.byref(self.struct)
 
 
+class TemplateDelta:
+    """Owns the numpy arrays behind one ``cae_template_delta`` struct: ``tails`` (a NodeDelta without dirty rows that
+    carries the dictionary tails the new rows use, or None), the removed and changed template indices and the rows of the
+    changed templates followed by the added ones.  Field names are the header's."""
+
+    _I32 = ("removed", "changed", "name", "labelset", "taint_list", "allowed_pods", "pod_off", "pod_spec")
+
+    def __init__(self, tails: Optional[NodeDelta] = None, **arrays) -> None:
+        a: Dict[str, np.ndarray] = {}
+        for nm in self._I32:
+            a[nm] = _i32(arrays.get(nm, [0] if nm == "pod_off" else []))
+        ns = len(a["name"])
+        for nm in ("unschedulable", "has_alloc_cpu", "has_alloc_mem"):
+            a[nm] = np.ascontiguousarray(arrays.get(nm, np.zeros(ns)), np.uint8)
+        for nm in ("cap_cpu", "cap_mem"):
+            a[nm] = np.ascontiguousarray(arrays.get(nm, np.zeros(ns)), np.int64)
+        a["alloc"] = np.ascontiguousarray(np.asarray(arrays.get("alloc", np.zeros((ns, MAX_RES))), np.int64).reshape(ns, MAX_RES))
+        self.arrays = a
+        self.tails = tails
+        s = capi.cae_template_delta()
+        s.abi_version = capi.CONST["CAE_ABI_VERSION"]
+        s.tails = C.pointer(tails.struct) if tails is not None else None
+        s.num_removed = len(a["removed"])
+        s.num_changed = len(a["changed"])
+        s.num_added = ns - len(a["changed"])
+        for name, ctype in capi.cae_template_delta._fields_:
+            if name in a:
+                setattr(s, name, a[name].ctypes.data_as(ctype))
+        self.struct = s
+
+    def replace(self, **arrays) -> "TemplateDelta":
+        """A copy with some arrays (or ``tails``) replaced (the counts follow the arrays)."""
+        tails = arrays.pop("tails", self.tails)
+        return TemplateDelta(tails, **{**self.arrays, **arrays})
+
+    @property
+    def num_removed(self) -> int:
+        return self.struct.num_removed
+
+    @property
+    def num_changed(self) -> int:
+        return self.struct.num_changed
+
+    @property
+    def num_added(self) -> int:
+        return self.struct.num_added
+
+    def ptr(self):
+        return C.byref(self.struct)
+
+
 class PodDelta:
     """Owns the numpy arrays behind one ``cae_pod_delta`` struct: the dictionary tails and new pod specs (continuing the
     resident tables; offsets relative to the tail) and the complete new pending list.  Field names are the header's."""
@@ -788,6 +874,7 @@ class Encoder:
         self.b = TableBuilder()
         self._podspec_cache: Dict[int, int] = {}
         self._ns_objects: Dict[str, Namespace] = {}
+        self.template_keys: Optional[List] = None   # the caller's key of each template (node-group id); None = position
 
     # ---- interning helpers --------------------------------------------------------------
     def _val(self, v: str) -> int:
@@ -980,6 +1067,15 @@ class Encoder:
         self._cluster = [(b.node_rows[r][0], (b.node_rows[r][1], b.node_rows[r][2], b.node_rows[r][3], tuple(b.node_alloc[r]),
                                               b.node_rows[r][4], tuple(b.node_pod_spec[off[r]:off[r + 1]])))
                          for r in range(b.num_cluster_nodes)]
+        # the template rows the engine holds: (caller key, row state) per template, kept current by template_delta
+        N, T = b.num_cluster_nodes, b.num_templates
+        keys = list(range(T)) if self.template_keys is None else list(self.template_keys)
+        if len(keys) != T or len(set(keys)) != T:
+            raise ValueError("template_keys: one distinct key per template")
+        self._templates = [(keys[t], (b.node_rows[r][0], b.node_rows[r][1], b.node_rows[r][2], b.node_rows[r][3],
+                                      tuple(b.node_alloc[r]), b.node_rows[r][4], b.node_rows[r][5], b.node_rows[r][6],
+                                      b.node_rows[r][7], b.node_rows[r][8], tuple(b.node_pod_spec[off[r]:off[r + 1]])))
+                           for t, r in enumerate(range(N, N + T))]
         return enc
 
     def _resident_spec(self, pod: Pod, allow_new: bool = False) -> int:
@@ -1123,6 +1219,69 @@ class Encoder:
         self._cluster = new_list + added
         return churn
 
+    def _template_state(self, ni: NodeInfo) -> tuple:
+        """(name, label set, taint list, unschedulable, allocatable, allowed pods, capacity cpu / memory, has_alloc cpu /
+        memory, pod specs) of a template, interned append-only against the last load.  Its pods are incoming pods as far
+        as the volume filters go (podspec's non-resident rule), and their specs are looked up among the specs the engine
+        holds with nodeName ignored, as for a resident pod."""
+        n, b = ni.node, self.b
+        a = self._node_args(NodeInfo(n, []))
+        if len(self.resources) > self._num_res:
+            self._delta_ok = False
+            raise Unsupported("template %s has a resource the last load did not have" % n.name)
+        specs = []
+        for p in ni.pods:
+            if p.has_volumes_or_claims:
+                raise Unsupported("template pod %s/%s uses volumes or resource claims" % (p.namespace, p.name))
+            specs.append(self._resident_spec(p))
+        return (a["name"], a["labelset"], a["taint_list"], int(a["unschedulable"]), tuple(a["alloc"]), a["allowed_pods"],
+                a["cap_cpu"], a["cap_mem"], int(a["has_alloc_cpu"]), int(a["has_alloc_mem"]), tuple(specs))
+
+    def template_delta(self, new_templates: Sequence[NodeInfo], keys: Optional[Sequence] = None) -> "TemplateDelta":
+        """The shim's side of cae_load_templates: the complete new template list (what TemplateNodeInfoProvider returns,
+        keyed by node-group id; `keys` None = the position) as a TemplateDelta against what the engine holds.  Vanished
+        keys are removed, new keys are added, survivors whose state changed become changed rows.  The survivors must keep
+        their relative order and the new templates must all come after them; a template pod's spec must be one the engine
+        holds (run pod_delta(..., residents=templates) first for new ones); no new resource dimension.  Unsupported
+        otherwise: a full load."""
+        self._check_resident()
+        keys = list(range(len(new_templates))) if keys is None else list(keys)
+        if len(keys) != len(new_templates) or len(set(keys)) != len(keys):
+            raise ValueError("template delta: one distinct key per template")
+        old = {k: t for t, (k, _) in enumerate(self._templates)}
+        last, seen_new = -1, False
+        for k in keys:
+            t = old.get(k)
+            if t is None:
+                seen_new = True
+            elif seen_new or t < last:
+                raise Unsupported("template delta: the surviving templates are reordered or a new one comes before one of them")
+            else:
+                last = t
+        states = [self._template_state(ni) for ni in new_templates]
+        kept = {old[k] for k in keys if k in old}
+        removed = [t for t in range(len(self._templates)) if t not in kept]
+        changed, rows, added = [], [], []
+        for k, st in zip(keys, states):
+            t = old.get(k)
+            if t is None:
+                added.append(st)
+            elif st != self._templates[t][1]:
+                changed.append(t)
+                rows.append(st)
+        rows += added
+        po = [0]
+        for st in rows:
+            po.append(po[-1] + len(st[10]))
+        col = lambda i: [st[i] for st in rows]
+        delta = TemplateDelta(NodeDelta(**self._tails(_NODE_TABLES)), removed=removed, changed=changed, name=col(0),
+                              labelset=col(1), taint_list=col(2), unschedulable=col(3),
+                              alloc=np.asarray(col(4), np.int64).reshape(len(rows), MAX_RES), allowed_pods=col(5),
+                              cap_cpu=col(6), cap_mem=col(7), has_alloc_cpu=col(8), has_alloc_mem=col(9), pod_off=po,
+                              pod_spec=[x for st in rows for x in st[10]])
+        self._templates = list(zip(keys, states))
+        return delta
+
     def pod_delta(self, groups: Sequence[PodEquivalenceGroup], residents: Sequence[NodeInfo] = ()) -> "PodDelta":
         """The shim's side of cae_load_pods: `groups` become the complete new pending list, and every spec and dictionary
         entry interned since the last load or delta becomes a tail.  The pods of `residents` (the changed or added nodes
@@ -1147,9 +1306,13 @@ class Encoder:
 
 def encode(cluster: Sequence[NodeInfo], templates: Sequence[NodeInfo],
            groups: Sequence[PodEquivalenceGroup],
-           namespaces: Sequence[Namespace] = (), encoder: Optional[Encoder] = None) -> EncodedObjects:
-    """encoder: the Encoder to intern with (a fresh one by default), for a caller that needs its dictionaries afterwards."""
+           namespaces: Sequence[Namespace] = (), encoder: Optional[Encoder] = None,
+           template_keys: Optional[Sequence] = None) -> EncodedObjects:
+    """encoder: the Encoder to intern with (a fresh one by default), for a caller that needs its dictionaries afterwards.
+    template_keys: the caller's key of each template (node-group id) that Encoder.template_delta matches by."""
     enc = encoder or Encoder()
+    if template_keys is not None:
+        enc.template_keys = list(template_keys)
     for ns in namespaces:
         enc.add_namespace(ns)
     for ni in cluster:

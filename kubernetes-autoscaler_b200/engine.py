@@ -164,6 +164,19 @@ class Engine:
         self._check(rc)
         return True
 
+    def load_templates(self, delta, enc: Optional[EncodedObjects] = None) -> bool:
+        """The per-tick delta of the node-group templates (cae_load_templates): removed, changed and added templates plus
+        the dictionary tails they need (encode.TemplateDelta).  Returns False when the engine answers "use a full load"
+        (status 2); the engine is unchanged then.  `enc`: the objects the engine now holds
+        (EncodedObjects.apply_template_delta), kept as this engine's shapes (the template count changes)."""
+        rc = self.lib.cae_load_templates(self.h, delta.ptr())
+        if rc == 2:
+            return False
+        self._check(rc)
+        if enc is not None:
+            self.enc = enc
+        return True
+
     def load_pods(self, delta, enc: Optional[EncodedObjects] = None) -> int:
         """The per-tick delta of the pod specs (cae_load_pods): new pod specs with the dictionary tails they need and the
         complete new pending list (encode.PodDelta).  Returns the status: 0 applied, 1 a limit of the engine (use the stock

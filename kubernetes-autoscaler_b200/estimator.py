@@ -22,7 +22,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import capi
-from .encode import EncodedObjects, Encoder, encode
+from .encode import EncodedObjects, Encoder, Unsupported, encode
 from .engine import Engine
 from .objects import NodeInfo, Pod, PodEquivalenceGroup
 
@@ -198,14 +198,39 @@ class ScaleUpSimulation:
 
     def __init__(self, cluster: Sequence[NodeInfo], templates: Dict[str, NodeInfo],
                  groups: Sequence[PodEquivalenceGroup], engine: Optional[Engine] = None, namespaces=()) -> None:
+        self.cluster = list(cluster)
+        self.namespaces = list(namespaces)
+        self.groups = list(groups)
+        self.engine = engine or shared_engine()
+        self._full_load(templates)
+
+    def _full_load(self, templates: Dict[str, NodeInfo]) -> None:
         self.ids = list(templates.keys())
         self.templates = [templates[i] for i in self.ids]
-        self.groups = list(groups)
         self.encoder = Encoder()
-        self.enc: EncodedObjects = encode(cluster, self.templates, groups, namespaces, encoder=self.encoder)
+        self.enc: EncodedObjects = encode(self.cluster, self.templates, self.groups, self.namespaces, encoder=self.encoder,
+                                          template_keys=self.ids)
         self.sng_limit: Optional[np.ndarray] = None
-        self.engine = engine or shared_engine()
         self.engine.load(self.enc)
+
+    def update_templates(self, templates: Dict[str, NodeInfo]) -> bool:
+        """A new TemplateNodeInfoProvider result (node-group id -> template) against the resident snapshot: a template
+        delta (cae_load_templates) matched by node-group id, or a full load when the delta cannot express the change
+        (encode.Unsupported) or the engine refuses it (status 2).  ids and templates follow the new order either way;
+        the similar-groups caps of an earlier similar_node_groups call are dropped.  Returns True when the delta applied."""
+        ids = list(templates.keys())
+        tl = [templates[i] for i in ids]
+        try:
+            delta = self.encoder.template_delta(tl, keys=ids)
+        except Unsupported:
+            self._full_load(templates)
+            return False
+        after = self.enc.apply_template_delta(delta)
+        if not self.engine.load_templates(delta, after):
+            self._full_load(templates)
+            return False
+        self.ids, self.templates, self.enc, self.sng_limit = ids, tl, after, None
+        return True
 
     def schedulable_pod_groups(self) -> Dict[str, List[int]]:
         """orchestrator.go:603-638 for every node group: indices of the groups whose exemplar fits."""

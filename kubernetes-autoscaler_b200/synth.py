@@ -454,6 +454,110 @@ def node_scale(enc: EncodedObjects, seed: int, n_remove: int, n_add: int, n_dirt
     return churn, pending
 
 
+def _template_rows(enc: EncodedObjects, ts) -> dict:
+    """The cae_template_delta row columns of templates ``ts`` of ``enc`` as they are."""
+    a, N = enc.arrays, enc.struct.num_cluster_nodes
+    rows = [N + int(t) for t in ts]
+    off, spec = a["node_pod_off"], a["node_pod_spec"]
+    out = {nm: [a["node_" + nm][r] for r in rows] for nm in ("name", "labelset", "taint_list", "unschedulable", "allowed_pods",
+                                                             "cap_cpu", "cap_mem", "has_alloc_cpu", "has_alloc_mem")}
+    out["alloc"] = [a["node_alloc"][r].copy() for r in rows]
+    out["pods"] = [list(spec[off[r]:off[r + 1]]) for r in rows]
+    return out
+
+
+def _template_delta(enc: EncodedObjects, tails: dict, removed, changed, rows: dict):
+    from .encode import MAX_RES, NodeDelta, TemplateDelta
+    po = [0]
+    for p in rows["pods"]:
+        po.append(po[-1] + len(p))
+    nrow = len(rows["name"])
+    cols = {nm: rows[nm] for nm in ("name", "labelset", "taint_list", "unschedulable", "allowed_pods", "cap_cpu", "cap_mem",
+                                    "has_alloc_cpu", "has_alloc_mem")}
+    return TemplateDelta(NodeDelta(**tails), removed=sorted(removed), changed=sorted(changed), pod_off=po,
+                         pod_spec=[x for p in rows["pods"] for x in p],
+                         alloc=np.asarray(rows["alloc"], np.int64).reshape(nrow, MAX_RES), **cols)
+
+
+def template_churn(enc: EncodedObjects, seed: int, n_change: int, n_remove: int, n_add: int):
+    """A deterministic random tick of node-group template churn against a snapshot of ``generate``: ``n_remove`` random
+    templates go away, ``n_change`` others change and ``n_add`` new ones (copies of random templates under a new name and
+    pool) are appended.  A changed template gets a new name (the provider's random suffix) and, by turns, a zone value of
+    another template (the first changed one a zone value no row had: a new domain), another taint list, other allocatable
+    and allowed pods; an added one every third time a new zone value too.  DaemonSet pods stay those of the source.
+    Returns the encode.TemplateDelta; ``enc.apply_template_delta(delta)`` is the snapshot after the tick."""
+    a, s = enc.arrays, enc.struct
+    N, T = s.num_cluster_nodes, s.num_templates
+    rng = SplitMix64(0x7E3A0000 + seed)
+    perm = rng.next(T).argsort() if T else np.zeros(0, np.int64)
+    n_remove = min(n_remove, T)
+    n_change = min(n_change, T - n_remove)
+    removed = [int(t) for t in perm[:n_remove]]
+    changed = sorted(int(t) for t in perm[n_remove:n_remove + n_change])
+    src = changed + ([int(x) for x in rng.randint(n_add, T)] if T else [])
+    n_add = len(src) - len(changed)
+    rows = _template_rows(enc, src)
+    nv, nl, nt = s.num_values, s.num_labelsets, s.num_taint_lists
+    new_vals, new_ls = [], {}
+    zones = []
+    for r in range(N, N + T):
+        ls = int(a["node_labelset"][r])
+        zones += [int(v) for k, v in zip(a["ls_key"][a["ls_off"][ls]:a["ls_off"][ls + 1]],
+                                         a["ls_val"][a["ls_off"][ls]:a["ls_off"][ls + 1]]) if k == K_ZONE]
+    name0 = int(a["node_name"].max()) + 1 if len(a["node_name"]) else 0
+    r8 = rng.next(8 * max(len(src), 1)).reshape(-1, 8)
+    u = rng.uniform(4 * max(len(src), 1)).reshape(-1, 4)
+    for i in range(len(src)):
+        ri = [int(x) for x in r8[i]]
+        ls = int(rows["labelset"][i])
+        lab = {int(k): int(v) for k, v in zip(a["ls_key"][a["ls_off"][ls]:a["ls_off"][ls + 1]],
+                                              a["ls_val"][a["ls_off"][ls]:a["ls_off"][ls + 1]])}
+        rows["name"][i] = name0 + i
+        new_zone = (i == 0 and n_change > 0) or (i >= len(changed) and ri[0] % 3 == 0)
+        if new_zone:
+            new_vals.append(0)
+            lab[K_ZONE] = nv + len(new_vals) - 1
+        elif zones and (i >= len(changed) or ri[1] % 2 == 0):
+            lab[K_ZONE] = zones[ri[2] % len(zones)]
+        if i >= len(changed) or ri[3] % 3 == 0:
+            lab[K_POOL] = 16 + ri[4] % 8
+        key = tuple(sorted(lab.items()))
+        rows["labelset"][i] = new_ls.setdefault(key, nl + len(new_ls))
+        if i < len(changed) and ri[5] % 2 == 0 and nt:
+            rows["taint_list"][i] = ri[6] % nt
+        if i < len(changed) and u[i][0] < 0.5:
+            rows["alloc"][i][0] = max(1, int(rows["alloc"][i][0] * (0.5 + u[i][1])))
+            rows["alloc"][i][1] = max(1, int(rows["alloc"][i][1] * (0.5 + u[i][2])))
+            rows["allowed_pods"][i] = max(len(rows["pods"][i]) + 1, int(ri[7] % 121))
+    ls_items = sorted(new_ls.items(), key=lambda kv: kv[1])
+    ls_off = [0]
+    for k, _ in ls_items:
+        ls_off.append(ls_off[-1] + len(k))
+    tails = dict(value_is_int=[0] * len(new_vals), value_int=[0] * len(new_vals), ls_off=ls_off,
+                 ls_key=[kk for k, _ in ls_items for kk, _v in k], ls_val=[v for k, _ in ls_items for _k, v in k])
+    return _template_delta(enc, tails, removed, changed, rows)
+
+
+def daemonset_rollout(enc: EncodedObjects, seed: int):
+    """A DaemonSet created or rolled out: every template's DaemonSet pod list changes (every other template loses its
+    first pod, the others gain one pod of a spec already on a template or resident).  Returns the encode.TemplateDelta
+    with every template changed."""
+    a, s = enc.arrays, enc.struct
+    N, T = s.num_cluster_nodes, s.num_templates
+    rng = SplitMix64(0xDA350000 + seed)
+    rows = _template_rows(enc, range(T))
+    pool = sorted(set(int(x) for x in a["node_pod_spec"]))
+    pick = rng.randint(max(T, 1), max(len(pool), 1))
+    for t in range(T):
+        pods = rows["pods"][t]
+        if t % 2 and pods:
+            pods.pop(0)
+        elif pool:
+            pods.append(pool[int(pick[t])])
+        rows["allowed_pods"][t] = max(int(rows["allowed_pods"][t]), len(pods) + 1)
+    return _template_delta(enc, {}, [], range(T), rows)
+
+
 def pod_churn(enc: EncodedObjects, seed: int, arrive: int, leave: int):
     """A deterministic random tick of workload churn against a snapshot of ``generate``: ``leave`` random pending groups
     finish, and ``arrive`` new workloads come, each a new spec copied from a random pending spec with a new cpu request

@@ -8,6 +8,7 @@
     python scripts/delta_tick.py --kind churn --config 3 --scale 1,10,100 --dirty 20 --reps 5 [--check]
     python scripts/delta_tick.py --kind pods --config 3 --scale 1,10,100 --reps 5 [--check]
     python scripts/delta_tick.py --kind placed --config 3 --reps 5 [--check]
+    python scripts/delta_tick.py --kind templates --config 3 --scale 0,1,10,50 --reps 5 [--check]
 
 Kinds, with the change `scale` stands for and the delta call:
   nodes  synth.node_churn on `scale` dirty nodes (binds, evictions, moves, cordons, taints, allocatable, relabels):
@@ -16,6 +17,8 @@ Kinds, with the change `scale` stands for and the delta call:
          cae_load_node_churn(removed, added and dirty rows) + cae_load_pending(pending rows);
   pods   synth.pod_churn: `scale` new workloads arrive, `scale` pending groups finish: cae_load_pods(new specs + the new
          pending list).  The caller-side encode is not part of either tick (synth builds tables, not objects).
+  templates  synth.template_churn: `scale` templates change, scale // 4 are removed and scale // 4 added (scale 0: a
+         DaemonSet rollout, synth.daemonset_rollout, which changes every template's pod list): cae_load_templates.
   placed the reference's tick, filter pass then scale-up on ONE snapshot, three ways (`scale` is not used): every tick is
          cae_load + cae_filter_schedulable over all pending pods, then the placements become residents, then estimate_all +
          expander_best.  Tick A: cae_force_add_pods(what the pass assigned).  Tick B: the same placements as host-built
@@ -37,7 +40,7 @@ import time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 
-SCALES = {"nodes": "1,20,200,2000", "churn": "1,10,100", "pods": "1,10,100", "placed": "0"}
+SCALES = {"nodes": "1,20,200,2000", "churn": "1,10,100", "pods": "1,10,100", "placed": "0", "templates": "0,1,10,50"}
 
 
 def _card():
@@ -66,6 +69,10 @@ def _change(synth, kind, enc, seed, scale, dirty):
     if kind == "churn":
         churn, pending = synth.node_scale(enc, seed, scale, scale, dirty)
         return pending.apply_node_churn(churn), lambda eng: eng.load_node_churn(churn), lambda eng: eng.load_pending(pending)
+    if kind == "templates":
+        delta = synth.template_churn(enc, seed, scale, scale // 4, scale // 4) if scale else synth.daemonset_rollout(enc, seed)
+        after = enc.apply_template_delta(delta)
+        return after, lambda eng: eng.load_templates(delta, after), None
     delta = synth.pod_churn(enc, seed, scale, scale)
     after = enc.apply_pod_delta(delta)
     return after, lambda eng: eng.load_pods(delta, after) == 0, None
@@ -205,6 +212,7 @@ def main():
         for rep in range(args.reps):
             after, call, pend = _change(synth, args.kind, enc, 1000 * scale + rep, scale, args.dirty)
             a.load(enc)
+            caps = np.full(after.T, args.cap, np.int32)   # a template delta changes T
 
             def delta_tick():
                 t0 = time.perf_counter()

@@ -7,7 +7,7 @@ self-cleaning accumulators, last-block election, shared-memory state and block-w
 
 Dense pass (K1, both variants), Estimate() of every template (K0 + K3: plain closed form, capacity form with the cluster
 fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals), a cluster-node delta
-(cae_load_nodes), a cluster-node churn (cae_load_node_churn), new pod specs (cae_load_pods), the placements of a filter pass made resident (cae_force_add_pods) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
+(cae_load_nodes), a cluster-node churn (cae_load_node_churn), new pod specs (cae_load_pods), node-group template changes (cae_load_templates), the placements of a filter pass made resident (cae_force_add_pods) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
 against the CPU oracle so that a "clean" run also means "correct results under the tool"."""
 import os
 import sys
@@ -93,6 +93,16 @@ def main():
             got = eng.filter_schedulable(order_p)
             ref = pyoracle.filter_schedulable(after, order_p)
             assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
+            # node-group templates changed, removed and added (cae_load_templates: column gather through the template map,
+            # template domains, rank tables, full class matrix, template counter columns)
+            tdelta = synth.template_churn(after, cfg, 4, 3, 5)
+            after = after.apply_template_delta(tdelta)
+            assert eng.load_templates(tdelta, after)
+            _, reasons, _ = eng.feasibility()
+            assert np.array_equal(reasons, pyoracle.feasibility_dense(after)[0])
+            caps = np.full(after.T, 30, np.int32)
+            got_e, ref_e = eng.estimate_all(caps), pyoracle.estimate_all(after, caps)
+            assert all(np.array_equal(x, y) for x, y in zip(got_e, ref_e[:4]))
             # the filter pass's placements made resident (cae_force_add_pods: CSR append, row state, feed tables, recount),
             # then what the scale-up asks; pod limits out of reach, see tests/test_gpu_force_add.py
             after.arrays["node_allowed_pods"][:after.struct.num_cluster_nodes] += 4000
