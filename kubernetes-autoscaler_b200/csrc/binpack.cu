@@ -708,9 +708,11 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
       }
       int placed = 0;
 
-      // spare capacity of node x for this pod by NodePorts + NodeResourcesFit alone (pod slots, free resources)
+      // spare capacity of node x for this pod by NodePorts + NodeResourcesFit alone (pod slots, free resources); a node
+      // holding more pods than it allows (slots < 0: a lowered max-pods, a force-added list) takes none, not a negative
+      // count that the clamped sums below would take off the other nodes
       auto res_cap_of = [&](auto frf, int slots, unsigned long long ports, int want) -> int {
-        int k = min(min(slots, want), kcap);
+        int k = max(min(min(slots, want), kcap), 0);
         if (k > 0 && (ports & pconf)) k = 0;
 #pragma unroll
         for (int a = 0; a < A; ++a) {
@@ -1227,7 +1229,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
               h_caps(x, cp, ci);
               const int k_other = min(rc, ci);
               g_kc[x] = min(k_other, cp);
-              if (k_other == 0 && hp >= 0 && (!RM || p.rm.live_w[x])) {   // a removed node is no domain's eligible node
+              if (k_other <= 0 && hp >= 0 && (!RM || p.rm.live_w[x])) {   // a removed node is no domain's eligible node
                 const int sl = slot_of(hp, x);
                 if (sl >= 0 && elig_of(hp, x) && rd_cnt(hp, sl) == 0 && rd_pres(hp, sl) == 1) blocked = 1;
               }
@@ -1718,12 +1720,15 @@ __global__ void lpt_rank_kernel(const long long* __restrict__ cost, int t_begin,
 }
 
 // `need` bytes of slab under the layout of p (bp_slab_of).  The slot versions in a block's slab persist across launches
-// but are only meaningful within one layout: bytes that a new allocation or a new layout hands out are zeroed.
+// but are only meaningful within one layout: bytes that a new allocation or a new layout hands out are zeroed.  A grown
+// buffer is a new allocation even when the memory pool hands back the old address (its bytes are then whatever the pool
+// last held there), so growth is told by the capacity, not by the pointer.
 static int slab_reserve(Engine* e, Engine::Slab& s, BpParams& p, bool fm, size_t need) {
   const size_t sig = p.scratch_per_cta * 1000003u + (size_t)bp_xg(p, fm) * 10007u + (size_t)p.dstride * 101u + (size_t)p.log_cap * 7u + (size_t)std::max(e->A, 1);
   const void* old = s.buf.p;
+  const size_t old_cap = s.buf.cap;
   if (devbuf_reserve(e, s.buf, need)) return -1;
-  if (s.buf.p != old || sig != s.sig) { s.sig = sig; s.zeroed = 0; }
+  if (s.buf.p != old || s.buf.cap != old_cap || sig != s.sig) { s.sig = sig; s.zeroed = 0; }
   if (need > s.zeroed) {
     CAE_CUDA(cudaMemsetAsync(static_cast<unsigned char*>(s.buf.p) + s.zeroed, 0, need - s.zeroed, e->stream));
     s.zeroed = need;

@@ -346,9 +346,11 @@ def node_churn(enc: EncodedObjects, seed: int, n_dirty: int, bind: float = 0.3, 
             key = tuple(sorted(lab.items()))
             ls = new_ls.setdefault(key, nl + len(new_ls))
         lsets.append(ls)
-    # allowed pods stay above the final resident count: the estimator's fallback onto cluster nodes that are already at
-    # their pod limit disagrees with the oracle (DESIGN.md §4), which is not what these deltas test
-    allowed = [max(ap, len(p) + 1) for ap, p in zip(allowed, lists)]
+    # about one dirty row in four ends at or past its pod limit (pod slots 0 .. -3): a kubelet whose max-pods is lowered
+    # keeps the pods it runs
+    for i, p in enumerate(lists):
+        if int(r8[i][7]) % 8 < 2:
+            allowed[i] = max(0, len(p) - (int(r8[i][7]) >> 3) % 4)
     ls_items = sorted(new_ls.items(), key=lambda kv: kv[1])
     tl_items = sorted(new_tl.items(), key=lambda kv: kv[1])
     ls_off, tl_off = [0], [0]
@@ -378,8 +380,8 @@ def node_scale(enc: EncodedObjects, seed: int, n_remove: int, n_add: int, n_dirt
     cluster rows leave, ``n_add`` nodes shaped like the generator's cluster nodes join, and ``n_dirty`` other rows change
     as in ``node_churn`` (same seed).  Every added node has a new hostname value; about one in four has a new zone value
     (a domain appears); when ``n_remove`` allows, the removals include every node of the smallest zone (a domain
-    disappears).  Residents of the added nodes are drawn from the specs resident at the load; allowed pods stay above the
-    resident count (DESIGN.md §4).
+    disappears).  Residents of the added nodes are drawn from the specs resident at the load; about one added node in four
+    allows no more pods than it holds.
     Returns (churn, pending): the NodeChurn and ``enc`` with the pods bound by the dirty rows removed from the pending rows.
     ``pending.apply_node_churn(churn)`` is the snapshot after the tick."""
     from .encode import NodeChurn, NodeDelta
@@ -432,7 +434,13 @@ def node_scale(enc: EncodedObjects, seed: int, n_remove: int, n_add: int, n_dirt
         pods = [int(resident_pool[i]) for i in rng.randint(k, len(resident_pool))] if k else []
         pod_spec.extend(pods)
         pod_off.append(len(pod_spec))
-        allowed.append(max(110, len(pods) + 1))
+        allowed.append(110)
+    # about one added node in four joins at or past its pod limit (pod slots 0 .. -3), as one whose max-pods is set below
+    # what it already runs
+    under = rng.randint(max(n_add, 1), 16)
+    for j in range(n_add):
+        if under[j] < 4:
+            allowed[j] = max(0, (pod_off[j + 1] - pod_off[j]) - int(under[j]))
     n_new_vals = n_add + (1 if n_add else 0)
     ls_off = list(delta.arrays["ls_off"]) if delta is not None else [0]
     for it in ls_items:
@@ -528,7 +536,8 @@ def template_churn(enc: EncodedObjects, seed: int, n_change: int, n_remove: int,
         if i < len(changed) and u[i][0] < 0.5:
             rows["alloc"][i][0] = max(1, int(rows["alloc"][i][0] * (0.5 + u[i][1])))
             rows["alloc"][i][1] = max(1, int(rows["alloc"][i][1] * (0.5 + u[i][2])))
-            rows["allowed_pods"][i] = max(len(rows["pods"][i]) + 1, int(ri[7] % 121))
+            # one time in four at or past the DaemonSet pods it holds: every pod fails NodeResourcesFit there
+            rows["allowed_pods"][i] = int(ri[7] % 121) if ri[7] % 4 else max(0, len(rows["pods"][i]) - (ri[7] >> 2) % 2)
     ls_items = sorted(new_ls.items(), key=lambda kv: kv[1])
     ls_off = [0]
     for k, _ in ls_items:
@@ -554,7 +563,8 @@ def daemonset_rollout(enc: EncodedObjects, seed: int):
             pods.pop(0)
         elif pool:
             pods.append(pool[int(pick[t])])
-        rows["allowed_pods"][t] = max(int(rows["allowed_pods"][t]), len(pods) + 1)
+        if t % 5 == 4:   # a template whose DaemonSet pods now fill its pod limit
+            rows["allowed_pods"][t] = len(pods)
     return _template_delta(enc, {}, [], range(T), rows)
 
 

@@ -104,8 +104,7 @@ def main():
             got_e, ref_e = eng.estimate_all(caps), pyoracle.estimate_all(after, caps)
             assert all(np.array_equal(x, y) for x, y in zip(got_e, ref_e[:4]))
             # the filter pass's placements made resident (cae_force_add_pods: CSR append, row state, feed tables, recount),
-            # then what the scale-up asks; pod limits out of reach, see tests/test_gpu_force_add.py
-            after.arrays["node_allowed_pods"][:after.struct.num_cluster_nodes] += 4000
+            # then what the scale-up asks; nodes the filter pass fills to their pod limit and rows the deltas left past it included
             eng.load(after)
             order_p = np.arange(after.P, dtype=np.int32)[::-1].copy()
             assigned = eng.filter_schedulable(order_p)[0]

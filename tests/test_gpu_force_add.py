@@ -21,15 +21,6 @@ from test_gpu_pod_delta import _synth_delta
 pytestmark = pytest.mark.gpu
 
 
-def _roomy(shape):
-    """The shape with pod limits no placement can reach: a cluster node at its pod limit (c_slots <= 0) is where the
-    estimator's hostname-spread fallback is known to differ from the oracle (DESIGN.md §4), with or without this call,
-    and a filter pass fills nodes to exactly that limit.  Resources, not pod slots, bound the placements here."""
-    enc = _gen(shape)
-    enc.arrays["node_allowed_pods"][:enc.struct.num_cluster_nodes] += 4000
-    return enc
-
-
 def _emptied(before, after):
     return int(((np.diff(after.arrays["group_off"]) == 0) & (np.diff(before.arrays["group_off"]) > 0)).sum())
 
@@ -45,7 +36,7 @@ def test_filter_then_scale_up(engines, oracle, shape, want_reasons):
     """one tick of the reference on one engine: the filter pass (hints, similarity classes, a RAW lastIndex) over every
     pending pod, its placements handed back, then everything the scale-up asks"""
     eng, fresh = engines(want_reasons)
-    enc = _roomy(shape)
+    enc = _gen(shape)
     eng.load(enc)
     _, hint, cls, ctrl, ok, _ = _filter_args(enc)
     order = np.arange(enc.P, dtype=np.int32)[::-1].copy()
@@ -54,7 +45,6 @@ def test_filter_then_scale_up(engines, oracle, shape, want_reasons):
     after, want_index = enc.apply_force_add(placed, assigned[placed])
     # not vacuous: a real fraction of the pods moves and a group empties
     assert len(placed) >= enc.P // 10 and after.P > 0 and _emptied(enc, after) >= 1
-    assert _slots_left(after).min() > 0
     new_index = eng.force_add_pods(placed, assigned[placed], after)
     assert np.array_equal(new_index, want_index)
     _check(eng, fresh, oracle, after, want_reasons)
@@ -73,7 +63,7 @@ def test_arbitrary_force_adds(engines, oracle, shape):
     """lists no filter pass produced: random ones, onto unschedulable nodes, all pods of a spread and of an anti-affinity
     group onto one node, and onto full nodes (negative free resources and pod slots)"""
     eng, fresh = engines(True)
-    enc = _roomy(shape)
+    enc = _gen(shape)
     P, N = enc.P, enc.struct.num_cluster_nodes
     go = enc.arrays["group_off"]
     enc.arrays["node_unschedulable"][[2, 7, 11]] = 1
@@ -94,7 +84,6 @@ def test_arbitrary_force_adds(engines, oracle, shape):
         eng.load(enc)
         after, want_index = enc.apply_force_add(pods, nodes)
         assert np.array_equal(eng.force_add_pods(pods, nodes, after), want_index), name
-        assert _slots_left(after).min() > 0
         _check(eng, fresh, oracle, after, True)
     # pod slots that bind without reaching zero: every receiving row ends with 1..3 free slots, so the filter pass and the
     # fallback of the estimate stop on the slots this call took off, and the oracle still applies
@@ -108,17 +97,17 @@ def test_arbitrary_force_adds(engines, oracle, shape):
     assert _slots_left(after).min() == 1 and _slots_left(after).max() == 3
     assert eng.force_add_pods(pods, nodes, after) is not False
     _check(eng, fresh, oracle, after, True)
-    # full nodes: three rows take 60 % of the pods and end far below zero free resources, one of them at a pod limit of
-    # 5.  Compared with the fresh load only: c_slots <= 0 is the fallback divergence from the oracle that _roomy avoids.
-    tight = _roomy(shape)
+    # full nodes: three rows take 60 % of the pods and end far below zero free resources and pod slots, one of them at a pod
+    # limit of 5
+    tight = _gen(shape)
     tight.arrays["node_allowed_pods"][1] = 5
     eng.load(tight)
     pods = rng.permutation(P)[:P * 6 // 10]
     nodes = rng.integers(0, 3, len(pods))
     after, _ = tight.apply_force_add(pods, nodes)
-    assert _slots_left(after)[1] < 0
+    assert (_slots_left(after)[:3] < 0).all()
     assert eng.force_add_pods(pods, nodes, after) is not False
-    _check(eng, fresh, oracle, after, True, with_oracle=False)
+    _check(eng, fresh, oracle, after, True)
 
 
 def _node(name, cpu, pods=30):
@@ -255,7 +244,7 @@ def _placements(eng, enc, n=900):
 @pytest.mark.parametrize("shape", sorted(SHAPES))
 def test_combined_with_the_delta_calls(engines, oracle, shape):
     eng, fresh = engines(True)
-    enc = _roomy(shape)
+    enc = _gen(shape)
     # force_add twice, then a node delta and the pending rows that go with it
     eng.load(enc)
     pods, nodes = _placements(eng, enc)
@@ -266,11 +255,11 @@ def test_combined_with_the_delta_calls(engines, oracle, shape):
     eng.force_add_pods(index[pods[1::2]], nodes[1::2], cur)
     both, _ = enc.apply_force_add(np.concatenate([pods[::2], pods[1::2]]), np.concatenate([nodes[::2], nodes[1::2]]))
     assert np.array_equal(cur.arrays["pend_spec"], both.arrays["pend_spec"])
-    _check(eng, fresh, oracle, cur, True, with_oracle=False)
+    _check(eng, fresh, oracle, cur, True)
     nd, pending = synth.node_churn(cur, 31, 6)
     assert eng.load_nodes(nd) and eng.load_pending(pending)
     cur = pending.apply_node_delta(nd)
-    _check(eng, fresh, oracle, cur, True, with_oracle=False)
+    _check(eng, fresh, oracle, cur, True)
     # new specs arrive, a filter pass places some of their pods too, the placements are handed back
     delta = _synth_delta(cur, 5, 4, keep=1.0)
     cur = cur.apply_pod_delta(delta)
@@ -278,7 +267,7 @@ def test_combined_with_the_delta_calls(engines, oracle, shape):
     pods, nodes = _placements(eng, cur, cur.P)
     cur, _ = cur.apply_force_add(pods, nodes)
     assert eng.force_add_pods(pods, nodes, cur) is not False
-    _check(eng, fresh, oracle, cur, True, with_oracle=False)
+    _check(eng, fresh, oracle, cur, True)
     # the scale-down batch reads the same resident snapshot
     fresh.load(cur)
     move_off = np.array([0, 3, 3, 8], np.int32)

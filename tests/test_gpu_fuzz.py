@@ -128,7 +128,28 @@ def _apply_dims(seed, dims, nodes, pods):
                 p.requests[synth.DIMS[a]] = v
 
 
-def _scenario(seed, big=False, dims=None):
+def _overfill(seed, cluster, extra):
+    """About a quarter of the cluster nodes end up holding more pods than they allow (pod slots 0, -1 or -3), as a kubelet
+    whose max-pods was lowered keeps the pods it runs: such a node gets residents from extra() up to at least three, then
+    allowed pods below that count.  Draws from its own stream (returned), so the scenarios without it stay as they were."""
+    ro = random.Random(seed ^ 0x0F11)
+    for ni in cluster:
+        if ro.random() < 0.25:
+            while len(ni.pods) < 3:
+                ni.pods.append(extra(ro))
+            ni.node.allocatable["pods"] = len(ni.pods) + ro.choice([0, -1, -3])
+    return ro
+
+
+def _host_spread_only(ro, p):
+    """Half the time: p spreads over hostnames against its own app and has no other counter, so the estimator takes its
+    capacity form and the fallback onto the cluster nodes (binpacking_estimator.go:186-205) runs."""
+    if ro.random() < 0.5:
+        p.topology_spread = [TopologySpreadConstraint(ro.randint(1, 2), HOST, LabelSelector(match_labels={"app": p.labels["app"]}))]
+        p.pod_affinity, p.pod_anti_affinity = [], []
+
+
+def _scenario(seed, big=False, dims=None, overfull=False):
     rng = random.Random(seed)
     residents = [_rand_pod(rng, "r%d" % i) for i in range(6)]
     for r in residents:
@@ -148,6 +169,10 @@ def _scenario(seed, big=False, dims=None):
     caps = [rng.choice([0, 0, 3, 8, 20, -1] if big else [0, 0, 1, 2, 5, -1]) for _ in templates]
     if dims is not None:
         _apply_dims(seed, dims, [ni.node for ni in cluster + templates], [g.pods[0] for g in groups])
+    if overfull:
+        ro = _overfill(seed, cluster, lambda ro: ro.choice(residents))
+        for g in groups:
+            _host_spread_only(ro, g.pods[0])
     return cluster, templates, groups, namespaces, caps
 
 
@@ -164,12 +189,12 @@ def test_random_scenarios_every_dim_count(eng, oracle, A):
     _check_random_scenarios(eng, oracle, range(90_000 + 100 * A, 90_000 + 100 * A + 8), rank_layout.DIM_SETS[A])
 
 
-def _check_random_scenarios(eng, oracle, seeds, dims):
+def _check_random_scenarios(eng, oracle, seeds, dims, big=False, overfull=False):
     from kubernetes_autoscaler_b200.engine import EngineUnsupported, unpack_bits
     refused = 0
     fails = []
     for seed in seeds:
-        cluster, templates, groups, namespaces, caps = _scenario(seed, dims=dims)
+        cluster, templates, groups, namespaces, caps = _scenario(seed, big=big, dims=dims, overfull=overfull)
         enc = encode(cluster, templates, groups, namespaces=namespaces)
         try:
             eng.load(enc)
@@ -236,7 +261,7 @@ def test_random_scenarios_larger(eng, oracle, block):
     assert not fails, "Estimate() differs from the oracle: " + "; ".join(fails)
 
 
-def _filter_scenario(seed, dims=None):
+def _filter_scenario(seed, dims=None, overfull=False):
     rng = random.Random(seed)
     residents = [_rand_pod(rng, "r%d" % i) for i in range(8)]
     for r in residents:
@@ -251,6 +276,10 @@ def _filter_scenario(seed, dims=None):
     protos = [_rand_pod(rng, "p%d" % i) for i in range(rng.randint(1, 7))]
     if dims is not None:
         _apply_dims(seed, dims, [ni.node for ni in cluster], protos)
+    if overfull:   # before the pods are cloned from the protos; the main stream draws the same either way
+        ro = _overfill(seed, cluster, lambda ro: ro.choice(residents))
+        for p in protos:
+            _host_spread_only(ro, p)
     pods = []
     for i in range(rng.randint(1, 70)):
         p = rng.choice(protos).clone()
@@ -284,12 +313,12 @@ def test_random_filter_scenarios_every_dim_count(eng, oracle, A):
     _check_filter_scenarios(eng, oracle, range(95_000 + 100 * A, 95_000 + 100 * A + 12), rank_layout.DIM_SETS[A])
 
 
-def _check_filter_scenarios(eng, oracle, seeds, dims):
+def _check_filter_scenarios(eng, oracle, seeds, dims, overfull=False):
     from kubernetes_autoscaler_b200 import podlistprocessor as plp
     from kubernetes_autoscaler_b200.engine import EngineUnsupported
     refused = placed = 0
     for seed in seeds:
-        cluster, pods, hints, namespaces, banned, brk, li = _filter_scenario(seed, dims)
+        cluster, pods, hints, namespaces, banned, brk, li = _filter_scenario(seed, dims, overfull)
         h = plp.Hints()
         for name, node in hints.items():
             h.Set(("default", name), node)

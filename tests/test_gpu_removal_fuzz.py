@@ -19,7 +19,7 @@ from kubernetes_autoscaler_b200 import podlistprocessor as plp
 from kubernetes_autoscaler_b200 import synth
 from kubernetes_autoscaler_b200.objects import (BuildTestPod, LabelSelector, Namespace, NodeInfo, PodAffinityTerm, Taint,
                                                 Toleration, TopologySpreadConstraint, WithLabels)
-from test_gpu_fuzz import _apply_dims, _rand_node, _rand_pod
+from test_gpu_fuzz import _apply_dims, _host_spread_only, _overfill, _rand_node, _rand_pod
 from test_removal_batch import _node, batch, oracle_loop
 
 HOST, ZONE = "kubernetes.io/hostname", "topology.kubernetes.io/zone"
@@ -45,10 +45,11 @@ def _admits(node, pods, p):
     return all(not v or sum(q.requests.get(r, 0) for q in pods) + v <= node.allocatable.get(r, 0) for r, v in p.requests.items())
 
 
-def removal_scenario(seed, dims=None):
+def removal_scenario(seed, dims=None, overfull=False):
     """A random snapshot and a batch over it: dict(cluster, cands, dest, kw) with kw the keyword arguments of both arms.
     `dims`: requests in exactly these resource dims (test_gpu_fuzz._apply_dims); the first candidate's first pod requests
-    all of them and moves, so the pending specs have exactly these active dims."""
+    all of them and moves, so the pending specs have exactly these active dims.  `overfull`: test_gpu_fuzz._overfill,
+    with residents the kubelet would not have admitted."""
     rng = random.Random(seed)
     nodes = [_rand_node(rng, "n%d" % i, False) for i in range(rng.randint(3, 14))]
     pods = []
@@ -106,6 +107,16 @@ def removal_scenario(seed, dims=None):
         pods_to_move.append(keep)
     kw = dict(last_index=rng.randint(len(nodes) + 1, 4 * len(nodes)), hints=hints, pods_to_move=pods_to_move,
               namespaces=[Namespace("other", {"team": "a"})] if rng.random() < 0.5 else [])
+    if overfull:   # residents past what _admits lets in, on about a quarter of the nodes; from a stream of its own
+        extra = []
+
+        def resident(ro):
+            p = _rand_pod(ro, "o%d" % len(extra))
+            p.owner_uid, p.owner_kind = "rs-" + p.labels["app"], "ReplicaSet"
+            _host_spread_only(ro, p)
+            extra.append(p)
+            return p
+        _overfill(seed, cluster, resident)
     return dict(cluster=cluster, cands=cands, dest=dest, kw=kw)
 
 

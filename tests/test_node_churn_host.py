@@ -88,7 +88,7 @@ def test_empty_churn_is_a_no_op(oracle):
     _same_results(oracle, enc0.apply_node_churn(churn), enc0)
 
 
-def test_node_scale_is_deterministic_and_consistent():
+def test_node_scale_is_deterministic_and_draws_rows_past_their_pod_limit():
     enc = synth.generate(3, pods=3000, templates=16, cluster_nodes=40)
     c1, p1 = synth.node_scale(enc, 7, 6, 5, 8)
     c2, p2 = synth.node_scale(enc, 7, 6, 5, 8)
@@ -104,7 +104,9 @@ def test_node_scale_is_deterministic_and_consistent():
     assert after.struct.num_cluster_nodes == 40 - 6 + 5
     assert a["node_pod_off"][-1] == len(a["node_pod_spec"])
     N = after.struct.num_cluster_nodes
-    assert np.all(a["node_allowed_pods"][:N] > np.diff(a["node_pod_off"])[:N])
+    # some rows, dirty or added, allow no more pods than they hold (pod slots <= 0); none allows a negative count
+    slots = a["node_allowed_pods"][:N] - np.diff(a["node_pod_off"])[:N]
+    assert (slots <= 0).any() and (slots > 0).any() and (a["node_allowed_pods"][:N] >= 0).all()
     # every added node has a new hostname value; the residents of an added node are specs resident at the load
     resident = set(enc.arrays["node_pod_spec"].tolist())
     assert set(c1.arrays["pod_spec"].tolist()) <= resident
