@@ -540,6 +540,39 @@ int32_t cae_feasibility(cae_engine* e, uint32_t* fit_bits, uint8_t* reasons, int
  *   reasons [T][E] uint8 */
 int32_t cae_feasibility_groups(cae_engine* e, uint8_t* reasons);
 
+/* Rejection reasons of every pending pod group, counted over the node groups, for the status of the pods that stay
+ * unschedulable.
+ * Replaces: the SchedulingErrors that SchedulablePodGroups (orchestrator.go:603-638) records per (exemplar, node group),
+ * GetRemainingPods (orchestrator.go:843-857) and the aggregation of ReasonsMessage (processors/status/
+ * eventing_scale_up_processor.go) over RejectedNodeGroups, without copying the [T][E] reason matrix to the host.
+ * Reason keys: one column per string PredicateError.Reasons() can hold here.  Keys 1..12 are the enum cae_reason codes,
+ * with two exceptions:
+ *   key CAE_R_PREFILTER_NODEAFFINITY counts only "PreFilterResult excluded the node";
+ *   key CAE_R_FIT counts node groups whose first failing plugin is NodeResourcesFit; its reasons are the keys
+ *   CAE_RK_TOO_MANY_PODS and CAE_RK_INSUFFICIENT + r (fitsRequest, noderesources/fit.go:649-736, lists every one that
+ *   applies).  Keys 0 and 15 stay 0.
+ *   considered [T]    1 = the node group was simulated (a valid scale-up candidate); NULL = all
+ *   exist [T]         1 = NodeGroup.Exist(); ReasonsMessage skips the others; NULL = all
+ *   schedulable [E]   eg.Schedulable: the exemplar of group g fits at least one considered template
+ *   reason_count [E][CAE_REASON_KEYS]
+ *                     templates that are considered, exist and reject group g with key k
+ *   detail [T][E]     may be NULL: RejectedNodeGroups itself, for every template (masks not applied), 0 where the exemplar
+ *                     fits: bits 0-3 the cae_reason code, CAE_RD_PREFILTER_FAILED, CAE_RD_TOO_MANY_PODS, bit 8 + r
+ *                     (CAE_RD_INSUFFICIENT << r) resource dim r insufficient.
+ * A group without pods (emptied by cae_force_add_pods) has no exemplar: all its outputs are 0.  Under
+ * CAE_CFG_PODS_PRESHARDED a rank answers for the groups it holds; no collective is needed.  The call's D2H bytes go to
+ * cae_stats.d2h_bytes.
+ * Status -2 (nothing done): before a load, schedulable or reason_count NULL, a mask byte > 1. */
+#define CAE_RK_PREFILTER_FAILED 13   /* NodeAffinity PreFilter failed: conflicting metadata.name terms */
+#define CAE_RK_TOO_MANY_PODS 14
+#define CAE_RK_INSUFFICIENT 16       /* + resource dim r: "Insufficient <name of dim r>" */
+#define CAE_REASON_KEYS 24           /* CAE_RK_INSUFFICIENT + CAE_MAX_RES */
+#define CAE_RD_PREFILTER_FAILED 16
+#define CAE_RD_TOO_MANY_PODS 32
+#define CAE_RD_INSUFFICIENT 256
+int32_t cae_group_reasons(cae_engine* e, const uint8_t* considered, const uint8_t* exist, uint8_t* schedulable,
+                          int32_t* reason_count, uint16_t* detail);
+
 /* Bin-packing estimate for every template at once.
  * Replaces: BinpackingNodeEstimator.Estimate (estimator/binpacking_estimator.go:97-139) called per
  * node group from ComputeExpansionOption (orchestrator.go:462-520), incl. DecreasingPodOrderer.Order

@@ -175,6 +175,8 @@ def load_engine_lib() -> C.CDLL:
     lib.cae_feasibility.restype = C.c_int32
     lib.cae_feasibility_groups.argtypes = [C.c_void_p, C.c_void_p]
     lib.cae_feasibility_groups.restype = C.c_int32
+    lib.cae_group_reasons.argtypes = [C.c_void_p] + [C.c_void_p] * 5
+    lib.cae_group_reasons.restype = C.c_int32
     lib.cae_estimate_all.argtypes = [C.c_void_p] + [C.c_void_p] * 5
     lib.cae_estimate_all.restype = C.c_int32
     lib.cae_estimate_all_ex.argtypes = [C.c_void_p] + [C.c_void_p] * 7

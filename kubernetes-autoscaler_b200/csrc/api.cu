@@ -1660,6 +1660,55 @@ static int do_similar(Engine* e, const cae_similarity_inputs* in, uint32_t* bits
   return 0;
 }
 
+// cae_group_reasons.  The masks travel in one H2D copy, schedulable and the counts in one D2H copy; the detail matrix goes
+// from the device straight into the caller's buffer.
+static int do_group_reasons(Engine* e, const uint8_t* considered, const uint8_t* exist, uint8_t* sched_out, int32_t* count_out,
+                            uint16_t* detail_out) {
+  const int T = e->T, E = e->E, K = CAE_REASON_KEYS;
+  if (!sched_out || !count_out) { set_error("cae_group_reasons: schedulable and reason_count are required"); return -2; }
+  for (int t = 0; t < T; ++t)
+    if ((considered && considered[t] > 1) || (exist && exist[t] > 1)) { set_error("cae_group_reasons: mask byte > 1"); return -2; }
+  e->stats.h2d_bytes = 0;
+  e->stats.d2h_bytes = 0;
+  if (E == 0) return 0;
+  if (T == 0) {   // no node group: nothing fits, nothing rejects
+    std::fill(sched_out, sched_out + E, (uint8_t)0);
+    std::fill(count_out, count_out + (size_t)E * K, 0);
+    return 0;
+  }
+  Engine::Staging& st = e->gr;
+  GroupReasonLaunch a{};
+  size_t in_end = 0, out_end = 0;
+  auto walk = [&](Layout& l) {
+    l.add(a.mask, T);
+    in_end = l.bytes;
+    l.add(a.sched, E); l.add(a.count, (size_t)E * K);
+    out_end = l.bytes;
+    if (detail_out) l.add(a.detail, (size_t)T * E);
+  };
+  const size_t bytes = layout_bytes(walk);   // sets out_end: a separate statement, argument order is unspecified
+  if (stage_reserve(e, st, bytes, out_end)) return -1;
+  layout_bind(st.dev.p, walk);
+  if (!detail_out) a.detail = nullptr;
+  uint8_t* h_mask = st.host_of(a.mask);
+  for (int t = 0; t < T; ++t)
+    h_mask[t] = (uint8_t)((!considered || considered[t] ? GR_CONSIDERED : 0) | (!exist || exist[t] ? GR_EXIST : 0));
+  if (stage_upload(e, st, in_end)) return -1;
+  CAE_CUDA(cudaMemsetAsync(a.sched, 0, out_end - in_end, e->stream));
+  if (launch_group_reason_counts(e, a)) return -1;
+  CAE_CUDA(cudaMemcpyAsync(st.host_of(a.sched), a.sched, out_end - in_end, cudaMemcpyDeviceToHost, e->stream));
+  size_t d2h = out_end - in_end;
+  if (detail_out) {
+    CAE_CUDA(cudaMemcpyAsync(detail_out, a.detail, sizeof(uint16_t) * (size_t)T * E, cudaMemcpyDeviceToHost, e->stream));
+    d2h += sizeof(uint16_t) * (size_t)T * E;
+  }
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
+  e->stats.d2h_bytes = (int64_t)d2h;
+  std::copy(st.host_of(a.sched), st.host_of(a.sched) + E, sched_out);
+  std::copy(st.host_of(a.count), st.host_of(a.count) + (size_t)E * K, count_out);
+  return 0;
+}
+
 }  // namespace cae
 
 using cae::Engine;
@@ -1929,6 +1978,14 @@ int32_t cae_feasibility_groups(cae_engine* h, uint8_t* reasons) {
     CAE_CUDA(cudaMemcpyAsync(reasons, e->d_group_reason, (size_t)e->T * e->E, cudaMemcpyDeviceToHost, e->stream));
   CAE_CUDA(cudaStreamSynchronize(e->stream));
   return 0;
+}
+
+int32_t cae_group_reasons(cae_engine* h, const uint8_t* considered, const uint8_t* exist, uint8_t* schedulable,
+                          int32_t* reason_count, uint16_t* detail) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_group_reasons before cae_load"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_group_reasons(e, considered, exist, schedulable, reason_count, detail);
 }
 
 int32_t cae_estimate_all(cae_engine* h, const int32_t* max_nodes, int32_t* node_count, int32_t* pod_count,

@@ -356,6 +356,7 @@ struct Engine {
   DevBuf tp_dyn;                          // dom [K][N+T] | elig [Q][U]
   // buffers of cae_similar_node_groups (similar.cu)
   Staging sim;                            // inputs | outputs (one D2H copy) | operand rows | schedulable bit rows (device only)
+  Staging gr;                             // cae_group_reasons: masks | schedulable, counts (one D2H copy) | detail (device only)
   int sm_count = 132;
   int smem_optin = 227 * 1024;             // opt-in shared memory per thread block
   size_t hbm_bytes = (size_t)80 << 30;     // device memory (sizes the estimator's global slabs)
@@ -427,6 +428,22 @@ int launch_expand_pods(Engine* e);
 int launch_port_conflicts(Engine* e, int num_port_lists);
 int launch_feasibility(Engine* e, bool want_reasons);
 int launch_group_feasibility(Engine* e);
+// cae_group_reasons (kernels.cu).  In: mask [T] (GR_CONSIDERED | GR_EXIST).  Out (pre-zeroed by api.cu): sched [E],
+// count [E][CAE_REASON_KEYS], detail [T][E] or NULL.  The launch fills in the shapes and the engine's tables, and computes
+// the group reasons first when they are stale.
+static_assert(CAE_REASON_KEYS == CAE_RK_INSUFFICIENT + CAE_MAX_RES, "one key per resource dim after the fixed keys");
+enum : int { GR_CONSIDERED = 1, GR_EXIST = 2 };
+struct GroupReasonLaunch {
+  int E, T, span;                         // span: templates per block row
+  const uint8_t* code;                    // [T][E] group reasons
+  const int64_t* free_all;                // [R][T]
+  const int32_t* slots;                   // [T]
+  const uint8_t* mask;
+  uint8_t* sched;
+  int32_t* count;
+  uint16_t* detail;
+};
+int launch_group_reason_counts(Engine* e, GroupReasonLaunch a);
 int launch_order(Engine* e);
 int launch_group_records(Engine* e);     // GroupRec[E] (after the class / counter tables of a load)
 GroupRecSrc group_rec_src(const Engine* e);

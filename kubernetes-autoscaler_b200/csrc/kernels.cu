@@ -4,11 +4,13 @@
 //   pack_ok_bits_kernel   byte matrix -> per-class template bit words
 //   (K1, the dense pods x templates pass, lives in feas.cu; K3, the estimator, in binpack.cu)
 //   group_reason_kernel   exemplar x template reasons (what SchedulablePodGroups asks)
+//   group_reason_count_kernel   the same reasons counted per group and reason key (cae_group_reasons)
 //   order_kernel          K0: DecreasingPodOrderer per template (float64 score, stable bitonic sort)
 //   waste_kernel          K4: least-waste score per option
 //
 // Integer / bitset work only: no tensor cores (SURVEY.md §2.4).  Grid sizes are multiples of the SM
 // count where the work allows; per-template rows are staged in shared memory and broadcast.
+#include <algorithm>
 #include <cfloat>
 #include <climits>
 
@@ -74,11 +76,8 @@ __global__ void group_reason_kernel(DevObjects o, int E, int T, int N, int U, co
     int spec = o.pend_spec[o.group_off[g]];
     r = pre_code[(size_t)spec_sc[spec] * U + N + t] & 0x0F;
     if (r == 0) {
-      bool fail = tmpl_slots[t] < 1;
-      for (int a = 0; a < R; ++a) {
-        int64_t q = o.ps_req[(size_t)spec * R + a];
-        fail |= (q > 0 && q > tmpl_free_all[(size_t)a * T + t]);
-      }
+      const uint32_t fail = fit_fail_mask(o.ps_req + (size_t)spec * R, tmpl_slots[t],
+                                          [&](int a) { return tmpl_free_all[(size_t)a * T + t]; });
       r = fail ? CAE_R_FIT : post_code[(size_t)spec_dc[spec] * T + t];
     }
   }
@@ -94,6 +93,102 @@ int launch_group_feasibility(Engine* e) {
   e->stats.kernel_launches++;
   CAE_KERNEL_OK();
   e->group_reason_valid = true;
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// cae_group_reasons: the group reasons counted per reason key
+// ------------------------------------------------------------------------------------------------
+// Thread = group, block = GR_GROUPS groups x a span of templates, walked in staged chunks of GR_TCH: the codes [t][g] are
+// read along g (coalesced), a NodeResourcesFit code is expanded into its failure set from the staged template columns.
+// Counters live in shared memory ([key][thread]: a run-time key index into a register array would go to local memory)
+// and are added to the pre-zeroed [E][K] result with integer atomics, so the sums do not depend on block order.
+constexpr int GR_GROUPS = 128;
+constexpr int GR_TCH = 64;
+
+__global__ void __launch_bounds__(GR_GROUPS) group_reason_count_kernel(DevObjects o, GroupReasonLaunch a) {
+  __shared__ int32_t s_cnt[CAE_REASON_KEYS][GR_GROUPS];
+  __shared__ int64_t s_free[R][GR_TCH];
+  __shared__ int32_t s_slots[GR_TCH];
+  __shared__ uint8_t s_mask[GR_TCH];
+  const int tid = threadIdx.x, g = blockIdx.x * GR_GROUPS + tid;
+  const int tb = blockIdx.y * a.span, te = min(a.T, tb + a.span);
+#pragma unroll
+  for (int k = 0; k < CAE_REASON_KEYS; ++k) s_cnt[k][tid] = 0;
+  const bool live = g < a.E && o.group_off[g + 1] > o.group_off[g];
+  int64_t req[R];
+  bool pf_failed = false;
+  {
+    const int spec = live ? o.pend_spec[o.group_off[g]] : 0;
+#pragma unroll
+    for (int r = 0; r < R; ++r) req[r] = live ? o.ps_req[(size_t)spec * R + r] : 0;
+    // "PreFilter failed" (conflicting metadata.name terms) depends on the pod alone: any node answers it
+    if (live) pf_failed = naff_prefilter(o, o.ps_naff[spec], unode(o, o.N)) == 3;
+  }
+  bool sched = false;
+  for (int t0 = tb; t0 < te; t0 += GR_TCH) {
+    const int n = min(GR_TCH, te - t0);
+    __syncthreads();   // every read of the previous chunk is done
+    for (int i = tid; i < R * GR_TCH; i += GR_GROUPS) {
+      const int r = i / GR_TCH, j = i % GR_TCH;
+      if (j < n) s_free[r][j] = a.free_all[(size_t)r * a.T + t0 + j];
+    }
+    for (int j = tid; j < n; j += GR_GROUPS) {
+      s_slots[j] = a.slots[t0 + j];
+      s_mask[j] = a.mask[t0 + j];
+    }
+    __syncthreads();
+    if (g >= a.E) continue;
+    for (int j = 0; j < n; ++j) {
+      const int t = t0 + j;
+      const uint32_t c = live ? a.code[(size_t)t * a.E + g] : 0u;
+      uint32_t d = c;
+      if (c == CAE_R_FIT) d |= fit_fail_mask(req, s_slots[j], [&](int r) { return s_free[r][j]; });
+      else if (c == CAE_R_PREFILTER_NODEAFFINITY && pf_failed) d |= CAE_RD_PREFILTER_FAILED;
+      if (a.detail) a.detail[(size_t)t * a.E + g] = (uint16_t)d;
+      const int m = s_mask[j];
+      if (!(m & GR_CONSIDERED)) continue;
+      if (c == CAE_R_OK) {
+        sched |= live;
+        continue;
+      }
+      if (!(m & GR_EXIST)) continue;
+      s_cnt[(d & CAE_RD_PREFILTER_FAILED) ? CAE_RK_PREFILTER_FAILED : (int)c][tid] += 1;
+      if (c == CAE_R_FIT) {
+        if (d & CAE_RD_TOO_MANY_PODS) s_cnt[CAE_RK_TOO_MANY_PODS][tid] += 1;
+#pragma unroll
+        for (int r = 0; r < R; ++r)
+          if (d & ((uint32_t)CAE_RD_INSUFFICIENT << r)) s_cnt[CAE_RK_INSUFFICIENT + r][tid] += 1;
+      }
+    }
+  }
+  if (g >= a.E) return;
+  if (sched) a.sched[g] = 1;
+#pragma unroll
+  for (int k = 0; k < CAE_REASON_KEYS; ++k) {
+    const int c = s_cnt[k][tid];
+    if (c) atomicAdd(&a.count[(size_t)g * CAE_REASON_KEYS + k], c);
+  }
+}
+
+int launch_group_reason_counts(Engine* e, GroupReasonLaunch a) {
+  if (e->E == 0 || e->T == 0) return 0;
+  if (!e->group_reason_valid && launch_group_feasibility(e)) return -1;
+  // at least two waves of blocks: the template span per block follows from the resident blocks per SM
+  int per_sm = 1;
+  CAE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, group_reason_count_kernel, GR_GROUPS, 0));
+  const int gx = (e->E + GR_GROUPS - 1) / GR_GROUPS;
+  const long long want = 2LL * e->sm_count * std::max(per_sm, 1);
+  const int gy = (int)std::min<long long>(e->T, (want + gx - 1) / gx);
+  a.E = e->E;
+  a.T = e->T;
+  a.span = (e->T + gy - 1) / gy;
+  a.code = e->d_group_reason;
+  a.free_all = e->d_tmpl_free_all;
+  a.slots = e->d_tmpl_slots;
+  group_reason_count_kernel<<<dim3(gx, (e->T + a.span - 1) / a.span), GR_GROUPS, 0, e->stream>>>(e->dobj, a);
+  e->stats.kernel_launches++;
+  CAE_KERNEL_OK();
   return 0;
 }
 

@@ -194,6 +194,18 @@ __device__ __forceinline__ bool port_lists_conflict(const DevObjects& o, int a, 
   return false;
 }
 
+// NodeResourcesFit fitsRequest (noderesources/fit.go:649-736) on a node with `slots` free pod slots and free(r) =
+// allocatable - requested in dim r: every failing part as cae_group_reasons detail bits (CAE_RD_TOO_MANY_PODS,
+// CAE_RD_INSUFFICIENT << r), 0 = the pod fits.  A dim the pod does not request is never checked (fit.go:670-704).
+template <class Free>
+__device__ __forceinline__ uint32_t fit_fail_mask(const int64_t* req, int slots, Free free) {
+  uint32_t m = slots < 1 ? (uint32_t)CAE_RD_TOO_MANY_PODS : 0u;
+#pragma unroll
+  for (int r = 0; r < R; ++r)
+    if (req[r] > 0 && req[r] > free(r)) m |= (uint32_t)CAE_RD_INSUFFICIENT << r;
+  return m;
+}
+
 // ---- static (pod-state independent) part of RunFiltersOnNode for (static class, universe node) ----
 // code byte: low nibble = first failing reason among PREFILTER, NodeUnschedulable, NodeName,
 // TaintToleration, NodeAffinity, NodePorts-vs-pods-already-on-the-node (0 = none);

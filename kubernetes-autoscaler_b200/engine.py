@@ -234,6 +234,23 @@ class Engine:
         self._check(self.lib.cae_feasibility_groups(self.h, out.ctypes.data_as(C.c_void_p)))
         return out
 
+    def group_reasons(self, considered=None, exist=None, want_detail: bool = False):
+        """cae_group_reasons: every group's rejection reasons counted over the node groups.  considered / exist: [T] flags
+        (None = all).  Returns (schedulable [E] uint8, counts [E][CAE_REASON_KEYS] int32, detail [T][E] uint16 | None)."""
+        enc = self.enc
+        T, E = enc.T, enc.E
+        opt = lambda a: None if a is None else np.ascontiguousarray(a, np.uint8)
+        cons, ex = opt(considered), opt(exist)
+        for m in (cons, ex):
+            if m is not None and m.shape != (T,):
+                raise ValueError("group_reasons: a mask needs one flag per template")
+        sched = np.zeros(E, np.uint8)
+        counts = np.zeros((E, capi.CONST["CAE_REASON_KEYS"]), np.int32)
+        detail = np.zeros((T, E), np.uint16) if want_detail else None
+        vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+        self._check(self.lib.cae_group_reasons(self.h, vp(cons), vp(ex), vp(sched), vp(counts), vp(detail)))
+        return sched, counts, detail
+
     def estimate_all_li(self, max_nodes, last_index_in):
         """cae_estimate_all_ex: Estimate of every template with the plugin runner's lastIndex carried in per template.
         Returns node_count, pod_count, sched, order, last_index_out."""

@@ -25,6 +25,7 @@ from . import capi
 from .encode import EncodedObjects, Encoder, Unsupported, encode
 from .engine import Engine
 from .objects import NodeInfo, Pod, PodEquivalenceGroup
+from .scaleupstatus import GetRemainingPods, NoScaleUpInfo, count_reasons, detail_reasons, reason_key_strings
 
 
 # ---- limiter (host logic; integer only) -----------------------------------------------------
@@ -236,6 +237,23 @@ class ScaleUpSimulation:
         """orchestrator.go:603-638 for every node group: indices of the groups whose exemplar fits."""
         reasons = self.engine.feasibility_groups()
         return {ng: [g for g in range(len(self.groups)) if reasons[t][g] == 0] for t, ng in enumerate(self.ids)}
+
+    def no_scale_up_infos(self, exist: Optional[Dict[str, bool]] = None, skipped: Optional[Dict[str, List[str]]] = None,
+                          want_detail: bool = False, all_unschedulable: bool = False) -> List[NoScaleUpInfo]:
+        """ScaleUpStatus.PodsRemainUnschedulable (GetRemainingPods, orchestrator.go:843-857) from cae_group_reasons: every
+        loaded template is a considered node group.  exist: node-group id -> Exist() (missing ids exist); skipped: the
+        SkippedNodeGroups reasons; want_detail: also fill RejectedNodeGroups (copies the [T][E] detail);
+        all_unschedulable: every group counts as unschedulable (stopAllOrNothingScaleUp)."""
+        ex = None if exist is None else [1 if exist.get(i, True) else 0 for i in self.ids]
+        sched, counts, detail = self.engine.group_reasons(None, ex, want_detail)
+        keys = reason_key_strings(self.encoder.resources.items)
+        rejected = None
+        if detail is not None:
+            rejected = [{self.ids[t]: detail_reasons(detail[t, g], keys) for t in np.flatnonzero(detail[:, g])}
+                        for g in range(len(self.groups))]
+        if all_unschedulable:
+            sched = np.zeros_like(sched)
+        return GetRemainingPods(self.groups, sched, [count_reasons(row, keys) for row in counts], rejected, dict(skipped or {}))
 
     def similar_node_groups(self, node_groups: Sequence[NodeGroupInfo], extra_ignored_labels: Sequence[str] = (),
                             ratios: NodeGroupDifferenceRatios = NodeGroupDifferenceRatios(), safe=None,
