@@ -149,7 +149,8 @@ def _host_spread_only(ro, p):
         p.pod_affinity, p.pod_anti_affinity = [], []
 
 
-def _scenario(seed, big=False, dims=None, overfull=False):
+def _scenario(seed, big=False, dims=None, overfull=False, nodes=None, group_pods=None):
+    """`nodes`: that many cluster nodes; `group_pods`: groups of 1..group_pods pods.  Unset, the draws are as they were."""
     rng = random.Random(seed)
     residents = [_rand_pod(rng, "r%d" % i) for i in range(6)]
     for r in residents:
@@ -158,12 +159,12 @@ def _scenario(seed, big=False, dims=None, overfull=False):
         if rng.random() < 0.1:
             r.terminating = True
     cluster = [NodeInfo(_rand_node(rng, "c%d" % i, False), [rng.choice(residents) for _ in range(rng.randint(0, 3))])
-               for i in range(rng.randint(8, 40) if big else rng.randint(0, 6))]
+               for i in range(nodes if nodes is not None else rng.randint(8, 40) if big else rng.randint(0, 6))]
     ds = BuildTestPod("ds", 50, 1 << 24)
     ds.labels = {"app": rng.choice(APPS)}
     ds.tolerations = [Toleration("", "Exists", "", "")]
     templates = [NodeInfo(_rand_node(rng, "t%d" % i, True), [ds] if rng.random() < 0.5 else []) for i in range(rng.randint(1, 5))]
-    groups = [makePodEquivalenceGroup(_rand_pod(rng, "p%d" % i), rng.randint(1, 60) if big else rng.randint(1, 9))
+    groups = [makePodEquivalenceGroup(_rand_pod(rng, "p%d" % i), rng.randint(1, group_pods or (60 if big else 9)))
               for i in range(rng.randint(3, 14) if big else rng.randint(1, 8))]
     namespaces = [Namespace("other", {"team": "a"})] if rng.random() < 0.5 else []
     caps = [rng.choice([0, 0, 3, 8, 20, -1] if big else [0, 0, 1, 2, 5, -1]) for _ in templates]
@@ -261,14 +262,16 @@ def test_random_scenarios_larger(eng, oracle, block):
     assert not fails, "Estimate() differs from the oracle: " + "; ".join(fails)
 
 
-def _filter_scenario(seed, dims=None, overfull=False):
+def _filter_scenario(seed, dims=None, overfull=False, nodes=None, pod_range=(1, 70)):
+    """`nodes`: that many cluster nodes; `pod_range`: the bounds of the pending pod count.  Unset, the draws are as they
+    were."""
     rng = random.Random(seed)
     residents = [_rand_pod(rng, "r%d" % i) for i in range(8)]
     for r in residents:
         r.requests = {"cpu": rng.choice([100, 400]), "memory": 1 << 26}
         r.host_ports = []
     cluster = []
-    for i in range(rng.randint(1, 45)):
+    for i in range(nodes if nodes is not None else rng.randint(1, 45)):
         n = _rand_node(rng, "c%d" % i, False)
         if rng.random() < 0.1:
             n.unschedulable = True
@@ -281,7 +284,7 @@ def _filter_scenario(seed, dims=None, overfull=False):
         for p in protos:
             _host_spread_only(ro, p)
     pods = []
-    for i in range(rng.randint(1, 70)):
+    for i in range(rng.randint(*pod_range)):
         p = rng.choice(protos).clone()
         p.name = "q%d" % i
         if rng.random() < 0.7:
@@ -313,12 +316,12 @@ def test_random_filter_scenarios_every_dim_count(eng, oracle, A):
     _check_filter_scenarios(eng, oracle, range(95_000 + 100 * A, 95_000 + 100 * A + 12), rank_layout.DIM_SETS[A])
 
 
-def _check_filter_scenarios(eng, oracle, seeds, dims, overfull=False):
+def _check_filter_scenarios(eng, oracle, seeds, dims, overfull=False, scenario=_filter_scenario):
     from kubernetes_autoscaler_b200 import podlistprocessor as plp
     from kubernetes_autoscaler_b200.engine import EngineUnsupported
     refused = placed = 0
     for seed in seeds:
-        cluster, pods, hints, namespaces, banned, brk, li = _filter_scenario(seed, dims, overfull)
+        cluster, pods, hints, namespaces, banned, brk, li = scenario(seed, dims, overfull)
         h = plp.Hints()
         for name, node in hints.items():
             h.Set(("default", name), node)

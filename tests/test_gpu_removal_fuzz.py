@@ -45,13 +45,13 @@ def _admits(node, pods, p):
     return all(not v or sum(q.requests.get(r, 0) for q in pods) + v <= node.allocatable.get(r, 0) for r, v in p.requests.items())
 
 
-def removal_scenario(seed, dims=None, overfull=False):
+def removal_scenario(seed, dims=None, overfull=False, nodes=None):
     """A random snapshot and a batch over it: dict(cluster, cands, dest, kw) with kw the keyword arguments of both arms.
     `dims`: requests in exactly these resource dims (test_gpu_fuzz._apply_dims); the first candidate's first pod requests
     all of them and moves, so the pending specs have exactly these active dims.  `overfull`: test_gpu_fuzz._overfill,
-    with residents the kubelet would not have admitted."""
+    with residents the kubelet would not have admitted.  `nodes`: that many nodes (unset: 3-14, drawn as before)."""
     rng = random.Random(seed)
-    nodes = [_rand_node(rng, "n%d" % i, False) for i in range(rng.randint(3, 14))]
+    nodes = [_rand_node(rng, "n%d" % i, False) for i in range(nodes if nodes is not None else rng.randint(3, 14))]
     pods = []
     for i in range(rng.randint(1, 3) * len(nodes)):
         p = _rand_pod(rng, "r%d" % i)
@@ -157,12 +157,12 @@ def _gpu_check(eng, scn, persist):
     return got
 
 
-def _run_seeds(eng, seeds):
+def _run_seeds(eng, seeds, scenario=removal_scenario):
     from kubernetes_autoscaler_b200.engine import EngineUnsupported
     refused = 0
     mix = Mix()
     for seed in seeds:
-        scn = removal_scenario(seed) if not isinstance(seed, tuple) else removal_scenario(*seed)
+        scn = scenario(seed) if not isinstance(seed, tuple) else scenario(*seed)
         for persist in (False, True):
             try:
                 got = _gpu_check(eng, scn, persist)
