@@ -1,9 +1,9 @@
 """ctypes view of ``include/caengine.h``.
 
-The struct layouts are parsed from the header at import time so that the header stays the single
-source of truth for the ABI (a field added there is picked up here; a mismatch cannot happen
-silently).  Only ``int32_t`` / ``int64_t`` / ``double`` scalars, arrays of them and ``const T*``
-pointers appear in the ABI structs.
+The struct layouts and the function signatures are parsed from the header so that the header stays
+the single source of truth for the ABI (a field or parameter added there is picked up here; a
+mismatch cannot happen silently).  Only ``int32_t`` / ``int64_t`` / ``double`` scalars, arrays of
+them and ``const T*`` pointers appear in the ABI structs.
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ HEADER = os.path.join(REPO_ROOT, "include", "caengine.h")
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 ENGINE_LIB = os.path.join(PKG_DIR, "libcaengine.so")
 
-_SCALARS = {"int32_t": C.c_int32, "int64_t": C.c_int64, "uint8_t": C.c_uint8,
+_SCALARS = {"int32_t": C.c_int32, "int64_t": C.c_int64, "uint8_t": C.c_uint8, "uint16_t": C.c_uint16,
             "uint32_t": C.c_uint32, "double": C.c_double, "size_t": C.c_size_t}
 
 
@@ -112,9 +112,48 @@ class cae_similarity_inputs(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_similarity_inputs")
 
 
+_STRUCTS = {s.__name__: s for s in (cae_objects, cae_config, cae_stats, cae_price_inputs, cae_node_delta, cae_node_churn,
+                                     cae_template_delta, cae_pod_delta, cae_similarity_inputs)}
+
+
+def _ctype(decl: str, opaque, where: str):
+    """ctypes type of one C declaration (a return type or a parameter, its name optional); None for ``void``."""
+    m = re.fullmatch(r"(?:const\s+)?(\w+)\s*(\**)\s*(?:\w+)?", decl.strip())
+    base, stars = (m.group(1), len(m.group(2))) if m else (None, 0)
+    if stars and (base in _SCALARS or base in _STRUCTS or base in opaque or base in ("void", "char")):
+        if stars > 1:
+            return C.POINTER(C.c_void_p)
+        if base == "char":
+            return C.c_char_p
+        if base == "size_t":
+            return C.POINTER(C.c_size_t)
+        return C.POINTER(_STRUCTS[base]) if base in _STRUCTS else C.c_void_p
+    if not stars and (base in _SCALARS or base == "void"):
+        return _SCALARS.get(base)
+    raise RuntimeError("cannot map the C type %r of %s" % (decl.strip(), where))
+
+
+def signatures(src: str) -> Dict[str, Tuple[object, List[object]]]:
+    """{function: (restype, argtypes)} of every prototype in the comment-stripped header source `src`."""
+    opaque = set(re.findall(r"typedef struct (\w+) \1;", src))
+    out: Dict[str, Tuple[object, List[object]]] = {}
+    for m in re.finditer(r"^((?:const\s+)?\w+\s*\**)\s*(cae_\w+)\s*\(([^()]*)\)\s*;", src, flags=re.M):
+        name, params = m.group(2), [p for p in m.group(3).split(",") if p.strip()]
+        if [p.strip() for p in params] == ["void"]:
+            params = []
+        args = [_ctype(p, opaque, name) for p in params]
+        if None in args:
+            raise RuntimeError("%s has a void parameter" % name)
+        out[name] = (_ctype(m.group(1), opaque, name), args)
+    missed = set(re.findall(r"\b(cae_\w+)\s*\(", src)) - set(out)
+    if missed:
+        raise RuntimeError("cannot parse the prototypes of %s" % sorted(missed))
+    return out
+
+
 def declared_functions() -> List[str]:
     """Names of every function the header declares (used by the symbol-export test)."""
-    return sorted(set(re.findall(r"\b(cae_\w+)\s*\(", _SRC)))
+    return sorted(signatures(_SRC))
 
 
 REASON_NAMES = {v: k for k, v in CONST.items() if k.startswith("CAE_R_")}
@@ -150,65 +189,8 @@ def load_engine_lib() -> C.CDLL:
             "libcaengine.so is missing (%s): build it with `python -c 'import __graft_entry__ as g; "
             "g.build()'`. The engine has no CPU fallback." % path)
     lib = C.CDLL(path, mode=C.RTLD_GLOBAL)
-    P = C.POINTER
-    lib.cae_create.argtypes = [P(cae_config), P(C.c_void_p)]
-    lib.cae_create.restype = C.c_int32
-    lib.cae_destroy.argtypes = [C.c_void_p]
-    lib.cae_destroy.restype = None
-    lib.cae_last_error.restype = C.c_char_p
-    lib.cae_version.restype = C.c_char_p
-    lib.cae_load.argtypes = [C.c_void_p, P(cae_objects)]
-    lib.cae_load.restype = C.c_int32
-    lib.cae_load_pending.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
-    lib.cae_load_pending.restype = C.c_int32
-    lib.cae_load_nodes.argtypes = [C.c_void_p, P(cae_node_delta)]
-    lib.cae_load_nodes.restype = C.c_int32
-    lib.cae_load_node_churn.argtypes = [C.c_void_p, P(cae_node_churn)]
-    lib.cae_load_node_churn.restype = C.c_int32
-    lib.cae_load_templates.argtypes = [C.c_void_p, P(cae_template_delta)]
-    lib.cae_load_templates.restype = C.c_int32
-    lib.cae_load_pods.argtypes = [C.c_void_p, P(cae_pod_delta)]
-    lib.cae_load_pods.restype = C.c_int32
-    lib.cae_force_add_pods.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.cae_force_add_pods.restype = C.c_int32
-    lib.cae_feasibility.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.cae_feasibility.restype = C.c_int32
-    lib.cae_feasibility_groups.argtypes = [C.c_void_p, C.c_void_p]
-    lib.cae_feasibility_groups.restype = C.c_int32
-    lib.cae_group_reasons.argtypes = [C.c_void_p] + [C.c_void_p] * 5
-    lib.cae_group_reasons.restype = C.c_int32
-    lib.cae_estimate_all.argtypes = [C.c_void_p] + [C.c_void_p] * 5
-    lib.cae_estimate_all.restype = C.c_int32
-    lib.cae_estimate_all_ex.argtypes = [C.c_void_p] + [C.c_void_p] * 7
-    lib.cae_estimate_all_ex.restype = C.c_int32
-    lib.cae_expander_best.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
-                                      C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.cae_expander_best.restype = C.c_int32
-    lib.cae_get_stats.argtypes = [C.c_void_p, P(cae_stats)]
-    lib.cae_get_stats.restype = C.c_int32
-    lib.cae_peer_handle.argtypes = [C.c_void_p, C.c_void_p]
-    lib.cae_peer_handle.restype = C.c_int32
-    lib.cae_peer_attach.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
-    lib.cae_peer_attach.restype = C.c_int32
-    lib.cae_device_buffer.argtypes = [C.c_void_p, C.c_int32, P(C.c_size_t)]
-    lib.cae_device_buffer.restype = C.c_void_p
-    lib.cae_filter_schedulable.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
-                                           C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.cae_filter_schedulable.restype = C.c_int32
-    lib.cae_simulate_removals.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 7 + [C.c_int32] * 3 + [C.c_void_p] * 3 + \
-        [C.c_int32, C.c_void_p]
-    lib.cae_simulate_removals.restype = C.c_int32
-    lib.cae_price_scores.argtypes =[C.c_void_p, P(cae_price_inputs), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.cae_price_scores.restype = C.c_int32
-    lib.cae_expander_chain_ex.argtypes = [C.c_void_p, C.c_int32, C.c_int32] + [C.c_void_p] * 7
-    lib.cae_expander_chain_ex.restype = C.c_int32
-    lib.cae_waste_scores.argtypes = [C.c_void_p, C.c_void_p]
-    lib.cae_waste_scores.restype = C.c_int32
-    lib.cae_expander_chain.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.cae_expander_chain.restype = C.c_int32
-    lib.cae_similar_node_groups.argtypes = [C.c_void_p, P(cae_similarity_inputs), C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.cae_similar_node_groups.restype = C.c_int32
-    lib.cae_stream.argtypes = [C.c_void_p]
-    lib.cae_stream.restype = C.c_void_p
+    for name, (restype, argtypes) in signatures(_SRC).items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _engine_lib = lib
     return lib

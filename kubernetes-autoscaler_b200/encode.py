@@ -457,10 +457,7 @@ class EncodedObjects:
         s.num_templates = b.num_templates
         s.num_groups = len(b.group_off) - 1
         s.num_pending = int(b.group_off[-1])
-        for name, ctype in capi.cae_objects._fields_:
-            if name in a:
-                arr = a[name]
-                setattr(s, name, arr.ctypes.data_as(ctype))
+        _fill_pointers(s, a)
         missing = [n for n, t in capi.cae_objects._fields_
                    if n not in a and hasattr(t, "contents")]
         if missing:
@@ -476,13 +473,7 @@ class EncodedObjects:
         go = np.clip(self.arrays["group_off"], p_begin, p_end) - p_begin
         out.arrays["group_off"] = np.ascontiguousarray(go.astype(np.int32))
         out.arrays["pend_spec"] = np.ascontiguousarray(self.arrays["pend_spec"][p_begin:p_end])
-        s = capi.cae_objects()
-        C.memmove(C.byref(s), C.byref(self.struct), C.sizeof(s))
-        s.num_pending = p_end - p_begin
-        for name, ctype in capi.cae_objects._fields_:
-            if name in ("group_off", "pend_spec"):
-                setattr(s, name, out.arrays[name].ctypes.data_as(ctype))
-        out.struct = s
+        out.struct = self._restruct(out.arrays, num_pending=p_end - p_begin)
         return out
 
     def with_pending(self, pend_spec, group_off) -> "EncodedObjects":
@@ -655,9 +646,7 @@ class EncodedObjects:
         C.memmove(C.byref(s), C.byref(self.struct), C.sizeof(s))
         for k, v in counts.items():
             setattr(s, k, v)
-        for name, ctype in capi.cae_objects._fields_:
-            if name in arrays:
-                setattr(s, name, arrays[name].ctypes.data_as(ctype))
+        _fill_pointers(s, arrays)
         return s
 
     # convenience
@@ -677,182 +666,132 @@ class EncodedObjects:
         return C.byref(self.struct)
 
 
-class NodeDelta:
-    """Owns the numpy arrays behind one ``cae_node_delta`` struct: the dictionary tails (values, label sets, taint lists
-    that continue the resident tables; offsets relative to the tail) and the complete new state of the dirty cluster
-    rows.  Field names are the header's."""
+def _fill_pointers(s, arrays: Dict[str, np.ndarray]) -> None:
+    """Point every field of the ctypes struct `s` that names one of `arrays` at that array."""
+    for name, ctype in s._fields_:
+        if name in arrays:
+            setattr(s, name, arrays[name].ctypes.data_as(ctype))
 
-    _I32 = ("ls_off", "ls_key", "ls_val", "taint_off", "taint_key", "taint_val", "taint_effect", "row", "labelset",
-            "taint_list", "allowed_pods", "pod_off", "pod_spec")
 
-    def __init__(self, **arrays) -> None:
-        a: Dict[str, np.ndarray] = {}
-        for nm in self._I32:
-            a[nm] = _i32(arrays.get(nm, [0] if nm in ("ls_off", "taint_off", "pod_off") else []))
-        a["value_is_int"] = np.ascontiguousarray(arrays.get("value_is_int", []), np.uint8)
-        a["value_int"] = np.ascontiguousarray(arrays.get("value_int", []), np.int64)
-        a["unschedulable"] = np.ascontiguousarray(arrays.get("unschedulable", []), np.uint8)
-        nd = len(a["row"])
-        a["alloc"] = np.ascontiguousarray(np.asarray(arrays.get("alloc", np.zeros((nd, MAX_RES))), np.int64).reshape(nd, MAX_RES))
-        self.arrays = a
-        s = capi.cae_node_delta()
-        s.abi_version = capi.CONST["CAE_ABI_VERSION"]
-        s.num_new_values = len(a["value_is_int"])
-        s.num_new_labelsets = len(a["ls_off"]) - 1
-        s.num_new_taint_lists = len(a["taint_off"]) - 1
-        s.num_dirty = nd
-        for name, ctype in capi.cae_node_delta._fields_:
-            if name in a:
-                setattr(s, name, a[name].ctypes.data_as(ctype))
-        self.struct = s
+def _count(field: str) -> property:
+    return property(lambda self: getattr(self.struct, field))
 
-    def replace(self, **arrays) -> "NodeDelta":
-        """A copy with some arrays replaced (the counts follow the arrays)."""
-        return NodeDelta(**{**self.arrays, **arrays})
 
-    @property
-    def num_dirty(self) -> int:
-        return self.struct.num_dirty
+class AbiArrays:
+    """Owns the numpy arrays behind one ABI struct and the struct that points at them.  A subclass states its struct as a
+    table; the fields, their dtypes and pointer types are the header's.  The constructor takes fields by name: an array
+    left out is empty (an offsets array, which the header names ``*_off``, is ``[0]``; a per-row array is zeros of the
+    row count), None is a NULL pointer and a scalar is set as given.  Every count follows its array."""
+
+    STRUCT: type
+    COUNTS: Dict[str, str] = {}       # count field -> the array whose length gives it (an offsets array's length - 1)
+    ROWS: Optional[str] = None        # the array whose length is the row count
+    PER_ROW: Tuple[str, ...] = ()     # the arrays of one entry per row
+    PER_ROW_RES: Tuple[str, ...] = ()  # the per-row arrays of [rows][MAX_RES]
+    NESTED: Optional[str] = None      # the field that points to an optional nested NodeDelta
+
+    def __init__(self, **fields) -> None:
+        nested = fields.pop(self.NESTED, None) if self.NESTED else None
+        rows = len(fields.get(self.ROWS, ())) if self.ROWS else 0
+        s, a = self.STRUCT(), {}
+        fields.setdefault("abi_version", capi.CONST["CAE_ABI_VERSION"])
+        for name, ctype in self.STRUCT._fields_:
+            if name == self.NESTED:
+                continue
+            if not hasattr(ctype, "contents"):
+                if name in fields:
+                    setattr(s, name, fields[name])
+                continue
+            shape = (rows, MAX_RES) if name in self.PER_ROW_RES else (rows,)
+            x = fields.get(name, np.zeros(shape) if name in self.PER_ROW else [0] if name.endswith("_off") else [])
+            if x is not None:
+                x = np.ascontiguousarray(x, np.dtype(ctype._type_))
+                a[name] = np.ascontiguousarray(x.reshape(shape)) if name in self.PER_ROW_RES else x
+        for cnt, nm in self.COUNTS.items():
+            setattr(s, cnt, len(a[nm]) - nm.endswith("_off"))
+        if self.NESTED:
+            setattr(self, self.NESTED, nested)
+            setattr(s, self.NESTED, C.pointer(nested.struct) if nested is not None else None)
+        _fill_pointers(s, a)
+        self.arrays, self.struct = a, s
+
+    def replace(self, **arrays):
+        """A copy with some arrays (or the nested struct) replaced (the counts follow the arrays)."""
+        if self.NESTED:
+            arrays.setdefault(self.NESTED, getattr(self, self.NESTED))
+        return type(self)(**{**self.arrays, **arrays})
 
     def ptr(self):
         return C.byref(self.struct)
 
 
-class NodeChurn:
-    """Owns the numpy arrays behind one ``cae_node_churn`` struct: ``changed`` (a NodeDelta with the dirty rows and the
-    dictionary tails the dirty and the added rows use, or None), the removed rows and the added nodes.  Field names are
-    the header's."""
+class NodeDelta(AbiArrays):
+    """``cae_node_delta``: the dictionary tails (values, label sets, taint lists that continue the resident tables; offsets
+    relative to the tail) and the complete new state of the dirty cluster rows."""
 
-    _I32 = ("removed", "name", "labelset", "taint_list", "allowed_pods", "pod_off", "pod_spec")
+    STRUCT = capi.cae_node_delta
+    COUNTS = {"num_new_values": "value_is_int", "num_new_labelsets": "ls_off", "num_new_taint_lists": "taint_off",
+              "num_dirty": "row"}
+    ROWS, PER_ROW, PER_ROW_RES = "row", ("labelset", "taint_list", "unschedulable", "alloc", "allowed_pods"), ("alloc",)
+    num_dirty = _count("num_dirty")
+
+
+class NodeChurn(AbiArrays):
+    """``cae_node_churn``: ``changed`` (a NodeDelta with the dirty rows and the dictionary tails the dirty and the added
+    rows use, or None), the removed rows and the added nodes."""
+
+    STRUCT, NESTED = capi.cae_node_churn, "changed"
+    COUNTS = {"num_removed": "removed", "num_added": "name"}
+    ROWS, PER_ROW, PER_ROW_RES = "name", ("labelset", "taint_list", "unschedulable", "alloc", "allowed_pods"), ("alloc",)
+    num_removed, num_added = _count("num_removed"), _count("num_added")
 
     def __init__(self, changed: Optional[NodeDelta] = None, **arrays) -> None:
-        a: Dict[str, np.ndarray] = {}
-        for nm in self._I32:
-            a[nm] = _i32(arrays.get(nm, [0] if nm == "pod_off" else []))
-        a["unschedulable"] = np.ascontiguousarray(arrays.get("unschedulable", np.zeros(len(a["name"]))), np.uint8)
-        na = len(a["name"])
-        a["alloc"] = np.ascontiguousarray(np.asarray(arrays.get("alloc", np.zeros((na, MAX_RES))), np.int64).reshape(na, MAX_RES))
-        self.arrays = a
-        self.changed = changed
-        s = capi.cae_node_churn()
-        s.abi_version = capi.CONST["CAE_ABI_VERSION"]
-        s.changed = C.pointer(changed.struct) if changed is not None else None
-        s.num_removed = len(a["removed"])
-        s.num_added = na
-        for name, ctype in capi.cae_node_churn._fields_:
-            if name in a:
-                setattr(s, name, a[name].ctypes.data_as(ctype))
-        self.struct = s
-
-    def replace(self, **arrays) -> "NodeChurn":
-        """A copy with some arrays (or ``changed``) replaced (the counts follow the arrays)."""
-        changed = arrays.pop("changed", self.changed)
-        return NodeChurn(changed, **{**self.arrays, **arrays})
-
-    @property
-    def num_removed(self) -> int:
-        return self.struct.num_removed
-
-    @property
-    def num_added(self) -> int:
-        return self.struct.num_added
-
-    def ptr(self):
-        return C.byref(self.struct)
+        super().__init__(changed=changed, **arrays)
 
 
-class TemplateDelta:
-    """Owns the numpy arrays behind one ``cae_template_delta`` struct: ``tails`` (a NodeDelta without dirty rows that
-    carries the dictionary tails the new rows use, or None), the removed and changed template indices and the rows of the
-    changed templates followed by the added ones.  Field names are the header's."""
+class TemplateDelta(AbiArrays):
+    """``cae_template_delta``: ``tails`` (a NodeDelta without dirty rows that carries the dictionary tails the new rows
+    use, or None), the removed and changed template indices and the rows of the changed templates followed by the added
+    ones."""
 
-    _I32 = ("removed", "changed", "name", "labelset", "taint_list", "allowed_pods", "pod_off", "pod_spec")
+    STRUCT, NESTED = capi.cae_template_delta, "tails"
+    COUNTS = {"num_removed": "removed", "num_changed": "changed"}
+    ROWS, PER_ROW_RES = "name", ("alloc",)
+    PER_ROW = ("labelset", "taint_list", "unschedulable", "alloc", "allowed_pods", "cap_cpu", "cap_mem", "has_alloc_cpu",
+               "has_alloc_mem")
+    num_removed, num_changed, num_added = _count("num_removed"), _count("num_changed"), _count("num_added")
 
     def __init__(self, tails: Optional[NodeDelta] = None, **arrays) -> None:
-        a: Dict[str, np.ndarray] = {}
-        for nm in self._I32:
-            a[nm] = _i32(arrays.get(nm, [0] if nm == "pod_off" else []))
-        ns = len(a["name"])
-        for nm in ("unschedulable", "has_alloc_cpu", "has_alloc_mem"):
-            a[nm] = np.ascontiguousarray(arrays.get(nm, np.zeros(ns)), np.uint8)
-        for nm in ("cap_cpu", "cap_mem"):
-            a[nm] = np.ascontiguousarray(arrays.get(nm, np.zeros(ns)), np.int64)
-        a["alloc"] = np.ascontiguousarray(np.asarray(arrays.get("alloc", np.zeros((ns, MAX_RES))), np.int64).reshape(ns, MAX_RES))
-        self.arrays = a
-        self.tails = tails
-        s = capi.cae_template_delta()
-        s.abi_version = capi.CONST["CAE_ABI_VERSION"]
-        s.tails = C.pointer(tails.struct) if tails is not None else None
-        s.num_removed = len(a["removed"])
-        s.num_changed = len(a["changed"])
-        s.num_added = ns - len(a["changed"])
-        for name, ctype in capi.cae_template_delta._fields_:
-            if name in a:
-                setattr(s, name, a[name].ctypes.data_as(ctype))
-        self.struct = s
-
-    def replace(self, **arrays) -> "TemplateDelta":
-        """A copy with some arrays (or ``tails``) replaced (the counts follow the arrays)."""
-        tails = arrays.pop("tails", self.tails)
-        return TemplateDelta(tails, **{**self.arrays, **arrays})
-
-    @property
-    def num_removed(self) -> int:
-        return self.struct.num_removed
-
-    @property
-    def num_changed(self) -> int:
-        return self.struct.num_changed
-
-    @property
-    def num_added(self) -> int:
-        return self.struct.num_added
-
-    def ptr(self):
-        return C.byref(self.struct)
+        super().__init__(tails=tails, **arrays)
+        self.struct.num_added = len(self.arrays["name"]) - self.struct.num_changed
 
 
-class PodDelta:
-    """Owns the numpy arrays behind one ``cae_pod_delta`` struct: the dictionary tails and new pod specs (continuing the
-    resident tables; offsets relative to the tail) and the complete new pending list.  Field names are the header's."""
+class PodDelta(AbiArrays):
+    """``cae_pod_delta``: the dictionary tails and new pod specs (continuing the resident tables; offsets relative to the
+    tail) and the complete new pending list."""
 
-    # count field -> the array whose length gives it (minus one for an offsets array)
-    _COUNTS = {"num_new_values": "value_is_int", "num_new_namespaces": "ns_labelset", "num_new_labelsets": "ls_off",
-               "num_new_reqs": "req_key", "num_new_selectors": "sel_kind", "num_new_naff": "naff_nodesel",
-               "num_new_naff_terms": "term_expr_sel", "num_new_tol_lists": "tol_off", "num_new_port_lists": "port_off",
-               "num_new_pts_lists": "pts_off", "num_new_aff_lists": "aff_off", "num_new_aterms": "aterm_selector",
-               "num_new_specs": "ps_namespace", "num_groups": "group_off", "num_pending": "pend_spec"}
-    _OFFSETS = ("ls_off", "req_val_off", "sel_req_off", "naff_term_off", "term_field_off", "tol_off", "port_off", "pts_off",
-                "aff_off", "aterm_ns_off", "group_off")
+    STRUCT = capi.cae_pod_delta
+    COUNTS = {"num_new_values": "value_is_int", "num_new_namespaces": "ns_labelset", "num_new_labelsets": "ls_off",
+              "num_new_reqs": "req_key", "num_new_selectors": "sel_kind", "num_new_naff": "naff_nodesel",
+              "num_new_naff_terms": "term_expr_sel", "num_new_tol_lists": "tol_off", "num_new_port_lists": "port_off",
+              "num_new_pts_lists": "pts_off", "num_new_aff_lists": "aff_off", "num_new_aterms": "aterm_selector",
+              "num_new_specs": "ps_namespace", "num_groups": "group_off", "num_pending": "pend_spec"}
+    ROWS, PER_ROW_RES = "ps_namespace", ("ps_req",)
+    PER_ROW = tuple(f for f, _ in capi.cae_pod_delta._fields_ if f.startswith("ps_"))
+    num_new_specs = _count("num_new_specs")
 
-    def __init__(self, **arrays) -> None:
-        a: Dict[str, np.ndarray] = {}
-        for name, ctype in capi.cae_pod_delta._fields_:
-            if not hasattr(ctype, "contents"):
-                continue
-            dt = {C.c_uint8: np.uint8, C.c_int64: np.int64}.get(ctype._type_, np.int32)
-            a[name] = np.ascontiguousarray(arrays.get(name, [0] if name in self._OFFSETS else []), dt)
-        a["ps_req"] = np.ascontiguousarray(a["ps_req"].reshape(len(a["ps_namespace"]), MAX_RES))
-        self.arrays = a
-        s = capi.cae_pod_delta()
-        s.abi_version = capi.CONST["CAE_ABI_VERSION"]
-        for cnt, nm in self._COUNTS.items():
-            setattr(s, cnt, len(a[nm]) - (nm in self._OFFSETS))
-        for name, ctype in capi.cae_pod_delta._fields_:
-            if name in a:
-                setattr(s, name, a[name].ctypes.data_as(ctype))
-        self.struct = s
 
-    def replace(self, **arrays) -> "PodDelta":
-        """A copy with some arrays replaced (the counts follow the arrays)."""
-        return PodDelta(**{**self.arrays, **arrays})
+class PriceInputs(AbiArrays):
+    """``cae_price_inputs`` of cae_price_scores."""
 
-    @property
-    def num_new_specs(self) -> int:
-        return self.struct.num_new_specs
+    STRUCT = capi.cae_price_inputs
 
-    def ptr(self):
-        return C.byref(self.struct)
+
+class SimilarityInputs(AbiArrays):
+    """``cae_similarity_inputs`` of cae_similar_node_groups."""
+
+    STRUCT = capi.cae_similarity_inputs
+    COUNTS = {"num_ignored_keys": "ignored_keys"}
 
 
 # ----------------------------------------------------------------------------------------------

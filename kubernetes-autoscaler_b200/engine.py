@@ -10,7 +10,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 
 from . import capi
-from .encode import EncodedObjects
+from .encode import EncodedObjects, PriceInputs, SimilarityInputs
 
 
 class EngineError(RuntimeError):
@@ -19,6 +19,16 @@ class EngineError(RuntimeError):
 
 class EngineUnsupported(EngineError):
     """Status > 0: the input uses something the engine refuses; the caller must use the stock path."""
+
+
+def _vp(a: Optional[np.ndarray]):
+    """The array's data as a void*, NULL for None."""
+    return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _opt(a, dtype) -> Optional[np.ndarray]:
+    """A contiguous array of `dtype`, None for None (a NULL argument)."""
+    return None if a is None else np.ascontiguousarray(a, dtype)
 
 
 class PinnedArray:
@@ -66,10 +76,6 @@ class Engine:
     def __init__(self, device: int = 0, rank: int = 0, world_size: int = 1, want_reasons: bool = False,
                  pods_presharded: bool = False, feature_gates: Optional[int] = None) -> None:
         self.lib = capi.load_engine_lib()
-        self.lib.cae_host_alloc.argtypes = [C.c_size_t]
-        self.lib.cae_host_alloc.restype = C.c_void_p
-        self.lib.cae_host_free.argtypes = [C.c_void_p]
-        self.lib.cae_host_free.restype = None
         cfg = capi.cae_config()
         cfg.abi_version = capi.CONST["CAE_ABI_VERSION"]
         cfg.device, cfg.rank, cfg.world_size, cfg.want_reasons = device, rank, world_size, int(want_reasons)
@@ -94,6 +100,13 @@ class Engine:
         if rc > 0:
             raise EngineUnsupported(msg)
         raise EngineError("caengine status %d: %s" % (rc, msg))
+
+    def _applied(self, rc: int) -> bool:
+        """A delta call's status: False on 2 ("use a full load"; the engine is unchanged), True on 0, raises otherwise."""
+        if rc == 2:
+            return False
+        self._check(rc)
+        return True
 
     def close(self) -> None:
         if getattr(self, "h", None):
@@ -135,47 +148,33 @@ class Engine:
     def load_pending(self, enc: EncodedObjects) -> bool:
         """The per-tick delta (cae_load_pending): only the pending-pod rows of `enc` travel; nodes, templates and pod specs
         must be the ones of the last load().  Returns False when the engine answers "use a full load" (status 2)."""
-        a = enc.arrays
-        rc = self.lib.cae_load_pending(self.h, enc.P, a["pend_spec"].ctypes.data_as(C.c_void_p), enc.E,
-                                       a["group_off"].ctypes.data_as(C.c_void_p))
-        if rc == 2:
-            return False
-        self._check(rc)
-        self.enc = enc
-        return True
+        ok = self._applied(self.lib.cae_load_pending(self.h, enc.P, _vp(enc.arrays["pend_spec"]), enc.E,
+                                                     _vp(enc.arrays["group_off"])))
+        if ok:
+            self.enc = enc
+        return ok
 
     def load_nodes(self, delta) -> bool:
         """The per-tick delta of the cluster nodes (cae_load_nodes): new rows of existing cluster nodes plus the dictionary
         tails they need (encode.NodeDelta).  Returns False when the engine answers "use a full load" (status 2); the engine
         is unchanged then."""
-        rc = self.lib.cae_load_nodes(self.h, delta.ptr())
-        if rc == 2:
-            return False
-        self._check(rc)
-        return True
+        return self._applied(self.lib.cae_load_nodes(self.h, delta.ptr()))
 
     def load_node_churn(self, churn) -> bool:
         """The per-tick delta of the cluster-node list (cae_load_node_churn): removed and added cluster nodes plus the
         dirty rows of the survivors (encode.NodeChurn).  Returns False when the engine answers "use a full load" (status 2);
         the engine is unchanged then."""
-        rc = self.lib.cae_load_node_churn(self.h, churn.ptr())
-        if rc == 2:
-            return False
-        self._check(rc)
-        return True
+        return self._applied(self.lib.cae_load_node_churn(self.h, churn.ptr()))
 
     def load_templates(self, delta, enc: Optional[EncodedObjects] = None) -> bool:
         """The per-tick delta of the node-group templates (cae_load_templates): removed, changed and added templates plus
         the dictionary tails they need (encode.TemplateDelta).  Returns False when the engine answers "use a full load"
         (status 2); the engine is unchanged then.  `enc`: the objects the engine now holds
         (EncodedObjects.apply_template_delta), kept as this engine's shapes (the template count changes)."""
-        rc = self.lib.cae_load_templates(self.h, delta.ptr())
-        if rc == 2:
-            return False
-        self._check(rc)
-        if enc is not None:
+        ok = self._applied(self.lib.cae_load_templates(self.h, delta.ptr()))
+        if ok and enc is not None:
             self.enc = enc
-        return True
+        return ok
 
     def load_pods(self, delta, enc: Optional[EncodedObjects] = None) -> int:
         """The per-tick delta of the pod specs (cae_load_pods): new pod specs with the dictionary tails they need and the
@@ -199,13 +198,10 @@ class Engine:
         pd, nd = np.ascontiguousarray(pods, np.int32), np.ascontiguousarray(nodes, np.int32)
         if pd.ndim != 1 or pd.shape != nd.shape:
             raise ValueError("force_add_pods: pods and nodes must be two lists of one length")
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)
         # new_index is worked out here, not asked of the library: the library writes one entry per pending pod IT holds, and
         # this object's shapes (self.enc) are only as current as the caller kept them
-        rc = self.lib.cae_force_add_pods(self.h, len(pd), vp(pd), vp(nd), None)
-        if rc == 2:
+        if not self._applied(self.lib.cae_force_add_pods(self.h, len(pd), _vp(pd), _vp(nd), None)):
             return False
-        self._check(rc)
         keep = np.ones(self.enc.P, bool)
         keep[pd] = False
         new_index = np.where(keep, np.cumsum(keep) - 1, -1).astype(np.int32)
@@ -222,16 +218,13 @@ class Engine:
         bits = self._pin("bits", (T, (Pl + 31) // 32), np.uint32) if want_bits else None
         reasons = self._pin("reasons", (T, Pl), np.uint8) if self.want_reasons else None
         count = self._pin("count", (T,), np.int32)
-        self._check(self.lib.cae_feasibility(
-            self.h, bits.ctypes.data_as(C.c_void_p) if bits is not None else None,
-            reasons.ctypes.data_as(C.c_void_p) if reasons is not None else None,
-            count.ctypes.data_as(C.c_void_p)))
+        self._check(self.lib.cae_feasibility(self.h, _vp(bits), _vp(reasons), _vp(count)))
         return bits, reasons, count
 
     def feasibility_groups(self) -> np.ndarray:
         enc = self.enc
         out = np.zeros((enc.T, enc.E), np.uint8)
-        self._check(self.lib.cae_feasibility_groups(self.h, out.ctypes.data_as(C.c_void_p)))
+        self._check(self.lib.cae_feasibility_groups(self.h, _vp(out)))
         return out
 
     def group_reasons(self, considered=None, exist=None, want_detail: bool = False):
@@ -239,16 +232,14 @@ class Engine:
         (None = all).  Returns (schedulable [E] uint8, counts [E][CAE_REASON_KEYS] int32, detail [T][E] uint16 | None)."""
         enc = self.enc
         T, E = enc.T, enc.E
-        opt = lambda a: None if a is None else np.ascontiguousarray(a, np.uint8)
-        cons, ex = opt(considered), opt(exist)
+        cons, ex = _opt(considered, np.uint8), _opt(exist, np.uint8)
         for m in (cons, ex):
             if m is not None and m.shape != (T,):
                 raise ValueError("group_reasons: a mask needs one flag per template")
         sched = np.zeros(E, np.uint8)
         counts = np.zeros((E, capi.CONST["CAE_REASON_KEYS"]), np.int32)
         detail = np.zeros((T, E), np.uint16) if want_detail else None
-        vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-        self._check(self.lib.cae_group_reasons(self.h, vp(cons), vp(ex), vp(sched), vp(counts), vp(detail)))
+        self._check(self.lib.cae_group_reasons(self.h, _vp(cons), _vp(ex), _vp(sched), _vp(counts), _vp(detail)))
         return sched, counts, detail
 
     def estimate_all_li(self, max_nodes, last_index_in):
@@ -256,13 +247,12 @@ class Engine:
         Returns node_count, pod_count, sched, order, last_index_out."""
         enc = self.enc
         T, E = enc.T, enc.E
-        mn = None if max_nodes is None else np.ascontiguousarray(max_nodes, np.int32)
+        mn = _opt(max_nodes, np.int32)
         li = np.ascontiguousarray(last_index_in, np.int32)
         nc, pc = np.zeros(T, np.int32), np.zeros(T, np.int32)
         sched, order = np.zeros((T, E), np.int32), np.zeros((T, E), np.int32)
         lo = np.zeros(T, np.int32)
-        vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-        self._check(self.lib.cae_estimate_all_ex(self.h, vp(mn), vp(li), vp(nc), vp(pc), vp(sched), vp(order), vp(lo)))
+        self._check(self.lib.cae_estimate_all_ex(self.h, _vp(mn), _vp(li), _vp(nc), _vp(pc), _vp(sched), _vp(order), _vp(lo)))
         return nc, pc, sched, order, lo
 
     def estimate_all(self, max_nodes: Optional[Sequence[int]] = None, want_sched: bool = True, copy: bool = True):
@@ -271,13 +261,12 @@ class Engine:
         views that the next call overwrites; want_sched=False skips the two [T][E] matrices."""
         enc = self.enc
         T, E = enc.T, enc.E
-        mn = None if max_nodes is None else np.ascontiguousarray(max_nodes, np.int32)
+        mn = _opt(max_nodes, np.int32)
         node_count = self._pin("node_count", (T,), np.int32)
         pod_count = self._pin("pod_count", (T,), np.int32)
         sched = self._pin("sched", (T, E), np.int32) if want_sched else None
         order = self._pin("order", (T, E), np.int32) if want_sched else None
-        vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-        self._check(self.lib.cae_estimate_all(self.h, vp(mn), vp(node_count), vp(pod_count), vp(sched), vp(order)))
+        self._check(self.lib.cae_estimate_all(self.h, _vp(mn), _vp(node_count), _vp(pod_count), _vp(sched), _vp(order)))
         if copy:
             return (node_count.copy(), pod_count.copy(), None if sched is None else sched.copy(),
                     None if order is None else order.copy())
@@ -289,50 +278,29 @@ class Engine:
         ch = np.asarray(chain, np.int32)
         nc = np.ascontiguousarray(node_count, np.int32)
         pc = np.ascontiguousarray(pod_count, np.int32)
-        sc = None if sched is None else np.ascontiguousarray(sched, np.int32)
+        sc = _opt(sched, np.int32)
         mask = np.zeros(enc.T, np.uint8)
         waste = np.zeros(enc.T, np.float64)
-        vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-        self._check(self.lib.cae_expander_best(self.h, vp(ch), len(ch), vp(nc), vp(pc), vp(sc), vp(mask), vp(waste)))
+        self._check(self.lib.cae_expander_best(self.h, _vp(ch), len(ch), _vp(nc), _vp(pc), _vp(sc), _vp(mask), _vp(waste)))
         return mask, waste
 
     def waste_scores(self) -> np.ndarray:
         """Least-waste score of this rank's template shard from the device-resident result of the last estimate_all
         (0.0 for the rows of other ranks: a sum all-reduce of float64[T] assembles the vector)."""
         waste = np.zeros(self.enc.T, np.float64)
-        self._check(self.lib.cae_waste_scores(self.h, waste.ctypes.data_as(C.c_void_p)))
+        self._check(self.lib.cae_waste_scores(self.h, _vp(waste)))
         return waste
 
     def price_scores(self, node_price, pod_price, stabilization_price: float, preferred_cpu_milli: int = 0, unfitness=None,
                      has_gpu=None, exists=None, node_count=None, sched=None, order=None) -> np.ndarray:
         """Price expander score per option (expander/price/price.go).  node_count/sched/order None = the device-resident
         result of the last estimate_all."""
-        T = self.enc.T
-        keep = []
-
-        def arr(a, dt):
-            if a is None:
-                return None
-            a = np.ascontiguousarray(a, dt)
-            keep.append(a)
-            return a
-        pin = capi.cae_price_inputs()
-        f64p, u8p = C.POINTER(C.c_double), C.POINTER(C.c_uint8)
-        pin.node_price = arr(node_price, np.float64).ctypes.data_as(f64p)
-        pin.pod_price = arr(pod_price, np.float64).ctypes.data_as(f64p)
-        u = arr(unfitness, np.float64)
-        pin.unfitness = u.ctypes.data_as(f64p) if u is not None else None
-        g = arr(has_gpu, np.uint8)
-        pin.has_gpu = g.ctypes.data_as(u8p) if g is not None else None
-        x = arr(exists, np.uint8)
-        pin.exists = x.ctypes.data_as(u8p) if x is not None else None
-        pin.price_error = None
-        pin.stabilization_price = float(stabilization_price)
-        pin.preferred_cpu_milli = int(preferred_cpu_milli)
-        score = np.zeros(T, np.float64)
-        vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-        self._check(self.lib.cae_price_scores(self.h, C.byref(pin), vp(arr(node_count, np.int32)), vp(arr(sched, np.int32)),
-                                              vp(arr(order, np.int32)), vp(score)))
+        pin = PriceInputs(node_price=node_price, pod_price=pod_price, unfitness=unfitness, has_gpu=has_gpu, exists=exists,
+                          price_error=None, stabilization_price=float(stabilization_price),
+                          preferred_cpu_milli=int(preferred_cpu_milli))
+        score = np.zeros(self.enc.T, np.float64)
+        nc, sc, od = _opt(node_count, np.int32), _opt(sched, np.int32), _opt(order, np.int32)
+        self._check(self.lib.cae_price_scores(self.h, pin.ptr(), _vp(nc), _vp(sc), _vp(od), _vp(score)))
         return score
 
     def filter_schedulable(self, pod_order: Sequence[int], hint_node=None, sim_class=None, class_ctrl=None, node_ok=None,
@@ -341,16 +309,15 @@ class Engine:
         index or -1, lastIndex afterwards, overflowing controller count)."""
         enc = self.enc
         order = np.ascontiguousarray(pod_order, np.int32)
-        hn = None if hint_node is None else np.ascontiguousarray(hint_node, np.int32)
-        sc = None if sim_class is None else np.ascontiguousarray(sim_class, np.int32)
-        cc = None if class_ctrl is None else np.ascontiguousarray(class_ctrl, np.int32)
-        ok = None if node_ok is None else np.ascontiguousarray(node_ok, np.uint8)
+        hn = _opt(hint_node, np.int32)
+        sc = _opt(sim_class, np.int32)
+        cc = _opt(class_ctrl, np.int32)
+        ok = _opt(node_ok, np.uint8)
         assigned = np.full(max(enc.P, 1), -1, np.int32)
         li, ov = np.zeros(1, np.int32), np.zeros(1, np.int32)
-        vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-        self._check(self.lib.cae_filter_schedulable(self.h, vp(order), len(order), vp(hn), vp(sc), vp(cc),
-                                                    0 if cc is None else len(cc), vp(ok), int(last_index), int(break_on_failure),
-                                                    vp(assigned), vp(li), vp(ov)))
+        self._check(self.lib.cae_filter_schedulable(self.h, _vp(order), len(order), _vp(hn), _vp(sc), _vp(cc),
+                                                    0 if cc is None else len(cc), _vp(ok), int(last_index), int(break_on_failure),
+                                                    _vp(assigned), _vp(li), _vp(ov)))
         return assigned[:enc.P], int(li[0]), int(ov[0])
 
     def simulate_removals(self, cand_node, move_off, move_pod, dest_ok=None, hint_node=None, sim_class=None, class_ctrl=None,
@@ -375,17 +342,16 @@ class Engine:
         cn = np.ascontiguousarray(cand_node, np.int32)
         mo = np.ascontiguousarray(move_off, np.int32)
         mp = np.ascontiguousarray(move_pod, np.int32)
-        ok = None if dest_ok is None else np.ascontiguousarray(dest_ok, np.uint8)
-        hn = None if hint_node is None else np.ascontiguousarray(hint_node, np.int32)
-        sc = None if sim_class is None else np.ascontiguousarray(sim_class, np.int32)
-        cc = None if class_ctrl is None else np.ascontiguousarray(class_ctrl, np.int32)
+        ok = _opt(dest_ok, np.uint8)
+        hn = _opt(hint_node, np.int32)
+        sc = _opt(sim_class, np.int32)
+        cc = _opt(class_ctrl, np.int32)
         res = np.zeros(max(len(cn), 1), np.int32)
         log = np.zeros((max(log_cap, 1), 3), np.int32)
         li, n = np.zeros(1, np.int32), np.zeros(1, np.int32)
-        vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-        rc = self.lib.cae_simulate_removals(self.h, len(cn), vp(cn), vp(mo), vp(mp), vp(ok), vp(hn), vp(sc), vp(cc),
-                                            0 if cc is None else len(cc), int(last_index), int(bool(persist)), vp(res), vp(li),
-                                            vp(log), int(log_cap), vp(n))
+        rc = self.lib.cae_simulate_removals(self.h, len(cn), _vp(cn), _vp(mo), _vp(mp), _vp(ok), _vp(hn), _vp(sc), _vp(cc),
+                                            0 if cc is None else len(cc), int(last_index), int(bool(persist)), _vp(res), _vp(li),
+                                            _vp(log), int(log_cap), _vp(n))
         if rc == 1:
             return rc, None, None, np.zeros((int(n[0]), 3), np.int32)
         return rc, res[:len(cn)], int(li[0]), log[:int(n[0])]
@@ -396,30 +362,14 @@ class Engine:
         (bits [T, ceil(T/32)] uint32: bit s of row t = s is similar to t, count [T] int32, sng_limit [T] int64).  Raises
         EngineUnsupported on status 1 (a quantity past INT64_MAX / 1000)."""
         T = self.enc.T
-        keep = []
-
-        def arr(a, dt, ctype):
-            a = np.ascontiguousarray(a, dt)
-            keep.append(a)
-            return a.ctypes.data_as(C.POINTER(ctype))
-        si = capi.cae_similarity_inputs()
-        si.abi_version = capi.CONST["CAE_ABI_VERSION"]
-        ign = np.ascontiguousarray(list(ignored_keys), np.int32)
-        si.num_ignored_keys = len(ign)
-        si.ignored_keys = arr(ign, np.int32, C.c_int32)
-        si.max_allocatable_difference_ratio, si.max_free_difference_ratio, si.max_capacity_memory_difference_ratio = \
-            (float(r) for r in ratios)
-        si.res_sig = arr(res_sig, np.int32, C.c_int32)
-        si.free_dims = arr(free_dims, np.uint32, C.c_uint32)
-        si.eligible = arr(eligible, np.uint8, C.c_uint8)
-        si.safe = None if safe is None else arr(safe, np.uint8, C.c_uint8)
-        si.max_size = arr(max_size, np.int32, C.c_int32)
-        si.target_size = arr(target_size, np.int32, C.c_int32)
+        alloc_ratio, free_ratio, mem_ratio = (float(r) for r in ratios)
+        si = SimilarityInputs(ignored_keys=list(ignored_keys), res_sig=res_sig, free_dims=free_dims, eligible=eligible, safe=safe,
+                              max_size=max_size, target_size=target_size, max_allocatable_difference_ratio=alloc_ratio,
+                              max_free_difference_ratio=free_ratio, max_capacity_memory_difference_ratio=mem_ratio)
         bits = np.zeros((T, (T + 31) // 32), np.uint32)
         count = np.zeros(T, np.int32)
         limit = np.zeros(T, np.int64)
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)
-        self._check(self.lib.cae_similar_node_groups(self.h, C.byref(si), vp(bits), vp(count), vp(limit)))
+        self._check(self.lib.cae_similar_node_groups(self.h, si.ptr(), _vp(bits), _vp(count), _vp(limit)))
         return bits, count, limit
 
     # ---- fused histogram exchange over peer memory (multi-GPU dense pass) -------------------------
@@ -448,35 +398,28 @@ class Engine:
         return int(p or 0), int(n.value)
 
 
-def expander_chain(chain: Sequence[int], node_count, pod_count, waste) -> np.ndarray:
-    """The expander filter chain on the host (cae_expander_chain): needs the library, not a GPU."""
+def _expander_chain(fn: str, chain: Sequence[int], node_count, pod_count, *scores) -> np.ndarray:
+    """One call of the host-side filter chain `fn` (cae_expander_chain or cae_expander_chain_ex): the best-option mask."""
     lib = capi.load_engine_lib()
     ch = np.asarray(chain, np.int32)
     nc = np.ascontiguousarray(node_count, np.int32)
     pc = np.ascontiguousarray(pod_count, np.int32)
-    w = np.ascontiguousarray(waste, np.float64)
     mask = np.zeros(len(nc), np.uint8)
-    vp = lambda a: a.ctypes.data_as(C.c_void_p)
-    rc = lib.cae_expander_chain(vp(ch), len(ch), len(nc), vp(nc), vp(pc), vp(w), vp(mask))
+    rc = getattr(lib, fn)(_vp(ch), len(ch), len(nc), _vp(nc), _vp(pc), *map(_vp, scores), _vp(mask))
     if rc != 0:
-        raise EngineError("cae_expander_chain status %d: %s" % (rc, (lib.cae_last_error() or b"").decode()))
+        raise EngineError("%s status %d: %s" % (fn, rc, (lib.cae_last_error() or b"").decode()))
     return mask
+
+
+def expander_chain(chain: Sequence[int], node_count, pod_count, waste) -> np.ndarray:
+    """The expander filter chain on the host (cae_expander_chain): needs the library, not a GPU."""
+    return _expander_chain("cae_expander_chain", chain, node_count, pod_count, np.ascontiguousarray(waste, np.float64))
 
 
 def expander_chain_ex(chain: Sequence[int], node_count, pod_count, waste=None, price=None, price_error=None, priority=None) -> np.ndarray:
     """cae_expander_chain_ex: the chain with the price (price.go:166-173) and priority (priority.go:119-165) filters."""
-    lib = capi.load_engine_lib()
-    ch = np.asarray(chain, np.int32)
-    nc = np.ascontiguousarray(node_count, np.int32)
-    pc = np.ascontiguousarray(pod_count, np.int32)
-    opt = lambda a, dt: None if a is None else np.ascontiguousarray(a, dt)
-    w, pr, pe, prio = opt(waste, np.float64), opt(price, np.float64), opt(price_error, np.uint8), opt(priority, np.int32)
-    mask = np.zeros(len(nc), np.uint8)
-    vp = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-    rc = lib.cae_expander_chain_ex(vp(ch), len(ch), len(nc), vp(nc), vp(pc), vp(w), vp(pr), vp(pe), vp(prio), vp(mask))
-    if rc != 0:
-        raise EngineError("cae_expander_chain_ex status %d: %s" % (rc, (lib.cae_last_error() or b"").decode()))
-    return mask
+    return _expander_chain("cae_expander_chain_ex", chain, node_count, pod_count, _opt(waste, np.float64),
+                           _opt(price, np.float64), _opt(price_error, np.uint8), _opt(priority, np.int32))
 
 
 def resolve_priorities(config: dict, group_ids: Sequence[str]) -> np.ndarray:

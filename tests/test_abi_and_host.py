@@ -3,12 +3,14 @@ the ctypes structs match the header, the encoder builds consistent tables, and t
 logic (product code, Python) agrees with the reference tables and the oracle."""
 import ctypes
 import os
+import re
 
 import numpy as np
 import pytest
 
 from kubernetes_autoscaler_b200 import capi, synth
-from kubernetes_autoscaler_b200.encode import encode
+from kubernetes_autoscaler_b200.encode import (NodeChurn, NodeDelta, PodDelta, SimilarityInputs, TemplateDelta,
+                                               encode)
 from kubernetes_autoscaler_b200.estimator import (ClusterCapacityThreshold, EstimationContext, NodeGroupInfo,
                                                   SngCapacityThreshold, StaticThreshold,
                                                   ThresholdBasedEstimationLimiter, getMinLimit)
@@ -43,6 +45,63 @@ def test_create_without_gpu_fails_loudly():
     from kubernetes_autoscaler_b200.engine import Engine, EngineError
     with pytest.raises(EngineError):
         Engine()
+
+
+def test_signatures_cover_every_declared_function():
+    sigs = capi.signatures(capi._SRC)
+    assert sorted(sigs) == sorted(set(re.findall(r"\b(cae_\w+)\s*\(", capi._SRC))) == capi.declared_functions()
+    assert {"cae_host_alloc", "cae_host_free", "cae_similar_node_groups"} <= set(sigs)
+
+
+def test_signatures_follow_the_mapping_rule():
+    sigs, P, V, I32 = capi.signatures(capi._SRC), ctypes.POINTER, ctypes.c_void_p, ctypes.c_int32
+    assert sigs["cae_create"] == (I32, [P(capi.cae_config), P(V)])              # struct pointer, cae_engine**
+    assert sigs["cae_device_buffer"] == (V, [V, I32, P(ctypes.c_size_t)])       # void* return, size_t*
+    assert sigs["cae_last_error"] == (ctypes.c_char_p, [])
+    assert sigs["cae_destroy"] == (None, [V])
+    assert sigs["cae_host_alloc"] == (V, [ctypes.c_size_t])
+    assert sigs["cae_price_scores"] == (I32, [V, P(capi.cae_price_inputs), V, V, V, V])
+    assert sigs["cae_simulate_removals"] == (I32, [V, I32] + [V] * 7 + [I32] * 3 + [V] * 3 + [I32, V])
+
+
+@pytest.mark.parametrize("proto", ["int32_t cae_x(cae_engine* e, float f);", "foo_t cae_x(void);",
+                                   "int32_t cae_x(cae_config cfg);", "int32_t cae_x(bar_t* p);",
+                                   "int32_t cae_x(void (*cb)(int));"])
+def test_signatures_refuse_what_the_rule_does_not_know(proto):
+    with pytest.raises(RuntimeError):
+        capi.signatures("typedef struct cae_engine cae_engine;\n" + proto + "\n")
+
+
+def test_abi_struct_owners_counts_follow_their_arrays():
+    R = capi.CONST["CAE_MAX_RES"]
+    nd = NodeDelta(value_is_int=[0, 1], value_int=[0, 5], ls_off=[0, 1, 3], ls_key=[1, 2, 3], ls_val=[0, 0, 0], row=[2, 4, 7])
+    s = nd.struct
+    assert (s.num_new_values, s.num_new_labelsets, s.num_new_taint_lists, nd.num_dirty) == (2, 2, 0, 3)
+    assert nd.arrays["alloc"].shape == (3, R) and nd.arrays["labelset"].tolist() == [0, 0, 0]
+    c = NodeChurn(nd, removed=[0, 5], name=[8, 9])
+    assert (c.num_removed, c.num_added) == (2, 2) and c.struct.changed.contents.num_dirty == 3
+    assert c.replace(removed=[1]).num_removed == 1 and c.replace(removed=[1]).changed is nd
+    assert not c.replace(changed=None).struct.changed
+    t = TemplateDelta(NodeDelta(value_is_int=[0, 1], value_int=[0, 5]), removed=[3], changed=[0, 1], name=[5, 6, 7, 8])
+    assert (t.num_removed, t.num_changed, t.num_added) == (1, 2, 2) and t.struct.tails.contents.num_new_values == 2
+    assert t.arrays["cap_cpu"].tolist() == [0] * 4 and t.arrays["alloc"].shape == (4, R)
+    assert t.replace(name=[5, 6], alloc=np.zeros((2, R))).num_added == 0
+    p = PodDelta(ps_namespace=[0, 1], ps_req=np.ones((2, R)), ls_off=[0, 2, 3], group_off=[0, 1, 3], pend_spec=[0, 1, 1])
+    assert (p.num_new_specs, p.struct.num_new_labelsets, p.struct.num_groups, p.struct.num_pending) == (2, 2, 2, 3)
+    assert p.replace(ps_namespace=[], ps_req=[]).num_new_specs == 0
+    for o in (nd, c, t, p):
+        assert o.struct.abi_version == capi.CONST["CAE_ABI_VERSION"]
+        for name, ctype in o.struct._fields_:                 # every array has its header field's dtype
+            if name in o.arrays:
+                assert o.arrays[name].dtype == np.dtype(ctype._type_), name
+    si = SimilarityInputs(ignored_keys=[4, 7], safe=None, res_sig=[1, 2], max_free_difference_ratio=0.5)
+    assert si.struct.num_ignored_keys == 2 and not si.struct.safe and si.struct.res_sig[1] == 2
+    assert si.struct.max_free_difference_ratio == 0.5
+
+
+def test_node_delta_per_row_arrays_default_to_zeros():
+    d = NodeDelta(row=[1], labelset=[0], taint_list=[0], allowed_pods=[10], pod_off=[0, 2], pod_spec=[3, 4])
+    assert d.arrays["unschedulable"].tolist() == [0] and d.arrays["alloc"].tolist() == [[0] * capi.CONST["CAE_MAX_RES"]]
 
 
 def test_struct_layout_matches_header():
