@@ -775,6 +775,53 @@ typedef struct cae_similarity_inputs {
 int32_t cae_similar_node_groups(cae_engine* e, const cae_similarity_inputs* in, uint32_t* similar_bits, int32_t* similar_count,
                                 int64_t* sng_limit);
 
+/* Scale-down eligibility of the candidate nodes on the resident snapshot, in one call.
+ * Replaces: eligibility.Checker.FilterOutUnremovable (core/scaledown/eligibility/eligibility.go) from the utilization on:
+ * utilization.Calculate (simulator/utilization/info.go) of every candidate, then the unready and threshold tests.  The
+ * checks before the utilization (recently unremovable, being deleted, the scale-down-disabled annotation, NotAutoscaled,
+ * a provider or config error) are host facts about the node: the caller passes their outcome in pre_reason.
+ * Per candidate i, in order:
+ *   pre_reason[i] != 0          reason CAE_ELIG_PRE, no utilization;
+ *   utilization (below) fails   CAE_ELIG_UNEXPECTED_ERROR, no utilization;
+ *   unready[i] != 0             CAE_ELIG_UNREADY_DISABLED;
+ *   !(Utilization < threshold)  CAE_ELIG_NOT_UNDERUTILIZED (NaN counts as below, +Inf as not);
+ *   otherwise                   CAE_ELIG_UNNEEDED, and i is appended to `unneeded`.
+ * Utilization: with a GpuConfig (gpu_dim >= 0) U(gpu_dim) alone (cpu and mem reported as 0); otherwise cpu = U(0),
+ * mem = U(1) and Utilization = math.Max(cpu, mem) (NaN-propagating, +Inf first; gpu reported as 0).  U(r) over the row's
+ * resident pods in order: a DaemonSet pod with skip_ds, else a mirror pod with skip_mirror, adds its request of dim r to
+ * `excluded`; else a long-terminating pod is skipped; else the request adds to `counted`.  U(r) =
+ * float64(milli(counted)) / float64(milli(alloc) - milli(excluded)) in IEEE double (0/0 = NaN, x/0 = +-Inf, the int64
+ * difference wraps as Go's does), where milli(v) = v for cpu and v * 1000 for every other dim (Quantity.MilliValue()).
+ * U fails when allocatable of dim r is 0 (absent or MilliValue() == 0) or gpu_dim is -2.  The request of a pod is its
+ * spec's ps_req row.  Templates are ignored and no pending-side table is read: the call is valid after any load or delta.
+ * Every rank holds all cluster rows and answers for all of them.  The call's H2D and D2H bytes go to cae_stats.
+ *   util [n_cand][4]   cpu, mem, gpu, Utilization; defined for reasons 0, 3 and 4 (0.0 otherwise)
+ *   reason [n_cand]    enum cae_eligibility
+ *   unneeded [n_cand]  candidate indices with reason 0, in input order; n_unneeded of them
+ * Status -2 (nothing written): before a load, n_cand < 0, a NULL required array, a row outside [0, num_cluster_nodes),
+ *   a gpu_dim outside [-2, CAE_MAX_RES), n_pod_flags different from the resident pods of the cluster rows (flags given).
+ * Status 1 (nothing written): a sum of requests, or an allocatable or sum times 1000, that a candidate's utilization
+ *   reads leaves int64, where Go's Quantity would not wrap: use the stock path. */
+typedef struct cae_eligibility_inputs {
+  int32_t n_cand;
+  const int32_t* cand_node;   /* [n_cand] cluster rows in scaleDownCandidates order (duplicates allowed) */
+  const uint8_t* pod_flags;   /* [n_pod_flags] one byte per resident pod of the cluster rows, rows in order, each row's pods in
+                                 the engine's current order (the load's, a node delta's new list, force-added pods appended):
+                                 bit 0 DaemonSet, bit 1 mirror, bit 2 long-terminating, other bits ignored; NULL = all 0 */
+  int64_t n_pod_flags;
+  const uint8_t* skip_ds;     /* [n_cand] ignoreDaemonSetsUtilization of the node's group; NULL = 0 */
+  int32_t skip_mirror;        /* IgnoreMirrorPodsUtilization */
+  const int32_t* gpu_dim;     /* [n_cand] -1 no GpuConfig, >= 0 the dim of GpuConfig.ResourceName, -2 a name the load has no
+                                 dim for */
+  const double* threshold;    /* [n_cand] the group's GPU threshold for a GPU node, its utilization threshold otherwise */
+  const uint8_t* pre_reason;  /* [n_cand] != 0: the caller's reason from the checks before the utilization; NULL = 0 */
+  const uint8_t* unready;     /* [n_cand] unready and ScaleDownUnreadyEnabled off; NULL = 0 */
+} cae_eligibility_inputs;
+enum cae_eligibility { CAE_ELIG_UNNEEDED = 0, CAE_ELIG_PRE = 1, CAE_ELIG_UNEXPECTED_ERROR = 2, CAE_ELIG_UNREADY_DISABLED = 3,
+                       CAE_ELIG_NOT_UNDERUTILIZED = 4 };
+int32_t cae_scale_down_eligibility(cae_engine* e, const cae_eligibility_inputs* in, double* util, uint8_t* reason,
+                                   int32_t* unneeded, int32_t* n_unneeded);
+
 int32_t cae_get_stats(cae_engine* e, cae_stats* out);
 
 /* Raw device pointers of the engine's result buffers, for zero-copy collectives (torch.distributed

@@ -1709,6 +1709,75 @@ static int do_group_reasons(Engine* e, const uint8_t* considered, const uint8_t*
   return 0;
 }
 
+// cae_scale_down_eligibility.  The inputs travel in one H2D copy (a NULL byte vector as zeros, the pod flags last and only
+// when given), util, reason, the list, its length and the status in one D2H copy; nothing is written to the caller's
+// buffers unless the status is 0.
+static int do_eligibility(Engine* e, const cae_eligibility_inputs* in, double* util_out, uint8_t* reason_out,
+                          int32_t* unneeded_out, int32_t* n_unneeded) {
+  auto bad = [](const char* m) { set_error(std::string("cae_scale_down_eligibility: ") + m); return -2; };
+  const int n = in->n_cand, N = e->N;
+  if (n < 0) return bad("n_cand < 0");
+  if (!n_unneeded || (n && (!in->cand_node || !in->gpu_dim || !in->threshold || !util_out || !reason_out || !unneeded_out)))
+    return bad("a required array is NULL");
+  for (int i = 0; i < n; ++i) {
+    if (in->cand_node[i] < 0 || in->cand_node[i] >= N) return bad("a candidate row outside the cluster rows");
+    if (in->gpu_dim[i] < -2 || in->gpu_dim[i] >= CAE_MAX_RES) return bad("a gpu_dim outside [-2, CAE_MAX_RES)");
+  }
+  int64_t resident = 0;
+  for (int r = 0; r < N; ++r) resident += e->nh.pod_cnt[r];
+  if (in->pod_flags && in->n_pod_flags != resident) return bad("n_pod_flags is not the resident pod count of the cluster rows");
+  e->stats.h2d_bytes = 0;
+  e->stats.d2h_bytes = 0;
+  if (n == 0) {
+    *n_unneeded = 0;
+    return 0;
+  }
+  Engine::Staging& st = e->el;
+  EligLaunch a{};
+  a.n = n;
+  a.skip_mirror = in->skip_mirror != 0;
+  const size_t nf = in->pod_flags ? (size_t)resident : 0;
+  size_t in_end = 0, out_end = 0;
+  auto walk = [&](Layout& l) {
+    l.add(a.cand, n); l.add(a.gpu_dim, n); l.add(a.threshold, n); l.add(a.skip_ds, n); l.add(a.pre, n); l.add(a.unready, n);
+    l.add(a.flags, nf);
+    in_end = l.bytes;
+    l.add(a.util, (size_t)n * 4); l.add(a.reason, n); l.add(a.list, n); l.add(a.count, 1); l.add(a.status, 1);
+    out_end = l.bytes;
+  };
+  const size_t bytes = layout_bytes(walk);
+  if (stage_reserve(e, st, bytes, bytes)) return -1;
+  layout_bind(st.dev.p, walk);
+  if (!nf) a.flags = nullptr;
+  std::copy(in->cand_node, in->cand_node + n, st.host_of(a.cand));
+  std::copy(in->gpu_dim, in->gpu_dim + n, st.host_of(a.gpu_dim));
+  std::copy(in->threshold, in->threshold + n, st.host_of(a.threshold));
+  for (auto [src, dst] : {std::make_pair(in->skip_ds, a.skip_ds), std::make_pair(in->pre_reason, a.pre),
+                          std::make_pair(in->unready, a.unready)}) {
+    uint8_t* h = st.host_of(dst);
+    if (src) std::copy(src, src + n, h);
+    else std::fill(h, h + n, (uint8_t)0);
+  }
+  if (nf) memcpy(st.host_of(a.flags), in->pod_flags, nf);
+  if (stage_upload(e, st, in_end)) return -1;
+  CAE_CUDA(cudaMemsetAsync(a.status, 0, sizeof(int32_t), e->stream));
+  if (launch_eligibility(e, a)) return -1;
+  CAE_CUDA(cudaMemcpyAsync(st.host_of(a.util), a.util, out_end - in_end, cudaMemcpyDeviceToHost, e->stream));
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
+  e->stats.d2h_bytes = (int64_t)(out_end - in_end);
+  if (*st.host_of(a.status)) {
+    set_error("cae_scale_down_eligibility: a sum of requests or a milli value leaves int64, where Go's Quantity does not wrap: "
+              "use the stock path");
+    return 1;
+  }
+  const int m = *st.host_of(a.count);
+  std::copy(st.host_of(a.util), st.host_of(a.util) + (size_t)n * 4, util_out);
+  std::copy(st.host_of(a.reason), st.host_of(a.reason) + n, reason_out);
+  std::copy(st.host_of(a.list), st.host_of(a.list) + m, unneeded_out);
+  *n_unneeded = m;
+  return 0;
+}
+
 }  // namespace cae
 
 using cae::Engine;
@@ -2162,6 +2231,15 @@ int32_t cae_similar_node_groups(cae_engine* h, const cae_similarity_inputs* in, 
   if (!in) { cae::set_error("cae_similar_node_groups: no inputs"); return -2; }
   cudaSetDevice(e->cfg.device);
   return cae::do_similar(e, in, similar_bits, similar_count, sng_limit);
+}
+
+int32_t cae_scale_down_eligibility(cae_engine* h, const cae_eligibility_inputs* in, double* util, uint8_t* reason,
+                                   int32_t* unneeded, int32_t* n_unneeded) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_scale_down_eligibility before cae_load"); return -2; }
+  if (!in) { cae::set_error("cae_scale_down_eligibility: no inputs"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_eligibility(e, in, util, reason, unneeded, n_unneeded);
 }
 
 int32_t cae_get_stats(cae_engine* h, cae_stats* out) {

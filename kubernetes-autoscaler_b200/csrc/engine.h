@@ -357,6 +357,7 @@ struct Engine {
   // buffers of cae_similar_node_groups (similar.cu)
   Staging sim;                            // inputs | outputs (one D2H copy) | operand rows | schedulable bit rows (device only)
   Staging gr;                             // cae_group_reasons: masks | schedulable, counts (one D2H copy) | detail (device only)
+  Staging el;                             // cae_scale_down_eligibility: inputs | util, reason, list, count, status (one D2H copy)
   int sm_count = 132;
   int smem_optin = 227 * 1024;             // opt-in shared memory per thread block
   size_t hbm_bytes = (size_t)80 << 30;     // device memory (sizes the estimator's global slabs)
@@ -509,5 +510,18 @@ struct SimLaunch {
   uint32_t* sched;                        // scratch [T][ceil(E/32)]
 };
 int launch_similar(Engine* e, const SimLaunch& s);
+// scaledown.cu: cae_scale_down_eligibility.  In (device, uploaded by api.cu): the caller's arrays, flags NULL = all 0,
+// skip_ds / pre / unready as bytes (api.cu turns NULL into zeros).  Out: util [n][4], reason [n], list [n], count and status
+// (1 = a value left int64), every one written by the launch.
+struct EligLaunch {
+  int n, skip_mirror;
+  const int32_t *cand, *gpu_dim;
+  const uint8_t *flags, *skip_ds, *pre, *unready;
+  const double* threshold;
+  double* util;
+  uint8_t* reason;
+  int32_t *list, *count, *status;
+};
+int launch_eligibility(Engine* e, const EligLaunch& a);
 
 }  // namespace cae

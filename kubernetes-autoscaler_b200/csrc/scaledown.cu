@@ -1,0 +1,159 @@
+// scaledown.cu — cae_scale_down_eligibility: every scale-down candidate's utilization (utilization.Calculate) and its
+// eligibility reason (the end of eligibility.Checker.FilterOutUnremovable), then the unneeded candidates in input order.
+//
+//   * elig_kernel, one warp per candidate: the lanes stride over the row's resident pods (coalesced reads of node_pod_spec
+//     and the pod flags; a row can hold thousands of pods after cae_force_add_pods), gather the request of the one or two
+//     dims the utilization reads and add it to the counted or the excluded bucket as a 128-bit integer.  The warp reduces
+//     the buckets with shuffles once every lane has read its share: integer sums, so the result is exact and does not
+//     depend on the order.  Lane 0 then does the milli conversion, the IEEE divisions, Go's math.Max and the threshold test;
+//   * elig_compact_kernel, one block: the candidates with reason CAE_ELIG_UNNEEDED in input order (a block-wide scan per
+//     chunk of candidates).
+#include <climits>
+#include <cub/block/block_scan.cuh>
+
+#include "engine.h"
+
+namespace cae {
+
+constexpr int EL_WARPS = 8;                        // candidates per block of elig_kernel
+constexpr int EL_COMPACT = 1024;                   // threads of elig_compact_kernel
+constexpr long long EL_MILLI_LIM = LLONG_MAX / 1000;
+enum : int { PF_DAEMONSET = 1, PF_MIRROR = 2, PF_LONG_TERMINATING = 4 };
+
+// Two's-complement 128-bit sum of int64 terms: exact for any count of terms an int32 offset can address
+struct Sum128 {
+  unsigned long long lo = 0, hi = 0;
+  __device__ __forceinline__ void add(unsigned long long l2, unsigned long long h2) {
+    const unsigned long long l = lo + l2;
+    hi += h2 + (l < lo);
+    lo = l;
+  }
+  __device__ __forceinline__ void add(long long v) { add((unsigned long long)v, v < 0 ? ~0ull : 0ull); }
+  __device__ __forceinline__ void warp_sum() {     // every lane ends with the warp's sum
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) add(__shfl_xor_sync(0xffffffffu, lo, d), __shfl_xor_sync(0xffffffffu, hi, d));
+  }
+  __device__ __forceinline__ bool fits() const { return hi == (unsigned long long)((long long)lo >> 63); }
+};
+
+// Quantity.MilliValue() of a value in the engine's units: cpu is held in milli already, every other dim is multiplied by
+// 1000.  False: the product leaves int64.
+__device__ __forceinline__ bool to_milli(int r, long long v, long long& m) {
+  if (r == CAE_RES_CPU) { m = v; return true; }
+  if (v > EL_MILLI_LIM || v < -EL_MILLI_LIM) return false;
+  m = v * 1000;
+  return true;
+}
+
+enum : int { U_OK = 0, U_ERROR = 1, U_BIG = 2 };
+// CalculateUtilizationOfResource of dim r: float64(counted.MilliValue()) / float64(alloc.MilliValue() - excluded.MilliValue()).
+// The int64 difference wraps as Go's does; the division is IEEE (0/0 = NaN, x/0 = +-Inf).
+__device__ __forceinline__ int util_of(int r, long long alloc, const Sum128& counted, const Sum128& excluded, double& u) {
+  long long am, cm, em;
+  if (!to_milli(r, alloc, am)) return U_BIG;
+  if (am == 0) return U_ERROR;                     // allocatable absent or MilliValue() == 0
+  if (!counted.fits() || !excluded.fits() || !to_milli(r, (long long)counted.lo, cm) || !to_milli(r, (long long)excluded.lo, em))
+    return U_BIG;
+  const long long den = (long long)((unsigned long long)am - (unsigned long long)em);
+  u = __ddiv_rn(__ll2double_rn(cm), __ll2double_rn(den));
+  return U_OK;
+}
+
+// Go's math.Max: +Inf wins over NaN, NaN over everything else, +0 over -0 (fmax would drop a NaN)
+__device__ __forceinline__ double go_max(double x, double y) {
+  if ((isinf(x) && x > 0) || (isinf(y) && y > 0)) return __longlong_as_double(0x7ff0000000000000ll);
+  if (isnan(x) || isnan(y)) return __longlong_as_double(0x7ff8000000000001ll);   // math.NaN()
+  if (x == 0 && x == y) return signbit(x) ? y : x;
+  return x > y ? x : y;
+}
+
+__global__ void __launch_bounds__(EL_WARPS * 32) elig_kernel(DevObjects o, EligLaunch a) {
+  const int lane = threadIdx.x & 31, i = blockIdx.x * EL_WARPS + (threadIdx.x >> 5);
+  if (i >= a.n) return;                            // warp-uniform, as is every branch before the shuffles
+  uint8_t reason = CAE_ELIG_PRE;
+  double cpu = 0.0, mem = 0.0, gpu = 0.0, util = 0.0;
+  if (!a.pre[i]) {
+    const int row = a.cand[i], g = a.gpu_dim[i];
+    reason = CAE_ELIG_UNEXPECTED_ERROR;            // gpu_dim -2: GpuConfig names a resource the node cannot have
+    if (g != -2) {
+      const bool two = g < 0;                      // no GpuConfig: cpu and memory
+      const int d0 = two ? CAE_RES_CPU : g;
+      const bool skip_ds = a.skip_ds[i] != 0, skip_mirror = a.skip_mirror != 0;
+      Sum128 c0, x0, c1, x1;                       // counted / excluded of d0 and of memory
+      const int b = o.node_pod_off[row], e = o.node_pod_off[row + 1];
+      for (int k = b + lane; k < e; k += 32) {
+        const int f = a.flags ? a.flags[k] : 0;
+        const int64_t* req = o.ps_req + (size_t)o.node_pod_spec[k] * R;
+        const long long v0 = req[d0], v1 = two ? req[CAE_RES_MEM] : 0;
+        if ((skip_ds && (f & PF_DAEMONSET)) || (skip_mirror && (f & PF_MIRROR))) {
+          x0.add(v0);
+          x1.add(v1);
+        } else if (!(f & PF_LONG_TERMINATING)) {
+          c0.add(v0);
+          c1.add(v1);
+        }
+      }
+      c0.warp_sum();
+      x0.warp_sum();
+      if (two) {
+        c1.warp_sum();
+        x1.warp_sum();
+      }
+      if (lane == 0) {
+        const int64_t* al = o.node_alloc + (size_t)row * R;
+        int rc;
+        if (two) {
+          rc = util_of(CAE_RES_CPU, al[CAE_RES_CPU], c0, x0, cpu);
+          if (rc == U_OK) rc = util_of(CAE_RES_MEM, al[CAE_RES_MEM], c1, x1, mem);
+          util = go_max(cpu, mem);
+        } else {
+          rc = util_of(g, al[g], c0, x0, gpu);
+          util = gpu;
+        }
+        if (rc == U_BIG) *a.status = 1;
+        if (rc != U_OK) {
+          cpu = mem = gpu = util = 0.0;
+        } else if (a.unready[i]) {
+          reason = CAE_ELIG_UNREADY_DISABLED;
+        } else {
+          reason = !(util >= a.threshold[i]) ? CAE_ELIG_UNNEEDED : CAE_ELIG_NOT_UNDERUTILIZED;   // NaN is below any threshold
+        }
+      }
+    }
+  }
+  if (lane == 0) {
+    double* u = a.util + (size_t)i * 4;
+    u[0] = cpu;
+    u[1] = mem;
+    u[2] = gpu;
+    u[3] = util;
+    a.reason[i] = reason;
+  }
+}
+
+__global__ void __launch_bounds__(EL_COMPACT) elig_compact_kernel(EligLaunch a) {
+  using Scan = cub::BlockScan<int, EL_COMPACT>;
+  __shared__ typename Scan::TempStorage tmp;
+  int base = 0;
+  for (int c0 = 0; c0 < a.n; c0 += EL_COMPACT) {
+    const int i = c0 + threadIdx.x;
+    const int keep = i < a.n && a.reason[i] == CAE_ELIG_UNNEEDED;
+    int pos, total;
+    Scan(tmp).ExclusiveSum(keep, pos, total);
+    if (keep) a.list[base + pos] = i;
+    base += total;
+    __syncthreads();                               // tmp is reused by the next chunk
+  }
+  if (threadIdx.x == 0) *a.count = base;
+}
+
+int launch_eligibility(Engine* e, const EligLaunch& a) {
+  if (a.n <= 0) return 0;
+  elig_kernel<<<(a.n + EL_WARPS - 1) / EL_WARPS, EL_WARPS * 32, 0, e->stream>>>(e->dobj, a);
+  elig_compact_kernel<<<1, EL_COMPACT, 0, e->stream>>>(a);
+  e->stats.kernel_launches += 2;
+  CAE_KERNEL_OK();
+  return 0;
+}
+
+}  // namespace cae

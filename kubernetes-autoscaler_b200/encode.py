@@ -794,6 +794,21 @@ class SimilarityInputs(AbiArrays):
     COUNTS = {"num_ignored_keys": "ignored_keys"}
 
 
+class EligibilityInputs(AbiArrays):
+    """``cae_eligibility_inputs`` of cae_scale_down_eligibility.  The optional arrays left out are NULL; n_pod_flags follows
+    pod_flags unless given."""
+
+    STRUCT = capi.cae_eligibility_inputs
+    COUNTS = {"n_cand": "cand_node"}
+
+    def __init__(self, **fields) -> None:
+        for nm in ("pod_flags", "skip_ds", "pre_reason", "unready"):
+            fields.setdefault(nm, None)
+        super().__init__(**fields)
+        if "n_pod_flags" not in fields:
+            self.struct.n_pod_flags = len(self.arrays["pod_flags"]) if "pod_flags" in self.arrays else 0
+
+
 # ----------------------------------------------------------------------------------------------
 class Encoder:
     """Interns objects.py dataclasses into a TableBuilder (the Go shim's job in production)."""

@@ -10,7 +10,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 
 from . import capi
-from .encode import EncodedObjects, PriceInputs, SimilarityInputs
+from .encode import EligibilityInputs, EncodedObjects, PriceInputs, SimilarityInputs
 
 
 class EngineError(RuntimeError):
@@ -371,6 +371,29 @@ class Engine:
         limit = np.zeros(T, np.int64)
         self._check(self.lib.cae_similar_node_groups(self.h, si.ptr(), _vp(bits), _vp(count), _vp(limit)))
         return bits, count, limit
+
+    def scale_down_eligibility(self, cand_node, gpu_dim, threshold, pod_flags=None, skip_ds=None, skip_mirror: bool = False,
+                               pre_reason=None, unready=None):
+        """cae_scale_down_eligibility on the resident snapshot: every candidate's utilization and eligibility reason.
+        cand_node [n] cluster rows; gpu_dim [n] (-1 no GpuConfig, -2 a resource the load has no dim for); threshold [n];
+        pod_flags [resident pods of the cluster rows] bits DaemonSet | mirror << 1 | long-terminating << 2 (None = all 0);
+        skip_ds / pre_reason / unready [n] flags (None = all 0).  Returns (util [n][4] float64: cpu, mem, gpu, Utilization;
+        reason [n] uint8 CAE_ELIG_*; unneeded: the candidate indices with reason CAE_ELIG_UNNEEDED, in input order).
+        Raises EngineUnsupported on status 1 (a quantity that leaves int64)."""
+        cn = np.ascontiguousarray(cand_node, np.int32).reshape(-1)
+        n = len(cn)
+        ei = EligibilityInputs(cand_node=cn, gpu_dim=np.ascontiguousarray(gpu_dim, np.int32), skip_mirror=int(bool(skip_mirror)),
+                               threshold=np.ascontiguousarray(threshold, np.float64), pod_flags=_opt(pod_flags, np.uint8),
+                               skip_ds=_opt(skip_ds, np.uint8), pre_reason=_opt(pre_reason, np.uint8), unready=_opt(unready, np.uint8))
+        for nm in ("gpu_dim", "threshold", "skip_ds", "pre_reason", "unready"):
+            if nm in ei.arrays and ei.arrays[nm].shape != (n,):
+                raise ValueError("scale_down_eligibility: %s needs one entry per candidate" % nm)
+        util = np.zeros((max(n, 1), 4), np.float64)
+        reason = np.zeros(max(n, 1), np.uint8)
+        unneeded = np.zeros(max(n, 1), np.int32)
+        m = np.zeros(1, np.int32)
+        self._check(self.lib.cae_scale_down_eligibility(self.h, ei.ptr(), _vp(util), _vp(reason), _vp(unneeded), _vp(m)))
+        return util[:n], reason[:n], unneeded[:int(m[0])]
 
     # ---- fused histogram exchange over peer memory (multi-GPU dense pass) -------------------------
     def peer_handle(self) -> bytes:

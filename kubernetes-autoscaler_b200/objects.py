@@ -106,6 +106,12 @@ class Pod:
     owner_kind: str = ""
     # spec.priority (corev1helpers.PodPriority: 0 when unset); only the filter-out-schedulable ordering reads it
     priority: int = 0
+    # read only by the scale-down eligibility (IsMirrorPod, IsPodLongTerminating in eligibility.py); pod grouping ignores
+    # them: metadata.annotations, metadata.deletionTimestamp in seconds since the epoch (None = not being deleted;
+    # `terminating` is the flag the filters read) and spec.terminationGracePeriodSeconds (None = unset)
+    annotations: Dict[str, str] = field(default_factory=dict)
+    deletion_timestamp: Optional[float] = None
+    termination_grace_period_seconds: Optional[int] = None
 
     def clone(self) -> "Pod":
         return copy.deepcopy(self)

@@ -70,9 +70,9 @@ def pod_requests(containers: Sequence[Container], init_containers: Sequence[Cont
 
 
 def _spec_key(p: Pod):
-    """utils.PodSpecSemanticallyEqual on the fields this model carries (names / UIDs excluded)."""
+    """utils.PodSpecSemanticallyEqual on the fields this model carries (names / UIDs and metadata excluded)."""
     d = dataclasses.asdict(p)
-    for k in ("name", "labels", "owner_uid", "owner_kind"):
+    for k in ("name", "labels", "owner_uid", "owner_kind", "annotations", "deletion_timestamp", "termination_grace_period_seconds"):
         d.pop(k, None)
     return repr(sorted(d.items()))
 

@@ -25,6 +25,10 @@ from .podlistprocessor import HintingSimulator, HintKeyFromPod, RemovalInputs, p
 
 # simulator/cluster.go:55-95
 NoReason, NoPlaceToMovePods, NoNodeInfo = "NoReason", "NoPlaceToMovePods", "NoNodeInfo"
+# the reasons of the scale-down eligibility checks (eligibility.py)
+ScaleDownDisabledAnnotation, NotAutoscaled, NotUnderutilized = "ScaleDownDisabledAnnotation", "NotAutoscaled", "NotUnderutilized"
+CurrentlyBeingDeleted, RecentlyUnremovable = "CurrentlyBeingDeleted", "RecentlyUnremovable"
+ScaleDownUnreadyDisabled, UnexpectedError = "ScaleDownUnreadyDisabled", "UnexpectedError"
 
 
 @dataclass

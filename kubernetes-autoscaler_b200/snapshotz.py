@@ -50,6 +50,12 @@ def quantity_milli(q: Any) -> int:       # Quantity.MilliValue(): rounds up
     return math.ceil(parse_quantity(q) * 1000)
 
 
+def parse_time(t: str) -> float:
+    """metav1.Time (RFC 3339, as the API server writes it, e.g. "2024-05-01T12:00:00Z") in seconds since the epoch."""
+    from datetime import datetime
+    return datetime.fromisoformat(t.replace("Z", "+00:00")).timestamp()
+
+
 def resource_list(rl: Optional[Dict[str, Any]]) -> Dict[str, int]:
     out: Dict[str, int] = {}
     for name, q in (rl or {}).items():
@@ -104,6 +110,11 @@ def pod_from_json(p: Dict[str, Any]) -> Pod:
     pod.pod_affinity = _affinity_terms((aff.get("podAffinity") or {}).get("requiredDuringSchedulingIgnoredDuringExecution"))
     pod.pod_anti_affinity = _affinity_terms((aff.get("podAntiAffinity") or {}).get("requiredDuringSchedulingIgnoredDuringExecution"))
     pod.terminating = meta.get("deletionTimestamp") is not None
+    pod.annotations = dict(meta.get("annotations") or {})
+    if pod.terminating:
+        pod.deletion_timestamp = parse_time(meta["deletionTimestamp"])
+    grace = spec.get("terminationGracePeriodSeconds")
+    pod.termination_grace_period_seconds = None if grace is None else int(grace)
     pod.priority = int(spec.get("priority") or 0)
     # pods the engine must hand to the stock path (SURVEY §7 hard part 7): PVC / ephemeral volumes, DRA claims
     vols = spec.get("volumes") or []

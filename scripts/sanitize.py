@@ -7,7 +7,7 @@ self-cleaning accumulators, last-block election, shared-memory state and block-w
 
 Dense pass (K1, both variants), Estimate() of every template (K0 + K3: plain closed form, capacity form with the cluster
 fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals), a cluster-node delta
-(cae_load_nodes), a cluster-node churn (cae_load_node_churn), new pod specs (cae_load_pods), node-group template changes (cae_load_templates), the placements of a filter pass made resident (cae_force_add_pods) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
+(cae_load_nodes), a cluster-node churn (cae_load_node_churn), new pod specs (cae_load_pods), node-group template changes (cae_load_templates), the placements of a filter pass made resident (cae_force_add_pods), the scale-down eligibility (cae_scale_down_eligibility) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
 against the CPU oracle so that a "clean" run also means "correct results under the tool"."""
 import os
 import sys
@@ -117,6 +117,19 @@ def main():
             caps = np.full(after.T, 30, np.int32)
             got_e, ref_e = eng.estimate_all(caps), pyoracle.estimate_all(after, caps)
             assert all(np.array_equal(x, y) for x, y in zip(got_e, ref_e[:4]))
+        # scale-down eligibility (cae_scale_down_eligibility: the warp-per-row sums, the one-block compaction) on the load
+        # of the last delta, every cluster row a candidate twice, against a fresh load of the same objects
+        if enc.struct.num_cluster_nodes:
+            N = after.struct.num_cluster_nodes
+            rng = np.random.default_rng(cfg)
+            rows = np.concatenate([np.arange(N), np.arange(N)[::-1]]).astype(np.int32)
+            flags = rng.integers(0, 8, int(after.arrays["node_pod_off"][N])).astype(np.uint8)
+            args = (rows, rng.choice([-1, -1, 1, 2], 2 * N).astype(np.int32), np.full(2 * N, 0.5), flags,
+                    rng.integers(0, 2, 2 * N).astype(np.uint8), True)
+            got = eng.scale_down_eligibility(*args)
+            eng.load(after)
+            want = eng.scale_down_eligibility(*args)
+            assert all(np.array_equal(x, y, equal_nan=True) for x, y in zip(got, want))
         # similar node groups (cae_similar_node_groups: operand / bit-row prep, the pair kernel's staged tiles and ballots)
         infos, groups, ngs = synth.node_group_families(cfg, 45, 4, seed=cfg, groups=40)
         sim = ScaleUpSimulation([], infos, groups, eng)
