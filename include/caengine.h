@@ -689,6 +689,39 @@ int32_t cae_simulate_removals(cae_engine* e, int32_t n_cand, const int32_t* cand
                               int32_t persist, int32_t* result, int32_t* last_index_out, int32_t* log, int32_t log_cap,
                               int32_t* log_len);
 
+/* The ProvisioningRequest capacity check: the check-capacity.autoscaling.x-k8s.io class's bookCapacity and its loop over
+ * requests (cluster-autoscaler/provisioningrequest/checkcapacity/provisioningclass.go, orchestrator/orchestrator.go), in
+ * one launch.  Every output equals what this loop returns on ONE HintingSimulator (hints and lastIndex carried from call to
+ * call, SimilarPodsScheduling restarting per call) over the cluster rows of the resident snapshot:
+ *   for r in 0 .. n_req-1:
+ *     BOOK:  TrySchedulePods(pods of r, ScheduleAnywhere, breakOnFailure=false); every placement is kept
+ *     CHECK: Fork; TrySchedulePods(pods of r, ScheduleAnywhere, breakOnFailure=true); Commit if every pod was placed,
+ *            else Revert (later requests see a committed request's capacity as taken)
+ *   finally the outer Revert: the resident snapshot and every later answer stay exactly as they were, after any load or
+ *   delta.  A caller that wants the kept placements as residents passes them to cae_force_add_pods.
+ * Templates are ignored.
+ *   n_req, req_kind [n_req]     cae_capacity_kind of each request, in processing order
+ *   req_off [n_req + 1], req_pod []  pending-pod indices of each request in the order they are tried; a pod is listed at
+ *                               most once in the whole call.  A request with no pods is FOUND (0 placed == 0 asked).
+ *   hint_node, sim_class, class_ctrl, n_classes, last_index_in  as for cae_filter_schedulable (last_index_in may be raw)
+ * Outputs: result [n_req] cae_capacity_result: a CHECK request is FOUND iff it was committed, a BOOK request iff every pod
+ * was placed (it is kept either way); assigned_node [num_pending] the cluster row each pod was placed on in its request's
+ * simulation, whether or not the request was kept, -1 when it fitted nowhere, was not tried because of an earlier break, or
+ * is not listed (the caller sets its hints from this); last_index_out, raw when no scan placed a pod.
+ * At world_size > 1 the call runs on the pending pods this engine holds (this rank's pods under CAE_CFG_PODS_PRESHARDED)
+ * and each rank answers on its own, like cae_simulate_removals.  The placements of one request fit the per-simulation
+ * placement log by construction; should it overflow the call returns -1, like cae_simulate_removals.
+ * n_req == 0 is a valid call that changes nothing (assigned_node all -1, last_index_out = last_index_in).
+ * Status -2 (nothing runs): before cae_load, n_req < 0, a NULL array that is needed, req_off[0] != 0 or req_off
+ * decreasing, a kind other than BOOK or CHECK, a pod out of range or listed twice, a hinted row out of range, classes
+ * cae_filter_schedulable would refuse. */
+enum cae_capacity_kind { CAE_CAPACITY_BOOK = 0, CAE_CAPACITY_CHECK = 1 };
+enum cae_capacity_result { CAE_CAPACITY_FOUND = 0, CAE_CAPACITY_NOT_FOUND = 1 };
+int32_t cae_check_capacity(cae_engine* e, int32_t n_req, const int32_t* req_kind, const int32_t* req_off,
+                           const int32_t* req_pod, const int32_t* hint_node, const int32_t* sim_class,
+                           const int32_t* class_ctrl, int32_t n_classes, int32_t last_index_in,
+                           int32_t* result, int32_t* assigned_node, int32_t* last_index_out);
+
 /* The two halves of cae_expander_best for templates sharded over ranks (no [T][E] matrix ever leaves a GPU):
  * cae_waste_scores returns the least-waste score (expander/waste/waste.go:44-72) of this rank's template shard from
  * the device-resident result of the last cae_estimate_all, 0.0 for the rows of other ranks, so that a SUM all-reduce of

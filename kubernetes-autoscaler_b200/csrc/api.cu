@@ -2422,6 +2422,91 @@ int32_t cae_simulate_removals(cae_engine* h, int32_t n_cand, const int32_t* cand
   return 0;
 }
 
+int32_t cae_check_capacity(cae_engine* h, int32_t n_req, const int32_t* req_kind, const int32_t* req_off, const int32_t* req_pod,
+                           const int32_t* hint_node, const int32_t* sim_class, const int32_t* class_ctrl, int32_t n_classes,
+                           int32_t last_index_in, int32_t* result, int32_t* assigned_node, int32_t* last_index_out) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_check_capacity before cae_load"); return -2; }
+  const int P = e->P, N = e->N;
+  if (n_req < 0 || (n_req > 0 && (!req_kind || !req_off || !result)) || (P > 0 && !assigned_node) || !last_index_out ||
+      (sim_class && n_classes > 0 && !class_ctrl)) {
+    cae::set_error("cae_check_capacity: bad arguments");
+    return -2;
+  }
+  if (!sim_class) n_classes = 0;
+  // everything is checked before the first device write
+  const int M = n_req > 0 ? req_off[n_req] : 0;
+  if (n_req > 0 && req_off[0] != 0) { cae::set_error("cae_check_capacity: req_off[0] must be 0"); return -2; }
+  for (int r = 0; r < n_req; ++r) {
+    if (req_kind[r] != CAE_CAPACITY_BOOK && req_kind[r] != CAE_CAPACITY_CHECK) { cae::set_error("cae_check_capacity: unknown request kind"); return -2; }
+    if (req_off[r + 1] < req_off[r]) { cae::set_error("cae_check_capacity: req_off decreases"); return -2; }
+  }
+  if (M > 0 && !req_pod) { cae::set_error("cae_check_capacity: bad arguments"); return -2; }
+  {
+    std::vector<int32_t>& seen = e->rm_seen;   // a pod is placed at most once in the whole batch
+    seen.assign(std::max(P, 1), 0);
+    for (int k = 0; k < M; ++k) {
+      const int pod = req_pod[k];
+      if (pod < 0 || pod >= P) { cae::set_error("cae_check_capacity: pod index out of range"); return -2; }
+      if (seen[pod]++) { cae::set_error("cae_check_capacity: a pod is listed twice"); return -2; }
+    }
+  }
+  if (hint_node)
+    for (int i = 0; i < P; ++i)
+      if (hint_node[i] < -1 || hint_node[i] >= N) { cae::set_error("cae_check_capacity: hinted row out of range"); return -2; }
+  const int nctrl = sim_class_check("cae_check_capacity", sim_class, class_ctrl, n_classes, P, -1);
+  if (nctrl < 0) return -2;
+  e->stats.h2d_bytes = 0;
+  e->stats.d2h_bytes = 0;
+  if (n_req == 0) {
+    std::fill(assigned_node, assigned_node + P, -1);
+    *last_index_out = last_index_in;
+    return 0;
+  }
+  cudaSetDevice(e->cfg.device);
+  // one staged blob: kind | req_off | req_pod | hint | class | class_ctrl, then the outputs result | out[3] | assigned, which
+  // come back in one copy; an absent hint or class array stays NULL
+  Engine::Staging& st = e->fm;
+  cae::RemovalLaunch r{};
+  r.ncand = n_req; r.persist = 1; r.ncls = n_classes; r.nctrl = nctrl; r.log_cap = 0; r.last_index = last_index_in;
+  size_t in_end = 0, out_end = 0;
+  auto walk = [&](cae::Layout& l) {
+    l.add(r.kind, n_req); l.add(r.move_off, n_req + 1); l.add(r.move_pod, std::max(M, 1));
+    if (hint_node) l.add(r.hint, P);
+    if (sim_class) l.add(r.cls, P);
+    l.add(r.class_ctrl, std::max(n_classes, 1));
+    in_end = l.bytes;
+    l.add(r.result, n_req); l.add(r.out, 3); l.add(r.assigned, std::max(P, 1));
+    out_end = l.bytes;
+  };
+  const size_t bytes = cae::layout_bytes(walk);
+  if (cae::stage_reserve(e, st, bytes, out_end)) return -1;
+  cae::layout_bind(st.dev.p, walk);
+  r.status = r.out + 2;   // out = {lastIndex, log length (unused), placement log overflow}
+  std::copy(req_kind, req_kind + n_req, st.host_of(r.kind));
+  std::copy(req_off, req_off + n_req + 1, st.host_of(r.move_off));
+  if (M) std::copy(req_pod, req_pod + M, st.host_of(r.move_pod));
+  if (hint_node) std::copy(hint_node, hint_node + P, st.host_of(r.hint));
+  if (sim_class) std::copy(sim_class, sim_class + P, st.host_of(r.cls));
+  if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, st.host_of(r.class_ctrl));
+  if (cae::stage_upload(e, st, in_end)) return -1;
+  const size_t o_assigned = reinterpret_cast<const char*>(r.assigned) - static_cast<const char*>(st.dev.p);
+  CAE_CUDA(cudaMemsetAsync(r.result, 0, o_assigned - in_end, e->stream));
+  CAE_CUDA(cudaMemsetAsync(r.assigned, 0xFF, out_end - o_assigned, e->stream));   // -1 = not placed
+  cudaEventRecord(e->ev0, e->stream);
+  if (cae::launch_removals(e, r)) return -1;
+  cudaEventRecord(e->ev1, e->stream);
+  CAE_CUDA(cudaMemcpyAsync(st.host_of(r.result), r.result, out_end - in_end, cudaMemcpyDeviceToHost, e->stream));
+  if (fm_finish(e, nullptr, nullptr, 0, nullptr)) return -1;
+  e->stats.d2h_bytes = (int64_t)(out_end - in_end);
+  const int32_t* out = st.host_of(r.out);
+  if (out[2]) { cae::set_error("placement log overflow in the capacity batch"); return -1; }
+  std::copy(st.host_of(r.result), st.host_of(r.result) + n_req, result);
+  std::copy(st.host_of(r.assigned), st.host_of(r.assigned) + P, assigned_node);
+  *last_index_out = out[0];
+  return 0;
+}
+
 void* cae_stream(cae_engine* h) {
   Engine* e = reinterpret_cast<Engine*>(h);
   return e ? reinterpret_cast<void*>(e->stream) : nullptr;

@@ -249,7 +249,9 @@ __device__ __forceinline__ int bp_div_f(int64_t f, int64_t r, float rinv, int kb
 // RM = true (implies FM): RemovalSimulator.SimulateNodeRemoval called on every candidate in order (simulator/cluster.go:
 // 126-217), one work item per candidate on the same block.  rm_begin takes the candidate out of a working copy of the
 // snapshot (live mask, counter tables), builds its pod list and runs; the FM body simulates; rm_end records the outcome
-// and, for a persisted success, makes the working copy the committed one.
+// and, for a persisted success, makes the working copy the committed one.  The same instantiation runs a ProvisioningRequest
+// capacity batch (cae_check_capacity, RemovalState::kind set): item t is request t, no node leaves, and rm_end commits a
+// BOOK request always and a CHECK request when every pod was placed.
 template <int A, int TPB, bool WIN, bool FM, bool RM = false>
 __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack_kernel(DevObjects o, DynTables d, BpParams p) {
   constexpr int NW = TPB / 32;
@@ -340,8 +342,9 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
         if (tid == 0) { S.rm_li_raw = r.li_in; S.rm_log_n = 0; }
         __syncthreads();
       }
-      const int cand = r.cand[t];
-      const bool exists = cand >= 0 && r.live[cand];
+      // a capacity batch (r.kind set) has no candidate: no row leaves, its requests list their pods like move_pod
+      const int cand = r.kind ? -1 : r.cand[t];
+      const bool exists = r.kind || (cand >= 0 && r.live[cand]);
       if (!exists) {
         if (tid == 0) { S.rm_mode = 0; S.rm_runs = 0; S.rm_len = 0; S.rm_li = 0; }
       } else {
@@ -356,7 +359,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
         __syncthreads();
         // the candidate's resident pods and the pods earlier persisted simulations moved onto it stop counting, and its
         // domains lose one eligible node (dyn_base_kernel's sums without this row)
-        for (int q = tid; q < d.Q; q += TPB) {
+        for (int q = tid; q < d.Q && cand >= 0; q += TPB) {
           if (!d.elig[(size_t)q * p.U + cand]) continue;
           const int dm = d.dom[(size_t)d.q_k[q] * NTd + cand];
           if (dm < 0) continue;
@@ -372,7 +375,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
         for (int i = tid; i < L0; i += TPB) list[i] = r.move_pod[mb + i];
         if (tid == 0) {
           int L = L0;
-          for (int pod = r.head[cand]; pod >= 0; pod = r.next[pod]) list[L++] = pod;
+          for (int pod = cand >= 0 ? r.head[cand] : -1; pod >= 0; pod = r.next[pod]) list[L++] = pod;
           S.rm_len = L;
         }
         __syncthreads();
@@ -452,6 +455,12 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
     int n_new = 0, nodes_with_pods = 0, pods_total = 0,
         last_index = RM ? S.rm_li : FM ? p.fm_last_index : (p.last_index_in ? p.last_index_in[t] : 0);
     auto li_eff = [&]() -> int { const int len = N + n_new; return len > 0 ? last_index % len : 0; };
+    // breakOnFailure: per request in a capacity batch (a CHECK breaks, a BOOK does not), else the launch's.  Read at each use,
+    // as p.fm_break was: the filter instantiation compiles to the same code as before.
+    auto fm_brk = [&]() -> int {
+      if constexpr (RM) { if (p.rm.kind) return p.rm.kind[t]; }
+      return p.fm_break;
+    };
     bool new_nodes_available = !FM, cl_init = false, fm_stop = false, fm_moved = false;
     auto ensure_cluster = [&]() {  // run state of the cluster nodes, needed once a placement can reach them
       if (cl_init) return;
@@ -861,7 +870,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
       if (FM && dc == 0 && fm_hint < 0) {
         // ======================= plain run on the cluster nodes: dealt lap by lap ==================
         if (fm_stop || fm_blocked || N == 0) {
-          if (p.fm_break && n > 0) fm_stop = true;     // every pod of the run stays unschedulable (breakOnFailure, :71-73)
+          if (fm_brk() && n > 0) fm_stop = true;     // every pod of the run stays unschedulable (breakOnFailure, :71-73)
         } else {
           int total = 0, zero = 0, zero2 = 0;
           const int clampv = n < (1 << 26) ? n + 1 : (1 << 26);
@@ -876,7 +885,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
           fm_deal(m);
           if (m < n) {                      // the next pod fits nowhere: the identical pods behind it see the same state
             fm_mark_failed();
-            if (p.fm_break) fm_stop = true;
+            if (fm_brk()) fm_stop = true;
           }
         }
       } else if (FM && dc == 0) {
@@ -909,7 +918,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
               placed += 1;
             } else fm_mark_failed();
           }
-          if (where < 0 && p.fm_break) fm_stop = true;
+          if (where < 0 && fm_brk()) fm_stop = true;
         }
         if (tid == 0) p.fm_assigned[p.fm_pods[pb]] = where;
       } else if (dc == 0) {
@@ -1245,7 +1254,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
             // hostname counters only: per-node capacities over the cluster nodes, dealt like a plain run
             fast = true;
             if (fm_stop || fm_blocked || N == 0) {
-              if (p.fm_break && n > 0) fm_stop = true;
+              if (fm_brk() && n > 0) fm_stop = true;
             } else {
               if (!caps_done) cluster_caps();
               const int clampv = n < (1 << 26) ? n + 1 : (1 << 26);
@@ -1256,7 +1265,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
               fm_deal(m);
               if (m < n) {
                 fm_mark_failed();
-                if (p.fm_break) fm_stop = true;
+                if (fm_brk()) fm_stop = true;
               }
             }
           } else if (ok) {
@@ -1506,7 +1515,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
                   fm_mark_failed();
                 }
               }
-              if (where < 0 && p.fm_break) fm_stop = true;   // breakOnFailure (:71-73)
+              if (where < 0 && fm_brk()) fm_stop = true;   // breakOnFailure (:71-73)
             }
             if (tid == 0) p.fm_assigned[pod] = where;
           }
@@ -1582,16 +1591,19 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
     if (p.prof && tid == 0) atomicAdd((unsigned long long*)&p.prof[7], (unsigned long long)(clock64() - prof_tmpl0));
     if constexpr (RM) {
       // ---- rm_end: outcome, log, hints, lastIndex; a persisted success commits the working copy ----
+      // A capacity batch commits a BOOK request whatever it placed and a CHECK request that placed every pod; its
+      // output is fm_assigned itself (every pod is listed once in the whole batch), so it keeps no log.
       const RemovalState& r = p.rm;
       const int mode = S.rm_mode, L = S.rm_len, base = S.rm_log_n;
-      const int cand = r.cand[t];
+      const int cand = r.kind ? -1 : r.cand[t];
       const bool ok = pods_total == L;      // breakOnFailure: every pod placed, or the simulation stopped
+      const bool commit = mode != 0 && (r.kind ? ok || r.kind[t] == CAE_CAPACITY_BOOK : ok && r.persist);
       for (int i = tid; i < L; i += TPB) {  // one log entry per pod tried; hints set by placed pods survive in every case
         const int pod = p.fm_pods[i], x = p.fm_assigned[pod];
         if (base + i < r.log_cap) { r.log[(size_t)(base + i) * 3] = t; r.log[(size_t)(base + i) * 3 + 1] = pod; r.log[(size_t)(base + i) * 3 + 2] = x; }
         if (x >= 0) r.hint[pod] = x;
       }
-      if (mode != 0 && ok && r.persist) {
+      if (commit) {
         // Commit.  Undo needs no log: every candidate starts from a full copy of the committed state (rm_begin copies the
         // counters, ensure_cluster the node state), so a simulation that is not committed leaves nothing behind, and one that
         // is committed is copied back whole — the committed state is always exactly what the loop of single calls leaves.
@@ -1605,6 +1617,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
         for (int k = tid; k < L * d.Q; k += TPB) {
           const int i = k / d.Q, q = k - i * d.Q;
           const int pod = p.fm_pods[i], x = p.fm_assigned[pod];
+          if (x < 0) continue;   // a BOOK request keeps what it placed
           const int w = d.wmat[(size_t)q * d.S + o.pend_spec[pod]];
           if (w == 0 || !d.elig[(size_t)q * p.U + x]) continue;
           const int dm = d.dom[(size_t)d.q_k[q] * (N + p.T) + x];
@@ -1616,9 +1629,10 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
         for (int i = tid; i < d.pool; i += TPB) { r.ccnt[i] = r.wcnt[i]; r.cpres[i] = r.wpres[i]; }
         for (int q = tid; q < d.Q; q += TPB) r.ctot[q] = r.wtot[q];
         if (tid == 0) {
-          r.live[cand] = 0;
+          if (cand >= 0) r.live[cand] = 0;
           for (int i = 0; i < L; ++i) {   // NodeInfo order: appended to their destination in processing order
             const int pod = p.fm_pods[i], x = p.fm_assigned[pod];
+            if (x < 0) continue;
             r.next[pod] = -1;
             if (r.tail[x] < 0) r.head[x] = pod; else r.next[r.tail[x]] = pod;
             r.tail[x] = pod;
@@ -1626,7 +1640,8 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
         }
       }
       if (tid == 0) {
-        r.result[t] = mode == 0 ? CAE_REMOVAL_NO_NODE_INFO : ok ? CAE_REMOVAL_REMOVABLE : CAE_REMOVAL_NO_PLACE;
+        if (r.kind) r.result[t] = ok ? CAE_CAPACITY_FOUND : CAE_CAPACITY_NOT_FOUND;
+        else r.result[t] = mode == 0 ? CAE_REMOVAL_NO_NODE_INFO : ok ? CAE_REMOVAL_REMOVABLE : CAE_REMOVAL_NO_PLACE;
         // lastIndex leaves as a position among the live nodes; it stays raw when no scan placed a pod (plugin_runner.go:123)
         if (fm_moved && S.rm_nlive > 0) S.rm_li_raw = r.rank[last_index] % S.rm_nlive;
         S.rm_log_n = base + L;
@@ -1868,7 +1883,7 @@ int launch_removals(Engine* e, const RemovalLaunch& rl) {
   const size_t A1 = std::max(e->A, 1), ncls = std::max(rl.ncls, 1), nctrl = std::max(rl.nctrl, 1);
   RemovalState& r = p.rm;
   r.persist = rl.persist; r.log_cap = rl.log_cap; r.li_in = rl.last_index; r.ncls = rl.ncls; r.nctrl = rl.nctrl;
-  r.cand = rl.cand; r.move_off = rl.move_off; r.move_pod = rl.move_pod; r.dest_ok = rl.dest_ok;
+  r.cand = rl.cand; r.move_off = rl.move_off; r.move_pod = rl.move_pod; r.dest_ok = rl.dest_ok; r.kind = rl.kind;
   r.result = rl.result; r.log = rl.log; r.out = rl.out;
   r.grs = group_rec_src(e);
   // batch state, one buffer
@@ -1884,9 +1899,10 @@ int launch_removals(Engine* e, const RemovalLaunch& rl) {
   };
   if (devbuf_reserve(e, e->rm_state, layout_bytes(walk))) return -1;
   layout_bind(e->rm_state.p, walk);
+  if (rl.kind) { p.fm_assigned = rl.assigned; p.status = rl.status; }   // a capacity batch writes its outputs in place
   if (rl.hint) CAE_CUDA(cudaMemcpyAsync(r.hint, rl.hint, sizeof(int32_t) * e->P, cudaMemcpyDeviceToDevice, e->stream));
   else CAE_CUDA(cudaMemsetAsync(r.hint, 0xFF, sizeof(int32_t) * P, e->stream));
-  // one placement log entry per pod of a candidate at most
+  // one placement log entry per pod of a candidate (or a request) at most
   if (fm_slab_setup(e, p, e->P + 1024, 0)) return -1;
   { int unused = 0; if (launch_binpack_any(e, 1, 0, p, &unused, false, BP_REMOVALS)) return -1; }
   e->stats.kernel_launches += 1;

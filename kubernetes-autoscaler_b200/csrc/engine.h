@@ -301,7 +301,7 @@ struct Engine {
   Slab pack_slab, fm_slab;                // estimator / filter-out-schedulable pass (binpack.cu)
   Staging fm;                             // inputs, then outputs of the filter pass / the scale-down batch
   DevBuf rm_state;                        // scale-down batch state (RemovalState)
-  std::vector<int32_t> rm_owner, rm_seen; // [P] argument checks of the scale-down batch (kept to avoid per-call allocation)
+  std::vector<int32_t> rm_owner, rm_seen; // [P] argument checks of the scale-down and capacity batches (kept to avoid per-call allocation)
   DevBuf x_rows;                          // caller-supplied option rows: node_count | sched | order
   DevBuf x_price;                         // price inputs: node_price | pod_price | unfitness | score, then has_gpu | exists
   // fused histogram exchange over peer memory (feas.cu)
@@ -457,12 +457,16 @@ struct FilterLaunch {
   uint8_t *class_mark, *ctrl_over;
 };
 int launch_filter(Engine* e, const FilterLaunch& f);
-// cae_simulate_removals (api.cu lays out the inputs and outputs, launch_removals the batch state behind them)
+// cae_simulate_removals and cae_check_capacity (api.cu lays out the inputs and outputs, launch_removals the batch state
+// behind them).  A capacity batch sets `kind` and leaves cand, dest_ok and log NULL: item t lists its pods in
+// move_off / move_pod, no node leaves, and `assigned` [P] (set to -1 by the caller) takes every pod's node.
 struct RemovalLaunch {
   int ncand, persist, ncls, nctrl, log_cap, last_index;
   const int32_t *cand, *move_off, *move_pod, *hint, *cls, *class_ctrl;   // hint [P] (-1 = none) is read once
   const uint8_t* dest_ok;                                                // [N] or NULL
+  const int32_t* kind;                                                   // [ncand] CAE_CAPACITY_*, NULL for removals
   int32_t *result, *log, *out;                                           // out = {lastIndex, log length}
+  int32_t *assigned, *status;                                            // capacity batch: [P] output, status word
 };
 // Device view of a batch: inputs and outputs of RemovalLaunch, the committed state of the snapshot (what the persisted
 // simulations left) and the working copy of the candidate being simulated.  All of it lives in one engine-owned buffer.
@@ -470,6 +474,7 @@ struct RemovalState {
   int persist, log_cap, li_in, ncls, nctrl;
   const int32_t *cand, *move_off, *move_pod;
   const uint8_t* dest_ok;
+  const int32_t* kind;             // [T] capacity batch (cae_check_capacity): CAE_CAPACITY_BOOK | CHECK; NULL = removals
   int32_t *result, *log, *out;
   int64_t* cfree;                  // [A1][N] committed free resources
   int32_t* cslots;                 // [N]     committed pod slots

@@ -356,6 +356,23 @@ class Engine:
             return rc, None, None, np.zeros((int(n[0]), 3), np.int32)
         return rc, res[:len(cn)], int(li[0]), log[:int(n[0])]
 
+    def check_capacity(self, req_kind, req_off, req_pod, hint_node=None, sim_class=None, class_ctrl=None, last_index: int = 0):
+        """The ProvisioningRequest capacity batch on the snapshot of the last load (cae_check_capacity): BOOK requests keep
+        what they place, a CHECK request is committed only when every pod fits, and nothing stays in the snapshot.
+        Returns (result [n_req] CAE_CAPACITY_*, assigned [P] cluster row or -1 per pending pod, lastIndex afterwards)."""
+        kd = np.ascontiguousarray(req_kind, np.int32)
+        ro = np.ascontiguousarray(req_off, np.int32)
+        rp = np.ascontiguousarray(req_pod, np.int32)
+        hn = _opt(hint_node, np.int32)
+        sc = _opt(sim_class, np.int32)
+        cc = _opt(class_ctrl, np.int32)
+        res = np.zeros(max(len(kd), 1), np.int32)
+        assigned = np.full(max(self.enc.P, 1), -1, np.int32)
+        li = np.zeros(1, np.int32)
+        self._check(self.lib.cae_check_capacity(self.h, len(kd), _vp(kd), _vp(ro), _vp(rp), _vp(hn), _vp(sc), _vp(cc),
+                                                0 if cc is None else len(cc), int(last_index), _vp(res), _vp(assigned), _vp(li)))
+        return res[:len(kd)], assigned[:self.enc.P], int(li[0])
+
     def similar_node_groups(self, res_sig, free_dims, eligible, max_size, target_size, ignored_keys=(), safe=None,
                             ratios=(0.05, 0.05, 0.015)):
         """cae_similar_node_groups over the loaded templates.  ratios = (allocatable, free, memory capacity).  Returns

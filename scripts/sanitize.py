@@ -6,7 +6,7 @@ self-cleaning accumulators, last-block election, shared-memory state and block-w
     compute-sanitizer --tool racecheck python scripts/sanitize.py
 
 Dense pass (K1, both variants), Estimate() of every template (K0 + K3: plain closed form, capacity form with the cluster
-fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals), a cluster-node delta
+fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals), a ProvisioningRequest capacity batch (cae_check_capacity), a cluster-node delta
 (cae_load_nodes), a cluster-node churn (cae_load_node_churn), new pod specs (cae_load_pods), node-group template changes (cae_load_templates), the placements of a filter pass made resident (cae_force_add_pods), the scale-down eligibility (cae_scale_down_eligibility) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
 against the CPU oracle so that a "clean" run also means "correct results under the tool"."""
 import os
@@ -65,6 +65,14 @@ def main():
             cand = np.arange(n, dtype=np.int32)
             move_off = np.minimum(np.arange(n + 1, dtype=np.int32) * 4, len(order_p)).astype(np.int32)
             eng.simulate_removals(cand, move_off, order_p[:move_off[-1]], persist=True)
+            got = eng.filter_schedulable(order_p)
+            assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
+            # capacity batch (cae_check_capacity): one BOOK request of every pod is the filter pass; then BOOK + CHECK
+            # requests of 40 pods each, after which the filter pass on the same load is unchanged
+            res, assigned, li = eng.check_capacity([0], [0, len(order_p)], order_p)
+            assert np.array_equal(assigned[:len(ref[0])], ref[0]) and li == ref[1]
+            k = (len(order_p) + 39) // 40
+            eng.check_capacity([0] + [1] * (k - 1), np.minimum(np.arange(k + 1) * 40, len(order_p)), order_p, last_index=5)
             got = eng.filter_schedulable(order_p)
             assert np.array_equal(got[0], ref[0]) and got[1:] == ref[1:]
             # cluster-node churn (cae_load_node_churn: column gather, CSR rebuild, domains, full class matrix, recount)
