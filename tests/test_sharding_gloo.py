@@ -1,6 +1,6 @@
 """N>1 path on CPU: world_size-2 gloo.  The ranks shard pods (dense pass) / templates (pack) exactly
 like the engine does and assemble the result with ONE sum all-reduce each; the per-shard numbers come
-from the CPU oracle here (the GPU parity of a shard is covered by tests/test_gpu_parity.py)."""
+from the CPU oracle here (the GPU parity of every rank's shard is covered by tests/test_gpu_shards.py)."""
 import os
 import socket
 
