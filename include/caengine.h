@@ -689,6 +689,63 @@ int32_t cae_simulate_removals(cae_engine* e, int32_t n_cand, const int32_t* cand
                               int32_t persist, int32_t* result, int32_t* last_index_out, int32_t* log, int32_t log_cap,
                               int32_t* log_len);
 
+/* The removal batch of cae_simulate_removals on the resident snapshot, without a removal load: the pods to move are named
+ * as resident pods of the candidates' rows.  In a tick, scale-down runs after the scale-up load, its deltas, the filter
+ * pass's cae_force_add_pods and cae_scale_down_eligibility, on the snapshot those leave.
+ *   cand_node [n_cand]           cluster row of each candidate, -1 = a name the caller could not find (duplicates allowed)
+ *   move_off [n_cand + 1], move_slot []  per candidate, the position of each pod to move in its row's resident list, in the
+ *                                order the pods are tried (GetPodsToMove order).  Slots index each row's resident pods in
+ *                                the engine's current order, as cae_eligibility_inputs.pod_flags does (the load's order, a
+ *                                node delta's new list, force-added pods appended); a resident pod is its (row, slot) pair.
+ *                                A pair is listed at most once per candidate; listed again under a duplicate candidate it
+ *                                is the same pod.  Pods an earlier persisted simulation moved onto a row are appended
+ *                                automatically, as in cae_simulate_removals.
+ *   dest_ok [N]                  destinationMap, NULL = every node
+ *   hint_node [M], sim_class [M] per listed pod (M = move_off[n_cand]): hinted row (-1 none) and SimilarPodsScheduling
+ *                                class (-1 none), NULL = none; the listings of one pod must agree.  class_ctrl, n_classes,
+ *                                last_index_in (may be raw) and persist as for cae_simulate_removals.
+ * Answers: result, last_index_out and the log equal those of cae_simulate_removals on a cae_load of the same objects whose
+ * pending pods are the to-move copies (nodeName cleared), except that a log entry is (candidate, k, row or -1) with k the
+ * position in move_slot where that pod was FIRST listed (a moved-in pod that moves again keeps its first k).  The log
+ * capacity rule is cae_simulate_removals' (*log_len set to the size needed, status 1, nothing else defined; the state below
+ * is already in place, so a second call with the capacity answers the same).
+ * The nodeName-cleared twin: a pod whose spec names a node (ps_node_name >= 0) moves with the spec equal in every other
+ * column and ps_node_name = -1: the lowest such spec id, else a new spec appended with ids [S, S + n) in first-listing order.
+ * State afterwards: the state cae_load_pods leaves for the delta whose only tails are those twin specs, whose pending list is
+ * the distinct listed pods in first-listing order (pending index = rank among them, each with its own or its twin's spec)
+ * and which has one group per maximal run of consecutive pending pods with the same spec.  Every entry point then answers
+ * as a fresh cae_load of those objects would, and the rules the node calls judge "against the last cae_load or
+ * cae_load_pods" count this call as such a call.  The scale-up pending list is gone: the next tick starts with
+ * cae_load_pods.  Nodes are unchanged: persisted removals live in the batch state only (cae_load_node_churn makes them
+ * resident).  At world_size > 1 every rank may make the call, also under CAE_CFG_PODS_PRESHARDED, where the movers become
+ * this rank's pending pods; each rank answers for every candidate.  The call's H2D and D2H bytes go to cae_stats: the spec
+ * ids of the distinct pods travel to the host (4 B each), the resident lists do not.
+ * n_cand == 0 is a valid call: it empties the pending list.  Every check runs before anything observable changes.
+ * Status -2 (nothing changed): before a load, a NULL array that is needed, a row outside [-1, N), move_off[0] != 0 or
+ *   move_off decreasing, a slot at or past its row's resident pod count or any slot under row -1, a pair listed twice for
+ *   one candidate, hints or classes that differ between listings of one pod, a hinted row out of range, classes
+ *   cae_simulate_removals would refuse.
+ * Status 1 (nothing changed, *log_len = 0): a pending-side limit under which cae_load / cae_load_pods answer 1, judged on the
+ *   movers (more than 64 host-port sets, ...): use the stock path.
+ * Status 2 (nothing changed): a table would pass 2^31 - 1 entries.
+ * Status -1 (a CUDA error part way): the engine needs a cae_load. */
+typedef struct cae_resident_removals {
+  int32_t abi_version; /* CAE_ABI_VERSION */
+  int32_t n_cand;
+  const int32_t* cand_node;  /* [n_cand] */
+  const int32_t* move_off;   /* [n_cand + 1] */
+  const int32_t* move_slot;  /* [M] */
+  const uint8_t* dest_ok;    /* [N] or NULL */
+  const int32_t* hint_node;  /* [M] or NULL */
+  const int32_t* sim_class;  /* [M] or NULL */
+  const int32_t* class_ctrl; /* [n_classes] */
+  int32_t n_classes;
+  int32_t last_index_in;
+  int32_t persist;
+} cae_resident_removals;
+int32_t cae_simulate_resident_removals(cae_engine* e, const cae_resident_removals* in, int32_t* result, int32_t* last_index_out,
+                                       int32_t* log, int32_t log_cap, int32_t* log_len);
+
 /* The ProvisioningRequest capacity check: the check-capacity.autoscaling.x-k8s.io class's bookCapacity and its loop over
  * requests (cluster-autoscaler/provisioningrequest/checkcapacity/provisioningclass.go, orchestrator/orchestrator.go), in
  * one launch.  Every output equals what this loop returns on ONE HintingSimulator (hints and lastIndex carried from call to

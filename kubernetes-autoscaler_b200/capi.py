@@ -116,8 +116,13 @@ class cae_eligibility_inputs(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_eligibility_inputs")
 
 
+class cae_resident_removals(C.Structure):
+    _fields_ = _parse_struct(_SRC, "cae_resident_removals")
+
+
 _STRUCTS = {s.__name__: s for s in (cae_objects, cae_config, cae_stats, cae_price_inputs, cae_node_delta, cae_node_churn,
-                                     cae_template_delta, cae_pod_delta, cae_similarity_inputs, cae_eligibility_inputs)}
+                                     cae_template_delta, cae_pod_delta, cae_similarity_inputs, cae_eligibility_inputs,
+                                     cae_resident_removals)}
 
 
 def _ctype(decl: str, opaque, where: str):

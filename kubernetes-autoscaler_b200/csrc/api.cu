@@ -1435,25 +1435,11 @@ static int do_load_templates(Engine* e, const cae_template_delta* c) {
   return rc;
 }
 
-static int do_load_pods(Engine* e, const cae_pod_delta* d) {
-  LoadTimer lt("cae_load_pods");
-  auto bad = [](const char* m) { set_error(std::string("cae_load_pods: ") + m); return -2; };
-  if (d->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
-  const int P = d->num_pending, E = d->num_groups;
-  Tails v = pod_tails(d);
-  if (P < 0 || E < 0) return bad("negative count");
-  { const int rc = tails_present(v, bad); if (rc) return rc; }
-  if (!d->group_off || (P && !d->pend_spec)) return bad("NULL array with a non-zero count");
-  { const int rc = tails_offsets(v, bad); if (rc) return rc; }
-  if (!offsets_ok(d->group_off, E) || d->group_off[E] != P) return bad("group_off not covering pend_spec");
-  if (!tails_fit(e, v)) { set_error("cae_load_pods: a table would pass 2^31 - 1 entries"); return 2; }
-  { const int rc = tails_ids(e, v, bad); if (rc) return rc; }
-  const int S0 = e->num_podspecs, nsp = (int)v.n[CNT_SPECS], S = S0 + nsp;
-  for (int p = 0; p < P; ++p) if (d->pend_spec[p] < 0 || d->pend_spec[p] >= S) return bad("pending pod-spec id out of range");
-  for (int i = 0; i < nsp; ++i)   // a new resource dimension changes num_res: a full load
-    for (int r = e->dobj.num_res; r < R; ++r)
-      if (d->ps_req[(size_t)i * R + r] != 0) { set_error("cae_load_pods: a request in a dim past the load's num_res"); return 2; }
-  e->stats.h2d_bytes = 0;
+// The part of cae_load_pods after its checks, shared with cae_simulate_resident_removals: tails `v` (checked) and the new
+// pending list into the engine.  A limit the derivation meets (status 1 or 2) or a -2 takes the host mirrors back, so the
+// engine is as before the call; a CUDA error part way leaves an engine that needs a cae_load.
+static int commit_pod_delta(Engine* e, const Tails& v, int P, const int32_t* pend_spec, int E, const int32_t* group_off, LoadTimer& lt) {
+  const int S0 = e->num_podspecs, S = S0 + (int)v.n[CNT_SPECS];
   // ---- the node side the derivation reads on the host: the specs of the resident pods, each row's label set ----
   std::vector<uint8_t> resident(S, 0);
   std::vector<int32_t> row_ls((size_t)e->N + e->T);
@@ -1476,7 +1462,7 @@ static int do_load_pods(Engine* e, const cae_pod_delta* d) {
   o.num_values = tot(CNT_VALUES); o.num_labelsets = tot(CNT_LABELSETS); o.num_port_lists = tot(CNT_PORT_LISTS);
   o.num_pts_lists = tot(CNT_PTS_LISTS); o.num_aff_lists = tot(CNT_AFF_LISTS); o.num_aterms = tot(CNT_ATERMS); o.num_podspecs = S;
   o.num_cluster_nodes = e->N; o.num_templates = e->T; o.node_labelset = row_ls.data();
-  o.num_groups = E; o.num_pending = P; o.group_off = d->group_off; o.pend_spec = d->pend_spec;
+  o.num_groups = E; o.num_pending = P; o.group_off = group_off; o.pend_spec = pend_spec;
 
   // ---- commit: the H2D copy of the blob, then the device tables grow ----
   auto commit = [&]() -> int {
@@ -1489,6 +1475,28 @@ static int do_load_pods(Engine* e, const cae_pod_delta* d) {
   if (rc > 0 || rc == -2) take_back_mirrors(e);
   else if (rc) e->loaded = false;   // a CUDA error part way: the engine needs a cae_load
   return rc;
+}
+
+static int do_load_pods(Engine* e, const cae_pod_delta* d) {
+  LoadTimer lt("cae_load_pods");
+  auto bad = [](const char* m) { set_error(std::string("cae_load_pods: ") + m); return -2; };
+  if (d->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
+  const int P = d->num_pending, E = d->num_groups;
+  Tails v = pod_tails(d);
+  if (P < 0 || E < 0) return bad("negative count");
+  { const int rc = tails_present(v, bad); if (rc) return rc; }
+  if (!d->group_off || (P && !d->pend_spec)) return bad("NULL array with a non-zero count");
+  { const int rc = tails_offsets(v, bad); if (rc) return rc; }
+  if (!offsets_ok(d->group_off, E) || d->group_off[E] != P) return bad("group_off not covering pend_spec");
+  if (!tails_fit(e, v)) { set_error("cae_load_pods: a table would pass 2^31 - 1 entries"); return 2; }
+  { const int rc = tails_ids(e, v, bad); if (rc) return rc; }
+  const int nsp = (int)v.n[CNT_SPECS], S = e->num_podspecs + nsp;
+  for (int p = 0; p < P; ++p) if (d->pend_spec[p] < 0 || d->pend_spec[p] >= S) return bad("pending pod-spec id out of range");
+  for (int i = 0; i < nsp; ++i)   // a new resource dimension changes num_res: a full load
+    for (int r = e->dobj.num_res; r < R; ++r)
+      if (d->ps_req[(size_t)i * R + r] != 0) { set_error("cae_load_pods: a request in a dim past the load's num_res"); return 2; }
+  e->stats.h2d_bytes = 0;
+  return commit_pod_delta(e, v, P, d->pend_spec, E, d->group_off, lt);
 }
 
 // cae_force_add_pods: every check on the host first, then one pinned H2D copy of the arrivals grouped by receiving row (a
@@ -1866,6 +1874,204 @@ static int fm_finish(Engine* e, const int32_t* d_out, int32_t* out, int n_out, i
   float ms = 0;
   cudaEventElapsedTime(&ms, e->ev0, e->ev1);
   e->stats.estimate_ms = ms;
+  return 0;
+}
+
+// The removal batch after its checks (cae_simulate_removals, cae_simulate_resident_removals): move_pod [move_off[n_cand]]
+// pending pods, hint and cls [P] or NULL.  `d2h` (or NULL) takes the bytes copied back.
+static int run_removals(Engine* e, const char* who, int n_cand, const int32_t* cand_node, const int32_t* move_off,
+                        const int32_t* move_pod, const uint8_t* dest_ok, const int32_t* hint_node, const int32_t* sim_class,
+                        const int32_t* class_ctrl, int n_classes, int nctrl, int32_t last_index_in, int32_t persist, int32_t* result,
+                        int32_t* last_index_out, int32_t* log, int32_t log_cap, int32_t* log_len, int64_t* d2h) {
+  const int P = e->P, N = e->N, M = move_off[n_cand];
+  // one staged blob: cand | move_off | move_pod | hint | class | class_ctrl | dest_ok, then the outputs result | out[2] | log
+  // (device only); an absent hint, class or dest_ok array stays NULL
+  Engine::Staging& st = e->fm;
+  cae::RemovalLaunch r{};
+  r.ncand = n_cand; r.persist = persist ? 1 : 0; r.ncls = n_classes; r.nctrl = nctrl; r.log_cap = log_cap;
+  r.last_index = last_index_in;
+  size_t in_end = 0;
+  auto walk = [&](cae::Layout& l) {
+    l.add(r.cand, n_cand); l.add(r.move_off, n_cand + 1); l.add(r.move_pod, std::max(M, 1));
+    if (hint_node) l.add(r.hint, P);
+    if (sim_class) l.add(r.cls, P);
+    l.add(r.class_ctrl, std::max(n_classes, 1));
+    if (dest_ok) l.add(r.dest_ok, N);
+    in_end = l.bytes;
+    l.add(r.result, n_cand); l.add(r.out, 2); l.add(r.log, (size_t)std::max(log_cap, 1) * 3);
+  };
+  const size_t bytes = cae::layout_bytes(walk);
+  if (cae::stage_reserve(e, st, bytes, in_end)) return -1;
+  cae::layout_bind(st.dev.p, walk);
+  std::copy(cand_node, cand_node + n_cand, st.host_of(r.cand));
+  std::copy(move_off, move_off + n_cand + 1, st.host_of(r.move_off));
+  if (M) std::copy(move_pod, move_pod + M, st.host_of(r.move_pod));
+  if (hint_node) std::copy(hint_node, hint_node + P, st.host_of(r.hint));
+  if (sim_class) std::copy(sim_class, sim_class + P, st.host_of(r.cls));
+  if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, st.host_of(r.class_ctrl));
+  if (dest_ok) std::copy(dest_ok, dest_ok + N, st.host_of(r.dest_ok));
+  if (cae::stage_upload(e, st, in_end)) return -1;
+  cudaEventRecord(e->ev0, e->stream);
+  if (cae::launch_removals(e, r)) return -1;
+  cudaEventRecord(e->ev1, e->stream);
+  int32_t out[2] = {0, 0}, status = 0;
+  if (fm_finish(e, r.out, out, 2, &status)) return -1;
+  if (status) { cae::set_error("placement log overflow in the removal batch"); return -1; }
+  *log_len = out[1];
+  if (d2h) *d2h += 4 * 3;   // out[2] and the status word
+  if (out[1] > log_cap) { cae::set_error(std::string(who) + ": the log needs more entries than log_cap"); return 1; }
+  CAE_CUDA(cudaMemcpyAsync(result, r.result, sizeof(int32_t) * n_cand, cudaMemcpyDeviceToHost, e->stream));
+  if (out[1]) CAE_CUDA(cudaMemcpyAsync(log, r.log, sizeof(int32_t) * 3 * (size_t)out[1], cudaMemcpyDeviceToHost, e->stream));
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
+  if (d2h) *d2h += 4 * ((int64_t)n_cand + 3 * (int64_t)out[1]);
+  *last_index_out = out[0];
+  return 0;
+}
+
+// cae_simulate_resident_removals.  Every -2 check on the host first; then the spec ids of the distinct pods to move come up
+// in one D2H copy (launch_resident_specs), their nodeName-cleared twins are found in (or appended to) the spec table, the
+// movers become the pending list through cae_load_pods' commit (status 1 or 2: the engine is as before), and the removal
+// batch runs on them.  The log's pending indices are turned back into first-listing positions here.
+static int resident_removals(Engine* e, const cae_resident_removals* in, int32_t* result, int32_t* last_index_out, int32_t* log,
+                             int32_t log_cap, int32_t* log_len) {
+  auto bad = [](const char* m) { cae::set_error(std::string("cae_simulate_resident_removals: ") + m); return -2; };
+  if (in->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
+  const int n_cand = in->n_cand, N = e->N;
+  int n_classes = in->sim_class ? in->n_classes : 0;
+  if (n_cand < 0 || (n_cand > 0 && (!in->cand_node || !in->move_off || !result)) || !last_index_out || !log_len || log_cap < 0 ||
+      (log_cap > 0 && !log) || n_classes < 0 || (n_classes > 0 && !in->class_ctrl))
+    return bad("bad arguments");
+  if (n_cand > 0 && in->move_off[0] != 0) return bad("move_off[0] must be 0");
+  for (int c = 0; c < n_cand; ++c) {
+    if (in->cand_node[c] < -1 || in->cand_node[c] >= N) return bad("candidate row out of range");
+    if (in->move_off[c + 1] < in->move_off[c]) return bad("move_off decreases");
+  }
+  const int M = n_cand > 0 ? in->move_off[n_cand] : 0;
+  if (M > 0 && !in->move_slot) return bad("bad arguments");
+  // the distinct (row, slot) pairs in first-listing order: pending index of every listing, first listing of every pod
+  std::vector<int32_t> pend(M), first, prow, pslot, seen;
+  std::unordered_map<int64_t, int32_t> index_of;
+  for (int c = 0; c < n_cand; ++c) {
+    const int row = in->cand_node[c];
+    for (int k = in->move_off[c]; k < in->move_off[c + 1]; ++k) {
+      const int slot = in->move_slot[k];
+      if (row < 0 || slot < 0 || slot >= e->nh.pod_cnt[row]) return bad("a slot outside its row's resident pods");
+      auto it = index_of.emplace(((int64_t)row << 32) | (uint32_t)slot, (int32_t)first.size()).first;
+      const int p = it->second;
+      if (p == (int)first.size()) {
+        first.push_back(k); prow.push_back(row); pslot.push_back(slot); seen.push_back(-1);
+      } else {
+        if ((in->hint_node && in->hint_node[k] != in->hint_node[first[p]]) || (in->sim_class && in->sim_class[k] != in->sim_class[first[p]]))
+          return bad("a pod listed again with another hint or class");
+      }
+      if (seen[p] == c) return bad("a pod is listed twice for one candidate");
+      seen[p] = c;
+      pend[k] = p;
+    }
+  }
+  const int P = (int)first.size();
+  if (in->hint_node)
+    for (int k = 0; k < M; ++k)
+      if (in->hint_node[k] < -1 || in->hint_node[k] >= N) return bad("hinted row out of range");
+  const int nctrl = sim_class_check("cae_simulate_resident_removals", in->sim_class, in->class_ctrl, n_classes, M, -1);
+  if (nctrl < 0) return -2;
+  e->stats.h2d_bytes = 0;
+  e->stats.d2h_bytes = 0;
+  cudaSetDevice(e->cfg.device);
+  cae::LoadTimer lt("cae_simulate_resident_removals");
+
+  // ---- the spec of every pod to move, gathered from the resident CSR on the device ----
+  std::vector<int32_t> spec(P);
+  if (P) {
+    Engine::Staging& st = e->fm;
+    int32_t *d_row = nullptr, *d_slot = nullptr, *d_spec = nullptr;
+    size_t in_end = 0;
+    auto walk = [&](cae::Layout& l) { l.add(d_row, P); l.add(d_slot, P); in_end = l.bytes; l.add(d_spec, P); };
+    const size_t bytes = cae::layout_bytes(walk);
+    if (cae::stage_reserve(e, st, bytes, bytes)) return -1;
+    cae::layout_bind(st.dev.p, walk);
+    std::copy(prow.begin(), prow.end(), st.host_of(d_row));
+    std::copy(pslot.begin(), pslot.end(), st.host_of(d_slot));
+    if (cae::stage_upload(e, st, in_end)) return -1;
+    if (cae::launch_resident_specs(e, P, d_row, d_slot, d_spec)) return -1;
+    CAE_CUDA(cudaMemcpyAsync(st.host_of(d_spec), d_spec, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, e->stream));
+    CAE_CUDA(cudaStreamSynchronize(e->stream));
+    std::copy(st.host_of(d_spec), st.host_of(d_spec) + P, spec.begin());
+    e->stats.d2h_bytes += (int64_t)sizeof(int32_t) * P;
+  }
+
+  // ---- the nodeName-cleared twin of every spec that names a node: the lowest spec id equal in every other column, else a
+  // new spec appended in first-need order ----
+  const int S = e->num_podspecs;
+  auto col = [&](int t) { return e->host_tab<int32_t>(t); };
+  const int32_t* node_name = col(cae::TAB_ps_node_name);
+  const int64_t* req = e->host_tab<int64_t>(cae::TAB_ps_req);
+  const uint8_t* term = e->host_tab<uint8_t>(cae::TAB_ps_terminating);
+  const uint8_t* hs = e->host_tab<uint8_t>(cae::TAB_ps_hostname_spread);
+  static const int kCols[] = {cae::TAB_ps_namespace, cae::TAB_ps_labelset, cae::TAB_ps_tol_list, cae::TAB_ps_naff,
+                              cae::TAB_ps_port_list, cae::TAB_ps_pts_list, cae::TAB_ps_aff_list, cae::TAB_ps_anti_list};
+  auto key_of = [&](int s) {
+    std::string k;
+    for (int t : kCols) k.append(reinterpret_cast<const char*>(col(t) + s), 4);
+    k.append(reinterpret_cast<const char*>(req + (size_t)s * cae::R), 8 * cae::R);
+    k.push_back((char)term[s]);
+    k.push_back((char)hs[s]);
+    return k;
+  };
+  std::unordered_map<std::string, int32_t> twin_of;   // built only when a mover names a node
+  std::vector<int32_t> tw_ns, tw_ls, tw_tol, tw_naff, tw_port, tw_pts, tw_aff, tw_anti, tw_nn;
+  std::vector<int64_t> tw_req;
+  std::vector<uint8_t> tw_term, tw_hs;
+  std::vector<int32_t> pend_spec(P);
+  for (int p = 0; p < P; ++p) {
+    const int s = spec[p];
+    if (node_name[s] < 0) { pend_spec[p] = s; continue; }
+    if (twin_of.empty())
+      for (int x = S - 1; x >= 0; --x)
+        if (node_name[x] < 0) twin_of[key_of(x)] = x;
+    auto it = twin_of.emplace(key_of(s), S + (int32_t)tw_nn.size());
+    if (it.second) {
+      tw_ns.push_back(col(cae::TAB_ps_namespace)[s]); tw_ls.push_back(col(cae::TAB_ps_labelset)[s]);
+      tw_tol.push_back(col(cae::TAB_ps_tol_list)[s]); tw_naff.push_back(col(cae::TAB_ps_naff)[s]);
+      tw_port.push_back(col(cae::TAB_ps_port_list)[s]); tw_pts.push_back(col(cae::TAB_ps_pts_list)[s]);
+      tw_aff.push_back(col(cae::TAB_ps_aff_list)[s]); tw_anti.push_back(col(cae::TAB_ps_anti_list)[s]);
+      tw_nn.push_back(-1);
+      tw_req.insert(tw_req.end(), req + (size_t)s * cae::R, req + (size_t)(s + 1) * cae::R);
+      tw_term.push_back(term[s]); tw_hs.push_back(hs[s]);
+    }
+    pend_spec[p] = it.first->second;
+  }
+  // one group per maximal run of consecutive movers with the same spec
+  std::vector<int32_t> group_off(1, 0);
+  for (int p = 1; p <= P; ++p)
+    if (p == P || pend_spec[p] != pend_spec[p - 1]) group_off.push_back(p);
+  cae_pod_delta d{};
+  d.abi_version = CAE_ABI_VERSION;
+  d.num_new_specs = (int32_t)tw_nn.size();
+  d.ps_namespace = tw_ns.data(); d.ps_labelset = tw_ls.data(); d.ps_req = tw_req.data(); d.ps_tol_list = tw_tol.data();
+  d.ps_naff = tw_naff.data(); d.ps_node_name = tw_nn.data(); d.ps_port_list = tw_port.data(); d.ps_pts_list = tw_pts.data();
+  d.ps_aff_list = tw_aff.data(); d.ps_anti_list = tw_anti.data(); d.ps_terminating = tw_term.data(); d.ps_hostname_spread = tw_hs.data();
+  const cae::Tails v = cae::pod_tails(&d);
+  if (!cae::tails_fit(e, v)) { cae::set_error("cae_simulate_resident_removals: a table would pass 2^31 - 1 entries"); return 2; }
+  {   // the movers become the pending list, as cae_load_pods would leave it
+    const int rc = cae::commit_pod_delta(e, v, P, pend_spec.data(), (int)group_off.size() - 1, group_off.data(), lt);
+    if (rc) {
+      if (rc > 0) *log_len = 0;
+      return rc;
+    }
+  }
+  if (n_cand == 0) { *last_index_out = in->last_index_in; *log_len = 0; return 0; }
+
+  // ---- the batch on the movers: hint and class per pending pod ----
+  std::vector<int32_t> hint, cls;
+  if (in->hint_node) { hint.resize(P); for (int p = 0; p < P; ++p) hint[p] = in->hint_node[first[p]]; }
+  if (in->sim_class) { cls.resize(P); for (int p = 0; p < P; ++p) cls[p] = in->sim_class[first[p]]; }
+  const int rc = run_removals(e, "cae_simulate_resident_removals", n_cand, in->cand_node, in->move_off, pend.data(), in->dest_ok,
+                              in->hint_node ? hint.data() : nullptr, in->sim_class ? cls.data() : nullptr, in->class_ctrl,
+                              n_classes, nctrl, in->last_index_in, in->persist, result, last_index_out, log, log_cap, log_len,
+                              &e->stats.d2h_bytes);
+  if (rc) return rc;
+  for (int i = 0; i < *log_len; ++i) log[3 * i + 1] = first[log[3 * i + 1]];
   return 0;
 }
 
@@ -2380,46 +2586,16 @@ int32_t cae_simulate_removals(cae_engine* h, int32_t n_cand, const int32_t* cand
   e->stats.h2d_bytes = 0;
   if (n_cand == 0) { *last_index_out = last_index_in; *log_len = 0; return 0; }
   cudaSetDevice(e->cfg.device);
-  // one staged blob: cand | move_off | move_pod | hint | class | class_ctrl | dest_ok, then the outputs result | out[2] | log
-  // (device only); an absent hint, class or dest_ok array stays NULL
-  Engine::Staging& st = e->fm;
-  cae::RemovalLaunch r{};
-  r.ncand = n_cand; r.persist = persist ? 1 : 0; r.ncls = n_classes; r.nctrl = nctrl; r.log_cap = log_cap;
-  r.last_index = last_index_in;
-  size_t in_end = 0;
-  auto walk = [&](cae::Layout& l) {
-    l.add(r.cand, n_cand); l.add(r.move_off, n_cand + 1); l.add(r.move_pod, std::max(M, 1));
-    if (hint_node) l.add(r.hint, P);
-    if (sim_class) l.add(r.cls, P);
-    l.add(r.class_ctrl, std::max(n_classes, 1));
-    if (dest_ok) l.add(r.dest_ok, N);
-    in_end = l.bytes;
-    l.add(r.result, n_cand); l.add(r.out, 2); l.add(r.log, (size_t)std::max(log_cap, 1) * 3);
-  };
-  const size_t bytes = cae::layout_bytes(walk);
-  if (cae::stage_reserve(e, st, bytes, in_end)) return -1;
-  cae::layout_bind(st.dev.p, walk);
-  std::copy(cand_node, cand_node + n_cand, st.host_of(r.cand));
-  std::copy(move_off, move_off + n_cand + 1, st.host_of(r.move_off));
-  if (M) std::copy(move_pod, move_pod + M, st.host_of(r.move_pod));
-  if (hint_node) std::copy(hint_node, hint_node + P, st.host_of(r.hint));
-  if (sim_class) std::copy(sim_class, sim_class + P, st.host_of(r.cls));
-  if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, st.host_of(r.class_ctrl));
-  if (dest_ok) std::copy(dest_ok, dest_ok + N, st.host_of(r.dest_ok));
-  if (cae::stage_upload(e, st, in_end)) return -1;
-  cudaEventRecord(e->ev0, e->stream);
-  if (cae::launch_removals(e, r)) return -1;
-  cudaEventRecord(e->ev1, e->stream);
-  int32_t out[2] = {0, 0}, status = 0;
-  if (fm_finish(e, r.out, out, 2, &status)) return -1;
-  if (status) { cae::set_error("placement log overflow in the removal batch"); return -1; }
-  *log_len = out[1];
-  if (out[1] > log_cap) { cae::set_error("cae_simulate_removals: the log needs more entries than log_cap"); return 1; }
-  CAE_CUDA(cudaMemcpyAsync(result, r.result, sizeof(int32_t) * n_cand, cudaMemcpyDeviceToHost, e->stream));
-  if (out[1]) CAE_CUDA(cudaMemcpyAsync(log, r.log, sizeof(int32_t) * 3 * (size_t)out[1], cudaMemcpyDeviceToHost, e->stream));
-  CAE_CUDA(cudaStreamSynchronize(e->stream));
-  *last_index_out = out[0];
-  return 0;
+  return run_removals(e, "cae_simulate_removals", n_cand, cand_node, move_off, move_pod, dest_ok, hint_node, sim_class, class_ctrl,
+                      n_classes, nctrl, last_index_in, persist, result, last_index_out, log, log_cap, log_len, nullptr);
+}
+
+int32_t cae_simulate_resident_removals(cae_engine* h, const cae_resident_removals* in, int32_t* result, int32_t* last_index_out,
+                                       int32_t* log, int32_t log_cap, int32_t* log_len) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_simulate_resident_removals before cae_load"); return -2; }
+  if (!in) { cae::set_error("cae_simulate_resident_removals: no inputs"); return -2; }
+  return resident_removals(e, in, result, last_index_out, log, log_cap, log_len);
 }
 
 int32_t cae_check_capacity(cae_engine* h, int32_t n_req, const int32_t* req_kind, const int32_t* req_off, const int32_t* req_pod,

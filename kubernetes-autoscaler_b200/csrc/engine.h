@@ -34,7 +34,8 @@ enum DictCount : int {
 // appends them from this list).  X(field, element type, elements per entry, count, child count, carried by, host mirror):
 // an offsets table has count + 1 entries and indexes the tables of its child count (NONE: not an offsets table); "carried
 // by" names the delta structs with the field (NODE: cae_node_delta, POD: cae_pod_delta, BOTH); a host mirror is kept for
-// the pending-side derivation, which cae_load_pods reruns without the caller's cae_objects.
+// the pending-side derivation, which cae_load_pods reruns without the caller's cae_objects, and of every pod-spec column
+// for the nodeName-cleared twins of cae_simulate_resident_removals.
 #define CAE_DICT_TABLES(X)                                         \
   X(value_is_int, uint8_t, 1, VALUES, NONE, BOTH, 0)               \
   X(value_int, int64_t, 1, VALUES, NONE, BOTH, 0)                  \
@@ -92,8 +93,8 @@ enum DictCount : int {
   X(ps_pts_list, int32_t, 1, SPECS, NONE, POD, 1)                  \
   X(ps_aff_list, int32_t, 1, SPECS, NONE, POD, 1)                  \
   X(ps_anti_list, int32_t, 1, SPECS, NONE, POD, 1)                 \
-  X(ps_terminating, uint8_t, 1, SPECS, NONE, POD, 0)               \
-  X(ps_hostname_spread, uint8_t, 1, SPECS, NONE, POD, 0)
+  X(ps_terminating, uint8_t, 1, SPECS, NONE, POD, 1)               \
+  X(ps_hostname_spread, uint8_t, 1, SPECS, NONE, POD, 1)
 #define CAE_DICT_ID(field, type, per, cnt, child, by, host) TAB_##field,
 enum DictTable : int { CAE_DICT_TABLES(CAE_DICT_ID) NUM_DICT_TABLES };
 #undef CAE_DICT_ID
@@ -528,5 +529,8 @@ struct EligLaunch {
   int32_t *list, *count, *status;
 };
 int launch_eligibility(Engine* e, const EligLaunch& a);
+// scaledown.cu: cae_simulate_resident_removals.  spec[i] = the spec id of resident pod slot[i] of cluster row row[i], read
+// from the device-resident CSR (node_pod_off / node_pod_spec); n pairs, every one checked by api.cu.
+int launch_resident_specs(Engine* e, int n, const int32_t* row, const int32_t* slot, int32_t* spec);
 
 }  // namespace cae

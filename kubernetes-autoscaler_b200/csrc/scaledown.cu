@@ -8,6 +8,9 @@
 //     depend on the order.  Lane 0 then does the milli conversion, the IEEE divisions, Go's math.Max and the threshold test;
 //   * elig_compact_kernel, one block: the candidates with reason CAE_ELIG_UNNEEDED in input order (a block-wide scan per
 //     chunk of candidates).
+// cae_simulate_resident_removals:
+//   * resident_spec_kernel, one thread per distinct (row, slot) pair of the pods to move: the pod's spec id from the
+//     resident CSR, so that only these ids travel to the host, never the CSR.
 #include <climits>
 #include <cub/block/block_scan.cuh>
 
@@ -152,6 +155,20 @@ int launch_eligibility(Engine* e, const EligLaunch& a) {
   elig_kernel<<<(a.n + EL_WARPS - 1) / EL_WARPS, EL_WARPS * 32, 0, e->stream>>>(e->dobj, a);
   elig_compact_kernel<<<1, EL_COMPACT, 0, e->stream>>>(a);
   e->stats.kernel_launches += 2;
+  CAE_KERNEL_OK();
+  return 0;
+}
+
+__global__ void resident_spec_kernel(DevObjects o, int n, const int32_t* __restrict__ row, const int32_t* __restrict__ slot,
+                                     int32_t* __restrict__ spec) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) spec[i] = o.node_pod_spec[o.node_pod_off[row[i]] + slot[i]];
+}
+
+int launch_resident_specs(Engine* e, int n, const int32_t* row, const int32_t* slot, int32_t* spec) {
+  if (n <= 0) return 0;
+  resident_spec_kernel<<<(n + 255) / 256, 256, 0, e->stream>>>(e->dobj, n, row, slot, spec);
+  e->stats.kernel_launches += 1;
   CAE_KERNEL_OK();
   return 0;
 }

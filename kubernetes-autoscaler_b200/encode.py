@@ -632,6 +632,74 @@ class EncodedObjects:
         out.struct = self._restruct(a, num_pending=int(keep.sum()))
         return out, new_index
 
+    def apply_resident_removals(self, cand_node, move_off, move_slot) -> Tuple["EncodedObjects", np.ndarray, np.ndarray]:
+        """The objects after cae_simulate_resident_removals(cand_node, move_off, move_slot), stated on the host, and where
+        each pod sits: listing k names resident slot move_slot[k] of cluster row cand_node[c]; the distinct (row, slot)
+        pairs in first-listing order become the pending list, each with its spec or, when that spec names a node, its
+        nodeName-cleared twin (the lowest spec id equal in every other column, else a spec appended in first-need order);
+        one group per run of consecutive pending pods with the same spec.  Returns (objects, pend [M] = pending index of
+        every listing, first [P] = the listing where each pending pod first appears).  A cae_load of the objects must
+        answer like the engine after the call.  ValueError: what the engine answers with status -2 for the slot lists."""
+        import copy
+        cand = np.asarray(cand_node, np.int64).reshape(-1)
+        off = np.asarray(move_off, np.int64).reshape(-1)
+        slot = np.asarray(move_slot, np.int64).reshape(-1)
+        N, a = self.struct.num_cluster_nodes, dict(self.arrays)
+        if len(cand) and (len(off) != len(cand) + 1 or off[0] != 0 or (np.diff(off) < 0).any() or off[-1] != len(slot)):
+            raise ValueError("resident removals: move_off must start at 0, not decrease and cover move_slot")
+        if len(cand) and (cand.min() < -1 or cand.max() >= N):
+            raise ValueError("resident removals: a candidate row outside [-1, N)")
+        pod_off, pod_spec = a["node_pod_off"], a["node_pod_spec"]
+        index_of: Dict[Tuple[int, int], int] = {}
+        pend = np.zeros(len(slot), np.int32)
+        first, spec = [], []
+        for c in range(len(cand)):
+            row, listed = int(cand[c]), set()
+            for k in range(int(off[c]), int(off[c + 1])):
+                s = int(slot[k])
+                if row < 0 or s < 0 or s >= pod_off[row + 1] - pod_off[row]:
+                    raise ValueError("resident removals: slot %d outside the resident pods of row %d" % (s, row))
+                if (row, s) in listed:
+                    raise ValueError("resident removals: slot %d of row %d listed twice for candidate %d" % (s, row, c))
+                listed.add((row, s))
+                p = index_of.setdefault((row, s), len(first))
+                if p == len(first):
+                    first.append(k)
+                    spec.append(int(pod_spec[pod_off[row] + s]))
+                pend[k] = p
+        cols = [nm for nm in self.arrays if nm.startswith("ps_")]
+        S = self.struct.num_podspecs
+        twins: Dict[tuple, int] = {}
+        new_rows: List[int] = []
+
+        def key(s: int) -> tuple:
+            return tuple(a[nm][s].tobytes() for nm in cols if nm != "ps_node_name")
+
+        for i, s in enumerate(spec):
+            if a["ps_node_name"][s] < 0:
+                continue
+            if not twins:
+                for x in range(S - 1, -1, -1):
+                    if a["ps_node_name"][x] < 0:
+                        twins[key(x)] = x
+            t = twins.setdefault(key(s), S + len(new_rows))
+            if t == S + len(new_rows):
+                new_rows.append(s)
+            spec[i] = t
+        for nm in cols:
+            tail = a[nm][:S][new_rows].copy()
+            if nm == "ps_node_name":
+                tail[:] = -1
+            a[nm] = np.ascontiguousarray(np.concatenate([a[nm][:S], tail]))
+        ps = np.asarray(spec, np.int32)
+        starts = [p for p in range(len(ps)) if p == 0 or ps[p] != ps[p - 1]]
+        a["pend_spec"] = np.ascontiguousarray(ps)
+        a["group_off"] = _i32(starts + [len(ps)])
+        out = copy.copy(self)
+        out.arrays = a
+        out.struct = self._restruct(a, num_podspecs=S + len(new_rows), num_pending=len(ps), num_groups=len(starts))
+        return out, pend, np.asarray(first, np.int32)
+
     def _with_tails(self, d: Dict[str, np.ndarray], tables) -> Dict[str, np.ndarray]:
         """A copy of the arrays with the tails `d` of the dictionary tables `tables` appended (tail offsets made absolute)."""
         a, n = dict(self.arrays), _dict_counts(self.struct, self.arrays)
@@ -807,6 +875,18 @@ class EligibilityInputs(AbiArrays):
         super().__init__(**fields)
         if "n_pod_flags" not in fields:
             self.struct.n_pod_flags = len(self.arrays["pod_flags"]) if "pod_flags" in self.arrays else 0
+
+
+class ResidentRemovals(AbiArrays):
+    """``cae_resident_removals`` of cae_simulate_resident_removals.  The optional arrays left out are NULL."""
+
+    STRUCT = capi.cae_resident_removals
+    COUNTS = {"n_cand": "cand_node"}
+
+    def __init__(self, **fields) -> None:
+        for nm in ("dest_ok", "hint_node", "sim_class", "class_ctrl"):
+            fields.setdefault(nm, None)
+        super().__init__(**fields)
 
 
 # ----------------------------------------------------------------------------------------------

@@ -10,7 +10,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 
 from . import capi
-from .encode import EligibilityInputs, EncodedObjects, PriceInputs, SimilarityInputs
+from .encode import EligibilityInputs, EncodedObjects, PriceInputs, ResidentRemovals, SimilarityInputs
 
 
 class EngineError(RuntimeError):
@@ -352,6 +352,43 @@ class Engine:
         rc = self.lib.cae_simulate_removals(self.h, len(cn), _vp(cn), _vp(mo), _vp(mp), _vp(ok), _vp(hn), _vp(sc), _vp(cc),
                                             0 if cc is None else len(cc), int(last_index), int(bool(persist)), _vp(res), _vp(li),
                                             _vp(log), int(log_cap), _vp(n))
+        if rc == 1:
+            return rc, None, None, np.zeros((int(n[0]), 3), np.int32)
+        return rc, res[:len(cn)], int(li[0]), log[:int(n[0])]
+
+    def simulate_resident_removals(self, cand_node, move_off, move_slot, dest_ok=None, hint_node=None, sim_class=None,
+                                   class_ctrl=None, last_index: int = 0, persist: bool = False, log_cap: Optional[int] = None,
+                                   enc: Optional[EncodedObjects] = None):
+        """The removal batch of simulate_removals on the resident snapshot (cae_simulate_resident_removals): move_slot
+        names each pod to move by its position in its candidate row's resident list; hint_node / sim_class are per listed
+        pod.  Returns (result[n_cand], lastIndex afterwards, log [n][3] = (candidate, k, cluster row or -1) with k the
+        listing where the pod was first listed).  Afterwards the engine holds the movers as its pending pods; this object's
+        shapes follow through EncodedObjects.apply_resident_removals (`enc`: that result, when the caller has it).
+        Raises EngineUnsupported on status 1 (a limit judged on the movers) or 2 (a table would overflow)."""
+        move_off = np.ascontiguousarray(move_off, np.int32)
+        cap = int(log_cap) if log_cap is not None else int(move_off[-1]) + 64 if len(move_off) else 0
+        args = (cand_node, move_off, move_slot, dest_ok, hint_node, sim_class, class_ctrl, last_index, persist)
+        rc, res, li, log = self._simulate_resident_removals_raw(*args, cap)
+        if rc == 1 and len(log) > cap:   # the log needed more room: once more at the size it reported
+            rc, res, li, log = self._simulate_resident_removals_raw(*args, len(log))
+        self._check(rc)
+        self.enc = enc if enc is not None else self.enc.apply_resident_removals(cand_node, move_off, move_slot)[0]
+        return res, li, log
+
+    def _simulate_resident_removals_raw(self, cand_node, move_off, move_slot, dest_ok, hint_node, sim_class, class_ctrl,
+                                        last_index, persist, log_cap):
+        """One cae_simulate_resident_removals call: (status, result, lastIndex, log); on status 1 the log is zeros of the
+        needed length (0 for a limit)."""
+        cn = np.ascontiguousarray(cand_node, np.int32).reshape(-1)
+        cc = _opt(class_ctrl, np.int32)
+        rr = ResidentRemovals(cand_node=cn, move_off=np.ascontiguousarray(move_off, np.int32),
+                              move_slot=np.ascontiguousarray(move_slot, np.int32), dest_ok=_opt(dest_ok, np.uint8),
+                              hint_node=_opt(hint_node, np.int32), sim_class=_opt(sim_class, np.int32), class_ctrl=cc,
+                              n_classes=0 if cc is None else len(cc), last_index_in=int(last_index), persist=int(bool(persist)))
+        res = np.zeros(max(len(cn), 1), np.int32)
+        log = np.zeros((max(log_cap, 1), 3), np.int32)
+        li, n = np.zeros(1, np.int32), np.zeros(1, np.int32)
+        rc = self.lib.cae_simulate_resident_removals(self.h, rr.ptr(), _vp(res), _vp(li), _vp(log), int(log_cap), _vp(n))
         if rc == 1:
             return rc, None, None, np.zeros((int(n[0]), 3), np.int32)
         return rc, res[:len(cn)], int(li[0]), log[:int(n[0])]

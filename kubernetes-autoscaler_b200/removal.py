@@ -102,6 +102,67 @@ class RemovalSimulator:
                                                         x.class_ctrl, self.schedulingSimulator.last_index, self.canPersist)
         return self._apply_removals(x, result, last_index, log)
 
+    def SimulateNodeRemovalsResident(self, candidates: Sequence[str], destinationMap: Dict[str, bool],
+                                     pods_to_move: Optional[Sequence[Optional[Sequence[Pod]]]] = None
+                                     ) -> List[Tuple[Optional[NodeToBeRemoved], Optional[UnremovableNode]]]:
+        """SimulateNodeRemovals on the snapshot the engine already holds (cae_simulate_resident_removals), without a
+        removal load: ``self.cluster`` must be the engine's cluster rows in row order, each NodeInfo's pods in the engine's
+        order (the load's, a node delta's new list, force-added pods appended).  pods_to_move[i], when given, lists pods
+        of candidate i's NodeInfo (found by identity).  The same results, hints, lastIndex and (with persistence) cluster
+        as SimulateNodeRemovals; afterwards the engine's pending pods are the movers (the next tick starts with
+        cae_load_pods) and its nodes are unchanged, so with persistence ``self.cluster`` no longer mirrors its rows."""
+        if isinstance(candidates, str) or not all(isinstance(c, str) for c in candidates):
+            raise TypeError("candidates must be a sequence of node names")
+        candidates = list(candidates)
+        if pods_to_move is not None and len(pods_to_move) != len(candidates):
+            raise ValueError("pods_to_move needs one entry per candidate (%d != %d)" % (len(pods_to_move), len(candidates)))
+        sim = self.schedulingSimulator
+        eng = sim.engine or shared_engine()
+        cluster = list(self.cluster)
+        row_of = {ni.node.name: i for i, ni in enumerate(cluster)}
+        cand_node, move_slot, to_move, listed = [], [], [], []
+        for i, name in enumerate(candidates):
+            row = row_of.get(name, -1)
+            cand_node.append(row)
+            explicit = pods_to_move[i] if pods_to_move is not None else None
+            pods = [] if row < 0 else cluster[row].pods
+            slot_of = {id(p): s for s, p in enumerate(pods)}
+            objs = [] if row < 0 else (list(explicit) if explicit is not None else [p for p in pods if p.owner_kind != "DaemonSet"])
+            for p in objs:
+                if id(p) not in slot_of:
+                    raise ValueError("pod %s/%s is not a pod of node %s" % (p.namespace, p.name, name))
+                move_slot.append(slot_of[id(p)])
+            to_move.append(objs)
+            listed += objs
+        move_off = np.zeros(len(candidates) + 1, np.int32)
+        move_off[1:] = np.cumsum([len(o) for o in to_move]) if to_move else []
+        cand_node = np.array(cand_node, np.int32)
+        after, pend, _ = eng.enc.apply_resident_removals(cand_node, move_off, move_slot)
+        # hints and SimilarPodsScheduling classes per listing, keyed as prepare_removals keys them
+        hint = np.full(len(listed), -1, np.int32)
+        sim_class = np.full(len(listed), -1, np.int32)
+        classes: Dict[Tuple[str, int], int] = {}
+        ctrls: Dict[str, int] = {}
+        class_ctrl: List[int] = []
+        pend_spec = after.arrays["pend_spec"]
+        for k, p in enumerate(listed):
+            h = sim.hints.Get(HintKeyFromPod(p))
+            if h is not None and h in row_of:
+                hint[k] = row_of[h]
+            if p.owner_uid and p.owner_kind != "DaemonSet":
+                key = (p.owner_uid, int(pend_spec[pend[k]]))
+                if key not in classes:
+                    classes[key] = len(class_ctrl)
+                    class_ctrl.append(ctrls.setdefault(p.owner_uid, len(ctrls)))
+                sim_class[k] = classes[key]
+        dest = np.array([1 if destinationMap.get(ni.node.name) else 0 for ni in cluster], np.uint8)
+        result, last_index, log = eng.simulate_resident_removals(
+            cand_node, move_off, move_slot, None if dest.all() else dest, hint if (hint >= 0).any() else None,
+            sim_class if class_ctrl else None, class_ctrl or None, sim.last_index, self.canPersist, enc=after)
+        x = RemovalInputs(after, cluster, candidates, listed, cand_node, move_off, np.asarray(move_slot, np.int32), to_move,
+                          None, None, None, None)
+        return self._apply_removals(x, result, last_index, log)
+
     def _apply_removals(self, x: RemovalInputs, result, last_index: int, log) -> List[Tuple[Optional[NodeToBeRemoved], Optional[UnremovableNode]]]:
         """Rebuilds what the loop of single calls returns and leaves behind from the engine's log."""
         sim = self.schedulingSimulator

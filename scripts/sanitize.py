@@ -7,7 +7,7 @@ self-cleaning accumulators, last-block election, shared-memory state and block-w
 
 Dense pass (K1, both variants), Estimate() of every template (K0 + K3: plain closed form, capacity form with the cluster
 fallback, per-pod loop), expander scores, the filter-out-schedulable pass, a scale-down batch (cae_simulate_removals), a ProvisioningRequest capacity batch (cae_check_capacity), a cluster-node delta
-(cae_load_nodes), a cluster-node churn (cae_load_node_churn), new pod specs (cae_load_pods), node-group template changes (cae_load_templates), the placements of a filter pass made resident (cae_force_add_pods), the scale-down eligibility (cae_scale_down_eligibility) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
+(cae_load_nodes), a cluster-node churn (cae_load_node_churn), new pod specs (cae_load_pods), node-group template changes (cae_load_templates), the placements of a filter pass made resident (cae_force_add_pods), the scale-down eligibility (cae_scale_down_eligibility), a scale-down batch on the resident snapshot (cae_simulate_resident_removals) and the similar node groups (cae_similar_node_groups) — on miniatures of C2, C3 and C4 — each checked
 against the CPU oracle so that a "clean" run also means "correct results under the tool"."""
 import os
 import sys
@@ -138,6 +138,18 @@ def main():
             eng.load(after)
             want = eng.scale_down_eligibility(*args)
             assert all(np.array_equal(x, y, equal_nan=True) for x, y in zip(got, want))
+            # the scale-down batch on the resident snapshot (cae_simulate_resident_removals: the slot gather, the twin specs,
+            # the movers' derivation and the batch) against a removal load of the objects it leaves
+            off = after.arrays["node_pod_off"]
+            cand = np.concatenate([np.arange(min(N, 12)), [0]]).astype(np.int32)
+            move_off = np.concatenate([[0], np.cumsum(off[cand + 1] - off[cand])]).astype(np.int32)
+            slots = np.concatenate([np.arange(off[r + 1] - off[r]) for r in cand]).astype(np.int32)
+            moved, pend, first = after.apply_resident_removals(cand, move_off, slots)
+            got = eng.simulate_resident_removals(cand, move_off, slots, persist=True, enc=moved)
+            eng.load(moved)
+            res, li, log = eng.simulate_removals(cand, move_off, pend, persist=True)
+            assert np.array_equal(got[0], res) and got[1] == li and np.array_equal(got[2][:, [0, 2]], log[:, [0, 2]])
+            assert np.array_equal(got[2][:, 1], first[log[:, 1]])
         # similar node groups (cae_similar_node_groups: operand / bit-row prep, the pair kernel's staged tiles and ballots)
         infos, groups, ngs = synth.node_group_families(cfg, 45, 4, seed=cfg, groups=40)
         sim = ScaleUpSimulation([], infos, groups, eng)

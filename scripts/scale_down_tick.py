@@ -9,7 +9,11 @@ size of C3, and 15 000 x 30), every node a candidate.  Per size, one JSON line:
   * python_ref_ms: the CPU restatement (tests/utilization_ref.py) over every candidate, once.  It is Python: the cost of the
     Go loop it stands for (utilization.Calculate per candidate) is not measured;
   * tick_ms: the composed tick on the scale-up load, Checker.FilterOutUnremovable then RemovalSimulator.SimulateNodeRemovals
-    on the first --removals unneeded nodes (prepare, removal load and cae_simulate_removals), once after a warm-up.
+    on the first --removals unneeded nodes (prepare, removal load and cae_simulate_removals), once after a warm-up;
+  * resident_tick_ms: the same tick with RemovalSimulator.SimulateNodeRemovalsResident on the same engine, without the
+    removal load (slots, cae_simulate_resident_removals), once after a warm-up; resident_call_ms: CUDA events on the
+    engine's stream around that call (the slot upload, the spec gather, the movers' derivation, the batch and its log).
+    Both ticks must give the same outcome.
 The engine's answers are checked against the restatement.  The card name and power limit are read in the same run."""
 import argparse
 import copy
@@ -133,11 +137,39 @@ def main():
             return (time.perf_counter() - t0) * 1e3, res
         tick()
         tick_ms, res = tick()
+        call_ms = []
+        call = eng.simulate_resident_removals
+
+        def timed_call(*args, **kw):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            r = call(*args, **kw)
+            e1.record(stream)
+            e1.synchronize()
+            call_ms.append(e0.elapsed_time(e1))
+            return r
+        eng.simulate_resident_removals = timed_call
+
+        def resident_tick():
+            eng.load(enc)
+            t0 = time.perf_counter()
+            un, _, _ = checker.FilterOutUnremovable(cluster, names, NOW, groups)
+            res = RemovalSimulator(cluster, engine=eng).SimulateNodeRemovalsResident(un[:a.removals], dest)
+            return (time.perf_counter() - t0) * 1e3, res
+        resident_tick()
+        resident_ms, res2 = resident_tick()
+        del eng.simulate_resident_removals
+
+        def outcome(rs):
+            return [(r.node.name, [p.name for p in r.pods_to_reschedule], [p.name for p in r.daemonset_pods]) if r is not None
+                    else (u.node.name, u.reason) for r, u in rs]
+        assert outcome(res2) == outcome(res), "the resident tick differs from the tick with a removal load"
         row = dict(nodes=N, pods_per_node=a.pods, card=name, power_limit=power, candidates=N, unneeded=len(unneeded),
                    device_ms=round(statistics.median(dev), 4), host_ms=round(statistics.median(host), 4),
                    checker_ms=round(statistics.median(chk), 2), python_ref_ms=round(python_ms, 1),
                    h2d_bytes=h2d, tick_ms=round(tick_ms, 1), tick_removals=min(a.removals, len(unneeded)),
-                   tick_removable=sum(r[0] is not None for r in res))
+                   tick_removable=sum(r[0] is not None for r in res), resident_tick_ms=round(resident_ms, 1),
+                   resident_call_ms=round(call_ms[-1], 3))
         line = json.dumps(row)
         print(line, flush=True)
         if out:
