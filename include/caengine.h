@@ -682,7 +682,8 @@ int32_t cae_force_add_pods(cae_engine* e, int32_t n, const int32_t* pod, const i
  * pods_to_reschedule, the hints and the persisted cluster; log_len = entries written.  If the log needs more than
  * log_cap entries the call still runs every simulation, sets log_len to the size needed and returns 1 with no other output
  * defined: call again with that capacity.  Malformed input returns -2 before anything runs. */
-enum cae_removal_result { CAE_REMOVAL_REMOVABLE = 0, CAE_REMOVAL_NO_PLACE = 1, CAE_REMOVAL_NO_NODE_INFO = 2 };
+enum cae_removal_result { CAE_REMOVAL_REMOVABLE = 0, CAE_REMOVAL_NO_PLACE = 1, CAE_REMOVAL_NO_NODE_INFO = 2,
+                          CAE_REMOVAL_BLOCKED = 3, CAE_REMOVAL_NOT_SIMULATED = 4 /* cae_plan_removals only */ };
 int32_t cae_simulate_removals(cae_engine* e, int32_t n_cand, const int32_t* cand_node, const int32_t* move_off,
                               const int32_t* move_pod, const uint8_t* dest_ok, const int32_t* hint_node,
                               const int32_t* sim_class, const int32_t* class_ctrl, int32_t n_classes, int32_t last_index_in,
@@ -745,6 +746,93 @@ typedef struct cae_resident_removals {
 } cae_resident_removals;
 int32_t cae_simulate_resident_removals(cae_engine* e, const cae_resident_removals* in, int32_t* result, int32_t* last_index_out,
                                        int32_t* log, int32_t log_cap, int32_t* log_len);
+
+/* The scale-down planner's removal loop on the resident snapshot: Planner.categorizeNodes (core/scaledown/planner/
+ * planner.go) over the unneeded candidates, with GetPodsToMove's last two drainability rules (system, pdb), the
+ * RemainingPdbTracker, the unneeded-nodes limit and the destination map decided on the device, in one launch.  Every
+ * answer equals this loop, on the snapshot cae_simulate_resident_removals works on:
+ *   budget[b] = pdb_allowed[b]; counted = 0; dest = dest_ok (NULL = all)
+ *   for i in 0 .. n_cand-1:
+ *     if unneeded_limit >= 0 and counted >= unneeded_limit: result[i..] = NOT_SIMULATED; stop
+ *     row = cand_node[i]; row < 0, or removed by an earlier persisted success: NO_NODE_INFO; next
+ *     walk the row's NodeInfo pods, position j: resident slots in engine order, then pods earlier persisted simulations
+ *     moved onto it, in arrival order (a moved-in pod keeps the drain byte of its origin):
+ *       prefix SKIP -> next pod;  MOVE -> mover;  BLOCK -> blocked(j, caller reason)
+ *       prefix UNDEFINED:
+ *         kube_system_ns >= 0, ns(pod) == kube_system_ns and no PDB matches the pod -> blocked(j, CAE_BLOCK_KUBE_SYSTEM)
+ *         late reason != 0                                                           -> blocked(j, late reason)
+ *         a PDB b matching the pod has budget[b] < 1                                 -> blocked(j, CAE_BLOCK_NOT_ENOUGH_PDB)
+ *         otherwise mover
+ *     blocked: result BLOCKED, block_pos / block_reason set, no simulation (hints, lastIndex untouched); next
+ *     simulate the movers exactly as cae_simulate_resident_removals does -> REMOVABLE or NO_PLACE
+ *     REMOVABLE: count_b = movers matching b
+ *                pdb_slack[i] = min over b with count_b > 0 of (budget[b] - count_b), INT32_MAX if none
+ *                budget[b] -= count_b; dest[row] = 0 for later candidates (also without persist)
+ *                if !atomic[i]: counted++
+ * A PDB b matches a pod when ps_namespace == pdb_namespace[b] and the pod's label set matches PDB b's selector
+ * (labels.Selector.Matches; kind CAE_SEL_NOTHING matches nothing, an empty CAE_SEL_REQS everything).
+ * Drain byte (drain [n_res], one per resident pod of the cluster rows, indexed as cae_eligibility_inputs.pod_flags):
+ *   bits 0-1  cae_drain_prefix: the outcome of the drainability rules before `system` (DaemonSet pods are SKIP)
+ *   bits 2-3  0
+ *   bits 4-7  a reason 1..15: required for BLOCK; for UNDEFINED optional, the first static block among the rules between
+ *             `system` and `pdb` (not-safe-to-evict, local storage); 0 for SKIP and MOVE
+ * The potential movers of a candidate are its resident pods with prefix MOVE or UNDEFINED, in slot order: the log, the
+ * state afterwards and every status are those of cae_simulate_resident_removals with move_slot = the potential movers
+ * (hint_node / sim_class taken per resident pod); the log's k indexes that list, and blocked candidates write no entries.
+ *   unneeded_limit   -1 = no limit
+ *   atomic [n_cand]  the candidate's group has ZeroOrMaxNodeScaling (it does not count towards the limit); NULL = all 0
+ *   kube_system_ns   namespace id of kube-system; -1 = none, or SkipNodesWithSystemPods is off
+ *   PDBs: pdb_namespace [B] (any id >= 0), pdb_allowed [B] (DisruptionsAllowed), one selector per PDB in tables local
+ *         to the call (pdb_sel_kind [B] cae_sel_kind, pdb_req_off [B + 1] into req_key / req_op / req_val_off /
+ *         req_vals, laid out as cae_objects' requirement tables); key ids are open, value ids index the resident values
+ *         followed by the tail value_is_int / value_int [num_new_values] (values no label set holds).  Nothing of them
+ *         is kept: the call is idempotent.
+ * Outputs: result [n_cand]; block_pos [n_cand] the NodeInfo position j of the blocking pod, -1 when not blocked;
+ * block_reason [n_cand] the caller's 1..15, CAE_BLOCK_KUBE_SYSTEM or CAE_BLOCK_NOT_ENOUGH_PDB, 0 when not blocked;
+ * pdb_slack [n_cand] as above for REMOVABLE (INT32_MAX otherwise); pdb_left [B] the budgets after the loop;
+ * last_index_out, log, log_cap, log_len as for cae_simulate_resident_removals (status 1 with the size needed; a second
+ * call answers the same).  At world_size > 1 every rank may make the call and answers for every candidate.  The call's
+ * H2D and D2H bytes go to cae_stats.
+ * Status -2 (nothing changed): what cae_simulate_resident_removals refuses, n_res != the resident pods of the cluster
+ *   rows, a NULL array that is needed, reserved drain bits set, BLOCK with reason 0, a reason on SKIP or MOVE, a value id
+ *   out of range, a selector kind outside the enum, pdb_req_off or req_val_off not starting at 0 or decreasing, a
+ *   namespace id < 0, unneeded_limit < -1, an atomic byte > 1.
+ * Status 1 / 2 / -1: as for cae_simulate_resident_removals, judged on the potential movers; status 2 also when the distinct
+ *   specs of the potential movers times n_pdb pass 2^31 - 1 (the size of the match table). */
+enum cae_drain_prefix { CAE_DRAIN_UNDEFINED = 0, CAE_DRAIN_SKIP = 1, CAE_DRAIN_MOVE = 2, CAE_DRAIN_BLOCK = 3 };
+enum cae_block_reason { CAE_BLOCK_KUBE_SYSTEM = 16, CAE_BLOCK_NOT_ENOUGH_PDB = 17 };
+typedef struct cae_removal_plan {
+  int32_t abi_version; /* CAE_ABI_VERSION */
+  int32_t n_cand;
+  const int32_t* cand_node;     /* [n_cand] */
+  const uint8_t* dest_ok;       /* [N] or NULL */
+  const int32_t* class_ctrl;    /* [n_classes] */
+  int32_t n_classes;
+  int32_t last_index_in;
+  int32_t persist;
+  int32_t unneeded_limit;
+  const uint8_t* atomic;        /* [n_cand] or NULL */
+  int64_t n_res;
+  const uint8_t* drain;         /* [n_res] */
+  const int32_t* hint_node;     /* [n_res] or NULL */
+  const int32_t* sim_class;     /* [n_res] or NULL */
+  int32_t kube_system_ns;
+  int32_t n_pdb;
+  const int32_t* pdb_namespace; /* [n_pdb] */
+  const int32_t* pdb_allowed;   /* [n_pdb] */
+  const int32_t* pdb_sel_kind;  /* [n_pdb] */
+  const int32_t* pdb_req_off;   /* [n_pdb + 1] */
+  const int32_t* req_key;       /* [pdb_req_off[n_pdb]] */
+  const int32_t* req_op;        /* [pdb_req_off[n_pdb]] */
+  const int32_t* req_val_off;   /* [pdb_req_off[n_pdb] + 1] */
+  const int32_t* req_vals;      /* [req_val_off[last]] */
+  int32_t num_new_values;
+  const uint8_t* value_is_int;  /* [num_new_values] */
+  const int64_t* value_int;     /* [num_new_values] */
+} cae_removal_plan;
+int32_t cae_plan_removals(cae_engine* e, const cae_removal_plan* in, int32_t* result, int32_t* block_pos, int32_t* block_reason,
+                          int32_t* pdb_slack, int32_t* pdb_left, int32_t* last_index_out, int32_t* log, int32_t log_cap,
+                          int32_t* log_len);
 
 /* The ProvisioningRequest capacity check: the check-capacity.autoscaling.x-k8s.io class's bookCapacity and its loop over
  * requests (cluster-autoscaler/provisioningrequest/checkcapacity/provisioningclass.go, orchestrator/orchestrator.go), in

@@ -120,9 +120,13 @@ class cae_resident_removals(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_resident_removals")
 
 
+class cae_removal_plan(C.Structure):
+    _fields_ = _parse_struct(_SRC, "cae_removal_plan")
+
+
 _STRUCTS = {s.__name__: s for s in (cae_objects, cae_config, cae_stats, cae_price_inputs, cae_node_delta, cae_node_churn,
                                      cae_template_delta, cae_pod_delta, cae_similarity_inputs, cae_eligibility_inputs,
-                                     cae_resident_removals)}
+                                     cae_resident_removals, cae_removal_plan)}
 
 
 def _ctype(decl: str, opaque, where: str):

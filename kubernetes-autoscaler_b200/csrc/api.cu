@@ -1877,28 +1877,65 @@ static int fm_finish(Engine* e, const int32_t* d_out, int32_t* out, int n_out, i
   return 0;
 }
 
-// The removal batch after its checks (cae_simulate_removals, cae_simulate_resident_removals): move_pod [move_off[n_cand]]
-// pending pods, hint and cls [P] or NULL.  `d2h` (or NULL) takes the bytes copied back.
+// What cae_plan_removals adds to the resident batch: its checked inputs, the per-pending-pod facts the body derives once
+// the movers are the pending list, and where the planner's outputs go.
+struct PlanCall {
+  const cae_removal_plan* in;
+  int nreq = 0, nvals = 0;                  // requirement and value entries of the PDB selectors
+  std::vector<int32_t> move_off, move_slot, hint, cls;   // the potential movers as the resident batch's listing
+  std::vector<int64_t> res_off;             // [N + 1] first resident pod of each cluster row (the drain byte index)
+  std::vector<uint8_t> pod_byte;            // [P] drain byte of each pending pod
+  std::vector<int32_t> pod_ms, dspec;       // [P] index into dspec, [Sd] distinct pending specs
+  int32_t *block_pos, *block_reason, *pdb_slack, *pdb_left;
+};
+
+// The removal batch after its checks (cae_simulate_removals, cae_simulate_resident_removals, cae_plan_removals): move_pod
+// [move_off[n_cand]] pending pods, hint and cls [P] or NULL.  `d2h` (or NULL) takes the bytes copied back.
 static int run_removals(Engine* e, const char* who, int n_cand, const int32_t* cand_node, const int32_t* move_off,
                         const int32_t* move_pod, const uint8_t* dest_ok, const int32_t* hint_node, const int32_t* sim_class,
                         const int32_t* class_ctrl, int n_classes, int nctrl, int32_t last_index_in, int32_t persist, int32_t* result,
-                        int32_t* last_index_out, int32_t* log, int32_t log_cap, int32_t* log_len, int64_t* d2h) {
+                        int32_t* last_index_out, int32_t* log, int32_t log_cap, int32_t* log_len, int64_t* d2h,
+                        const PlanCall* plan = nullptr) {
   const int P = e->P, N = e->N, M = move_off[n_cand];
   // one staged blob: cand | move_off | move_pod | hint | class | class_ctrl | dest_ok, then the outputs result | out[2] | log
-  // (device only); an absent hint, class or dest_ok array stays NULL
+  // (device only); an absent hint, class or dest_ok array stays NULL.  A plan adds its inputs (the PlanState, the drain
+  // bytes, the PDB tables, the budgets it starts from) and outputs, and always stages dest_ok (its working copy).
   Engine::Staging& st = e->fm;
   cae::RemovalLaunch r{};
   r.ncand = n_cand; r.persist = persist ? 1 : 0; r.ncls = n_classes; r.nctrl = nctrl; r.log_cap = log_cap;
   r.last_index = last_index_in;
+  const cae_removal_plan* pi = plan ? plan->in : nullptr;
+  const int B = pi ? pi->n_pdb : 0, Sd = plan ? (int)plan->dspec.size() : 0, nch = plan ? cae::pdb_chunks(B) : 0;
+  const int V = e->dobj.num_values, Vt = pi ? V + pi->num_new_values : 0;
+  cae::PlanState hp{};                      // the PlanState's fields, bound here and staged as the struct at d_ps
+  cae::PlanState* d_ps = nullptr;
+  cae::PdbMatchLaunch pm{};
+  cae::DrainScanLaunch ds{};
+  int32_t *p_kind = nullptr, *p_roff = nullptr, *p_rkey = nullptr, *p_rop = nullptr, *p_rvoff = nullptr, *p_rvals = nullptr;
+  uint8_t* p_visint = nullptr;
+  int64_t* p_vint = nullptr;
   size_t in_end = 0;
   auto walk = [&](cae::Layout& l) {
     l.add(r.cand, n_cand); l.add(r.move_off, n_cand + 1); l.add(r.move_pod, std::max(M, 1));
     if (hint_node) l.add(r.hint, P);
     if (sim_class) l.add(r.cls, P);
     l.add(r.class_ctrl, std::max(n_classes, 1));
-    if (dest_ok) l.add(r.dest_ok, N);
+    if (dest_ok || plan) l.add(r.dest_ok, N);
+    if (plan) {
+      l.add(d_ps, 1);
+      l.add(ds.drain, (size_t)std::max<int64_t>(pi->n_res, 1)); l.add(hp.move_slot, std::max(M, 1));
+      l.add(hp.pod_byte, P); l.add(hp.pod_ms, P); l.add(pm.spec, Sd); l.add(hp.atomic, n_cand);
+      l.add(pm.pdb_ns, B); l.add(p_kind, B); l.add(p_roff, B + 1); l.add(p_rkey, plan->nreq); l.add(p_rop, plan->nreq);
+      l.add(p_rvoff, plan->nreq + 1); l.add(p_rvals, plan->nvals); l.add(p_visint, Vt); l.add(p_vint, Vt);
+      l.add(hp.budget, B);
+    }
     in_end = l.bytes;
     l.add(r.result, n_cand); l.add(r.out, 2); l.add(r.log, (size_t)std::max(log_cap, 1) * 3);
+    if (plan) {
+      l.add(hp.static_pos, n_cand); l.add(hp.static_reason, n_cand); l.add(hp.block_pos, n_cand);
+      l.add(hp.block_reason, n_cand); l.add(hp.slack_out, n_cand); l.add(hp.cnt, B);
+      l.add(pm.blk, (size_t)Sd * nch + 1); l.add(hp.m_off, Sd + 1);
+    }
   };
   const size_t bytes = cae::layout_bytes(walk);
   if (cae::stage_reserve(e, st, bytes, in_end)) return -1;
@@ -1910,7 +1947,65 @@ static int run_removals(Engine* e, const char* who, int n_cand, const int32_t* c
   if (sim_class) std::copy(sim_class, sim_class + P, st.host_of(r.cls));
   if (n_classes) std::copy(class_ctrl, class_ctrl + n_classes, st.host_of(r.class_ctrl));
   if (dest_ok) std::copy(dest_ok, dest_ok + N, st.host_of(r.dest_ok));
+  else if (plan) std::fill(st.host_of(r.dest_ok), st.host_of(r.dest_ok) + N, (uint8_t)1);
+  if (plan) {
+    hp.limit = pi->unneeded_limit; hp.npdb = B;
+    hp.dest = const_cast<uint8_t*>(r.dest_ok);
+    hp.m_pdb = nullptr;                     // known after the count pass
+    std::copy(pi->drain, pi->drain + pi->n_res, st.host_of(ds.drain));
+    std::copy(plan->move_slot.begin(), plan->move_slot.end(), st.host_of(hp.move_slot));
+    std::copy(plan->pod_byte.begin(), plan->pod_byte.end(), st.host_of(hp.pod_byte));
+    std::copy(plan->pod_ms.begin(), plan->pod_ms.end(), st.host_of(hp.pod_ms));
+    std::copy(plan->dspec.begin(), plan->dspec.end(), st.host_of(pm.spec));
+    if (pi->atomic) std::copy(pi->atomic, pi->atomic + n_cand, st.host_of(hp.atomic));
+    else std::fill(st.host_of(hp.atomic), st.host_of(hp.atomic) + n_cand, (uint8_t)0);
+    if (B) {
+      std::copy(pi->pdb_namespace, pi->pdb_namespace + B, st.host_of(pm.pdb_ns));
+      std::copy(pi->pdb_sel_kind, pi->pdb_sel_kind + B, st.host_of(p_kind));
+      std::copy(pi->pdb_req_off, pi->pdb_req_off + B + 1, st.host_of(p_roff));
+      std::copy(pi->pdb_allowed, pi->pdb_allowed + B, st.host_of(hp.budget));
+      std::copy(pi->req_key, pi->req_key + plan->nreq, st.host_of(p_rkey));
+      std::copy(pi->req_op, pi->req_op + plan->nreq, st.host_of(p_rop));
+      std::copy(pi->req_val_off, pi->req_val_off + plan->nreq + 1, st.host_of(p_rvoff));
+      std::copy(pi->req_vals, pi->req_vals + plan->nvals, st.host_of(p_rvals));
+      // the value tail behind the resident values (those are copied on the device after the upload)
+      std::copy(pi->value_is_int, pi->value_is_int + pi->num_new_values, st.host_of(p_visint) + V);
+      std::copy(pi->value_int, pi->value_int + pi->num_new_values, st.host_of(p_vint) + V);
+    }
+    *st.host_of(d_ps) = hp;
+    r.plan = d_ps;
+  }
   if (cae::stage_upload(e, st, in_end)) return -1;
+  if (plan) {
+    // the PDBs matching each distinct mover spec: count, offsets, then (once the total is known) the list
+    cae::DevObjects sel = e->dobj;
+    sel.req_key = p_rkey; sel.req_op = p_rop; sel.req_val_off = p_rvoff; sel.req_vals = p_rvals;
+    sel.sel_kind = p_kind; sel.sel_req_off = p_roff; sel.value_is_int = p_visint; sel.value_int = p_vint; sel.num_values = Vt;
+    if (B && V) {
+      CAE_CUDA(cudaMemcpyAsync(p_visint, e->dobj.value_is_int, V, cudaMemcpyDeviceToDevice, e->stream));
+      CAE_CUDA(cudaMemcpyAsync(p_vint, e->dobj.value_int, sizeof(int64_t) * V, cudaMemcpyDeviceToDevice, e->stream));
+    }
+    pm.nspec = Sd; pm.npdb = B; pm.m_off = const_cast<int32_t*>(hp.m_off);
+    if (cae::launch_pdb_count(e, sel, pm)) return -1;
+    int32_t total = 0;
+    if (Sd) {
+      CAE_CUDA(cudaMemcpyAsync(&total, pm.blk + (size_t)Sd * nch, sizeof(int32_t), cudaMemcpyDeviceToHost, e->stream));
+      CAE_CUDA(cudaStreamSynchronize(e->stream));
+      e->stats.d2h_bytes += 4;
+    }
+    if (total > 0) {
+      if (cae::devbuf_reserve(e, e->pdb_match, sizeof(int32_t) * (size_t)total)) return -1;
+      pm.m_pdb = static_cast<int32_t*>(e->pdb_match.p);
+      st.host_of(d_ps)->m_pdb = pm.m_pdb;
+      CAE_CUDA(cudaMemcpyAsync(&d_ps->m_pdb, &st.host_of(d_ps)->m_pdb, sizeof(pm.m_pdb), cudaMemcpyHostToDevice, e->stream));
+      e->stats.h2d_bytes += sizeof(pm.m_pdb);
+      if (cae::launch_pdb_fill(e, sel, pm)) return -1;
+    }
+    ds.n = n_cand; ds.kube_ns = pi->kube_system_ns; ds.cand = r.cand; ds.move_off = r.move_off; ds.move_pod = r.move_pod;
+    ds.pod_ms = hp.pod_ms; ds.m_off = hp.m_off;
+    ds.static_pos = const_cast<int32_t*>(hp.static_pos); ds.static_reason = const_cast<int32_t*>(hp.static_reason);
+    if (cae::launch_drain_scan(e, ds)) return -1;
+  }
   cudaEventRecord(e->ev0, e->stream);
   if (cae::launch_removals(e, r)) return -1;
   cudaEventRecord(e->ev1, e->stream);
@@ -1922,19 +2017,26 @@ static int run_removals(Engine* e, const char* who, int n_cand, const int32_t* c
   if (out[1] > log_cap) { cae::set_error(std::string(who) + ": the log needs more entries than log_cap"); return 1; }
   CAE_CUDA(cudaMemcpyAsync(result, r.result, sizeof(int32_t) * n_cand, cudaMemcpyDeviceToHost, e->stream));
   if (out[1]) CAE_CUDA(cudaMemcpyAsync(log, r.log, sizeof(int32_t) * 3 * (size_t)out[1], cudaMemcpyDeviceToHost, e->stream));
+  if (plan) {
+    CAE_CUDA(cudaMemcpyAsync(plan->block_pos, hp.block_pos, sizeof(int32_t) * n_cand, cudaMemcpyDeviceToHost, e->stream));
+    CAE_CUDA(cudaMemcpyAsync(plan->block_reason, hp.block_reason, sizeof(int32_t) * n_cand, cudaMemcpyDeviceToHost, e->stream));
+    CAE_CUDA(cudaMemcpyAsync(plan->pdb_slack, hp.slack_out, sizeof(int32_t) * n_cand, cudaMemcpyDeviceToHost, e->stream));
+    if (B) CAE_CUDA(cudaMemcpyAsync(plan->pdb_left, hp.budget, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, e->stream));
+  }
   CAE_CUDA(cudaStreamSynchronize(e->stream));
-  if (d2h) *d2h += 4 * ((int64_t)n_cand + 3 * (int64_t)out[1]);
+  if (d2h) *d2h += 4 * ((int64_t)n_cand + 3 * (int64_t)out[1]) + (plan ? 4 * (3 * (int64_t)n_cand + B) : 0);
   *last_index_out = out[0];
   return 0;
 }
 
-// cae_simulate_resident_removals.  Every -2 check on the host first; then the spec ids of the distinct pods to move come up
-// in one D2H copy (launch_resident_specs), their nodeName-cleared twins are found in (or appended to) the spec table, the
-// movers become the pending list through cae_load_pods' commit (status 1 or 2: the engine is as before), and the removal
-// batch runs on them.  The log's pending indices are turned back into first-listing positions here.
-static int resident_removals(Engine* e, const cae_resident_removals* in, int32_t* result, int32_t* last_index_out, int32_t* log,
-                             int32_t log_cap, int32_t* log_len) {
-  auto bad = [](const char* m) { cae::set_error(std::string("cae_simulate_resident_removals: ") + m); return -2; };
+// cae_simulate_resident_removals and the body of cae_plan_removals (`plan` set, its listing the potential movers).  Every -2
+// check on the host first; then the spec ids of the distinct pods to move come up in one D2H copy (launch_resident_specs),
+// their nodeName-cleared twins are found in (or appended to) the spec table, the movers become the pending list through
+// cae_load_pods' commit (status 1 or 2: the engine is as before), and the removal batch runs on them.  The log's pending
+// indices are turned back into first-listing positions here.
+static int resident_removals(Engine* e, const char* who, const cae_resident_removals* in, PlanCall* plan, int32_t* result,
+                             int32_t* last_index_out, int32_t* log, int32_t log_cap, int32_t* log_len) {
+  auto bad = [who](const char* m) { cae::set_error(std::string(who) + ": " + m); return -2; };
   if (in->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
   const int n_cand = in->n_cand, N = e->N;
   int n_classes = in->sim_class ? in->n_classes : 0;
@@ -1973,12 +2075,12 @@ static int resident_removals(Engine* e, const cae_resident_removals* in, int32_t
   if (in->hint_node)
     for (int k = 0; k < M; ++k)
       if (in->hint_node[k] < -1 || in->hint_node[k] >= N) return bad("hinted row out of range");
-  const int nctrl = sim_class_check("cae_simulate_resident_removals", in->sim_class, in->class_ctrl, n_classes, M, -1);
+  const int nctrl = sim_class_check(who, in->sim_class, in->class_ctrl, n_classes, M, -1);
   if (nctrl < 0) return -2;
   e->stats.h2d_bytes = 0;
   e->stats.d2h_bytes = 0;
   cudaSetDevice(e->cfg.device);
-  cae::LoadTimer lt("cae_simulate_resident_removals");
+  cae::LoadTimer lt(who);
 
   // ---- the spec of every pod to move, gathered from the resident CSR on the device ----
   std::vector<int32_t> spec(P);
@@ -2052,7 +2154,25 @@ static int resident_removals(Engine* e, const cae_resident_removals* in, int32_t
   d.ps_naff = tw_naff.data(); d.ps_node_name = tw_nn.data(); d.ps_port_list = tw_port.data(); d.ps_pts_list = tw_pts.data();
   d.ps_aff_list = tw_aff.data(); d.ps_anti_list = tw_anti.data(); d.ps_terminating = tw_term.data(); d.ps_hostname_spread = tw_hs.data();
   const cae::Tails v = cae::pod_tails(&d);
-  if (!cae::tails_fit(e, v)) { cae::set_error("cae_simulate_resident_removals: a table would pass 2^31 - 1 entries"); return 2; }
+  if (!cae::tails_fit(e, v)) { cae::set_error(std::string(who) + ": a table would pass 2^31 - 1 entries"); return 2; }
+  if (plan) {   // the drain byte of every mover and its spec among the distinct ones (the PDB match runs per spec)
+    const uint8_t* drain = plan->in->drain;
+    plan->pod_byte.resize(P);
+    plan->pod_ms.resize(P);
+    plan->dspec.clear();
+    std::unordered_map<int32_t, int32_t> ms_of;
+    for (int p = 0; p < P; ++p) {
+      plan->pod_byte[p] = drain[plan->res_off[prow[p]] + pslot[p]];
+      auto it = ms_of.emplace(pend_spec[p], (int32_t)plan->dspec.size());
+      if (it.second) plan->dspec.push_back(pend_spec[p]);
+      plan->pod_ms[p] = it.first->second;
+    }
+    // every (spec, PDB) pair may match: the match offsets are int32
+    if ((int64_t)plan->dspec.size() * plan->in->n_pdb > INT32_MAX) {
+      cae::set_error(std::string(who) + ": the (mover spec, PDB) match table would pass 2^31 - 1 entries");
+      return 2;
+    }
+  }
   {   // the movers become the pending list, as cae_load_pods would leave it
     const int rc = cae::commit_pod_delta(e, v, P, pend_spec.data(), (int)group_off.size() - 1, group_off.data(), lt);
     if (rc) {
@@ -2066,13 +2186,92 @@ static int resident_removals(Engine* e, const cae_resident_removals* in, int32_t
   std::vector<int32_t> hint, cls;
   if (in->hint_node) { hint.resize(P); for (int p = 0; p < P; ++p) hint[p] = in->hint_node[first[p]]; }
   if (in->sim_class) { cls.resize(P); for (int p = 0; p < P; ++p) cls[p] = in->sim_class[first[p]]; }
-  const int rc = run_removals(e, "cae_simulate_resident_removals", n_cand, in->cand_node, in->move_off, pend.data(), in->dest_ok,
+  const int rc = run_removals(e, who, n_cand, in->cand_node, in->move_off, pend.data(), in->dest_ok,
                               in->hint_node ? hint.data() : nullptr, in->sim_class ? cls.data() : nullptr, in->class_ctrl,
                               n_classes, nctrl, in->last_index_in, in->persist, result, last_index_out, log, log_cap, log_len,
-                              &e->stats.d2h_bytes);
+                              &e->stats.d2h_bytes, plan);
   if (rc) return rc;
   for (int i = 0; i < *log_len; ++i) log[3 * i + 1] = first[log[3 * i + 1]];
   return 0;
+}
+
+// cae_plan_removals: its own -2 checks (drain bytes, PDB tables, limit, atomic flags), then the potential movers of every
+// candidate from the drain bytes become the listing of the resident batch's body, which the planner's state rides along.
+static int plan_removals(Engine* e, const cae_removal_plan* in, int32_t* result, int32_t* block_pos, int32_t* block_reason,
+                         int32_t* pdb_slack, int32_t* pdb_left, int32_t* last_index_out, int32_t* log, int32_t log_cap,
+                         int32_t* log_len) {
+  static const char* who = "cae_plan_removals";
+  auto bad = [](const char* m) { cae::set_error(std::string("cae_plan_removals: ") + m); return -2; };
+  if (in->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
+  const int n_cand = in->n_cand, N = e->N, B = in->n_pdb;
+  if (n_cand < 0 || (n_cand > 0 && (!in->cand_node || !result || !block_pos || !block_reason || !pdb_slack)))
+    return bad("bad arguments");
+  for (int c = 0; c < n_cand; ++c)
+    if (in->cand_node[c] < -1 || in->cand_node[c] >= N) return bad("candidate row out of range");
+  PlanCall pc;
+  pc.in = in;
+  pc.block_pos = block_pos; pc.block_reason = block_reason; pc.pdb_slack = pdb_slack; pc.pdb_left = pdb_left;
+  pc.res_off.assign(N + 1, 0);
+  for (int x = 0; x < N; ++x) pc.res_off[x + 1] = pc.res_off[x] + e->nh.pod_cnt[x];
+  if (in->n_res != pc.res_off[N]) return bad("n_res differs from the resident pods of the cluster rows");
+  if (in->n_res > 0 && !in->drain) return bad("bad arguments");
+  for (int64_t k = 0; k < in->n_res; ++k) {
+    const int byte = in->drain[k], pre = byte & 3, why = byte >> 4;
+    if (byte & 0x0C) return bad("reserved drain bits set");
+    if (pre == CAE_DRAIN_BLOCK && why == 0) return bad("a BLOCK byte without a reason");
+    if ((pre == CAE_DRAIN_SKIP || pre == CAE_DRAIN_MOVE) && why != 0) return bad("a reason on a SKIP or MOVE byte");
+  }
+  if (in->unneeded_limit < -1) return bad("unneeded_limit < -1");
+  if (in->kube_system_ns < -1) return bad("kube_system_ns < -1");
+  if (in->atomic)
+    for (int c = 0; c < n_cand; ++c)
+      if (in->atomic[c] > 1) return bad("an atomic byte > 1");
+  if (B < 0 || (B > 0 && (!in->pdb_namespace || !in->pdb_allowed || !in->pdb_sel_kind || !in->pdb_req_off || !pdb_left)))
+    return bad("bad arguments");
+  if (B > 0) {
+    if (in->pdb_req_off[0] != 0) return bad("pdb_req_off[0] must be 0");
+    for (int b = 0; b < B; ++b) {
+      if (in->pdb_namespace[b] < 0) return bad("a PDB namespace id < 0");
+      if (in->pdb_sel_kind[b] != CAE_SEL_NOTHING && in->pdb_sel_kind[b] != CAE_SEL_REQS) return bad("a selector kind outside the enum");
+      if (in->pdb_req_off[b + 1] < in->pdb_req_off[b]) return bad("pdb_req_off decreases");
+    }
+    pc.nreq = in->pdb_req_off[B];
+    if (pc.nreq > 0 && (!in->req_key || !in->req_op)) return bad("bad arguments");
+    if (!in->req_val_off || in->req_val_off[0] != 0) return bad("req_val_off[0] must be 0");
+    for (int q = 0; q < pc.nreq; ++q) {
+      if (in->req_val_off[q + 1] < in->req_val_off[q]) return bad("req_val_off decreases");
+      if (in->req_op[q] < CAE_OP_IN || in->req_op[q] > CAE_OP_LT) return bad("a requirement operator outside the enum");
+    }
+    pc.nvals = in->req_val_off[pc.nreq];
+    if (in->num_new_values < 0 || (in->num_new_values > 0 && (!in->value_is_int || !in->value_int))) return bad("bad arguments");
+    if (pc.nvals > 0 && !in->req_vals) return bad("bad arguments");
+    const int64_t nv = (int64_t)e->dobj.num_values + in->num_new_values;
+    for (int k = 0; k < pc.nvals; ++k)
+      if (in->req_vals[k] < 0 || in->req_vals[k] >= nv) return bad("a value id out of range");
+  }
+  // the potential movers: every resident pod with prefix MOVE or UNDEFINED, in slot order, its hint and class per listing
+  pc.move_off.assign(n_cand + 1, 0);
+  for (int c = 0; c < n_cand; ++c) {
+    const int row = in->cand_node[c];
+    for (int sl = 0; row >= 0 && sl < e->nh.pod_cnt[row]; ++sl) {
+      const int64_t k = pc.res_off[row] + sl;
+      const int pre = in->drain[k] & 3;
+      if (pre != CAE_DRAIN_UNDEFINED && pre != CAE_DRAIN_MOVE) continue;
+      pc.move_slot.push_back(sl);
+      if (in->hint_node) pc.hint.push_back(in->hint_node[k]);
+      if (in->sim_class) pc.cls.push_back(in->sim_class[k]);
+    }
+    pc.move_off[c + 1] = (int32_t)pc.move_slot.size();
+  }
+  cae_resident_removals rr{};
+  rr.abi_version = CAE_ABI_VERSION;
+  rr.n_cand = n_cand; rr.cand_node = in->cand_node; rr.move_off = pc.move_off.data(); rr.move_slot = pc.move_slot.data();
+  rr.dest_ok = in->dest_ok; rr.hint_node = in->hint_node ? pc.hint.data() : nullptr;
+  rr.sim_class = in->sim_class ? pc.cls.data() : nullptr; rr.class_ctrl = in->class_ctrl; rr.n_classes = in->n_classes;
+  rr.last_index_in = in->last_index_in; rr.persist = in->persist;
+  const int rc = resident_removals(e, who, &rr, &pc, result, last_index_out, log, log_cap, log_len);
+  if (rc == 0 && n_cand == 0 && B > 0) std::copy(in->pdb_allowed, in->pdb_allowed + B, pdb_left);
+  return rc;
 }
 
 extern "C" {
@@ -2595,7 +2794,16 @@ int32_t cae_simulate_resident_removals(cae_engine* h, const cae_resident_removal
   Engine* e = reinterpret_cast<Engine*>(h);
   if (!e || !e->loaded) { cae::set_error("cae_simulate_resident_removals before cae_load"); return -2; }
   if (!in) { cae::set_error("cae_simulate_resident_removals: no inputs"); return -2; }
-  return resident_removals(e, in, result, last_index_out, log, log_cap, log_len);
+  return resident_removals(e, "cae_simulate_resident_removals", in, nullptr, result, last_index_out, log, log_cap, log_len);
+}
+
+int32_t cae_plan_removals(cae_engine* h, const cae_removal_plan* in, int32_t* result, int32_t* block_pos, int32_t* block_reason,
+                          int32_t* pdb_slack, int32_t* pdb_left, int32_t* last_index_out, int32_t* log, int32_t log_cap,
+                          int32_t* log_len) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_plan_removals before cae_load"); return -2; }
+  if (!in) { cae::set_error("cae_plan_removals: no inputs"); return -2; }
+  return plan_removals(e, in, result, block_pos, block_reason, pdb_slack, pdb_left, last_index_out, log, log_cap, log_len);
 }
 
 int32_t cae_check_capacity(cae_engine* h, int32_t n_req, const int32_t* req_kind, const int32_t* req_off, const int32_t* req_pod,

@@ -80,6 +80,10 @@ __host__ __device__ inline BpSlab bp_slab_of(const BpParams& p, int A1, bool fm)
   return bp_slab_layout(A1, bp_xg(p, fm), (size_t)DYN_MAX_Q * p.dstride, p.log_cap);
 }
 
+// rm_mode of a work item in the RM instantiation: no node, pods to simulate, nothing to move; cae_plan_removals adds a
+// candidate its drain rules block and one past the unneeded limit (equal to their cae_removal_result)
+enum : int { RM_NO_NODE = 0, RM_RUNS = 1, RM_EMPTY = 2, RM_BLOCKED = CAE_REMOVAL_BLOCKED, RM_NOT_SIMULATED = CAE_REMOVAL_NOT_SIMULATED };
+
 constexpr int BP_HIST = 256;   // capacities up to this use the histogram; above, a binary search
 
 // description of the dynamic group being placed (shared memory, uniform reads)
@@ -339,14 +343,20 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
         }
         for (int i = tid; i < d.pool; i += TPB) { r.ccnt[i] = d.base_cnt[i]; r.cpres[i] = d.base_pres[i]; }
         for (int q = tid; q < d.Q; q += TPB) r.ctot[q] = d.base_tot[q];
+        if (r.plan) {
+          for (int b = tid; b < r.plan->npdb; b += TPB) r.plan->cnt[b] = 0;
+          if (tid == 0) r.plan->counted = 0;
+        }
         if (tid == 0) { S.rm_li_raw = r.li_in; S.rm_log_n = 0; }
         __syncthreads();
       }
       // a capacity batch (r.kind set) has no candidate: no row leaves, its requests list their pods like move_pod
       const int cand = r.kind ? -1 : r.cand[t];
-      const bool exists = r.kind || (cand >= 0 && r.live[cand]);
+      // the planner's loop stops once `counted` reaches the unneeded limit (planner.go: categorizeNodes)
+      const bool limited = r.plan && r.plan->limit >= 0 && r.plan->counted >= r.plan->limit;
+      const bool exists = !limited && (r.kind || (cand >= 0 && r.live[cand]));
       if (!exists) {
-        if (tid == 0) { S.rm_mode = 0; S.rm_runs = 0; S.rm_len = 0; S.rm_li = 0; }
+        if (tid == 0) { S.rm_mode = limited ? RM_NOT_SIMULATED : RM_NO_NODE; S.rm_runs = 0; S.rm_len = 0; S.rm_li = 0; }
       } else {
         // working copy: counters, live mask, destinations (the candidate, removed nodes and nodes outside the map are none)
         for (int i = tid; i < d.pool; i += TPB) { r.wcnt[i] = r.ccnt[i]; r.wpres[i] = r.cpres[i]; }
@@ -377,8 +387,32 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
           int L = L0;
           for (int pod = cand >= 0 ? r.head[cand] : -1; pod >= 0; pod = r.next[pod]) list[L++] = pod;
           S.rm_len = L;
+          if (r.plan) r.plan->fail = INT_MAX;
         }
         __syncthreads();
+        // cae_plan_removals: GetPodsToMove's pdb rule over the UNDEFINED movers before the first static block, in NodeInfo
+        // order (resident slots, then moved-in pods behind every resident pod); a blocked candidate is not simulated
+        bool blocked = false;
+        if (r.plan) {
+          PlanState* pl = r.plan;
+          const int sp = pl->static_pos[t], nres = o.node_pod_off[cand + 1] - o.node_pod_off[cand];
+          for (int i = warp; i < S.rm_len; i += NW) {   // a warp per mover, its lanes over the mover's PDBs
+            const int pod = list[i], j = i < L0 ? pl->move_slot[mb + i] : nres + (i - L0);
+            if (j >= sp || (pl->pod_byte[pod] & 3) != CAE_DRAIN_UNDEFINED) continue;
+            const int ms = pl->pod_ms[pod];
+            for (int k = pl->m_off[ms] + lane; k < pl->m_off[ms + 1]; k += 32)
+              if (pl->budget[pl->m_pdb[k]] < 1) { atomicMin(&pl->fail, j); break; }
+          }
+          __syncthreads();
+          const int fj = *(volatile int*)&pl->fail;
+          blocked = min(fj, sp) != INT_MAX;        // block-uniform
+          if (blocked && tid == 0) {
+            pl->block_pos[t] = min(fj, sp);
+            pl->block_reason[t] = fj < sp ? CAE_BLOCK_NOT_ENOUGH_PDB : pl->static_reason[t];
+            S.rm_len = 0;                          // nothing is tried: no log entry, no hint, lastIndex untouched
+          }
+          __syncthreads();
+        }
         // statistics of every counter over the reduced node set (dyn_stats_kernel on the working copy): one warp per counter
         for (int q = warp; q < d.Q; q += NW) {
           const int off = d.q_base_off[q], len = d.q_base_off[q + 1] - off;
@@ -428,7 +462,7 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
           const int k = blk_excl_count<NW>(S, par, st, nruns);
           if (st) r.run_off[k] = i;
         }
-        if (tid == 0) { r.run_off[nruns] = L; S.rm_runs = nruns; S.rm_mode = L > 0 ? 1 : 2; }
+        if (tid == 0) { r.run_off[nruns] = L; S.rm_runs = nruns; S.rm_mode = blocked ? RM_BLOCKED : L > 0 ? RM_RUNS : RM_EMPTY; }
         __syncthreads();
         GroupRec* recs = const_cast<GroupRec*>(p.grec);
         for (int k = tid; k < nruns; k += TPB) {
@@ -1597,7 +1631,8 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
       const int mode = S.rm_mode, L = S.rm_len, base = S.rm_log_n;
       const int cand = r.kind ? -1 : r.cand[t];
       const bool ok = pods_total == L;      // breakOnFailure: every pod placed, or the simulation stopped
-      const bool commit = mode != 0 && (r.kind ? ok || r.kind[t] == CAE_CAPACITY_BOOK : ok && r.persist);
+      const bool simulated = mode == RM_RUNS || mode == RM_EMPTY;
+      const bool commit = simulated && (r.kind ? ok || r.kind[t] == CAE_CAPACITY_BOOK : ok && r.persist);
       for (int i = tid; i < L; i += TPB) {  // one log entry per pod tried; hints set by placed pods survive in every case
         const int pod = p.fm_pods[i], x = p.fm_assigned[pod];
         if (base + i < r.log_cap) { r.log[(size_t)(base + i) * 3] = t; r.log[(size_t)(base + i) * 3 + 1] = pod; r.log[(size_t)(base + i) * 3 + 2] = x; }
@@ -1639,9 +1674,48 @@ __global__ void __launch_bounds__(TPB, FM ? 1 : BP_MIN_CTAS * 256 / TPB) binpack
           }
         }
       }
+      if (r.plan) {
+        // cae_plan_removals on REMOVABLE (RemainingPdbTracker.CanRemovePods / RemovePods): count the movers of every PDB
+        // they match, the slack before the budgets drop, then the budgets; only the matched PDBs are touched.  The row
+        // stops being a destination, and the candidate counts towards the limit unless its group is atomic.
+        PlanState* pl = r.plan;
+        const bool removable = simulated && ok;   // block-uniform
+        if (removable) {
+          // a warp per mover, its lanes over the mover's PDBs (a pod may match thousands)
+          if (tid == 0) pl->slack = INT_MAX;
+          for (int i = warp; i < L; i += NW) {
+            const int ms = pl->pod_ms[p.fm_pods[i]];
+            for (int k = pl->m_off[ms] + lane; k < pl->m_off[ms + 1]; k += 32) atomicAdd(&pl->cnt[pl->m_pdb[k]], 1);
+          }
+          __syncthreads();
+          for (int i = warp; i < L; i += NW) {
+            const int ms = pl->pod_ms[p.fm_pods[i]];
+            for (int k = pl->m_off[ms] + lane; k < pl->m_off[ms + 1]; k += 32) {
+              const int b = pl->m_pdb[k];
+              atomicMin(&pl->slack, pl->budget[b] - *(volatile int*)&pl->cnt[b]);
+            }
+          }
+          __syncthreads();
+          for (int i = warp; i < L; i += NW) {
+            const int ms = pl->pod_ms[p.fm_pods[i]];
+            for (int k = pl->m_off[ms] + lane; k < pl->m_off[ms + 1]; k += 32) {
+              const int b = pl->m_pdb[k], c = atomicExch(&pl->cnt[b], 0);
+              if (c) pl->budget[b] -= c;           // one thread per PDB sees its count
+            }
+          }
+          if (tid == 0) {
+            pl->dest[cand] = 0;
+            if (!pl->atomic[t]) pl->counted += 1;
+          }
+        }
+        if (tid == 0) {
+          if (mode != RM_BLOCKED) { pl->block_pos[t] = -1; pl->block_reason[t] = 0; }
+          pl->slack_out[t] = removable ? *(volatile int*)&pl->slack : INT_MAX;
+        }
+      }
       if (tid == 0) {
         if (r.kind) r.result[t] = ok ? CAE_CAPACITY_FOUND : CAE_CAPACITY_NOT_FOUND;
-        else r.result[t] = mode == 0 ? CAE_REMOVAL_NO_NODE_INFO : ok ? CAE_REMOVAL_REMOVABLE : CAE_REMOVAL_NO_PLACE;
+        else r.result[t] = mode == RM_NO_NODE ? CAE_REMOVAL_NO_NODE_INFO : !simulated ? mode : ok ? CAE_REMOVAL_REMOVABLE : CAE_REMOVAL_NO_PLACE;
         // lastIndex leaves as a position among the live nodes; it stays raw when no scan placed a pod (plugin_runner.go:123)
         if (fm_moved && S.rm_nlive > 0) S.rm_li_raw = r.rank[last_index] % S.rm_nlive;
         S.rm_log_n = base + L;
@@ -1886,6 +1960,7 @@ int launch_removals(Engine* e, const RemovalLaunch& rl) {
   r.cand = rl.cand; r.move_off = rl.move_off; r.move_pod = rl.move_pod; r.dest_ok = rl.dest_ok; r.kind = rl.kind;
   r.result = rl.result; r.log = rl.log; r.out = rl.out;
   r.grs = group_rec_src(e);
+  r.plan = rl.plan;
   // batch state, one buffer
   auto walk = [&](Layout& l) {
     l.add(r.cfree, A1 * N); l.add(r.cslots, N); l.add(r.cports, N);

@@ -302,6 +302,7 @@ struct Engine {
   Slab pack_slab, fm_slab;                // estimator / filter-out-schedulable pass (binpack.cu)
   Staging fm;                             // inputs, then outputs of the filter pass / the scale-down batch
   DevBuf rm_state;                        // scale-down batch state (RemovalState)
+  DevBuf pdb_match;                       // cae_plan_removals: the PDBs matching each distinct mover spec (PlanState::m_pdb)
   std::vector<int32_t> rm_owner, rm_seen; // [P] argument checks of the scale-down and capacity batches (kept to avoid per-call allocation)
   DevBuf x_rows;                          // caller-supplied option rows: node_count | sched | order
   DevBuf x_price;                         // price inputs: node_price | pod_price | unfitness | score, then has_gpu | exists
@@ -461,8 +462,10 @@ int launch_filter(Engine* e, const FilterLaunch& f);
 // cae_simulate_removals and cae_check_capacity (api.cu lays out the inputs and outputs, launch_removals the batch state
 // behind them).  A capacity batch sets `kind` and leaves cand, dest_ok and log NULL: item t lists its pods in
 // move_off / move_pod, no node leaves, and `assigned` [P] (set to -1 by the caller) takes every pod's node.
+struct PlanState;
 struct RemovalLaunch {
   int ncand, persist, ncls, nctrl, log_cap, last_index;
+  PlanState* plan;                                                       // cae_plan_removals, NULL for the other batches
   const int32_t *cand, *move_off, *move_pod, *hint, *cls, *class_ctrl;   // hint [P] (-1 = none) is read once
   const uint8_t* dest_ok;                                                // [N] or NULL
   const int32_t* kind;                                                   // [ncand] CAE_CAPACITY_*, NULL for removals
@@ -489,6 +492,23 @@ struct RemovalState {
   int32_t *head, *tail, *next;     // [N], [N], [P] pods moved onto a node by persisted simulations, in arrival order
   int32_t* run_off;                // [P + 1] runs of the candidate's pod list
   GroupRecSrc grs;
+  PlanState* plan;                 // cae_plan_removals: the planner's loop (drain rules, budgets, limit); NULL otherwise
+};
+// cae_plan_removals: inputs, outputs and working values of the planner's loop, one struct in device memory (api.cu lays it
+// out in the call's staging blob).  dest_ok of the batch points at `dest`, so a REMOVABLE row stops being a destination.
+struct PlanState {
+  int limit, npdb;                          // unneeded_limit (-1 = none), B
+  int counted;                              // REMOVABLE candidates so far that count towards the limit
+  int fail, slack;                          // per candidate: first PDB-blocked NodeInfo position, pdb_slack (atomicMin)
+  const uint8_t* atomic;                    // [n_cand]
+  const int32_t* move_slot;                 // [M] resident slot of each potential-mover listing
+  const uint8_t* pod_byte;                  // [P] drain byte of each pending pod (of its resident origin)
+  const int32_t* pod_ms;                    // [P] index of the pending pod's spec among the distinct mover specs
+  const int32_t *m_off, *m_pdb;             // [Sd + 1], []: the PDBs matching each distinct spec, ascending
+  const int32_t *static_pos, *static_reason;   // [n_cand] first static block (INT_MAX = none), its reason (drain_scan_kernel)
+  int32_t *budget, *cnt;                    // [B] remaining disruptions (pdb_allowed in, pdb_left out), per-candidate counts
+  uint8_t* dest;                            // [N] destinationMap, rows of REMOVABLE candidates cleared
+  int32_t *block_pos, *block_reason, *slack_out;   // [n_cand] outputs
 };
 int launch_removals(Engine* e, const RemovalLaunch& r);
 // c_free [A][N], tmpl_free [A][T], tmpl_w [W][T] (scratch), rlut and (when e->d_tslice is set) tslice
@@ -532,5 +552,25 @@ int launch_eligibility(Engine* e, const EligLaunch& a);
 // scaledown.cu: cae_simulate_resident_removals.  spec[i] = the spec id of resident pod slot[i] of cluster row row[i], read
 // from the device-resident CSR (node_pod_off / node_pod_spec); n pairs, every one checked by api.cu.
 int launch_resident_specs(Engine* e, int n, const int32_t* row, const int32_t* slot, int32_t* spec);
+// scaledown.cu: cae_plan_removals.  `sel` is the engine's DevObjects with the requirement, selector and value tables of the
+// call's PDB selectors (selector b = PDB b).  launch_pdb_count writes blk [nspec * pdb_chunks(npdb) + 1] = the exclusive
+// offsets of every (spec, PDB chunk) block's matches and the total, and m_off [nspec + 1]; launch_pdb_fill writes m_pdb.
+struct PdbMatchLaunch {
+  int nspec, npdb;
+  const int32_t *spec, *pdb_ns;             // [nspec] distinct mover specs, [B] PDB namespaces
+  int32_t *blk, *m_off, *m_pdb;
+};
+int pdb_chunks(int npdb);
+int launch_pdb_count(Engine* e, const DevObjects& sel, const PdbMatchLaunch& a);
+int launch_pdb_fill(Engine* e, const DevObjects& sel, const PdbMatchLaunch& a);
+// the first static block of every candidate (BLOCK, the system rule, a late reason) over its row's resident drain bytes
+struct DrainScanLaunch {
+  int n, kube_ns;
+  const int32_t *cand, *move_off, *move_pod;   // potential movers as pending pods, in slot order
+  const uint8_t* drain;                     // [n_res]
+  const int32_t *pod_ms, *m_off;
+  int32_t *static_pos, *static_reason;
+};
+int launch_drain_scan(Engine* e, const DrainScanLaunch& a);
 
 }  // namespace cae

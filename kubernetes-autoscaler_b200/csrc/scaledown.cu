@@ -11,6 +11,15 @@
 // cae_simulate_resident_removals:
 //   * resident_spec_kernel, one thread per distinct (row, slot) pair of the pods to move: the pod's spec id from the
 //     resident CSR, so that only these ids travel to the host, never the CSR.
+// cae_plan_removals:
+//   * pdb_match_kernel, one thread per (distinct mover spec, PDB), a block per (spec, chunk of PD_CHUNK PDBs): namespace
+//     compare, then sel_matches_ls on the call's selector tables.  Run twice: the count pass writes each block's match
+//     count, pdb_scan_kernel (one block) turns them into offsets, the fill pass writes the matching PDB ids of every spec in
+//     ascending order (ballot ranks within the block).  S_cand x B selector evaluations per pass, B in the thousands;
+//   * drain_scan_kernel, one warp per candidate as elig_kernel: the first static block over the row's resident drain
+//     bytes (BLOCK, the system rule, a late reason) in slot order, the warp's movers ranked with a ballot to find their
+//     pending pods.
+#include <algorithm>
 #include <climits>
 #include <cub/block/block_scan.cuh>
 
@@ -168,6 +177,126 @@ __global__ void resident_spec_kernel(DevObjects o, int n, const int32_t* __restr
 int launch_resident_specs(Engine* e, int n, const int32_t* row, const int32_t* slot, int32_t* spec) {
   if (n <= 0) return 0;
   resident_spec_kernel<<<(n + 255) / 256, 256, 0, e->stream>>>(e->dobj, n, row, slot, spec);
+  e->stats.kernel_launches += 1;
+  CAE_KERNEL_OK();
+  return 0;
+}
+
+constexpr int PD_CHUNK = 256;                      // PDBs per block of pdb_match_kernel
+constexpr int PD_SCAN = 1024;                      // threads of pdb_scan_kernel
+constexpr int PD_MAX_Y = 65535;
+
+int pdb_chunks(int npdb) { return (npdb + PD_CHUNK - 1) / PD_CHUNK; }
+
+template <bool FILL>
+__global__ void __launch_bounds__(PD_CHUNK) pdb_match_kernel(DevObjects o, PdbMatchLaunch a, int nchunk) {
+  __shared__ int warp_n[PD_CHUNK / 32];
+  const int s = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int ns = o.ps_namespace[a.spec[s]], ls = o.ps_labelset[a.spec[s]];
+  for (int c = blockIdx.y; c < nchunk; c += gridDim.y) {   // block-uniform loop
+    const int b = c * PD_CHUNK + threadIdx.x;
+    const bool m = b < a.npdb && a.pdb_ns[b] == ns && sel_matches_ls(o, b, ls);
+    const size_t slot = (size_t)s * nchunk + c;
+    if (!FILL) {
+      const int n = __syncthreads_count(m);
+      if (threadIdx.x == 0) a.blk[slot] = n;
+    } else {
+      const unsigned bal = __ballot_sync(0xffffffffu, m);
+      if (lane == 0) warp_n[warp] = __popc(bal);
+      __syncthreads();
+      int pos = a.blk[slot] + __popc(bal & ((1u << lane) - 1));
+      for (int w = 0; w < warp; ++w) pos += warp_n[w];
+      if (m) a.m_pdb[pos] = b;
+      __syncthreads();                             // warp_n is reused by the next chunk
+    }
+  }
+}
+
+// exclusive offsets of the n block counts (blk[n] = total) and the per-spec offsets m_off [nspec + 1]
+__global__ void __launch_bounds__(PD_SCAN) pdb_scan_kernel(PdbMatchLaunch a, int nchunk) {
+  using Scan = cub::BlockScan<int, PD_SCAN>;
+  __shared__ typename Scan::TempStorage tmp;
+  const long long n = (long long)a.nspec * nchunk;
+  int base = 0;
+  for (long long c0 = 0; c0 < n; c0 += PD_SCAN) {
+    const long long i = c0 + threadIdx.x;
+    const int v = i < n ? a.blk[i] : 0;
+    int pos, total;
+    Scan(tmp).ExclusiveSum(v, pos, total);
+    if (i < n) {
+      a.blk[i] = base + pos;
+      if (i % nchunk == 0) a.m_off[i / nchunk] = base + pos;
+    }
+    base += total;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) { a.blk[n] = base; a.m_off[a.nspec] = base; }
+  if (nchunk == 0)                                 // no PDB: no spec matches any
+    for (int s = threadIdx.x; s < a.nspec; s += PD_SCAN) a.m_off[s] = 0;
+}
+
+static dim3 pdb_grid(const PdbMatchLaunch& a) { return dim3(a.nspec, std::min(pdb_chunks(a.npdb), PD_MAX_Y)); }
+
+int launch_pdb_count(Engine* e, const DevObjects& sel, const PdbMatchLaunch& a) {
+  if (a.nspec <= 0) return 0;
+  const int nchunk = pdb_chunks(a.npdb);
+  if (nchunk > 0) {
+    pdb_match_kernel<false><<<pdb_grid(a), PD_CHUNK, 0, e->stream>>>(sel, a, nchunk);
+    e->stats.kernel_launches += 1;
+  }
+  pdb_scan_kernel<<<1, PD_SCAN, 0, e->stream>>>(a, nchunk);
+  e->stats.kernel_launches += 1;
+  CAE_KERNEL_OK();
+  return 0;
+}
+
+int launch_pdb_fill(Engine* e, const DevObjects& sel, const PdbMatchLaunch& a) {
+  const int nchunk = pdb_chunks(a.npdb);
+  if (a.nspec <= 0 || nchunk == 0) return 0;
+  pdb_match_kernel<true><<<pdb_grid(a), PD_CHUNK, 0, e->stream>>>(sel, a, nchunk);
+  e->stats.kernel_launches += 1;
+  CAE_KERNEL_OK();
+  return 0;
+}
+
+__global__ void __launch_bounds__(EL_WARPS * 32) drain_scan_kernel(DevObjects o, DrainScanLaunch a) {
+  const int lane = threadIdx.x & 31, i = blockIdx.x * EL_WARPS + (threadIdx.x >> 5);
+  if (i >= a.n) return;                            // warp-uniform
+  const int row = a.cand[i];
+  int pos = INT_MAX, reason = 0;
+  if (row >= 0) {
+    const int b = o.node_pod_off[row], cnt = o.node_pod_off[row + 1] - b, mb = a.move_off[i];
+    int movers = 0;                                // potential movers in the slots before this chunk
+    for (int j0 = 0; j0 < cnt; j0 += 32) {
+      const int j = j0 + lane;
+      const int byte = j < cnt ? a.drain[b + j] : CAE_DRAIN_SKIP, pre = byte & 3;
+      const unsigned mv = __ballot_sync(0xffffffffu, pre == CAE_DRAIN_UNDEFINED || pre == CAE_DRAIN_MOVE);
+      int r = 0;
+      if (pre == CAE_DRAIN_BLOCK) {
+        r = byte >> 4;
+      } else if (pre == CAE_DRAIN_UNDEFINED) {
+        const int ms = a.pod_ms[a.move_pod[mb + movers + __popc(mv & ((1u << lane) - 1))]];
+        if (a.kube_ns >= 0 && o.ps_namespace[o.node_pod_spec[b + j]] == a.kube_ns && a.m_off[ms + 1] == a.m_off[ms])
+          r = CAE_BLOCK_KUBE_SYSTEM;
+        else
+          r = byte >> 4;
+      }
+      const unsigned blk = __ballot_sync(0xffffffffu, r != 0);
+      if (blk) {
+        const int f = __ffs(blk) - 1;
+        pos = j0 + f;
+        reason = __shfl_sync(0xffffffffu, r, f);
+        break;
+      }
+      movers += __popc(mv);
+    }
+  }
+  if (lane == 0) { a.static_pos[i] = pos; a.static_reason[i] = reason; }
+}
+
+int launch_drain_scan(Engine* e, const DrainScanLaunch& a) {
+  if (a.n <= 0) return 0;
+  drain_scan_kernel<<<(a.n + EL_WARPS - 1) / EL_WARPS, EL_WARPS * 32, 0, e->stream>>>(e->dobj, a);
   e->stats.kernel_launches += 1;
   CAE_KERNEL_OK();
   return 0;

@@ -889,6 +889,21 @@ class ResidentRemovals(AbiArrays):
         super().__init__(**fields)
 
 
+class RemovalPlan(AbiArrays):
+    """``cae_removal_plan`` of cae_plan_removals.  The optional arrays left out are NULL; n_res follows drain and n_pdb
+    pdb_namespace."""
+
+    STRUCT = capi.cae_removal_plan
+    COUNTS = {"n_cand": "cand_node", "n_res": "drain", "n_pdb": "pdb_namespace", "num_new_values": "value_is_int"}
+
+    def __init__(self, **fields) -> None:
+        for nm in ("dest_ok", "atomic", "hint_node", "sim_class", "class_ctrl"):
+            fields.setdefault(nm, None)
+        fields.setdefault("pdb_req_off", [0])
+        fields.setdefault("req_val_off", [0])
+        super().__init__(**fields)
+
+
 # ----------------------------------------------------------------------------------------------
 class Encoder:
     """Interns objects.py dataclasses into a TableBuilder (the Go shim's job in production)."""

@@ -10,7 +10,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 
 from . import capi
-from .encode import EligibilityInputs, EncodedObjects, PriceInputs, ResidentRemovals, SimilarityInputs
+from .encode import EligibilityInputs, EncodedObjects, PriceInputs, RemovalPlan, ResidentRemovals, SimilarityInputs
 
 
 class EngineError(RuntimeError):
@@ -392,6 +392,44 @@ class Engine:
         if rc == 1:
             return rc, None, None, np.zeros((int(n[0]), 3), np.int32)
         return rc, res[:len(cn)], int(li[0]), log[:int(n[0])]
+
+    def plan_removals(self, plan: RemovalPlan, log_cap: Optional[int] = None, enc: Optional[EncodedObjects] = None):
+        """The planner's removal loop on the resident snapshot (cae_plan_removals) for the inputs `plan`.  Returns a dict:
+        result [n_cand] CAE_REMOVAL_*, block_pos / block_reason / pdb_slack [n_cand], pdb_left [n_pdb], last_index, log
+        [n][3] = (candidate, k, cluster row or -1) with k the potential-mover listing where the pod was first listed, and
+        move_off / move_slot, that listing (every MOVE or UNDEFINED resident pod of each candidate's row, in slot order).
+        A log past `log_cap` (default: one entry per potential mover plus 64) is fetched again at the size the engine
+        reports.  Afterwards the engine holds the potential movers as its pending pods (`enc`: the objects after the call,
+        when the caller has them).  Raises EngineUnsupported on status 1 or 2."""
+        cand = plan.arrays["cand_node"]
+        drain = plan.arrays["drain"]
+        N = self.enc.struct.num_cluster_nodes
+        res_off = self.enc.arrays["node_pod_off"][:N + 1]
+        move_off, move_slot = [0], []
+        for row in cand.tolist():
+            if 0 <= row < N:   # (a row out of range is the engine's to refuse)
+                b = drain[res_off[row]:res_off[row + 1]] & 3
+                move_slot += np.flatnonzero((b == 0) | (b == 2)).tolist()
+            move_off.append(len(move_slot))
+        n, B = len(cand), plan.struct.n_pdb
+        cap = int(log_cap) if log_cap is not None else len(move_slot) + 64
+        out = {nm: np.zeros(max(n, 1), np.int32) for nm in ("result", "block_pos", "block_reason", "pdb_slack")}
+        out["pdb_left"] = np.zeros(max(B, 1), np.int32)
+        li, m = np.zeros(1, np.int32), np.zeros(1, np.int32)
+        for _ in range(2):
+            log = np.zeros((max(cap, 1), 3), np.int32)
+            rc = self.lib.cae_plan_removals(self.h, plan.ptr(), _vp(out["result"]), _vp(out["block_pos"]), _vp(out["block_reason"]),
+                                            _vp(out["pdb_slack"]), _vp(out["pdb_left"]), _vp(li), _vp(log), int(cap), _vp(m))
+            if rc != 1 or int(m[0]) <= cap:
+                break
+            cap = int(m[0])   # the log needed more room: once more at the size it reported
+        self._check(rc)
+        move_off = np.asarray(move_off, np.int32)
+        self.enc = enc if enc is not None else self.enc.apply_resident_removals(cand, move_off, move_slot)[0]
+        res = {nm: a[:n] for nm, a in out.items() if nm != "pdb_left"}
+        res.update(pdb_left=out["pdb_left"][:B], last_index=int(li[0]), log=log[:int(m[0])], move_off=move_off,
+                   move_slot=np.asarray(move_slot, np.int32))
+        return res
 
     def check_capacity(self, req_kind, req_off, req_pod, hint_node=None, sim_class=None, class_ctrl=None, last_index: int = 0):
         """The ProvisioningRequest capacity batch on the snapshot of the last load (cae_check_capacity): BOOK requests keep

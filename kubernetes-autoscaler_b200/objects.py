@@ -112,6 +112,11 @@ class Pod:
     annotations: Dict[str, str] = field(default_factory=dict)
     deletion_timestamp: Optional[float] = None
     termination_grace_period_seconds: Optional[int] = None
+    # read only by the drainability rules (drain.py): status.phase, spec.restartPolicy and whether the pod uses local storage
+    # (an emptyDir or hostPath volume that is not safe to lose)
+    phase: str = ""
+    restart_policy: str = "Always"
+    local_storage: bool = False
 
     def clone(self) -> "Pod":
         return copy.deepcopy(self)
@@ -132,6 +137,16 @@ class NodeInfo:
     """framework.NodeInfo: a node plus the pods already on it (resident / DaemonSet pods)."""
     node: Node
     pods: List[Pod] = field(default_factory=list)
+
+
+@dataclass
+class PodDisruptionBudget:
+    """policyv1.PodDisruptionBudget as the scale-down reads it: the selector (None = nil, matches nothing; LabelSelector()
+    = {}, matches everything in the namespace) and status.disruptionsAllowed."""
+    name: str
+    namespace: str
+    selector: Optional[LabelSelector]
+    disruptions_allowed: int
 
 
 @dataclass

@@ -150,6 +150,24 @@ def main():
             res, li, log = eng.simulate_removals(cand, move_off, pend, persist=True)
             assert np.array_equal(got[0], res) and got[1] == li and np.array_equal(got[2][:, [0, 2]], log[:, [0, 2]])
             assert np.array_equal(got[2][:, 1], first[log[:, 1]])
+            # the planner's loop on the resident snapshot (cae_plan_removals: both PDB match passes, the drain scan, the
+            # budgets and the limit in the batch): with every pod MOVE and no PDB it is the resident batch above, and a
+            # second call with PDBs, drain rules and a limit answers as the first
+            from kubernetes_autoscaler_b200.encode import RemovalPlan
+            nres = int(off[N])
+            eng.load(after)
+            pl = eng.plan_removals(RemovalPlan(cand_node=cand, drain=np.full(nres, 2, np.uint8), unneeded_limit=-1,
+                                               kube_system_ns=-1, persist=1))
+            assert np.array_equal(pl["result"], got[0]) and pl["last_index"] == got[1] and np.array_equal(pl["log"], got[2])
+            plan = RemovalPlan(cand_node=cand, drain=rng.choice([0, 1, 2, 0x40], nres).astype(np.uint8), unneeded_limit=6,
+                               kube_system_ns=0, persist=1, pdb_namespace=np.zeros(8, np.int32),
+                               pdb_allowed=rng.integers(0, 3, 8).astype(np.int32), pdb_sel_kind=np.ones(8, np.int32),
+                               pdb_req_off=np.zeros(9, np.int32))
+            answers = []
+            for _ in range(2):
+                eng.load(after)
+                answers.append(eng.plan_removals(plan))
+            assert all(np.array_equal(answers[0][k], answers[1][k]) for k in ("result", "block_pos", "pdb_left", "log"))
         # similar node groups (cae_similar_node_groups: operand / bit-row prep, the pair kernel's staged tiles and ballots)
         infos, groups, ngs = synth.node_group_families(cfg, 45, 4, seed=cfg, groups=40)
         sim = ScaleUpSimulation([], infos, groups, eng)
