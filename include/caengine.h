@@ -953,6 +953,40 @@ typedef struct cae_similarity_inputs {
 int32_t cae_similar_node_groups(cae_engine* e, const cae_similarity_inputs* in, uint32_t* similar_bits, int32_t* similar_count,
                                 int64_t* sng_limit);
 
+/* The DaemonSet pods of every loaded template, in one call, and optionally the template pod lists they imply.
+ * Replaces: the loop of daemonset.GetDaemonSetPodsForNode (utils/daemonset/daemonset.go) that podsExpectedOnFreshNode
+ * (simulator/node_info_utils.go) runs for every template TemplateNodeInfoProvider builds: daemon.NodeShouldRunDaemonPod
+ * (pkg/controller/daemon) for every (template, DaemonSet).  The caller loads the sanitized template (taints, name and
+ * hostname are host facts) and interns NewPod(ds, node) of every DaemonSet as a pod spec.
+ * Bit d of row t is set iff evaluate[t], the running bit of (t, d) is 0, and all of:
+ *   - ps_node_name of ds_spec[d] is -1 or equals the template's name id (the DaemonSet's spec.nodeName test);
+ *   - RequiredNodeAffinity.Match on the template row: nodeSelector AND the required terms, matchFields on metadata.name
+ *     against the template's name id (no PreFilter step);
+ *   - no NoSchedule or NoExecute taint of the template row is untolerated by the spec's tolerations.
+ * The three tests are independent, and node_unschedulable is not read.
+ *   run_bits [T][ceil(D/32)]  bit d%32 of word d/32 of row t.  May be NULL.
+ *   run_count [T]             bits set in row t.  May be NULL.
+ * Apply (keep != NULL): every evaluated template whose list changes gets the pod list "its first keep[t] pods, then
+ * ds_spec[d] for every bit d of its row, in d order", its other columns unchanged.  The engine then answers exactly as after
+ * cae_load_templates with those rows as `changed` (no tails), under that call's status rules: status 2 when a chosen spec
+ * has required anti-affinity terms and no pod of that spec was in the snapshot, or a table would pass 2^31 - 1; status 1
+ * with peers attached past 65536 templates.  A refused apply changes nothing and writes no output.
+ * At world_size > 1 every rank computes all T rows and applies the same change.  The call's H2D and D2H bytes go to
+ * cae_stats.
+ * Status -2 (nothing done): before a load; num_ds < 0; a NULL ds_spec with num_ds > 0; a spec id out of range; an evaluate
+ *   byte > 1; a running bit at or past num_ds; keep[t] < 0 or past template t's pod count. */
+typedef struct cae_daemonset_inputs {
+  int32_t abi_version;       /* CAE_ABI_VERSION */
+  int32_t num_ds;            /* D */
+  const int32_t* ds_spec;    /* [D] pod spec of NewPod(ds, node): the DaemonSet's pod template with the daemon tolerations
+                                added (AddOrUpdateDaemonPodTolerations); ps_node_name = the pod template's own spec.nodeName */
+  const uint8_t* evaluate;   /* [T] 1 = compute this template's row; NULL = all */
+  const uint32_t* running;   /* [T][ceil(D/32)] DaemonSets already running on the example node (podsExpectedOnFreshNode's
+                                runningDS): their bits stay 0; NULL = none */
+  const int32_t* keep;       /* [T] pods of the current list each template keeps before its DaemonSet pods; NULL = report only */
+} cae_daemonset_inputs;
+int32_t cae_template_daemonsets(cae_engine* e, const cae_daemonset_inputs* in, uint32_t* run_bits, int32_t* run_count);
+
 /* Scale-down eligibility of the candidate nodes on the resident snapshot, in one call.
  * Replaces: eligibility.Checker.FilterOutUnremovable (core/scaledown/eligibility/eligibility.go) from the utilization on:
  * utilization.Calculate (simulator/utilization/info.go) of every candidate, then the unready and threshold tests.  The

@@ -112,6 +112,10 @@ class cae_similarity_inputs(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_similarity_inputs")
 
 
+class cae_daemonset_inputs(C.Structure):
+    _fields_ = _parse_struct(_SRC, "cae_daemonset_inputs")
+
+
 class cae_eligibility_inputs(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_eligibility_inputs")
 
@@ -125,7 +129,8 @@ class cae_removal_plan(C.Structure):
 
 
 _STRUCTS = {s.__name__: s for s in (cae_objects, cae_config, cae_stats, cae_price_inputs, cae_node_delta, cae_node_churn,
-                                     cae_template_delta, cae_pod_delta, cae_similarity_inputs, cae_eligibility_inputs,
+                                     cae_template_delta, cae_pod_delta, cae_similarity_inputs, cae_daemonset_inputs,
+                                     cae_eligibility_inputs,
                                      cae_resident_removals, cae_removal_plan)}
 
 

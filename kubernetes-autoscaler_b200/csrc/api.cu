@@ -1668,6 +1668,143 @@ static int do_similar(Engine* e, const cae_similarity_inputs* in, uint32_t* bits
   return 0;
 }
 
+// The apply step of cae_template_daemonsets: the evaluated templates whose pod list changes become the `changed` rows of a
+// cae_template_delta, committed by do_load_templates, so the template-row derivation and its refusals are that call's.
+// The engine keeps no host copy of the template columns or pod lists: they are read back from the device, and only when
+// some evaluated row drops pods or gains DaemonSet pods.  `d2h` accumulates the bytes read.
+static int apply_daemonsets(Engine* e, const cae_daemonset_inputs* in, const uint32_t* bits, const int32_t* count, int Dw,
+                            int64_t* d2h) {
+  const int N = e->N, T = e->T;
+  std::vector<int> cand;
+  for (int t = 0; t < T; ++t)
+    if ((!in->evaluate || in->evaluate[t]) && (in->keep[t] != e->nh.tmpl_pods[t] || count[t])) cand.push_back(t);
+  if (cand.empty()) return 0;
+  const DevObjects& o = e->dobj;
+  std::vector<int32_t> name(T), ls(T), tl(T), allowed(T), off(T + 1);
+  std::vector<uint8_t> uns(T), hcpu(T), hmem(T);
+  std::vector<int64_t> alloc((size_t)T * R), ccpu(T), cmem(T);
+  auto get = [&](void* dst, const void* src, size_t n) {
+    *d2h += (int64_t)n;
+    return cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, e->stream);
+  };
+  CAE_CUDA(get(name.data(), o.node_name + N, 4 * (size_t)T));
+  CAE_CUDA(get(ls.data(), o.node_labelset + N, 4 * (size_t)T));
+  CAE_CUDA(get(tl.data(), o.node_taint_list + N, 4 * (size_t)T));
+  CAE_CUDA(get(allowed.data(), o.node_allowed_pods + N, 4 * (size_t)T));
+  CAE_CUDA(get(off.data(), o.node_pod_off + N, 4 * (size_t)(T + 1)));
+  CAE_CUDA(get(uns.data(), o.node_unschedulable + N, T));
+  CAE_CUDA(get(hcpu.data(), o.node_has_alloc_cpu + N, T));
+  CAE_CUDA(get(hmem.data(), o.node_has_alloc_mem + N, T));
+  CAE_CUDA(get(alloc.data(), o.node_alloc + (size_t)N * R, 8 * alloc.size()));
+  CAE_CUDA(get(ccpu.data(), o.node_cap_cpu + N, 8 * (size_t)T));
+  CAE_CUDA(get(cmem.data(), o.node_cap_mem + N, 8 * (size_t)T));
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
+  std::vector<int32_t> pods((size_t)(off[T] - off[0]));
+  if (!pods.empty()) {
+    CAE_CUDA(get(pods.data(), o.node_pod_spec + off[0], 4 * pods.size()));
+    CAE_CUDA(cudaStreamSynchronize(e->stream));
+  }
+  std::vector<int32_t> changed, r_name, r_ls, r_tl, r_allowed, r_off{0}, r_spec, list;
+  std::vector<uint8_t> r_uns, r_hcpu, r_hmem;
+  std::vector<int64_t> r_alloc, r_ccpu, r_cmem;
+  for (int t : cand) {
+    const int32_t* old = pods.data() + (off[t] - off[0]);
+    const int n_old = off[t + 1] - off[t];
+    list.assign(old, old + in->keep[t]);
+    for (int w = 0; w < Dw; ++w)
+      for (uint32_t m = bits[(size_t)t * Dw + w]; m; m &= m - 1) list.push_back(in->ds_spec[w * 32 + __builtin_ctz(m)]);
+    if ((int)list.size() == n_old && std::equal(list.begin(), list.end(), old)) continue;
+    changed.push_back(t);
+    r_name.push_back(name[t]); r_ls.push_back(ls[t]); r_tl.push_back(tl[t]); r_allowed.push_back(allowed[t]);
+    r_uns.push_back(uns[t]); r_hcpu.push_back(hcpu[t]); r_hmem.push_back(hmem[t]);
+    r_alloc.insert(r_alloc.end(), alloc.begin() + (size_t)t * R, alloc.begin() + (size_t)(t + 1) * R);
+    r_ccpu.push_back(ccpu[t]); r_cmem.push_back(cmem[t]);
+    r_spec.insert(r_spec.end(), list.begin(), list.end());
+    if (r_spec.size() > (size_t)INT32_MAX) {
+      set_error("cae_template_daemonsets: the new template pods would pass 2^31 - 1");
+      return 2;
+    }
+    r_off.push_back((int32_t)r_spec.size());
+  }
+  if (changed.empty()) return 0;
+  cae_template_delta c{};
+  c.abi_version = CAE_ABI_VERSION;
+  c.num_changed = (int32_t)changed.size();
+  c.changed = changed.data();
+  c.name = r_name.data(); c.labelset = r_ls.data(); c.taint_list = r_tl.data(); c.unschedulable = r_uns.data();
+  c.alloc = r_alloc.data(); c.allowed_pods = r_allowed.data(); c.cap_cpu = r_ccpu.data(); c.cap_mem = r_cmem.data();
+  c.has_alloc_cpu = r_hcpu.data(); c.has_alloc_mem = r_hmem.data(); c.pod_off = r_off.data(); c.pod_spec = r_spec.data();
+  return do_load_templates(e, &c);
+}
+
+// cae_template_daemonsets.  The inputs travel in one H2D copy, the counts and run bits in one D2H copy; nothing is written
+// to the caller's buffers unless the status is 0.
+static int do_template_daemonsets(Engine* e, const cae_daemonset_inputs* in, uint32_t* bits_out, int32_t* count_out) {
+  auto bad = [](const char* m) { set_error(std::string("cae_template_daemonsets: ") + m); return -2; };
+  if (in->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
+  const int N = e->N, T = e->T, D = in->num_ds;
+  if (D < 0) return bad("num_ds < 0");
+  if (D && !in->ds_spec) return bad("ds_spec is NULL");
+  const int Dw = (D + 31) / 32;
+  for (int d = 0; d < D; ++d)
+    if (in->ds_spec[d] < 0 || in->ds_spec[d] >= e->num_podspecs) return bad("a spec id out of range");
+  for (int t = 0; t < T; ++t) {
+    if (in->evaluate && in->evaluate[t] > 1) return bad("an evaluate byte > 1");
+    if (in->keep && (in->keep[t] < 0 || in->keep[t] > e->nh.tmpl_pods[t])) return bad("keep[t] < 0 or past the template's pods");
+  }
+  if (in->running && D % 32)
+    for (int t = 0; t < T; ++t)
+      if (in->running[(size_t)t * Dw + Dw - 1] >> (D % 32)) return bad("a running bit at or past num_ds");
+  e->stats.h2d_bytes = 0;
+  e->stats.d2h_bytes = 0;
+  if (T == 0) return 0;
+
+  Engine::Staging& st = e->ds;
+  DsLaunch a{};
+  a.N = N; a.T = T; a.D = D; a.Dw = Dw;
+  int32_t* d_spec = nullptr;
+  uint8_t* d_eval = nullptr;
+  uint32_t* d_run = nullptr;
+  size_t in_end = 0, o_bits = 0, out_end = 0;
+  auto walk = [&](Layout& l) {
+    l.add(d_spec, D); l.add(d_eval, in->evaluate ? T : 0); l.add(d_run, in->running ? (size_t)T * Dw : 0);
+    in_end = l.bytes;
+    l.add(a.count, T);
+    o_bits = l.bytes;
+    l.add(a.bits, (size_t)T * Dw);
+    out_end = l.bytes;
+  };
+  const size_t bytes = layout_bytes(walk);   // sets out_end: a separate statement, argument order is unspecified
+  if (stage_reserve(e, st, bytes, out_end)) return -1;
+  layout_bind(st.dev.p, walk);
+  if (D) std::copy(in->ds_spec, in->ds_spec + D, st.host_of(d_spec));
+  if (in->evaluate) std::copy(in->evaluate, in->evaluate + T, st.host_of(d_eval));
+  if (in->running) std::copy(in->running, in->running + (size_t)T * Dw, st.host_of(d_run));
+  if (stage_upload(e, st, in_end)) return -1;
+  a.ds_spec = d_spec;
+  a.evaluate = in->evaluate ? d_eval : nullptr;
+  a.running = in->running ? d_run : nullptr;
+  CAE_CUDA(cudaMemsetAsync(a.count, 0, sizeof(int32_t) * T, e->stream));
+  if (launch_ds_verdicts(e, a)) return -1;
+  int64_t d2h = (int64_t)(((bits_out || in->keep) ? out_end : o_bits) - in_end);
+  CAE_CUDA(cudaMemcpyAsync(st.host_of(a.count), a.count, (size_t)d2h, cudaMemcpyDeviceToHost, e->stream));
+  CAE_CUDA(cudaStreamSynchronize(e->stream));
+  const int32_t* h_count = st.host_of(a.count);
+  const uint32_t* h_bits = st.host_of(a.bits);
+  if (in->keep) {
+    const int64_t h2d = e->stats.h2d_bytes;
+    e->stats.h2d_bytes = 0;   // do_load_templates counts its own upload from 0
+    const int rc = apply_daemonsets(e, in, h_bits, h_count, Dw, &d2h);
+    e->stats.h2d_bytes += h2d;
+    e->stats.d2h_bytes = d2h;
+    if (rc) return rc;
+  }
+  e->stats.d2h_bytes = d2h;
+  if (count_out) std::copy(h_count, h_count + T, count_out);
+  if (bits_out) std::copy(h_bits, h_bits + (size_t)T * Dw, bits_out);
+  return 0;
+}
+
 // cae_group_reasons.  The masks travel in one H2D copy, schedulable and the counts in one D2H copy; the detail matrix goes
 // from the device straight into the caller's buffer.
 static int do_group_reasons(Engine* e, const uint8_t* considered, const uint8_t* exist, uint8_t* sched_out, int32_t* count_out,
@@ -2636,6 +2773,14 @@ int32_t cae_similar_node_groups(cae_engine* h, const cae_similarity_inputs* in, 
   if (!in) { cae::set_error("cae_similar_node_groups: no inputs"); return -2; }
   cudaSetDevice(e->cfg.device);
   return cae::do_similar(e, in, similar_bits, similar_count, sng_limit);
+}
+
+int32_t cae_template_daemonsets(cae_engine* h, const cae_daemonset_inputs* in, uint32_t* run_bits, int32_t* run_count) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_template_daemonsets before cae_load"); return -2; }
+  if (!in) { cae::set_error("cae_template_daemonsets: no inputs"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_template_daemonsets(e, in, run_bits, run_count);
 }
 
 int32_t cae_scale_down_eligibility(cae_engine* h, const cae_eligibility_inputs* in, double* util, uint8_t* reason,

@@ -360,6 +360,7 @@ struct Engine {
   Staging sim;                            // inputs | outputs (one D2H copy) | operand rows | schedulable bit rows (device only)
   Staging gr;                             // cae_group_reasons: masks | schedulable, counts (one D2H copy) | detail (device only)
   Staging el;                             // cae_scale_down_eligibility: inputs | util, reason, list, count, status (one D2H copy)
+  Staging ds;                             // cae_template_daemonsets: inputs | run bits, counts (one D2H copy)
   int sm_count = 132;
   int smem_optin = 227 * 1024;             // opt-in shared memory per thread block
   size_t hbm_bytes = (size_t)80 << 30;     // device memory (sizes the estimator's global slabs)
@@ -536,6 +537,17 @@ struct SimLaunch {
   uint32_t* sched;                        // scratch [T][ceil(E/32)]
 };
 int launch_similar(Engine* e, const SimLaunch& s);
+// daemonsets.cu: cae_template_daemonsets.  In (device, uploaded by api.cu): ds_spec [D], evaluate [T] or NULL, running
+// [T][Dw] or NULL.  Out: bits [T][Dw], every word written; count [T], zeroed by api.cu.
+struct DsLaunch {
+  int N, T, D, Dw;
+  const int32_t* ds_spec;
+  const uint8_t* evaluate;
+  const uint32_t* running;
+  uint32_t* bits;
+  int32_t* count;
+};
+int launch_ds_verdicts(Engine* e, const DsLaunch& a);
 // scaledown.cu: cae_scale_down_eligibility.  In (device, uploaded by api.cu): the caller's arrays, flags NULL = all 0,
 // skip_ds / pre / unready as bytes (api.cu turns NULL into zeros).  Out: util [n][4], reason [n], list [n], count and status
 // (1 = a value left int64), every one written by the launch.

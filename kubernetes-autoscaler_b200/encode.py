@@ -862,6 +862,18 @@ class SimilarityInputs(AbiArrays):
     COUNTS = {"num_ignored_keys": "ignored_keys"}
 
 
+class DaemonSetInputs(AbiArrays):
+    """``cae_daemonset_inputs`` of cae_template_daemonsets.  The optional arrays left out are NULL; num_ds follows ds_spec."""
+
+    STRUCT = capi.cae_daemonset_inputs
+    COUNTS = {"num_ds": "ds_spec"}
+
+    def __init__(self, **fields) -> None:
+        for nm in ("evaluate", "running", "keep"):
+            fields.setdefault(nm, None)
+        super().__init__(**fields)
+
+
 class EligibilityInputs(AbiArrays):
     """``cae_eligibility_inputs`` of cae_scale_down_eligibility.  The optional arrays left out are NULL; n_pod_flags follows
     pod_flags unless given."""
@@ -1330,6 +1342,14 @@ class Encoder:
                               pod_spec=[x for st in rows for x in st[10]])
         self._templates = list(zip(keys, states))
         return delta
+
+    def note_template_pods(self, enc: EncodedObjects) -> None:
+        """Take the template pod lists of `enc` as what the engine holds, after a call that changed them on the device
+        (cae_template_daemonsets with keep), so that the next template_delta compares against them."""
+        a, N = enc.arrays, enc.struct.num_cluster_nodes
+        off, spec = a["node_pod_off"], a["node_pod_spec"]
+        self._templates = [(k, st[:10] + (tuple(int(x) for x in spec[off[N + t]:off[N + t + 1]]),))
+                           for t, (k, st) in enumerate(self._templates)]
 
     def pod_delta(self, groups: Sequence[PodEquivalenceGroup], residents: Sequence[NodeInfo] = ()) -> "PodDelta":
         """The shim's side of cae_load_pods: `groups` become the complete new pending list, and every spec and dictionary

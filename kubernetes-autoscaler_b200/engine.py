@@ -10,7 +10,7 @@ from typing import Optional, Sequence, Tuple
 import numpy as np
 
 from . import capi
-from .encode import EligibilityInputs, EncodedObjects, PriceInputs, RemovalPlan, ResidentRemovals, SimilarityInputs
+from .encode import DaemonSetInputs, EligibilityInputs, EncodedObjects, PriceInputs, RemovalPlan, ResidentRemovals, SimilarityInputs
 
 
 class EngineError(RuntimeError):
@@ -463,6 +463,30 @@ class Engine:
         limit = np.zeros(T, np.int64)
         self._check(self.lib.cae_similar_node_groups(self.h, si.ptr(), _vp(bits), _vp(count), _vp(limit)))
         return bits, count, limit
+
+    def template_daemonsets(self, ds_spec, evaluate=None, running=None, keep=None, enc: Optional[EncodedObjects] = None):
+        """cae_template_daemonsets: NodeShouldRunDaemonPod of every loaded template and DaemonSet spec ds_spec [D].
+        evaluate [T] flags (None = all); running [T][ceil(D/32)] uint32 bits of the DaemonSets already on the example node
+        (None = none); keep [T] (None = report only): each evaluated template keeps its first keep[t] pods and gets the
+        pods of its bits after them.  Returns (bits [T][ceil(D/32)] uint32, count [T] int32).  After an apply this object's
+        shapes follow daemonset.apply_run_bits (`enc`: the objects after the call, when the caller has them).  Raises
+        EngineUnsupported when the apply is refused (status 1 or 2); the engine is unchanged then."""
+        T = self.enc.T
+        ds = np.ascontiguousarray(ds_spec, np.int32).reshape(-1)
+        Dw = (len(ds) + 31) // 32
+        di = DaemonSetInputs(ds_spec=ds, evaluate=_opt(evaluate, np.uint8), running=_opt(running, np.uint32), keep=_opt(keep, np.int32))
+        for nm, shape in (("evaluate", (T,)), ("keep", (T,)), ("running", (T, Dw))):
+            if nm in di.arrays and di.arrays[nm].size != int(np.prod(shape)):
+                raise ValueError("template_daemonsets: %s needs %s entries" % (nm, shape))
+        bits = np.zeros((T, Dw), np.uint32)
+        count = np.zeros(T, np.int32)
+        self._check(self.lib.cae_template_daemonsets(self.h, di.ptr(), _vp(bits), _vp(count)))
+        if keep is not None:
+            if enc is None:
+                from .daemonset import apply_run_bits, unpack_rows
+                enc = apply_run_bits(self.enc, ds, unpack_rows(bits, len(ds)), di.arrays["keep"], evaluate)[1]
+            self.enc = enc
+        return bits, count
 
     def scale_down_eligibility(self, cand_node, gpu_dim, threshold, pod_flags=None, skip_ds=None, skip_mirror: bool = False,
                                pre_reason=None, unready=None):

@@ -117,6 +117,8 @@ class Pod:
     phase: str = ""
     restart_policy: str = "Always"
     local_storage: bool = False
+    # spec.hostNetwork: read only by the daemon tolerations of a DaemonSet pod (daemonset.py)
+    host_network: bool = False
 
     def clone(self) -> "Pod":
         return copy.deepcopy(self)
