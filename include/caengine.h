@@ -386,6 +386,39 @@ typedef struct cae_node_churn {
 } cae_node_churn;
 int32_t cae_load_node_churn(cae_engine* e, const cae_node_churn* c);
 
+/* The scale-up's UPCOMING nodes as cluster rows: one copy of a node-group template per node a scale-up asked for that has
+ * not registered yet, together with the loop's node churn, in one rebuild of the resident snapshot.  Replaces: the fake
+ * nodes of StaticAutoscaler.getUpcomingNodeInfos (a SanitizedNodeInfo of the group's template per upcoming node, the
+ * registered-not-ready nodes left out), which the filter pass then packs pending pods onto, so that pods a scale-up already
+ * provisioned for do not trigger a second one.  Nothing but the copies' names and label sets travels: a copy's other
+ * columns and its resident pods are read from its template where they already are.
+ * The new cluster list is the surviving rows in their old order, then the churn's added rows, then the copies in the given
+ * order; template t moves to row N' + t.  A copy has its template's allocatable, allowed pods, taint list, unschedulable
+ * and resident pod list (the DaemonSet / mirror pods); its node name and label set are the caller's; like any added cluster
+ * row it has no capacity and no has_alloc_*.  Following SanitizedNodeInfo, the caller's label set is the template's labels
+ * with hostname_key set to the copy's name; the engine does not check that (any label set is valid), so the caller's
+ * interner stays the only one that mints ids.  The copies are ordinary rows afterwards: the next loop removes them
+ * through `churn->removed`, and they are kept out of scale-down through the callers' candidate lists and dest_ok.
+ * After the call every entry point answers bit-identically to a cae_load of the objects in that order (the churn's
+ * objects with the copies appended as added rows).  At world_size > 1 every rank applies the same call.
+ * Status -2 (malformed, nothing changed): every cause of cae_load_node_churn on `churn`; num_upcoming < 0; NULL arrays with
+ *   num_upcoming > 0; a template index outside [0, T); a negative node-name id; a label-set id outside the resident tables
+ *   plus the tails of `churn->changed`.
+ * Status 2 (the call does not apply: call cae_load with the full snapshot; nothing is changed): every cause of
+ *   cae_load_node_churn, counted with the copies: the node rows and template copies (N' + 2T, the copies included) or the
+ *   resident pods of all nodes (the copies' template pods included) would pass 2^31 - 1. */
+typedef struct cae_upcoming_nodes {
+  int32_t abi_version;           /* CAE_ABI_VERSION */
+  const cae_node_churn* churn;   /* the loop's real-node changes, applied in the same rebuild (dirty rows, removed rows: the
+                                    registered-not-ready nodes and the previous loop's copies, added real nodes); its
+                                    `changed` also carries the value / label-set tails the copies use; NULL = none */
+  int32_t num_upcoming;
+  const int32_t* template_idx;   /* [num_upcoming] template each copy is made from, in [0, T) */
+  const int32_t* name;           /* [num_upcoming] node-name id (>= 0) */
+  const int32_t* labelset;       /* [num_upcoming] the copy's label set (resident or tail) */
+} cae_upcoming_nodes;
+int32_t cae_add_upcoming_nodes(cae_engine* e, const cae_upcoming_nodes* u);
+
 /* The per-tick delta of the node-group TEMPLATES: templates removed (a node group went away), changed (a DaemonSet rolled
  * out, the template-from-real-node provider picked another sample node) and added (a new node group), against the
  * snapshot that is already resident.  Replaces: the TemplateNodeInfoProvider refresh between two loops, which the other

@@ -100,6 +100,10 @@ class cae_node_churn(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_node_churn", {"cae_node_delta": cae_node_delta})
 
 
+class cae_upcoming_nodes(C.Structure):
+    _fields_ = _parse_struct(_SRC, "cae_upcoming_nodes", {"cae_node_churn": cae_node_churn})
+
+
 class cae_template_delta(C.Structure):
     _fields_ = _parse_struct(_SRC, "cae_template_delta", {"cae_node_delta": cae_node_delta})
 
@@ -129,7 +133,7 @@ class cae_removal_plan(C.Structure):
 
 
 _STRUCTS = {s.__name__: s for s in (cae_objects, cae_config, cae_stats, cae_price_inputs, cae_node_delta, cae_node_churn,
-                                     cae_template_delta, cae_pod_delta, cae_similarity_inputs, cae_daemonset_inputs,
+                                     cae_upcoming_nodes, cae_template_delta, cae_pod_delta, cae_similarity_inputs, cae_daemonset_inputs,
                                      cae_eligibility_inputs,
                                      cae_resident_removals, cae_removal_plan)}
 

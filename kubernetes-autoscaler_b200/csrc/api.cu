@@ -967,13 +967,15 @@ struct RowsIn {
   const int64_t* alloc = nullptr;
 };
 
-// One cae_load_nodes or cae_load_node_churn call: its input, then what check_nodes derived from it
+// One cae_load_nodes, cae_load_node_churn or cae_add_upcoming_nodes call: its input, then what check_nodes derived from it
 struct NodePlan {
   const cae_node_delta* dl = nullptr;   // dictionary tails and dirty rows (row numbers before the call)
   Tails tails;
   RowsIn dirty, added;
   const int32_t *removed = nullptr, *name = nullptr;   // churn: removed rows, node names of the added rows
   int nr = 0;
+  int nu = 0;                                          // upcoming copies: template, node name and label set of each
+  const int32_t *up_tmpl = nullptr, *up_name = nullptr, *up_ls = nullptr;
   int64_t npods_d = 0, npods_a = 0, total = 0;
   int64_t rows_after = -1;   // cae_load_templates: the node rows and template copies after the call (-1: those of a churn)
   int64_t drop = 0;          // cae_load_templates: the pods of the templates the call replaces or removes
@@ -1008,10 +1010,10 @@ static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed)
   if (dl->abi_version != CAE_ABI_VERSION) return bad("abi_version mismatch");
   const Engine::NodeHost& nh = e->nh;
   const int N = e->N, S = e->num_podspecs;
-  const int nd = dl->num_dirty, na = p.added.n, nr = p.nr;
+  const int nd = dl->num_dirty, na = p.added.n, nr = p.nr, nu = p.nu;
   Tails& v = p.tails;
   v = node_tails(dl);
-  if (nd < 0 || na < 0 || nr < 0) return bad("negative count");
+  if (nd < 0 || na < 0 || nr < 0 || nu < 0) return bad("negative count");
   { const int rc = tails_present(v, bad); if (rc) return rc; }
   auto rows_null = [](const RowsIn& r) {
     return r.n && (!r.labelset || !r.taint_list || !r.unsched || !r.alloc || !r.allowed || !r.pod_off);
@@ -1019,7 +1021,8 @@ static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed)
   if (rows_null(p.dirty) || (nd && !dl->row)) return bad("dirty rows without arrays");
   if (nr && !p.removed) return bad("removed rows without an array");
   if (rows_null(p.added) || (na && !p.name)) return bad("added rows without arrays");
-  const int64_t rows_after = p.rows_after >= 0 ? p.rows_after : (int64_t)N - nr + na + 2 * (int64_t)e->T;
+  if (nu && (!p.up_tmpl || !p.up_name || !p.up_ls)) return bad("upcoming copies without arrays");
+  const int64_t rows_after = p.rows_after >= 0 ? p.rows_after : (int64_t)N - nr + na + nu + 2 * (int64_t)e->T;
   if (rows_after > INT32_MAX) return refuse("the node rows and template copies would pass 2^31 - 1");
   { const int rc = tails_offsets(v, bad); if (rc) return rc; }
   if (nd && !offsets_ok(dl->pod_off, nd)) return bad("resident-pod offsets");
@@ -1048,6 +1051,12 @@ static int check_nodes(Engine* e, const char* who, NodePlan& p, bool topo_fixed)
     if (p.name[i] < 0) return bad("node-name id of an added row out of range");
     if (p.added.labelset[i] < 0 || p.added.labelset[i] >= NL) return bad("label-set id of an added row out of range");
     if (p.added.taint_list[i] < 0 || p.added.taint_list[i] >= NTL) return bad("taint-list id of an added row out of range");
+  }
+  for (int i = 0; i < nu; ++i) {   // a copy's resident pods are its template's
+    if (p.up_tmpl[i] < 0 || p.up_tmpl[i] >= e->T) return bad("template index of an upcoming copy out of range");
+    if (p.up_name[i] < 0) return bad("node-name id of an upcoming copy out of range");
+    if (p.up_ls[i] < 0 || p.up_ls[i] >= NL) return bad("label-set id of an upcoming copy out of range");
+    total += nh.tmpl_pods[p.up_tmpl[i]];
   }
   total += p.npods_a;
   if (total > INT32_MAX) return refuse("more than 2^31 - 1 resident pods");
@@ -1089,23 +1098,23 @@ template <class T>
 static Extra extra_of(const std::vector<T>& v) { return {v.data(), v.size() * sizeof(T)}; }
 
 // One staged blob and one H2D copy: the dictionary tails, the staged rows (dirty rows, then added ones) with their run
-// state (cluster_row_state), and the caller's `extra` arrays (their device copies in xdev); then the dictionary tables
-// grow on the device.  After commit_nodes.
+// state (cluster_row_state), the upcoming copies' name, label set and template row, and the caller's `extra` arrays (their
+// device copies in xdev); then the dictionary tables grow on the device.  After commit_nodes.
 static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<Extra>& extra, NodeDeltaDev* dd, std::vector<const void*>* xdev) {
   const cae_node_delta* dl = p.dl;
   const int A = e->A;
-  const int nd = p.dirty.n, na = p.added.n, ns = nd + na;
+  const int nd = p.dirty.n, na = p.added.n, ns = nd + na, nu = p.nu;
   const int64_t npods = p.npods_d + p.npods_a;
   Engine::Staging& s = e->nd;
   char* tab[NUM_DICT_TABLES] = {};
   NodeDeltaDev d{};
-  d.nd = nd; d.na = na;
+  d.nd = nd; d.na = na; d.nu = nu;
   std::vector<char*> xd(extra.size());
   auto walk = [&](Layout& l) {
     tails_layout(l, p.tails, tab);
     l.add(d.alloc, (size_t)ns * R); l.add(d.cfree, (size_t)ns * A);
-    l.add(d.row, nd); l.add(d.name, na); l.add(d.labelset, ns); l.add(d.taint_list, ns); l.add(d.allowed, ns); l.add(d.cslots, ns);
-    l.add(d.pod_off, (size_t)ns + 1); l.add(d.pod_spec, npods); l.add(d.unsched, ns);
+    l.add(d.row, nd); l.add(d.name, na + nu); l.add(d.labelset, ns + nu); l.add(d.taint_list, ns); l.add(d.allowed, ns);
+    l.add(d.cslots, ns); l.add(d.up_row, nu); l.add(d.pod_off, (size_t)ns + 1); l.add(d.pod_spec, npods); l.add(d.unsched, ns);
     for (size_t x = 0; x < extra.size(); ++x) l.add(xd[x], extra[x].bytes);
   };
   const size_t bytes = layout_bytes(walk);
@@ -1114,6 +1123,9 @@ static int stage_nodes(Engine* e, const NodePlan& p, const std::vector<Extra>& e
   tails_put(e, p.tails, tab, s);
   std::copy(dl->row, dl->row + nd, s.host_of(d.row));
   std::copy(p.name, p.name + na, s.host_of(d.name));
+  std::copy(p.up_name, p.up_name + nu, s.host_of(d.name) + na);
+  std::copy(p.up_ls, p.up_ls + nu, s.host_of(d.labelset) + ns);
+  for (int j = 0; j < nu; ++j) s.host_of(d.up_row)[j] = e->N + p.up_tmpl[j];
   int32_t* poff = s.host_of(d.pod_off);
   poff[0] = 0;
   for (int part = 0, i0 = 0; part < 2; ++part) {   // the dirty rows, then the added ones
@@ -1167,33 +1179,40 @@ static int do_load_nodes(Engine* e, const cae_node_delta* dl) {
   return 0;
 }
 
-// cae_load_node_churn: the same checks and staging as cae_load_nodes plus the removed and added rows; then the row list is
-// rebuilt.  The host computes the new row -> source map, the resident counts and topology values of the new list and its
-// topology domains (assign_domains, as cae_load does); the device gathers the node columns and the resident CSR through
-// the map and reruns what a load derives from the node list: the class matrix over the whole universe, the template bits
-// and, with topology counters, the recount over every column.
-static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
-  if (c->abi_version != CAE_ABI_VERSION) { set_error("cae_load_node_churn: abi_version mismatch"); return -2; }
-  cae_node_delta none{};
-  none.abi_version = CAE_ABI_VERSION;
-  NodePlan p;
-  p.dl = c->changed ? c->changed : &none;
+static const cae_node_delta kNoNodeDelta = {CAE_ABI_VERSION};
+
+// The plan of a churn's rows (NULL: no churn)
+static int churn_plan(const char* who, const cae_node_churn* c, NodePlan& p) {
+  if (c && c->abi_version != CAE_ABI_VERSION) { set_error(std::string(who) + ": abi_version mismatch"); return -2; }
+  p.dl = c && c->changed ? c->changed : &kNoNodeDelta;
   p.dirty = dirty_rows(p.dl);
+  if (!c) return 0;
   p.added.n = c->num_added; p.added.labelset = c->labelset; p.added.taint_list = c->taint_list; p.added.allowed = c->allowed_pods;
   p.added.pod_off = c->pod_off; p.added.pod_spec = c->pod_spec; p.added.unsched = c->unschedulable; p.added.alloc = c->alloc;
   p.removed = c->removed; p.name = c->name; p.nr = c->num_removed;
-  { const int rc = check_nodes(e, "cae_load_node_churn", p, false); if (rc) return rc; }
+  return 0;
+}
+
+// cae_load_node_churn and cae_add_upcoming_nodes: the same checks and staging as cae_load_nodes plus the removed and added
+// rows and the upcoming copies; then the row list is rebuilt.  The host computes the new row -> source map, the resident
+// counts and topology values of the new list and its topology domains (assign_domains, as cae_load does); the device
+// gathers the node columns and the resident CSR through the map and reruns what a load derives from the node list: the
+// class matrix over the whole universe, the template bits and, with topology counters, the recount over every column.
+// A copy's resident count is its template's and its topology values are those of its own label set, so its domains are
+// the ones a load assigns to a cluster row with the copy's columns.
+static int apply_churn(Engine* e, const char* who, NodePlan& p) {
+  { const int rc = check_nodes(e, who, p, false); if (rc) return rc; }
   e->stats.h2d_bytes = 0;
   const cae_node_delta* dl = p.dl;
-  const int nd = p.dirty.n, na = p.added.n, nr = p.nr;
-  if (!dl->num_new_values && !dl->num_new_labelsets && !dl->num_new_taint_lists && !nd && !na && !nr) return 0;
+  const int nd = p.dirty.n, na = p.added.n, nr = p.nr, nu = p.nu;
+  if (!dl->num_new_values && !dl->num_new_labelsets && !dl->num_new_taint_lists && !nd && !na && !nr && !nu) return 0;
   commit_nodes(e, p);
-  if (!nd && !na && !nr) return stage_nodes(e, p, {}, nullptr, nullptr);
+  if (!nd && !na && !nr && !nu) return stage_nodes(e, p, {}, nullptr, nullptr);
 
-  // ---- the new row list on the host: survivors in their old order, the added nodes, the templates ----
+  // ---- the new row list on the host: survivors in their old order, the added nodes, the copies, the templates ----
   Engine::NodeHost& nh = e->nh;
   DynTables& dy = e->dyn;
-  const int oldN = e->N, T = e->T, N = oldN - nr + na, NT = N + T;
+  const int oldN = e->N, T = e->T, N = oldN - nr + na + nu, NT = N + T;
   const int K = e->has_dynamic ? dy.K : 0;
   std::vector<int32_t> src(NT), pod_cnt(N), key_val((size_t)K * N);
   int r = 0;
@@ -1211,6 +1230,11 @@ static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
     src[r] = -1 - (nd + j);
     pod_cnt[r] = p.added.pod_off[j + 1] - p.added.pod_off[j];
     for (int k = 0; k < K; ++k) key_val[(size_t)k * N + r] = label_of(e, dl, p.added.labelset[j], dy.key_id[k]);
+  }
+  for (int j = 0; j < nu; ++j, ++r) {
+    src[r] = -1 - (nd + na + j);
+    pod_cnt[r] = nh.tmpl_pods[p.up_tmpl[j]];
+    for (int k = 0; k < K; ++k) key_val[(size_t)k * N + r] = label_of(e, dl, p.up_ls[j], dy.key_id[k]);
   }
   for (int t = 0; t < T; ++t) src[N + t] = oldN + t;
   // topology domains of the new list, and the counter pool they size
@@ -1255,6 +1279,20 @@ static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
     if (launch_post_bits(e)) return -1;
   }
   return 0;
+}
+
+static int do_load_node_churn(Engine* e, const cae_node_churn* c) {
+  NodePlan p;
+  { const int rc = churn_plan("cae_load_node_churn", c, p); if (rc) return rc; }
+  return apply_churn(e, "cae_load_node_churn", p);
+}
+
+static int do_add_upcoming_nodes(Engine* e, const cae_upcoming_nodes* u) {
+  if (u->abi_version != CAE_ABI_VERSION) { set_error("cae_add_upcoming_nodes: abi_version mismatch"); return -2; }
+  NodePlan p;
+  { const int rc = churn_plan("cae_add_upcoming_nodes", u->churn, p); if (rc) return rc; }
+  p.nu = u->num_upcoming; p.up_tmpl = u->template_idx; p.up_name = u->name; p.up_ls = u->labelset;
+  return apply_churn(e, "cae_add_upcoming_nodes", p);
 }
 
 // The tables a load sizes by the template count (derive_pending and apply_dynamic allocate them in the arenas), laid out in
@@ -2516,6 +2554,14 @@ int32_t cae_load_node_churn(cae_engine* h, const cae_node_churn* c) {
   if (!c) { cae::set_error("cae_load_node_churn: no churn"); return -2; }
   cudaSetDevice(e->cfg.device);
   return cae::do_load_node_churn(e, c);
+}
+
+int32_t cae_add_upcoming_nodes(cae_engine* h, const cae_upcoming_nodes* u) {
+  Engine* e = reinterpret_cast<Engine*>(h);
+  if (!e || !e->loaded) { cae::set_error("cae_add_upcoming_nodes before cae_load"); return -2; }
+  if (!u) { cae::set_error("cae_add_upcoming_nodes: no input"); return -2; }
+  cudaSetDevice(e->cfg.device);
+  return cae::do_add_upcoming_nodes(e, u);
 }
 
 int32_t cae_load_templates(cae_engine* h, const cae_template_delta* d) {

@@ -404,8 +404,10 @@ int launch_class_matrix(Engine* e);      // pre_code[SC][U]: needs only the obje
 int launch_class_matrix_cols(Engine* e, const int32_t* d_cols, int ncols);   // pre_code[SC][cols] only
 int launch_dynamic_recount(Engine* e, const int32_t* d_cols, int ncols);     // elig of cols, cluster counters, post_code, qrec
 struct NodeDeltaDev {                    // device views into the staged rows of a delta or a churn (node_delta.cu)
-  int nd, na;                            // staged rows [0, nd) are dirty rows, [nd, nd + na) added nodes (churn)
-  const int32_t *row, *name;             // [nd] old row of a dirty row, [na] node name of an added one
+  int nd, na, nu;                        // staged rows [0, nd) are dirty rows, [nd, nd + na) added nodes (churn), then nu
+                                         // upcoming copies (cae_add_upcoming_nodes: name and label set only)
+  const int32_t *row, *name;             // [nd] old row of a dirty row, [na + nu] node name of an added row or a copy
+  const int32_t* up_row;                 // [nu] old row of each copy's template
   const int32_t *labelset, *taint_list, *allowed, *cslots, *pod_off, *pod_spec;
   const uint8_t* unsched;
   const int64_t *alloc, *cfree;          // [nd + na][R], [nd + na][A]
@@ -419,8 +421,9 @@ int launch_node_arrivals(Engine* e, const NodeDeltaDev& d, int64_t total);
 // force_add.cu: everything on the device that follows from the arrivals of launch_node_arrivals' `d`: the resident CSR, the
 // receiving rows' run state, their pre_code when an arrival holds host ports (`ports`), the topology counters
 int launch_force_add(Engine* e, const NodeDeltaDev& d, int64_t total, bool ports);
-// cae_load_node_churn and cae_load_templates: node columns, run state and resident CSR of the new row list of N' cluster rows
-// and T' templates; src [N'+T'] = old row, or -1 - staged row (staged rows are cluster rows of a churn or templates)
+// cae_load_node_churn, cae_add_upcoming_nodes and cae_load_templates: node columns, run state and resident CSR of the new row
+// list of N' cluster rows and T' templates; src [N'+T'] = old row, or -1 - staged row (staged rows are cluster rows of a
+// churn, upcoming copies, or templates)
 int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int N_new, int T_new, int64_t total);
 // cae_load_templates, after the domains of the new templates: elig of every column, ds_w and post_code (dyn_kernels.cu)
 int launch_template_dynamic(Engine* e);

@@ -7,8 +7,10 @@
 // cae_load_node_churn: the row list itself changes, so every node column is gathered into a new buffer through a map
 // new row -> source (an old row: a clean survivor or a shifted template; or a staged row: a dirty or an added node),
 // and the CSR is rebuilt through the same map.  Only the staged rows travel over PCIe; everything else is read where it
-// already is.  cae_load_templates uses the same gather with the cluster rows as their own sources and the templates routed
-// through the map (a surviving old template, or a staged changed / added one that carries its capacity columns).
+// already is.  cae_add_upcoming_nodes is a churn whose map has a third kind of source, a copy of template t: its name and
+// label set are staged, every other column, its run state and its list are read from the template.  cae_load_templates
+// uses the same gather with the cluster rows as their own sources and the templates routed through the map (a surviving
+// old template, or a staged changed / added one that carries its capacity columns).
 // cae_force_add_pods: the rows stay as they are and the receiving rows' lists grow: the same counts, scan and gather, with
 // the staged lists (the arrivals per receiving row) appended to the rows' old lists instead of replacing them.
 #include <cub/device/device_scan.cuh>
@@ -55,19 +57,27 @@ __global__ void nd_arrive_kernel(NodeDeltaDev d, int32_t* __restrict__ cnt, int3
   src[r] = -1 - i;
 }
 
-// one warp per new row: its list from the old CSR (src >= 0: old row) or from the staged rows (src < 0: row -1 - src);
+// The old row whose list a new row with source s takes: s itself (an old row), the template of an upcoming copy (staged
+// rows from nd + na on), or -1 (a dirty or added row: its list is staged)
+__device__ __forceinline__ int list_row(const NodeDeltaDev& d, int s) {
+  if (s >= 0) return s;
+  const int j = -1 - s - d.nd - d.na;
+  return j >= 0 ? d.up_row[j] : -1;
+}
+
+// one warp per new row: its list from the old CSR (list_row >= 0) or from the staged rows (src < 0: row -1 - src);
 // `append`: a staged list follows the old list of the row (which keeps its place) instead of replacing it
 __global__ void nd_gather_kernel(const int32_t* __restrict__ old_off, const int32_t* __restrict__ old_spec,
                                  const int32_t* __restrict__ new_off, int NT, const int32_t* __restrict__ src, NodeDeltaDev d,
                                  bool append, int32_t* __restrict__ new_spec) {
   const int r = (int)(((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (r >= NT) return;
-  const int s = src[r];
+  const int s = src[r], os = list_row(d, s);
   const int b = new_off[r], n = new_off[r + 1] - b;
   const int32_t *old = nullptr, *staged = nullptr;
   int n_old = n;
-  if (s >= 0) {
-    old = old_spec + old_off[s];
+  if (os >= 0) {
+    old = old_spec + old_off[os];
   } else {
     staged = d.pod_spec + d.pod_off[-1 - s];
     n_old = append ? n - (d.pod_off[-s] - d.pod_off[-1 - s]) : 0;
@@ -85,10 +95,14 @@ struct NodeCols {
 
 // one thread per new row: every node column, the run state of a cluster row and the resident count, from the row's source.
 // An added node has no capacity / has_alloc_* (read for templates only); a dirty row keeps those of its old row; a staged
-// template row (cae_load_templates: d.cap_cpu set) carries its own.
+// template row (cae_load_templates: d.cap_cpu set) carries its own.  An upcoming copy of template t (old row oldN + t) is
+// a cluster row with the template's columns but the staged name and label set, no capacity / has_alloc_*, and the run
+// state a load computes for it: allocatable minus the template pods' requests is the template's own (tmpl_free [A][T],
+// tmpl_slots [T] of the T templates before the call).
 __global__ void nc_columns_kernel(DevObjects o, NodeDeltaDev d, const int32_t* __restrict__ src, int NT, int N, int oldN, int A,
-                                  const int64_t* __restrict__ old_cfree, const int32_t* __restrict__ old_cslots, NodeCols c,
-                                  int32_t* __restrict__ cnt) {
+                                  const int64_t* __restrict__ old_cfree, const int32_t* __restrict__ old_cslots,
+                                  int T, const int64_t* __restrict__ tmpl_free, const int32_t* __restrict__ tmpl_slots,
+                                  NodeCols c, int32_t* __restrict__ cnt) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r > NT) return;
   if (r == NT) { cnt[NT] = 0; return; }
@@ -108,6 +122,18 @@ __global__ void nc_columns_kernel(DevObjects o, NodeDeltaDev d, const int32_t* _
     return;
   }
   const int i = -1 - s;
+  if (i >= d.nd + d.na) {   // an upcoming copy
+    const int u = list_row(d, s), t = u - oldN;
+    c.name[r] = d.name[i - d.nd]; c.labelset[r] = d.labelset[i];
+    c.taint_list[r] = o.node_taint_list[u]; c.unsched[r] = o.node_unschedulable[u]; c.allowed[r] = o.node_allowed_pods[u];
+    c.cap_cpu[r] = 0; c.cap_mem[r] = 0; c.has_cpu[r] = 0; c.has_mem[r] = 0;
+#pragma unroll
+    for (int k = 0; k < R; ++k) c.alloc[(size_t)r * R + k] = o.node_alloc[(size_t)u * R + k];
+    for (int a = 0; a < A; ++a) c.c_free[(size_t)a * N + r] = tmpl_free[(size_t)a * T + t];
+    c.c_slots[r] = tmpl_slots[t];
+    cnt[r] = o.node_pod_off[u + 1] - o.node_pod_off[u];
+    return;
+  }
   const int old = i < d.nd ? d.row[i] : -1, j = i - d.nd;
   const bool tmpl = d.cap_cpu != nullptr;
   c.name[r] = old >= 0 ? o.node_name[old] : d.name[j];
@@ -187,7 +213,8 @@ int launch_node_churn(Engine* e, const NodeDeltaDev& d, const int32_t* src, int 
   size_t tmp = 0;
   CAE_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp, cnt, new_off, NT + 1, e->stream));
   if (devbuf_reserve(e, e->nd_cub, tmp)) return -1;
-  nc_columns_kernel<<<(NT + 256) / 256, 256, 0, e->stream>>>(e->dobj, d, src, NT, N, e->N, e->A, e->d_c_free, e->d_c_slots, c, cnt);
+  nc_columns_kernel<<<(NT + 256) / 256, 256, 0, e->stream>>>(e->dobj, d, src, NT, N, e->N, e->A, e->d_c_free, e->d_c_slots, e->T,
+                                                             e->d_tmpl_free, e->d_tmpl_slots, c, cnt);
   CAE_CUDA(cub::DeviceScan::ExclusiveSum(e->nd_cub.p, tmp, cnt, new_off, NT + 1, e->stream));
   if (NT > 0)
     nd_gather_kernel<<<(unsigned)(((size_t)NT * 32 + 255) / 256), 256, 0, e->stream>>>(e->dobj.node_pod_off, e->dobj.node_pod_spec, new_off,

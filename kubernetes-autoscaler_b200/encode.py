@@ -542,6 +542,34 @@ class EncodedObjects:
         res.struct = out._restruct(a, num_cluster_nodes=len(keep) + na)
         return res
 
+    def apply_upcoming(self, up: "UpcomingNodes") -> "EncodedObjects":
+        """The objects after cae_add_upcoming_nodes(up), stated on the host: ``up.churn`` applied as apply_node_churn does,
+        then the copies appended after the cluster rows, before the templates.  A copy has its template's columns and
+        resident pods, its own node name and label set, and no capacity or has_alloc_*.  A cae_load of the result must
+        answer like the engine after the call."""
+        import copy
+        out = self.apply_node_churn(up.churn) if up.churn is not None else self
+        a, u = dict(out.arrays), up.arrays
+        N = out.struct.num_cluster_nodes
+        tr = N + np.asarray(u["template_idx"], np.int64)    # the template rows the copies are made from
+        nu = len(tr)
+        cols = {"node_name": u["name"], "node_labelset": u["labelset"], "node_cap_cpu": np.zeros(nu), "node_cap_mem": np.zeros(nu),
+                "node_has_alloc_cpu": np.zeros(nu), "node_has_alloc_mem": np.zeros(nu)}
+        for nm in ("node_name", "node_labelset", "node_taint_list", "node_unschedulable", "node_allowed_pods", "node_alloc",
+                   "node_cap_cpu", "node_cap_mem", "node_has_alloc_cpu", "node_has_alloc_mem"):
+            col = a[nm]
+            new = np.asarray(cols[nm], col.dtype) if nm in cols else col[tr]
+            a[nm] = np.ascontiguousarray(np.concatenate([col[:N], new.reshape((nu,) + col.shape[1:]), col[N:]]))
+        off, spec = a["node_pod_off"], a["node_pod_spec"]
+        rows = list(range(N)) + tr.tolist() + list(range(N, len(off) - 1))
+        pieces = [spec[off[r]:off[r + 1]] for r in rows]
+        a["node_pod_off"] = _i32(np.concatenate([[0], np.cumsum([len(p) for p in pieces], dtype=np.int64)]))
+        a["node_pod_spec"] = _i32(np.concatenate(pieces) if pieces else [])
+        res = copy.copy(out)
+        res.arrays = a
+        res.struct = out._restruct(a, num_cluster_nodes=N + nu)
+        return res
+
     def apply_template_delta(self, delta: "TemplateDelta") -> "EncodedObjects":
         """The objects after cae_load_templates(delta), stated on the host: the tails of ``delta.tails`` appended, then the
         template rows rebuilt: the surviving templates in their old order (a changed one replaced by its staged row in
@@ -815,6 +843,18 @@ class NodeChurn(AbiArrays):
 
     def __init__(self, changed: Optional[NodeDelta] = None, **arrays) -> None:
         super().__init__(changed=changed, **arrays)
+
+
+class UpcomingNodes(AbiArrays):
+    """``cae_upcoming_nodes``: ``churn`` (a NodeChurn with the loop's real-node changes and the dictionary tails the copies
+    use, or None) and the upcoming copies: template index, node-name id and label set of each."""
+
+    STRUCT, NESTED = capi.cae_upcoming_nodes, "churn"
+    COUNTS = {"num_upcoming": "template_idx"}
+    num_upcoming = _count("num_upcoming")
+
+    def __init__(self, churn: Optional[NodeChurn] = None, **arrays) -> None:
+        super().__init__(churn=churn, **arrays)
 
 
 class TemplateDelta(AbiArrays):
@@ -1279,6 +1319,30 @@ class Encoder:
                           allowed_pods=[st[4] for _, st in added], pod_off=po, pod_spec=[x for _, st in added for x in st[5]])
         self._cluster = new_list + added
         return churn
+
+    def upcoming_nodes(self, copies: Sequence[Tuple[int, NodeInfo]],
+                       new_cluster: Optional[Sequence[NodeInfo]] = None) -> "UpcomingNodes":
+        """The shim's side of cae_add_upcoming_nodes: `copies` = [(template index, sanitized copy)]
+        (upcoming.upcoming_node_infos) appended after the cluster nodes, with the loop's real cluster list `new_cluster` as
+        the churn of the same call (node_churn's rules; None = the real rows stay as they are).  Only each copy's node name
+        and label set are interned; its other columns and its pods are its template's as the engine holds them.  The
+        previous loop's copies are cluster rows like any other, so a `new_cluster` without them removes them.  The tails
+        the copies' label sets add travel in the churn's ``changed``."""
+        self._check_resident()
+        T = len(self._templates)
+        for t, _ in copies:
+            if not 0 <= t < T:
+                raise ValueError("upcoming nodes: template index %d out of range" % t)
+        names = [self.node_names(ni.node.name) for _, ni in copies]
+        ls = [self._labelset(ni.node.labels) for _, ni in copies]
+        if new_cluster is None:
+            churn = NodeChurn(self._tails_and_rows([], []))
+        else:
+            churn = self.node_churn(new_cluster)
+        for (t, _), nid, l in zip(copies, names, ls):
+            st = self._templates[t][1]
+            self._cluster.append((nid, (l, st[2], st[3], st[4], st[5], st[10])))
+        return UpcomingNodes(churn, template_idx=[t for t, _ in copies], name=names, labelset=ls)
 
     def _template_state(self, ni: NodeInfo) -> tuple:
         """(name, label set, taint list, unschedulable, allocatable, allowed pods, capacity cpu / memory, has_alloc cpu /

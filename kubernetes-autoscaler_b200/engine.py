@@ -166,6 +166,12 @@ class Engine:
         the engine is unchanged then."""
         return self._applied(self.lib.cae_load_node_churn(self.h, churn.ptr()))
 
+    def add_upcoming_nodes(self, up) -> bool:
+        """The scale-up's upcoming nodes as copies of their templates (cae_add_upcoming_nodes), applied with the loop's
+        node churn in one rebuild (encode.UpcomingNodes).  Returns False when the engine answers "use a full load" (status
+        2); the engine is unchanged then."""
+        return self._applied(self.lib.cae_add_upcoming_nodes(self.h, up.ptr()))
+
     def load_templates(self, delta, enc: Optional[EncodedObjects] = None) -> bool:
         """The per-tick delta of the node-group templates (cae_load_templates): removed, changed and added templates plus
         the dictionary tails they need (encode.TemplateDelta).  Returns False when the engine answers "use a full load"
